@@ -5,12 +5,12 @@
 
 One "step" = one eval forward of a batch of synthetic multi-view samples (4 views of 3x384x384 -> 17 joints,
 ResNet-152 backbone, 64^3 grid, softmax aggregation: BASELINE config #2, batch 8 per GPU) through the native
-sm_100a path.  Prints ONE JSON line (rank 0).  See the module docstrings / DESIGN.md for the field definitions.
+sm_90a path.  Prints ONE JSON line (rank 0).  See the module docstrings / DESIGN.md for the field definitions.
 
   value     device-timed throughput, inputs resident in HBM (CUDA events around K graph replays, max over ranks)
   e2e       same metric through the public nn.Module call with pinned-host images copied H2D and the keypoints
             read back D2H inside the timed region
-  roofline  dominant kernel (tcgen05 conv): algorithmic conv FLOPs / summed per-launch CUDA-event time, vs the
+  roofline  dominant kernel (tensor-core conv): algorithmic conv FLOPs / summed per-launch CUDA-event time, vs the
             measured dense bf16 peak (MEASURED_PEAKS.json); unprojection / soft-argmax HBM rooflines alongside
   cpu_baseline  the CPU oracle port of the reference path timed on this box's host cores (rank 0, bounded sample)
 
@@ -57,6 +57,7 @@ def parse():
     ap.add_argument("--no-config5", action="store_true", help="N = 1 only: skip the extra line for BASELINE config #5 (algebraic model)")
     ap.add_argument("--no-torch-gpu", action="store_true", help="skip the ATen/cuDNN secondary bars (fp32 and TF32) of the native arm")
     ap.add_argument("--no-calibrate", action="store_true", help="keep PyTorch default init (faster start, degenerate signal)")
+    ap.add_argument("--dump-outputs", metavar="DIR", help="single-GPU native arm: write the outputs of the last timed step as DIR/<name>.npy")
     return ap.parse_args()
 
 
@@ -65,11 +66,11 @@ def peaks():
     if os.path.exists(path):
         p = json.load(open(path))
         return {"hbm_gbs": p["hbm_gbs"], "bf16_tflops": p.get("bf16_tflops_sustained", p["bf16_tflops"]), "src": "measured"}
-    return {"hbm_gbs": 6650.0, "bf16_tflops": 1400.0, "src": "fallback"}
+    return {"hbm_gbs": 3350.0, "bf16_tflops": 989.0, "src": "H100 SXM data sheet (700 W)"}
 
 
 class ClockSampler(threading.Thread):
-    """nvidia-smi clock / throttle-reason samples during the timed region (B200_PROFILING.md recipe)."""
+    """nvidia-smi clock / throttle-reason samples during the timed region."""
 
     def __init__(self, index):
         super().__init__(daemon=True)
@@ -220,7 +221,7 @@ def algebraic_rate(args, dev, vol_model, images_dev, batch, flush):
 
 
 def main_torch_gpu(args, rank):
-    """Secondary bar (SURVEY 8d): the reference's own formulation -- torch ops through ATen/cuDNN -- on one B200, eval mode."""
+    """Secondary bar (SURVEY 8d): the reference's own formulation -- torch ops through ATen/cuDNN -- on one GPU, eval mode."""
     if rank != 0:
         return
     import lt_b200
@@ -401,6 +402,24 @@ def reduce_max(vals, dev, dist):
     return [float(v) for v in t]
 
 
+DUMP_SAMPLE = 1 << 20   # elements kept of an output larger than that (a fixed, seeded sample)
+
+
+def output_arrays(out):
+    """Host copies of what model(images, None, batch) returns (volumetric path), float32; outputs larger than DUMP_SAMPLE
+    elements are reduced to the same seeded sample of flat indices in every run (the indices go along as <name>_index)."""
+    kp, feats, vols, _, _, coords, base = out
+    arrays = {}
+    for name, t in (("keypoints_3d", kp), ("features", feats), ("volumes", vols), ("coord_volumes", coords), ("base_points", base)):
+        a = t.detach().float().cpu().numpy()
+        if a.size > DUMP_SAMPLE:
+            idx = np.sort(np.random.RandomState(0).choice(a.size, DUMP_SAMPLE, replace=False))
+            arrays[name + "_index"] = idx.astype(np.float64)
+            a = a.ravel()[idx]
+        arrays[name] = a.astype(np.float32)
+    return arrays
+
+
 def main_native(args, rank, world, local_rank):
     import lt_b200
     from lt_b200 import testing
@@ -409,6 +428,8 @@ def main_native(args, rank, world, local_rank):
     torch.cuda.set_device(local_rank)
     dev = torch.device("cuda", local_rank)
     dist = None
+    if world > 1 and args.dump_outputs:
+        raise SystemExit("bench.py --dump-outputs covers the single-GPU arm (--gpus 1)")
     if world > 1:
         import torch.distributed as dist
         dist.init_process_group("nccl", device_id=dev)
@@ -424,7 +445,7 @@ def main_native(args, rank, world, local_rank):
     model = model.to(dev).eval()
     eng = model.engine()
     model.clone_outputs = False
-    flush = torch.empty(256 * 1024 * 1024 // 4, dtype=torch.float32, device=dev)   # > 126 MB L2
+    flush = torch.empty(256 * 1024 * 1024 // 4, dtype=torch.float32, device=dev)   # > 50 MB L2 of the H100
 
     def barrier():
         torch.cuda.synchronize()
@@ -456,12 +477,13 @@ def main_native(args, rank, world, local_rank):
                 flush.zero_()
                 e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
                 e0.record()
-                step(images_dev)
+                timed_out = model(images_dev, None, batch)
                 e1.record()
                 evs.append((e0, e1))
             barrier()
             dev_ms = sum(a.elapsed_time(b) for a, b in evs)
             clocks = sampler.summary()
+            dumped = output_arrays(timed_out) if args.dump_outputs else None   # the model's output buffers are reused by later steps
 
             # ---- end-to-end arm, synchronous: pinned host images -> device, forward, keypoints -> host ----
             for _ in range(2):
@@ -585,11 +607,7 @@ def main_native(args, rank, world, local_rank):
     pk = peaks()
     roof = None
     extra = {}
-    traffic = {}
-    tpath = os.path.join(ROOT, "profiles", "ncu_traffic.json")   # DRAM bytes per launch from the committed ncu launch list
-    if os.path.exists(tpath):
-        traffic = json.load(open(tpath))
-    kernel_names = {"conv_tc": "conv_tc_kernel", "conv_pair": "conv_pair_kernel", "conv_fold": "conv_fold_kernel", "conv_tail": "v2v_tail_kernel",
+    kernel_names = {"conv_tc": "conv_tc_kernel", "conv_pair": "conv_tc_kernel", "conv_fold": "conv_tc_kernel", "conv_tail": "v2v_tail_kernel",
                     "conv_ffma": "conv_simt_kernel"}
     tensor_kernels = [k for k in kernel_names if k in agg]
     conv_key = max(tensor_kernels, key=lambda k: agg[k][0]) if tensor_kernels else None
@@ -601,7 +619,6 @@ def main_native(args, rank, world, local_rank):
         peak = pk["bf16_tflops"] if tc else 75.0
         r = {"kernel": kernel_names[key],
              "bound": "tensor", "achieved": ach, "peak": peak, "unit": "TFLOP/s", "frac": ach / peak,
-             "traffic": traffic.get(kernel_names[key]),
              "launches": cnt, "ms_per_step": ms,
              "peak_source": pk["src"] + (" sustained dense bf16/fp16 (cuBLAS)" if tc else " nominal fp32 FFMA"),
              "timing": "per-launch CUDA-event pairs in one eager (graph-free) step; graph replay is up to ~6 % faster"}
@@ -629,12 +646,8 @@ def main_native(args, rank, world, local_rank):
             ms, fl, nb, cnt = agg[key]
             ach = nb / (ms / 1e3) / 1e9
             extra["roofline_" + key] = {"bound": "hbm", "achieved": ach, "peak": pk["hbm_gbs"], "unit": "GB/s",
-                                        "frac": ach / pk["hbm_gbs"], "ms_per_step": ms, "launches": cnt, "traffic": traffic.get(key),
+                                        "frac": ach / pk["hbm_gbs"], "ms_per_step": ms, "launches": cnt,
                                         "peak_source": pk["src"] + " copy bandwidth"}
-    if traffic.get("_source") or traffic.get("source"):
-        traffic.setdefault("_source", traffic.get("source"))
-    if traffic.get("_source"):
-        extra["traffic_source"] = traffic["_source"]
     extra["step_breakdown_ms"] = {k: round(v[0], 3) for k, v in agg.items()}
 
     cpu = None
@@ -664,7 +677,7 @@ def main_native(args, rank, world, local_rank):
 
     torch_bars = {}
     if rank == 0 and world == 1 and not args.no_torch_gpu:
-        # secondary bar (SURVEY 8d): the reference's own torch formulation through ATen/cuDNN on the same B200, same weights/inputs
+        # secondary bar (SURVEY 8d): the reference's own torch formulation through ATen/cuDNN on the same GPU, same weights/inputs
         sd_dev = model.state_dict()
         for key, tf32 in (("torch_gpu", False), ("torch_gpu_tf32", True)):
             try:
@@ -677,7 +690,7 @@ def main_native(args, rank, world, local_rank):
         line = {
             "metric": METRIC, "value": value, "unit": "samples/s", "n_gpus": world, "steps": args.steps, "warmup": max(args.warmup, 3),
             "ms_per_step": dev_ms / args.steps, "higher_is_better": True, "scaling": "weak", "vs_baseline": None,
-            "dtype": {"tc": "fp16x3 (split-fp16 operands, 3 tcgen05 products per term, fp32 accumulate)", "tc1": "fp16", "simt": "f32"}[args.mode],
+            "dtype": {"tc": "fp16x3 (split-fp16 operands, 3 wgmma products per term, fp32 accumulate)", "tc1": "fp16", "simt": "f32"}[args.mode],
             "data": "synthetic",
             "config": {"workload": "Volumetric(softmax) ResNet-%d, %d views %dx%d, %d^3 grid, batch %d per GPU"
                                    % (args.layers, V, S, S, n, B),
@@ -705,6 +718,10 @@ def main_native(args, rank, world, local_rank):
         line.update(torch_bars)
         line.update(extra)
         print(json.dumps(line), flush=True)
+    if args.dump_outputs and rank == 0:
+        os.makedirs(args.dump_outputs, exist_ok=True)
+        for name, a in dumped.items():
+            np.save(os.path.join(args.dump_outputs, name + ".npy"), a)
     if dist is not None:
         dist.destroy_process_group()
 

@@ -1,5 +1,5 @@
 /*
- * lt_b200.h -- C ABI of liblt_b200.so: the B200 (sm_100a) kernels behind the volumetric
+ * lt_b200.h -- C ABI of liblt_b200.so: the H100 (sm_90a) kernels behind the volumetric
  * triangulation hot path of karfly/learnable-triangulation-pytorch.
  *
  * The reference is 100% Python/PyTorch: it has no FFI for this path.  Each entry point
@@ -44,47 +44,42 @@ enum lt_agg { LT_AGG_SUM = 0, LT_AGG_MAX = 1, LT_AGG_SOFTMAX = 2, LT_AGG_CONF = 
 /* conv implementation selector */
 enum lt_conv_impl {
   LT_CONV_SIMT = 0, /* fp32 FFMA implicit GEMM (exact, any shape) */
-  LT_CONV_TC = 1,   /* tcgen05, split-fp16 3-term products (fp32-grade) */
-  LT_CONV_TC1 = 2,  /* tcgen05, high parts only (plain fp16 precision, fast mode) */
-  LT_CONV_TC_FOLD = 3, /* tcgen05, kw taps folded into N, persistent (Cin = 32 cubic 3^3 / 7^3 stride-1 layers; weights from
+  LT_CONV_TC = 1,   /* wgmma, split-fp16 3-term products (fp32-grade) */
+  LT_CONV_TC1 = 2,  /* wgmma, high parts only (plain fp16 precision, fast mode) */
+  LT_CONV_TC_FOLD = 3, /* wgmma over all 32 output channels (Cin = 32 cubic 3^3 / 7^3 stride-1 layers; weights from
                          lt_conv_fold_pack_weights; desc->Cout = real channel count <= 32, FC = 32) */
-  LT_CONV_TC_PAIR = 4  /* tcgen05 cta_group::2: CTA pairs compute 256 x {128,256} tiles, persistent, 3-term products into one
-                         accumulator (layers with Cout % 128 == 0 that lt_conv_pair_eligible accepts; weights from
-                         lt_conv_pair_pack_weights) */
+  LT_CONV_TC_PAIR = 4  /* wgmma, 3-term products, weights padded to 128 output channels (layers with Cout % 128 == 0 that
+                         lt_conv_pair_eligible accepts; weights from lt_conv_pair_pack_weights) */
 };
 
 /* residual placement in the conv epilogue */
 enum lt_residual { LT_RES_NONE = 0, LT_RES_BEFORE_RELU = 1, LT_RES_AFTER_RELU = 2 };
 
 /* Kernel-selection options: the ONLY mutable process-wide state of the library besides its caches (encoded tensor maps,
- * per-device function attributes).  Every field defaults to the measured-best path; the alternatives stay reachable for A/B
- * measurements on the same box.  Set once before launching (lt_set_options is not synchronised against concurrent launches);
+ * per-device function attributes).  Set once before launching (lt_set_options is not synchronised against concurrent launches);
  * no entry point reads the environment. */
 typedef struct lt_options {
-  int tc_persist;          /* conv_tc: persistent variant 0 = never, 1 = tiny-tile layers (default), 2 = whenever possible */
+  /* sm_90a: the variants of the first (tensor-memory) kernels that these fields selected are one wgmma kernel; the fields
+     marked "no effect" are kept for ABI compatibility and ignored */
+  int tc_persist;          /* no effect */
   int tc_splitk;           /* conv_tc: split-K for grids below half the SMs (default 1) */
-  int tc_bres;             /* conv_tc: B-resident persistent variant for K-short 1x1 layers (default 1) */
-  int tc_direct_epilogue;  /* conv_tc: register epilogue with plain stores instead of the staged TMA epilogue (default 0) */
-  int fold_fast_issue;     /* conv_fold: unrolled uniform-register MMA issue loop (default 1) */
-  int fold_debug;          /* conv_fold: 0 = off; 1..3 = stage knock-outs of tools/fold_probe.py; 16 = wait counters to stderr */
+  int tc_bres;             /* no effect */
+  int tc_direct_epilogue;  /* no effect */
+  int fold_fast_issue;     /* no effect */
+  int fold_debug;          /* no effect */
   int softargmax_stream;   /* soft-argmax: streaming TMA kernels for compact channels-last logits (default 1) */
   int unproject_v2;        /* unprojection: production-shape kernel (default 1) */
   int unproject_cpl;       /* unprojection v2: channels per lane, 4 (default) or 8 */
   int unproject_lb;        /* unprojection v2: min CTAs / SM override (0 = per-variant default) */
-  int unproject_brick;     /* unprojection v2: side of the voxel bricks a CTA walks (0 = linear order, default: measured faster) */
+  int unproject_brick;     /* unprojection v2: side of the voxel bricks a CTA walks (0 = linear order, default) */
   int unproject_brick_order; /* voxel order inside a brick: 0 = z fastest, 1 = x fastest, 2 = 2 x 2 (x, y) tiles (voxels of a warp share taps) */
-  int pair_nt, pair_stages; /* conv_pair A/B overrides: N tile (0 = heuristic, 128, 256), operand ring depth cap (0 = as many as fit) */
-  int pair_prof;           /* conv_pair: 1 = per-role wait counters to stderr after every launch (debug; synchronises) */
-  int pair_direct_out;     /* conv_pair: split-fp16 outputs stored from registers (1, default) or staged + TMA store (0) */
-  int pair_two_acc;        /* conv_pair: the hi*lo + lo*hi products accumulate in their own TMEM accumulator (1, default) or share the main
-                              one (0: 2.4 % faster, but 3x as many TRUNCATING tcgen05 accumulation steps on the main accumulator: the
-                              full-size config #2 parity then misses the 1e-3 contract, profiles/r02i_accumulation.md) */
-  int fold_pair;           /* conv_fold: CTA-pair variant (cta_group::2, each CTA fetches half of every weight operand): 0 = never, 1 = layers
-                              whose weights are streamed (7^3; default: measured 8 % faster there, neutral on the weight-resident 3^3), 2 = always */
-  int fold_direct;         /* conv_fold: full-width split-fp16 tiles stored from registers, residual read from global memory (default 0:
-                              measured 15-20 % slower than the staged TMA epilogue on the 3^3 layers -- 32-sector row stores / loads) */
-  int fold_fullw;          /* conv_fold: full-width M tiles (W in {16, 32, 64}: every MMA row is an output position, the kw shift crosses
-                              warps through shared memory) (1, default) or 16/32-position x windows with K-1 wasted rows each (0) */
+  int pair_nt, pair_stages; /* no effect */
+  int pair_prof;           /* no effect */
+  int pair_direct_out;     /* no effect */
+  int pair_two_acc;        /* no effect: the hi*lo + lo*hi products always accumulate in their own accumulator */
+  int fold_pair;           /* no effect */
+  int fold_direct;         /* no effect */
+  int fold_fullw;          /* no effect */
 } lt_options;
 void lt_default_options(lt_options* o);
 int lt_get_options(lt_options* o);
@@ -225,7 +220,7 @@ typedef struct lt_conv_desc {
 int lt_conv_nd_fwd(const lt_conv_desc* desc, const void* in, const void* weight, const float* scale,
                    const float* shift, const void* residual, void* out, int impl, void* stream);
 
-/* Tensor-core (tcgen05) weight packing: float32 [taps][Cin][Cout] (host or device? -> DEVICE)
+/* Tensor-core weight packing: float32 [taps][Cin][Cout] (host or device? -> DEVICE)
  * to fp16 [taps][Cin/32][n tile][hi|lo][Nt][32] (64-byte rows; Nt = min(CoutP, 128), CoutP = round_up(Cout, 16));
  * Cin % 32 == 0. */
 size_t lt_conv_tc_weight_bytes(int taps, int Cin, int Cout);
@@ -236,9 +231,9 @@ int lt_conv_tc_pack_weights(const float* w_tap_ci_co, void* packed, int taps, in
  *   (td, th, tw, ci, co) is read from w[base + td*s_td + th*s_th + tw*s_tw + ci*s_ci + co*s_co] (nn.Conv: (Cout, Cin, k...);
  *   nn.ConvTranspose: (Cin, Cout, k...); stride phases of a transposed conv: a tap sub-lattice walked with negative strides).
  * lt_fold_bn_fwd: eval-mode BatchNorm (pose_resnet.py:30-31, v2v.py:12) + conv bias -> per-channel scale / shift [CP] (double
- *   arithmetic, rounded once); mean == NULL: no BatchNorm.  accum_steps: tcgen05.mma steps that accumulate into the main fp32
+ *   arithmetic, rounded once); mean == NULL: no BatchNorm.  accum_steps: tensor-core MMA steps that accumulate into the main fp32
  *   accumulator of the kernel that will consume this scale (taps x Cin / 16; 0 for the exact-fp32 kernels).  The tensor core adds
- *   with truncation, which shrinks a sum by an expected 0.28 x steps x 2^-24 (tools/accum_probe.py: 0.27-0.29 for K = 256..4608);
+ *   with truncation, which shrinks a sum by an expected 0.28 x steps x 2^-24 (rate measured on the tensor-memory MMA of the kernels' first target, not re-measured for wgmma);
  *   the scale is multiplied by 1 + that, which halves the rms accumulation error.
  * lt_absmax_fwd: float bit pattern of max|w| over n elements.  Passed (optionally, else NULL) to the two calls above it selects the
  *   power-of-two filter pre-scale S = 2^(9 - floor(log2 max|w|)) of the tensor-core path: the gathered filter is multiplied by S,
@@ -323,7 +318,7 @@ int lt_s32_to_f32(const void* in, float* out, long pixels, int C, void* stream);
 /* channels-last [N][P][Cs] (first C channels) -> channels-first [N][C][P] float32 */
 int lt_cl_to_cf_f32(const float* in, float* out, int N, long P, int Cs, int C, void* stream);
 
-/* Self test of the tcgen05/TMA GEMM core: D[M][N] = A[M][K] * B[N][K]^T with fp16 inputs
+/* Self test of the wgmma/TMA GEMM core: D[M][N] = A[M][K] * B[N][K]^T with fp16 inputs
  * (row-major, K contiguous), float32 output.  variant selects descriptor conventions
  * (bring-up aid; 0 is the shipped one). */
 int lt_tc_gemm_selftest(const void* a_fp16, const void* b_fp16, float* d, int M, int N, int K,
@@ -331,7 +326,7 @@ int lt_tc_gemm_selftest(const void* a_fp16, const void* b_fp16, float* d, int M,
 
 /* ------------------------------------------------------------------------------------------
  * Test hooks (NOT part of the product path): the per-item code of the two backward kernels executed on the CPU with HOST
- * pointers, so that the `-m "not gpu"` suite can check the gradient arithmetic against torch autograd without a B200.
+ * pointers, so that the `-m "not gpu"` suite can check the gradient arithmetic against torch autograd without a GPU.
  * Same arguments as the device entry points minus scratch / stream.
  * ---------------------------------------------------------------------------------------- */
 int lt_test_unproject_aggregate_bwd_host(const float* features, const float* proj, const float* coord, const float* conf,

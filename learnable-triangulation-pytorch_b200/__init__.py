@@ -1,4 +1,4 @@
-"""lt_b200 -- B200-native (sm_100a) implementation of the volumetric-triangulation hot path of
+"""lt_b200 -- H100-native (sm_90a) implementation of the volumetric-triangulation hot path of
 karfly/learnable-triangulation-pytorch, behind the reference's own nn.Module / op interface.
 
 Import as `lt_b200` (the directory name `learnable-triangulation-pytorch_b200` is not a valid
@@ -21,7 +21,7 @@ def install(mvn_package=None):
 
     `mvn_package` is the already-imported reference package (`import mvn`); if None it is imported.
     After this, the reference `train.py` (which does `from mvn.models.triangulation import
-    VolumetricTriangulationNet` at import time) picks up the B200 implementation unchanged.
+    VolumetricTriangulationNet` at import time) picks up the native implementation unchanged.
     """
     import importlib
     if mvn_package is None:

@@ -1,7 +1,7 @@
-"""Build liblt_b200.so (all CUDA kernels + the C ABI of include/lt_b200.h) for sm_100a, in-tree.
+"""Build liblt_b200.so (all CUDA kernels + the C ABI of include/lt_b200.h) for sm_90a (H100), in-tree.
 
-nvcc cross-compiles without a GPU; the .so is git-ignored but travels to the GPU box with the
-repo snapshot.  `python -m`-free usage: `from lt_b200 import build; build.build()`.
+nvcc cross-compiles without a GPU.  The .so, its object files and the source-digest stamp are build
+products (git-ignored).  `python -m`-free usage: `from lt_b200 import build; build.build()`.
 """
 import hashlib
 import os
@@ -12,9 +12,10 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 LIB = os.path.join(HERE, "liblt_b200.so")
 STAMP = os.path.join(HERE, ".liblt_b200.stamp")
-SOURCES = ["capi.cu", "unproject.cu", "softargmax.cu", "conv_simt.cu", "conv_tc.cu", "conv_pair.cu", "conv_tail.cu", "conv_tc_fold.cu", "misc.cu", "algebraic.cu", "backward.cu"]
-NVCC_FLAGS = ["-gencode", "arch=compute_100a,code=sm_100a", "-O3", "-lineinfo", "-std=c++17",
-              "--expt-relaxed-constexpr", "-Xcompiler", "-fPIC", "-Xptxas", "-v"]
+SOURCES = ["capi.cu", "unproject.cu", "softargmax.cu", "conv_simt.cu", "conv_tc.cu", "conv_tail.cu", "misc.cu", "algebraic.cu", "backward.cu"]
+ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]
+NVCC_FLAGS = ARCH + ["-O3", "-lineinfo", "-std=c++17",
+                     "--expt-relaxed-constexpr", "-Xcompiler", "-fPIC", "-Xptxas", "-v"]
 
 
 def _digest():
@@ -61,7 +62,7 @@ def build(force=False, verbose=False):
     if failed:
         sys.stderr.write("\n".join(log))
         raise RuntimeError("nvcc failed (see build/nvcc.log)")
-    link = [nvcc, "-shared", "-o", LIB] + objs + ["-gencode", "arch=compute_100a,code=sm_100a"]
+    link = [nvcc, "-shared", "-o", LIB] + objs + ARCH
     res = subprocess.run(link, stdout=subprocess.PIPE, stderr=subprocess.STDOUT, text=True)
     if res.returncode != 0:
         sys.stderr.write(res.stdout)

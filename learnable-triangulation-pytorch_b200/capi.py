@@ -42,7 +42,7 @@ class Options(ctypes.Structure):
                                      "softargmax_stream", "unproject_v2", "unproject_cpl", "unproject_lb", "unproject_brick", "unproject_brick_order", "pair_nt", "pair_stages", "pair_prof", "pair_direct_out", "pair_two_acc", "fold_pair", "fold_direct", "fold_fullw")]
 
 
-# The ONE place the environment is read (A/B tooling: tools/post_probe.py, tools/fold_probe.py): LT_OPT_<FIELD>=<int>
+# The ONE place the environment is read (A/B experiments): LT_OPT_<FIELD>=<int>
 OPTIONS_ENV_PREFIX = "LT_OPT_"
 
 # every symbol include/lt_b200.h declares: name -> (restype, argtypes)

@@ -17,7 +17,7 @@
 
 // The per-item bodies are __host__ __device__: the kernels run them on the GPU, and lt_test_*_bwd_host (bottom of the file)
 // runs the SAME code on the CPU so that `-m "not gpu"` tests can check the gradient arithmetic against torch autograd
-// without a B200 (test hook only: nothing on the product path calls it).
+// without a GPU (test hook only: nothing on the product path calls it).
 #ifdef __CUDA_ARCH__
 #define LT_LD(p) __ldg(p)
 #else

@@ -1,4 +1,4 @@
-// Shared helpers for the lt_b200 kernels (sm_100a only).
+// Shared helpers for the lt_b200 kernels (sm_90a).
 #pragma once
 #include <cuda_runtime.h>
 #include <cuda_fp16.h>
@@ -44,11 +44,11 @@ static inline int ceil_div(long a, long b) { return (int)((a + b - 1) / b); }
 // ---- split-fp16 ("S32") format ----------------------------------------------------------------
 // x ~= hi + lo with hi = fp16_rn(x), lo = fp16_rn(x - hi): two fp16 tensor-core operands carrying ~22 significand bits.
 // The low part is stored UNSCALED (round 2; it was pre-scaled by 2^11 in round 1), so the three products hi*hi, hi*lo,
-// lo*hi of a K slice can accumulate into ONE fp32 accumulator (half the TMEM columns and tcgen05.ld traffic, 256-wide N
-// tiles double-buffered).  Price: for |x| < ~0.125 the low part is an fp16 subnormal, i.e. the representation error is
+// lo*hi of a K slice are commensurable and may share an fp32 accumulator (the conv kernels keep the cross products in a second
+// one).  Price: for |x| < ~0.125 the low part is an fp16 subnormal, i.e. the representation error is
 // max(2^-22 |x|, 2^-25) absolute -- 3e-8, far below the 1e-3 contract for BatchNorm-scaled activations and Kaiming-scaled
-// weights (CPU emulation on the calibrated test model: per-layer relative error 1.9e-7..9.0e-7, tools/lo_scale_experiment.py;
-// measured on the B200 in tests/test_gpu_tc.py / test_gpu_forward.py).  |x| is saturated at the fp16 maximum (65504).
+// weights (CPU emulation on the calibrated test model: per-layer relative error 1.9e-7..9.0e-7;
+// checked on the GPU by tests/test_gpu_tc.py / test_gpu_forward.py).  |x| is saturated at the fp16 maximum (65504).
 typedef __half sh_t;
 constexpr float kLoScale = 1.0f;   // kept as named constants: the two-accumulator kernels (conv_tc.cu, conv_tc_fold.cu) form D1 + kLoInv * D2
 constexpr float kLoInv = 1.0f;
@@ -88,7 +88,7 @@ __device__ __forceinline__ float4 load_s32x4(const sh_t* row, int c) {
 // Power-of-two pre-scale of a layer's filter (tensor-core path): S = 2^(9 - floor(log2 max|w|)) puts max|w| * S into
 // [512, 1024), so that the UNSCALED low parts of every weight down to 2^-13 of the largest stay normal fp16 numbers (full
 // ~22-bit operands); Kaiming-sized filters (|w| ~ 0.03) would otherwise keep only ~2^-20 relative precision, which a
-// 152-layer trunk amplifies to ~1.5e-4 at the features (measured, profiles/r02_precision.md).  1 / S is folded into the
+// 152-layer trunk amplifies to ~1.5e-4 at the features (measured).  1 / S is folded into the
 // epilogue scale (exact).  absmax_bits: the float bit pattern of max|w| (lt_absmax_fwd), or null for "no scaling".
 __device__ __forceinline__ float weight_pow2_scale(const unsigned* absmax_bits) {
   if (!absmax_bits) return 1.0f;

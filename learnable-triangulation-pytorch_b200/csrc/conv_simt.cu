@@ -3,7 +3,7 @@
 // ReLU epilogue and the strided output mapping used for transposed-conv phases.
 //
 // Role: (1) "parity mode" of the conv path -- plain fp32 accumulation, so the whole network can
-// be checked against the fp32 oracle at ~1e-6; (2) on-GPU checker for the tcgen05 path
+// be checked against the fp32 oracle at ~1e-6; (2) on-GPU checker for the tensor-core path
 // (conv_tc.cu) at sizes the CPU oracle cannot reach; (3) executor for layers the tensor-core
 // kernel does not cover (Cin not a multiple of 32: the 7x7 stem).
 // Replaces the cuDNN/ATen convs behind pose_resnet.py:62-95,205-209,266-291 and v2v.py:7-66.

@@ -2,17 +2,15 @@
 // back_layers[2] (same) and output_layer (1x1x1 conv 32->J, bias) as ONE kernel.
 //
 // Unfused, each of the three point-wise layers reads and writes the whole 64^3 x 32-channel volume (2 x 268 MB per layer at
-// B = 8): ~0.41 ms of pure HBM round trips for 5 GFLOP.  Here a CTA streams 128-voxel tiles of the input once (TMA, 16 KB),
-// chains the three 128 x 32 x 32 GEMMs on the tensor cores (tcgen05, 3-term split-fp16 products, fp32 accumulators in TMEM)
-// with the two hidden activations going TMEM -> registers (scale / shift / ReLU / split) -> a swizzled shared-memory tile that
-// is the next GEMM's A operand, and writes only the logits (float32, `FC` floats per voxel: 17 joints rounded up to 20).
+// B = 8): pure HBM round trips for 5 GFLOP.  Here a CTA streams 128-voxel tiles of the input once (TMA, 16 KB), chains the
+// three 128 x 32 x 32 GEMMs on the tensor cores (wgmma, 3-term split-fp16 products, fp32 accumulators in registers) with the
+// two hidden activations going registers (scale / shift / ReLU / split) -> a swizzled shared-memory tile that is the next
+// GEMM's A operand, and writes only the logits (float32, `FC` floats per voxel: 17 joints rounded up to 20).
 // HBM traffic: 128 B in + 80 B out per voxel instead of 3 x 256 B.
 //
-// Per tile the chain GEMM1 -> act -> GEMM2 -> act -> GEMM3 -> store is serial (~2000 cycles of latency); throughput comes from
-// three co-resident CTAs per SM (76 KB of shared memory, 128 TMEM columns each) and the TMA prefetch of the next input tile.
-//
-// Warp roles (192 threads): warp 0 TMA producer, warp 1 TMEM allocator + MMA issuer, warps 2..5 activation / store warps
-// (one TMEM lane quadrant = 32 voxels each; a thread owns one voxel row).
+// Warp roles (384 threads): warpgroup 0 = TMA producer (weights once, then the input tiles through a two-stage ring),
+// warpgroups 1 and 2 = GEMM chain + activations for rows 0-63 / 64-127 of a tile, each with its own hidden tile.  Two CTAs
+// per SM overlap one CTA's serial chain with the other's.
 #include "conv_tc_params.cuh"
 #include "softargmax_common.cuh"
 
@@ -33,176 +31,216 @@ struct TailParams {
   float mult;
 };
 
-constexpr int kTailThreads = 192;
+constexpr int kTailThreads = 384;
 constexpr int kTailStages = 2;
 constexpr int kTailWBytes = 32 * 128;        // one 32 x [32 hi | 32 lo] weight tile
-// smem: A ring | H tile | W1 W2 W3 | barriers
+constexpr int kTailHBytes = 64 * 128;        // hidden tile of one consumer warpgroup: 64 rows x [32 hi | 32 lo]
+// smem: A ring | H tiles [2] | W1 W2 W3 | barriers
 constexpr int kTailOffH = kTailStages * kATileBytes;
-constexpr int kTailOffW = kTailOffH + kATileBytes;
+constexpr int kTailOffW = kTailOffH + 2 * kTailHBytes;
 constexpr int kTailOffBar = kTailOffW + 3 * kTailWBytes;
-// fused statistics: per activation warp a [32 rows][FC <= 20 floats] logit tile + [32][4] coordinates; the [4][32][5] merge scratch of
-// a flush aliases the first warp's tile (three CTAs of 74 880 bytes + 1 KB each still fit the SM's 228 KB)
+// fused statistics: per consumer warp a [16 rows][FC <= 20 floats] logit tile + [16][4] coordinates, then the [8][32][5] merge scratch
 constexpr int kTailStatMaxFC = 20;
 constexpr int kTailOffStat = kTailOffBar + 128;
-constexpr int kTailStatWarpBytes = 32 * kTailStatMaxFC * 4 + 32 * 16;
-constexpr int kTailStatBytes = 4 * kTailStatWarpBytes;
-static_assert(4 * 32 * 5 * 4 <= 32 * kTailStatMaxFC * 4, "merge scratch must fit the first warp's logit tile");
+constexpr int kTailStatWarpBytes = 16 * kTailStatMaxFC * 4 + 16 * 16;
+constexpr int kTailOffMerge = kTailOffStat + 8 * kTailStatWarpBytes;
 constexpr int kTailSmem = kTailOffBar + 128 + 1024;
-constexpr int kTailSmemStats = kTailOffStat + kTailStatBytes + 1024;
+constexpr int kTailSmemStats = kTailOffMerge + 8 * 32 * 5 * 4 + 1024;
 
-__device__ __forceinline__ void tail_bar_sync() { asm volatile("bar.sync 2, 128;" ::: "memory"); }
+__device__ __forceinline__ void tail_wg_sync(int g) {   // the 128 threads of consumer warpgroup g
+  if (g == 0) asm volatile("bar.sync 1, 128;" ::: "memory");
+  else asm volatile("bar.sync 2, 128;" ::: "memory");
+}
+__device__ __forceinline__ void tail_consumers_sync() { asm volatile("bar.sync 3, 256;" ::: "memory"); }
 
-__device__ __forceinline__ void issue_gemm32(uint32_t d, uint64_t ad, uint64_t bd, uint32_t idesc) {
-  // rows = [32 hi | 32 lo] fp16: K slices hi0 +0, hi1 +2, lo0 +4, lo1 +6 (16-byte units); three products into one accumulator
-  umma_f16(d, ad, bd, idesc, 0u);
-  umma_f16(d, ad + 2, bd + 2, idesc, 1u);
-  umma_f16(d, ad, bd + 4, idesc, 1u);
-  umma_f16(d, ad + 2, bd + 6, idesc, 1u);
-  umma_f16(d, ad + 4, bd, idesc, 1u);
-  umma_f16(d, ad + 6, bd + 2, idesc, 1u);
+// 64 x 32 x 32 GEMM of one warpgroup on split-fp16 rows [32 hi | 32 lo]: K slices hi0 +0, hi1 +2, lo0 +4, lo1 +6 (16-byte units);
+// hi*hi, hi*lo and lo*hi into one accumulator; returns once the MMAs have completed
+__device__ __forceinline__ void gemm32(float (&d)[16], uint64_t ad, uint64_t bd) {
+  wg_fence();
+  wgmma_f16<32>(d, ad, bd, 0u);
+  wgmma_f16<32>(d, ad + 2, bd + 2, 1u);
+  wgmma_f16<32>(d, ad, bd + 4, 1u);
+  wgmma_f16<32>(d, ad + 2, bd + 6, 1u);
+  wgmma_f16<32>(d, ad + 4, bd, 1u);
+  wgmma_f16<32>(d, ad + 6, bd + 2, 1u);
+  wg_commit();
+  wg_wait<0>();
+  wg_fence_regs(d);
+}
+
+// scale / shift / ReLU of a hidden layer and its split-fp16 store into the warpgroup's swizzled hidden tile (the next A operand):
+// this thread's accumulator elements are rows rl + 8 (k / 2 & 1), channels 8 (k / 4) + c2 + (k & 1)
+__device__ __forceinline__ void hidden_store(const float (&d)[16], const float* __restrict__ scale, const float* __restrict__ shift,
+                                             uint32_t hbase, int rl, int c2) {
+#pragma unroll
+  for (int i = 0; i < 4; ++i) {
+    const int c = 8 * i + c2;
+    const float2 sc = __ldg(reinterpret_cast<const float2*>(scale + c));
+    const float2 sh = __ldg(reinterpret_cast<const float2*>(shift + c));
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      const int r = rl + 8 * h;
+      const float v0 = fmaxf(fmaf(d[4 * i + 2 * h], sc.x, sh.x), 0.f), v1 = fmaxf(fmaf(d[4 * i + 2 * h + 1], sc.y, sh.y), 0.f);
+      uint32_t hi2, lo2;
+      split_s32x2(v0, v1, hi2, lo2);
+      // hi halves of channels 8i..8i+7 = 16-byte chunk i of the row, lo halves = chunk 4 + i; 128-byte swizzle
+      const uint32_t sw = (uint32_t)(r & 7);
+      asm volatile("st.shared.u32 [%0], %1;" ::"r"(hbase + r * 128 + (((uint32_t)i ^ sw) << 4) + c2 * 2), "r"(hi2) : "memory");
+      asm volatile("st.shared.u32 [%0], %1;" ::"r"(hbase + r * 128 + (((uint32_t)(4 + i) ^ sw) << 4) + c2 * 2), "r"(lo2) : "memory");
+    }
+  }
 }
 
 // STATS: 0 = logits only, 1 = + softmax statistics, 2 = + ReLU ("volume_softmax: false") statistics.  The logits a warp has just
-// produced (32 voxel rows x J joints, one row per lane) are transposed through a warp-private shared-memory tile so that lane j
-// folds joint j of the 32 rows into its online-softmax state (4 rows per step: one rescale + four ex2); the state lives in five
-// registers per lane for the whole kernel and is written per (sample, CTA) -- the logits are never re-read for the statistics.
+// produced (16 voxel rows x J joints) are transposed through a warp-private shared-memory tile so that lane j folds joint j of the
+// 16 rows into its online-softmax state (4 rows per step: one rescale + four ex2); the state lives in five registers per lane for
+// the whole kernel and is written per (sample, CTA) -- the logits are never re-read for the statistics.
 template <int STATS>
-__global__ void __launch_bounds__(kTailThreads, 3) v2v_tail_kernel(const __grid_constant__ CUtensorMap tmX,
+__global__ void __launch_bounds__(kTailThreads, 2) v2v_tail_kernel(const __grid_constant__ CUtensorMap tmX,
                                                                     const __grid_constant__ CUtensorMap tmW1,
                                                                     const __grid_constant__ CUtensorMap tmW2,
                                                                     const __grid_constant__ CUtensorMap tmW3, const TailParams p) {
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
-  uint8_t* h_tile = smem + kTailOffH;
   uint8_t* w_tiles = smem + kTailOffW;
   uint64_t* a_full = reinterpret_cast<uint64_t*>(smem + kTailOffBar);   // [2]
   uint64_t* a_empty = a_full + kTailStages;                             // [2]
-  uint64_t* d_full = a_empty + kTailStages;                             // [3] accumulator k complete
-  uint64_t* h_full = d_full + 3;                                        // [2] hidden tile k written
-  uint64_t* w_full = h_full + 2;                                        // [1]
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(w_full + 1);
+  uint64_t* w_full = a_empty + kTailStages;                             // [1]
 
-  const int warp = uniform_warp_idx(), lane = threadIdx.x & 31;
+  const int wg = __shfl_sync(0xffffffffu, (int)(threadIdx.x >> 7), 0);
+  const int lane = threadIdx.x & 31;
   if (threadIdx.x == 0) {
-    for (int s = 0; s < kTailStages; ++s) { mbar_init(&a_full[s], 1); mbar_init(&a_empty[s], 1); }
-    for (int i = 0; i < 3; ++i) mbar_init(&d_full[i], 1);
-    for (int i = 0; i < 2; ++i) mbar_init(&h_full[i], 4);     // one arrival per activation warp
+    for (int s = 0; s < kTailStages; ++s) { mbar_init(&a_full[s], 1); mbar_init(&a_empty[s], 2); }
     mbar_init(w_full, 1);
     fence_barrier_init();
   }
-  if (warp == 0 && lane == 0) { prefetch_tmap(&tmX); prefetch_tmap(&tmW1); }
-  if (warp == 1) tmem_alloc(tmem_slot, 128u);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
 
-  if (warp == 0) {
+  if (wg == 0) {
     // ================= producer: weights once, then the input tiles =================
-    if (elect_one()) {
-      mbar_expect_tx(w_full, 3u * kTailWBytes);
-      tma_load_2d(w_tiles, &tmW1, w_full, 0, 0);
-      tma_load_2d(w_tiles + kTailWBytes, &tmW2, w_full, 0, 0);
-      tma_load_2d(w_tiles + 2 * kTailWBytes, &tmW3, w_full, 0, 0);
+    if (threadIdx.x < 32) {
+      if (elect_one()) {
+        prefetch_tmap(&tmX);
+        mbar_expect_tx(w_full, 3u * kTailWBytes);
+        tma_load_2d(w_tiles, &tmW1, w_full, 0, 0);
+        tma_load_2d(w_tiles + kTailWBytes, &tmW2, w_full, 0, 0);
+        tma_load_2d(w_tiles + 2 * kTailWBytes, &tmW3, w_full, 0, 0);
+      }
+      __syncwarp();
+      uint32_t s = 0, ph = 0;
+      for (long t = blockIdx.x; t < p.tiles; t += gridDim.x) {
+        mbar_wait(&a_empty[s], ph ^ 1u);
+        if (elect_one()) {
+          mbar_expect_tx(&a_full[s], (uint32_t)kATileBytes);
+          tma_load_2d(smem + s * kATileBytes, &tmX, &a_full[s], 0, (int)(t * 128));
+        }
+        __syncwarp();
+        if (++s == kTailStages) { s = 0; ph ^= 1u; }
+      }
     }
-    __syncwarp();
-    uint32_t s = 0, ph = 0;
-    for (long t = blockIdx.x; t < p.tiles; t += gridDim.x) {
-      mbar_wait(&a_empty[s], ph ^ 1u);
-      if (elect_one()) {
-        mbar_expect_tx(&a_full[s], (uint32_t)kATileBytes);
-        tma_load_2d(smem + s * kATileBytes, &tmX, &a_full[s], 0, (int)(t * 128));
-      }
-      __syncwarp();
-      if (++s == kTailStages) { s = 0; ph ^= 1u; }
-    }
-  } else if (warp == 1) {
-    // ================= MMA issuer =================
-    const uint32_t idesc = make_idesc_f16(32);
-    const uint64_t a0 = make_sw128_desc(smem_u32(smem));
-    const uint64_t hd = make_sw128_desc(smem_u32(h_tile));
-    const uint64_t w1 = make_sw128_desc(smem_u32(w_tiles)), w2 = make_sw128_desc(smem_u32(w_tiles + kTailWBytes)),
-                   w3 = make_sw128_desc(smem_u32(w_tiles + 2 * kTailWBytes));
-    mbar_wait(w_full, 0);
-    uint32_t s = 0, ph = 0, tp = 0;
-    for (long t = blockIdx.x; t < p.tiles; t += gridDim.x, tp ^= 1u) {
-      mbar_wait(&a_full[s], ph);
-      tc_fence_after();
-      if (elect_one()) {
-        issue_gemm32(tmem_base, a0 + (uint64_t)(s * (kATileBytes >> 4)), w1, idesc);
-        umma_commit(&a_empty[s]);
-        umma_commit(&d_full[0]);
-      }
-      __syncwarp();
-      mbar_wait(&h_full[0], tp);
-      tc_fence_after();
-      if (elect_one()) {
-        issue_gemm32(tmem_base + 32u, hd, w2, idesc);
-        umma_commit(&d_full[1]);
-      }
-      __syncwarp();
-      mbar_wait(&h_full[1], tp);
-      tc_fence_after();
-      if (elect_one()) {
-        issue_gemm32(tmem_base + 64u, hd, w3, idesc);
-        umma_commit(&d_full[2]);
-      }
-      __syncwarp();
-      if (++s == kTailStages) { s = 0; ph ^= 1u; }
-    }
-  } else {
-    // ================= activation / store warps (2..5): thread = one voxel row of the tile =================
-    const int quad = warp & 3;
-    const int row = quad * 32 + lane;
-    const uint32_t tlane = tmem_base + ((uint32_t)(quad * 32) << 16);
-    const uint32_t hbase = smem_u32(h_tile);
-    uint32_t tp = 0;
-    // fused statistics state
-    constexpr bool SM = STATS == 1;
-    const int aw = warp - 2;                      // activation warp 0..3
-    float* lg_s = reinterpret_cast<float*>(smem + kTailOffStat + aw * kTailStatWarpBytes);     // [32][FC]
-    float4* cd_s = reinterpret_cast<float4*>(lg_s + 32 * kTailStatMaxFC);                       // [32] (x, y, z, -)
-    float* merge_s = reinterpret_cast<float*>(smem + kTailOffStat);                            // [4][32][5], aliases warp 0's logit tile
-    SoftState st;
+    return;
+  }
+
+  // ================= consumers: warpgroup g owns rows 64 g .. 64 g + 63 of every tile =================
+  const int g = wg - 1;
+  const int wq = (threadIdx.x >> 5) & 3;
+  const int rl = wq * 16 + (lane >> 2);          // this thread's rows rl and rl + 8 of the warpgroup's 64
+  const int c2 = 2 * (lane & 3);
+  const uint32_t hbase = smem_u32(smem + kTailOffH + g * kTailHBytes);
+  const uint64_t hd = make_sw128_desc(hbase);
+  const uint64_t w1 = make_sw128_desc(smem_u32(w_tiles)), w2 = make_sw128_desc(smem_u32(w_tiles + kTailWBytes)),
+                 w3 = make_sw128_desc(smem_u32(w_tiles + 2 * kTailWBytes));
+  // fused statistics state
+  constexpr bool SM = STATS == 1;
+  const int aw = g * 4 + wq;                     // consumer warp 0..7
+  float* lg_s = reinterpret_cast<float*>(smem + kTailOffStat + aw * kTailStatWarpBytes);     // [16][FC]
+  float4* cd_s = reinterpret_cast<float4*>(lg_s + 16 * kTailStatMaxFC);                      // [16] (x, y, z, -)
+  float* merge_s = reinterpret_cast<float*>(smem + kTailOffMerge);                          // [8][32][5]
+  SoftState st;
+  st_init(st, SM);
+  int cur_b = -1;
+  auto flush = [&](int b) {      // CTA merge of the eight warps' states -> partial[b][blockIdx.x][j], then reset (CTA-uniform call sites)
+    float* my = merge_s + (aw * 32 + lane) * 5;
+    my[0] = st.m; my[1] = st.d; my[2] = st.sx; my[3] = st.sy; my[4] = st.sz;
     st_init(st, SM);
-    int cur_b = -1;
-    auto flush = [&](int b) {      // CTA merge of the four warps' states -> partial[b][blockIdx.x][j], then reset (CTA-uniform call sites)
-      tail_bar_sync();             // every warp has consumed its last tile (the scratch aliases the first warp's)
-      float* my = merge_s + (aw * 32 + lane) * 5;
-      my[0] = st.m; my[1] = st.d; my[2] = st.sx; my[3] = st.sy; my[4] = st.sz;
-      st_init(st, SM);
-      tail_bar_sync();
-      if (aw == 0 && lane < p.J) {
-        SoftState a{merge_s[lane * 5], merge_s[lane * 5 + 1], merge_s[lane * 5 + 2], merge_s[lane * 5 + 3], merge_s[lane * 5 + 4]};
+    tail_consumers_sync();
+    if (aw == 0 && lane < p.J) {
+      SoftState a{merge_s[lane * 5], merge_s[lane * 5 + 1], merge_s[lane * 5 + 2], merge_s[lane * 5 + 3], merge_s[lane * 5 + 4]};
 #pragma unroll
-        for (int w = 1; w < 4; ++w) {
-          const float* o = merge_s + (w * 32 + lane) * 5;
-          SoftState t{o[0], o[1], o[2], o[3], o[4]};
-          st_merge(a, t, SM);
-        }
-        float* dst = p.partial + (((long)b * gridDim.x + blockIdx.x) * p.J + lane) * 5;
-        dst[0] = a.m; dst[1] = a.d; dst[2] = a.sx; dst[3] = a.sy; dst[4] = a.sz;
+      for (int w = 1; w < 8; ++w) {
+        const float* o = merge_s + (w * 32 + lane) * 5;
+        SoftState t{o[0], o[1], o[2], o[3], o[4]};
+        st_merge(a, t, SM);
       }
-      tail_bar_sync();
-    };
+      float* dst = p.partial + (((long)b * gridDim.x + blockIdx.x) * p.J + lane) * 5;
+      dst[0] = a.m; dst[1] = a.d; dst[2] = a.sx; dst[3] = a.sy; dst[4] = a.sz;
+    }
+    tail_consumers_sync();
+  };
+  if (STATS) {
+    // samples in which this CTA owns no tile still need an (identity) partial for the merge
+    for (int i = threadIdx.x - 128; i < p.B * p.J; i += 256) {
+      const int b = i / p.J, j = i % p.J;
+      const long lo = (long)b * p.tiles_per_sample, G = gridDim.x;
+      const long f0 = lo + (((long)blockIdx.x - lo) % G + G) % G;     // first tile >= lo owned by this CTA
+      if (!(f0 < lo + p.tiles_per_sample)) {
+        float* dst = p.partial + (((long)b * G + blockIdx.x) * p.J + j) * 5;
+        dst[0] = SM ? -INFINITY : 0.0f; dst[1] = 0.f; dst[2] = 0.f; dst[3] = 0.f; dst[4] = 0.f;
+      }
+    }
+  }
+
+  mbar_wait(w_full, 0);
+  uint32_t s = 0, ph = 0;
+  for (long t = blockIdx.x; t < p.tiles; t += gridDim.x) {
     if (STATS) {
-      // samples in which this CTA owns no tile still need an (identity) partial for the merge
-      for (int i = threadIdx.x - 64; i < p.B * p.J; i += 128) {
-        const int b = i / p.J, j = i % p.J;
-        const long lo = (long)b * p.tiles_per_sample, G = gridDim.x;
-        const long f0 = lo + (((long)blockIdx.x - lo) % G + G) % G;     // first tile >= lo owned by this CTA
-        if (!(f0 < lo + p.tiles_per_sample)) {
-          float* dst = p.partial + (((long)b * G + blockIdx.x) * p.J + j) * 5;
-          dst[0] = SM ? -INFINITY : 0.0f; dst[1] = 0.f; dst[2] = 0.f; dst[3] = 0.f; dst[4] = 0.f;
+      // rows = B x nvox with nvox % 128 == 0: every tile is full and lies inside one sample; a sample boundary closes the
+      // previous sample's partial (CTA-uniform)
+      const int b = (int)(t / p.tiles_per_sample);
+      if (b != cur_b) {
+        if (cur_b >= 0) flush(cur_b);
+        cur_b = b;
+      }
+    }
+    float d[16];
+    mbar_wait(&a_full[s], ph);
+    gemm32(d, make_sw128_desc(smem_u32(smem + s * kATileBytes + g * kTailHBytes)), w1);
+    if ((threadIdx.x & 127) == 0) mbar_arrive_local(&a_empty[s]);
+    if (++s == kTailStages) { s = 0; ph ^= 1u; }
+#pragma unroll
+    for (int layer = 0; layer < 2; ++layer) {
+      tail_wg_sync(g);           // the previous MMA that read the hidden tile has completed in every warp
+      hidden_store(d, layer == 0 ? p.scale1 : p.scale2, layer == 0 ? p.shift1 : p.shift2, hbase, rl, c2);
+      fence_proxy_async();       // generic-proxy stores -> visible to the MMA's operand reads
+      tail_wg_sync(g);
+      gemm32(d, hd, layer == 0 ? w2 : w3);
+    }
+    // ---- logits (and their statistics) ----
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      const int rw = (lane >> 2) + 8 * h;        // row within this warp's 16
+      const long vox = t * 128 + g * 64 + rl + 8 * h;
+#pragma unroll
+      for (int i = 0; i < 4; ++i) {
+        const int c = 8 * i + c2;
+        if (c < p.FC) {
+          const float2 a = __ldg(reinterpret_cast<const float2*>(p.scale3 + c));
+          const float2 bb = __ldg(reinterpret_cast<const float2*>(p.bias3 + c));
+          const float2 o = make_float2(fmaf(d[4 * i + 2 * h], a.x, bb.x), fmaf(d[4 * i + 2 * h + 1], a.y, bb.y));
+          if (vox < p.rows) *reinterpret_cast<float2*>(p.logits + vox * p.FC + c) = o;
+          if (STATS) *reinterpret_cast<float2*>(lg_s + rw * p.FC + c) = o;
         }
       }
     }
-    // statistics of the tile in lg_s / cd_s (rows [r_lo, r_hi) of this warp's 32): lane j folds joint j, four rows per step.
-    // They are computed ONE TILE LATE, in the two bubbles of the next tile's chain (after handing a hidden tile to the MMA warp the
-    // activation warp would otherwise just wait for the next accumulator), so the fused pass adds no latency to the GEMM chain.
-    auto stats_rows = [&](int r_lo, int r_hi) {
+    if (STATS) {
+      if (lane < 16) {
+        const long vox = t * 128 + g * 64 + wq * 16 + lane;
+        const float* cp = p.coord + vox * 3;
+        cd_s[lane] = make_float4(__ldg(cp), __ldg(cp + 1), __ldg(cp + 2), 0.f);
+      }
+      __syncwarp();
       if (lane < p.J) {
-        for (int r0 = r_lo; r0 < r_hi; r0 += 4) {
+        for (int r0 = 0; r0 < 16; r0 += 4) {
           float l[4], x[4], y[4], z[4];
 #pragma unroll
           for (int k = 0; k < 4; ++k) {
@@ -213,99 +251,10 @@ __global__ void __launch_bounds__(kTailThreads, 3) v2v_tail_kernel(const __grid_
           st_push4<SM>(st, l, x, y, z);
         }
       }
-    };
-    bool pending = false;          // lg_s / cd_s hold a tile (of sample cur_b) whose statistics are not folded in yet
-    for (long t = blockIdx.x; t < p.tiles; t += gridDim.x, tp ^= 1u) {
-#pragma unroll
-      for (int layer = 0; layer < 2; ++layer) {
-        mbar_wait(&d_full[layer], tp);
-        tc_fence_after();
-        uint32_t t0[16], t1[16];
-        tmem_ld16_nowait(tlane + (uint32_t)(layer * 32), t0);
-        tmem_ld16_nowait(tlane + (uint32_t)(layer * 32 + 16), t1);
-        tmem_wait_ld();
-        float v0[16], v1[16];
-#pragma unroll
-        for (int j = 0; j < 16; ++j) { v0[j] = __uint_as_float(t0[j]); v1[j] = __uint_as_float(t1[j]); }
-        const float* sc = layer == 0 ? p.scale1 : p.scale2;
-        const float* sh = layer == 0 ? p.shift1 : p.shift2;
-        epi_affine16(v0, sc, sh, 0);
-        epi_affine16(v1, sc, sh, 16);
-#pragma unroll
-        for (int j = 0; j < 16; ++j) { v0[j] = fmaxf(v0[j], 0.f); v1[j] = fmaxf(v1[j], 0.f); }
-        // the previous reader of the hidden tile (GEMM layer+1 of this tile's predecessor step) has completed: d_full[layer]
-        // of THIS step is committed after it in issue order
-        epi_store16(hbase, row, 0, LT_FMT_S32, v0);
-        epi_store16(hbase, row, 1, LT_FMT_S32, v1);
-        fence_proxy_async();
-        tc_fence_before();
-        __syncwarp();
-        if (lane == 0) mbar_arrive_local(&h_full[layer]);
-        if (STATS && pending) stats_rows(layer * 16, layer * 16 + 16);
-      }
-      if (STATS) {
-        // the pending tile is folded in; a sample boundary between it and this tile closes the sample's partial (CTA-uniform)
-        const int b = (int)(t / p.tiles_per_sample);
-        __syncwarp();
-        if (b != cur_b) {
-          if (cur_b >= 0) flush(cur_b);
-          cur_b = b;
-        }
-      }
-      mbar_wait(&d_full[2], tp);
-      tc_fence_after();
-      {
-        uint32_t t0[16], t1[16];
-        tmem_ld16_nowait(tlane + 64u, t0);
-        tmem_ld16_nowait(tlane + 80u, t1);
-        tmem_wait_ld();
-        const long vox = t * 128 + row;
-        float3 cxyz = make_float3(0.f, 0.f, 0.f);
-        if (STATS && vox < p.rows) { const float* cp = p.coord + vox * 3; cxyz = make_float3(__ldg(cp), __ldg(cp + 1), __ldg(cp + 2)); }
-        if (vox < p.rows) {
-          float* dst = p.logits + vox * p.FC;
-#pragma unroll
-          for (int j = 0; j < 16; j += 4) {
-            const float4 a = __ldg(reinterpret_cast<const float4*>(p.scale3 + j));
-            const float4 b = __ldg(reinterpret_cast<const float4*>(p.bias3 + j));
-            const float4 o = make_float4(fmaf(__uint_as_float(t0[j]), a.x, b.x), fmaf(__uint_as_float(t0[j + 1]), a.y, b.y),
-                                         fmaf(__uint_as_float(t0[j + 2]), a.z, b.z), fmaf(__uint_as_float(t0[j + 3]), a.w, b.w));
-            *reinterpret_cast<float4*>(dst + j) = o;
-            if (STATS) *reinterpret_cast<float4*>(lg_s + lane * p.FC + j) = o;
-          }
-#pragma unroll
-          for (int j = 0; j < 16; j += 4) {
-            if (16 + j < p.FC) {
-              const float4 a = __ldg(reinterpret_cast<const float4*>(p.scale3 + 16 + j));
-              const float4 b = __ldg(reinterpret_cast<const float4*>(p.bias3 + 16 + j));
-              const float4 o = make_float4(fmaf(__uint_as_float(t1[j]), a.x, b.x), fmaf(__uint_as_float(t1[j + 1]), a.y, b.y),
-                                           fmaf(__uint_as_float(t1[j + 2]), a.z, b.z), fmaf(__uint_as_float(t1[j + 3]), a.w, b.w));
-              *reinterpret_cast<float4*>(dst + 16 + j) = o;
-              if (STATS) *reinterpret_cast<float4*>(lg_s + lane * p.FC + 16 + j) = o;
-            }
-          }
-        }
-        if (STATS) {
-          // rows = B x nvox with nvox % 128 == 0: every tile is full and lies inside one sample
-          cd_s[lane] = make_float4(cxyz.x, cxyz.y, cxyz.z, 0.f);
-          __syncwarp();
-          pending = true;
-        }
-      }
-      tc_fence_before();   // accumulator reads of this tile are ordered before the next tile's h_full arrivals
-    }
-    if (STATS) {
-      if (pending) { stats_rows(0, 32); __syncwarp(); }
-      if (cur_b >= 0) flush(cur_b);
+      __syncwarp();
     }
   }
-
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, 128u);
-  }
+  if (STATS && cur_b >= 0) flush(cur_b);
 }
 
 }  // namespace lt
@@ -339,7 +288,7 @@ static int launch_tail(const void* x, const void* w1, const void* w2, const void
     if (e == cudaSuccess) e = cudaFuncSetAttribute(v2v_tail_kernel<2>, cudaFuncAttributeMaxDynamicSharedMemorySize, kTailSmemStats);
     if (e != cudaSuccess) return fail(LT_ERR_CUDA, "v2v_tail: cudaFuncSetAttribute: %s", cudaGetErrorString(e));
   }
-  long grid = 3L * sm_count();
+  long grid = 2L * sm_count();
   if (grid > p.tiles) grid = p.tiles;
   if (grid_out) *grid_out = (int)grid;
   cudaStream_t st = (cudaStream_t)stream;

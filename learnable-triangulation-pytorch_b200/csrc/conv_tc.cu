@@ -1,20 +1,24 @@
-// Tensor-core implicit-GEMM convolution for sm_100a: TMA-staged channels-last tiles ->
-// shared memory (128B swizzle) -> tcgen05.mma (UMMA 128 x Nt x 16, fp16 in, fp32 accumulate in
-// TMEM) -> tcgen05.ld epilogue with folded-BN scale/shift, residual, ReLU and strided
-// channels-last store (plain conv, stride-phase transposed conv).
+// Tensor-core implicit-GEMM convolution for sm_90a: TMA-staged channels-last tiles -> shared memory (128B swizzle) ->
+// wgmma (m64 x Nt x k16 per warpgroup, fp16 in, fp32 accumulators in registers) -> epilogue with folded-BN scale/shift,
+// residual, ReLU and strided channels-last store straight from the accumulator registers (plain conv, stride-phase
+// transposed conv, grouped outputs).
 //
 // GEMM view:  M = output positions (tile = a bw x bh x bd x bn box of 128 positions),
-//             N = output channels (tile Nt <= 256), K = taps x Cin.
+//             N = output channels (tile Nt = 16 / 32 / 64 / 128), K = taps x Cin.
 // For every filter tap the A tile is ONE TMA box load of the input tensor shifted by the tap
 // offset; out-of-range coordinates are zero-filled by TMA, which implements the padding.
 //
-// Precision: activations and weights travel as split-fp16 (x = hi + lo/2048, see common.cuh).  Per
-// 16-wide K slice the kernel issues hi*hi into accumulator D1 and hi*lo + lo*hi into accumulator D2
-// (3 MMAs; the epilogue forms D1 + D2/2048: ~22 significand bits per operand, dropped lo*lo term
-// 2^-22 relative -- fp32-grade results from the fp16 pipe), or hi*hi only (LT_CONV_TC1, fast mode).
+// Precision: activations and weights travel as split-fp16 rows [32 hi | 32 lo] (x = hi + lo, see common.cuh).  Per 16-wide K
+// slice the kernel accumulates hi*hi into D1 and hi*lo + lo*hi into D2 and the epilogue forms D1 + D2 (~22 significand bits per
+// operand, the dropped lo*lo term is 2^-22 relative: fp32-grade results from the fp16 pipe); keeping the small cross products out
+// of the big accumulator limits the rounding of the accumulation steps.  LT_CONV_TC1 (fast mode) issues hi*hi only.
 //
-// Warp roles (320 threads): warp 0 = TMA producer, warp 1 = TMEM allocator + MMA issuer,
-// warps 2-9 = epilogue (two warps per TMEM lane quadrant, each converting 16 of a block's 32 channels).
+// Weights: [tap][Cin/32][CoutP rows][32 hi | 32 lo] fp16 (128-byte rows), so the K slices of both operands are descriptor offsets
+// (+0, +2 hi; +4, +6 lo, in 16-byte units).
+//
+// Warp roles (384 threads): warpgroup 0 = TMA producer (one warp issues), warpgroups 1 and 2 = MMA + epilogue for rows 0-63 and
+// 64-127 of the M tile.  The operand ring is released per stage by one arrival of each consumer warpgroup once its MMAs that read
+// the stage have completed (wgmma.wait_group 1 keeps one chunk of MMAs in flight behind the issue).
 #include "tc_common.cuh"
 #include "conv_tc_params.cuh"
 #include <stdlib.h>
@@ -25,22 +29,22 @@ namespace lt {
 // ------------------------------------------------------------------------------------------------
 // Kernel
 // ------------------------------------------------------------------------------------------------
+constexpr int kTcThreads = 384;
 
-__global__ void __launch_bounds__(320) conv_tc_kernel(const __grid_constant__ CUtensorMap tmA,
-                                                      const __grid_constant__ CUtensorMap tmB,
-                                                      const __grid_constant__ OutMaps tmOut,
-                                                      const __grid_constant__ OutMaps tmRes, const TcParams p) {
+__device__ __forceinline__ void regs_release_producer() { asm volatile("setmaxnreg.dec.sync.aligned.u32 40;"); }
+__device__ __forceinline__ void regs_claim_consumer() { asm volatile("setmaxnreg.inc.sync.aligned.u32 232;"); }
+
+template <int NT>
+__global__ void __launch_bounds__(kTcThreads, 1) conv_tc_kernel(const __grid_constant__ CUtensorMap tmA,
+                                                                const __grid_constant__ CUtensorMap tmB, const TcParams p) {
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
-  const int b_bytes = p.Nt * 128;
-  const int stage_bytes = kATileBytes + b_bytes;
-  uint64_t* full = reinterpret_cast<uint64_t*>(smem + (size_t)p.stages * stage_bytes);
+  constexpr int kStage = kATileBytes + NT * 128;
+  uint64_t* full = reinterpret_cast<uint64_t*>(smem + (size_t)p.stages * kStage);
   uint64_t* empty = full + p.stages;
-  uint64_t* tmem_full = empty + p.stages;
-  uint64_t* res_full = tmem_full + 1;   // [2]
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(res_full + 2);
 
-  const int warp = uniform_warp_idx(), lane = threadIdx.x & 31;
+  const int wg = __shfl_sync(0xffffffffu, (int)(threadIdx.x >> 7), 0);
+  const int lane = threadIdx.x & 31;
 
   // tile coordinates
   int t = blockIdx.x;
@@ -49,444 +53,157 @@ __global__ void __launch_bounds__(320) conv_tc_kernel(const __grid_constant__ CU
   const int tdi = t % p.td; t /= p.td;
   const int tni = t;
   const int ow0 = twi * p.bw, oh0 = thi * p.bh, od0 = tdi * p.bd, nb0 = tni * p.bn;
-  const int n0 = blockIdx.y * p.Nt;
+  const int n0 = blockIdx.y * NT;
   const int nchunks_all = p.KD * p.KH * p.KW * p.CB;
   const int q_begin = (int)(((long)blockIdx.z * nchunks_all) / p.splits);
   const int nchunks = (int)(((long)(blockIdx.z + 1) * nchunks_all) / p.splits) - q_begin;   // chunks of this split
 
   if (threadIdx.x == 0) {
-    for (int s = 0; s < p.stages; ++s) { mbar_init(&full[s], 1); mbar_init(&empty[s], 1); }
-    mbar_init(tmem_full, 1);
-    mbar_init(&res_full[0], 1);
-    mbar_init(&res_full[1], 1);
+    for (int s = 0; s < p.stages; ++s) { mbar_init(&full[s], 1); mbar_init(&empty[s], 2); }
     fence_barrier_init();
+    prefetch_tmap(&tmA);
+    prefetch_tmap(&tmB);
   }
-  if (warp == 0 && lane == 0) { prefetch_tmap(&tmA); prefetch_tmap(&tmB); }
-  if (warp == 1) tmem_alloc(tmem_slot, (uint32_t)p.tmem_cols);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
 
-  if (warp == 0) {
-    // ================= TMA producer (whole warp runs the loop; one elected lane issues) =================
-    // chunk -> (tap, channel block) and ring slot / phase are advanced incrementally: no integer division in the loop
-    // (a handful of runtime divisions per chunk cost more issue latency than the chunk's MMAs take to execute)
-    int tap = q_begin / p.CB, cb = q_begin - tap * p.CB;
-    int kw = tap % p.KW, kh = (tap / p.KW) % p.KH, kd = tap / (p.KW * p.KH);
-    int s = 0;
-    uint32_t ph = 0;
-    const int ax = ow0 * p.sw - p.pw, ay = oh0 * p.sh - p.ph, az = od0 * p.sd - p.pd, bn0 = n0 * p.b_nmul;
-    for (int q = 0, qa = q_begin; q < nchunks; ++q, ++qa) {
-      mbar_wait(&empty[s], ph ^ 1u);
-      uint8_t* a_dst = smem + (size_t)s * stage_bytes;
-      uint8_t* b_dst = a_dst + kATileBytes;
-      if (elect_one()) {
-        mbar_expect_tx(&full[s], (uint32_t)stage_bytes);
-        tma_load_5d(a_dst, &tmA, &full[s], cb * 64, ax + kw, ay + kh, az + kd, nb0);
-        tma_load_2d(b_dst, &tmB, &full[s], qa * p.b_step0, qa * p.b_step1 + bn0);
+  if (wg == 0) {
+    // ================= TMA producer (warp 0 runs the loop; one elected lane issues) =================
+    regs_release_producer();
+    if (threadIdx.x < 32) {
+      // chunk -> (tap, channel block) and ring slot / phase are advanced incrementally: no integer division in the loop
+      int tap = q_begin / p.CB, cb = q_begin - tap * p.CB;
+      int kw = tap % p.KW, kh = (tap / p.KW) % p.KH, kd = tap / (p.KW * p.KH);
+      int s = 0;
+      uint32_t ph = 0;
+      const int ax = ow0 * p.sw - p.pw, ay = oh0 * p.sh - p.ph, az = od0 * p.sd - p.pd, bn0 = n0 * p.b_nmul;
+      for (int q = 0, qa = q_begin; q < nchunks; ++q, ++qa) {
+        mbar_wait(&empty[s], ph ^ 1u);
+        uint8_t* a_dst = smem + (size_t)s * kStage;
+        if (elect_one()) {
+          mbar_expect_tx(&full[s], (uint32_t)kStage);
+          tma_load_5d(a_dst, &tmA, &full[s], cb * 64, ax + kw, ay + kh, az + kd, nb0);
+          tma_load_2d(a_dst + kATileBytes, &tmB, &full[s], qa * p.b_step0, qa * p.b_step1 + bn0);
+        }
+        __syncwarp();
+        if (++cb == p.CB) { cb = 0; if (++kw == p.KW) { kw = 0; if (++kh == p.KH) { kh = 0; ++kd; } } }
+        if (++s == p.stages) { s = 0; ph ^= 1u; }
       }
-      __syncwarp();
-      if (++cb == p.CB) { cb = 0; if (++kw == p.KW) { kw = 0; if (++kh == p.KH) { kh = 0; ++kd; } } }
-      if (++s == p.stages) { s = 0; ph ^= 1u; }
     }
-  } else if (warp == 1) {
-    // ================= MMA issuer (whole warp runs the loop; one elected lane issues) =================
-    const uint32_t idesc = make_idesc_f16(p.Nt), idesc2 = make_idesc_f16(2 * p.Nt);
-    const uint32_t tmem_d2 = tmem_base + (uint32_t)p.Nt;   // second accumulator: cross terms (scaled by 2^11)
-    int s = 0;
+    return;
+  }
+
+  // ================= MMA + epilogue (warpgroups 1, 2: rows 64 (wg - 1) .. +63 of the M tile) =================
+  regs_claim_consumer();
+  const int g = wg - 1;
+  float d1[NT / 2], d2[NT / 2];
+#pragma unroll
+  for (int i = 0; i < NT / 2; ++i) { d1[i] = 0.f; d2[i] = 0.f; }
+  {
+    int s = 0, prev = -1;
     uint32_t ph = 0;
     const uint32_t ring0 = smem_u32(smem);
     for (int q = 0; q < nchunks; ++q) {
       mbar_wait(&full[s], ph);
-      tc_fence_after();
-      const uint32_t a_addr = ring0 + (uint32_t)(s * stage_bytes);
-      const uint32_t b_addr = a_addr + kATileBytes;
-      const uint64_t ad = make_sw128_desc(a_addr);
-      const uint64_t bd = (p.terms == 0) ? make_sw128_desc(b_addr) : make_sw64_desc(b_addr);
-      const uint32_t first = (q == 0) ? 0u : 1u;
-      if (elect_one()) {
-        if (p.terms == 3) {
-          // A row = [32 hi | 32 lo] fp16: hi slices at +0,+32 B, lo slices at +64,+96 B (descriptor units of 16 B).
-          // B tile = [Nt hi rows ; Nt lo rows] x 64 B (64B swizzle): one N = 2*Nt MMA per slice forms hi*hi -> D1 and
-          // hi*lo -> D2 from a single pass over A_hi; the lo*hi term is a second N = Nt MMA into D2.
-          umma_f16(tmem_base, ad, bd, idesc2, first);
-          umma_f16(tmem_d2, ad + 4, bd, idesc, 1);
-          umma_f16(tmem_base, ad + 2, bd + 2, idesc2, 1);
-          umma_f16(tmem_d2, ad + 6, bd + 2, idesc, 1);
-        } else if (p.terms == 1) {
-          // high parts only: A_hi x B_hi rows
-          umma_f16(tmem_base, ad, bd, idesc, first);
-          umma_f16(tmem_base, ad + 2, bd + 2, idesc, 1);
-        } else {
-          // plain fp16 rows (self test): 4 slices of 16
-          umma_f16(tmem_base, ad, bd, idesc, first);
-          umma_f16(tmem_base, ad + 2, bd + 2, idesc, 1);
-          umma_f16(tmem_base, ad + 4, bd + 4, idesc, 1);
-          umma_f16(tmem_base, ad + 6, bd + 6, idesc, 1);
-        }
-        umma_commit(&empty[s]);                       // frees the smem slot once these MMAs have read it
-        if (q == nchunks - 1) umma_commit(tmem_full); // accumulator complete
+      const uint32_t a_addr = ring0 + (uint32_t)(s * kStage) + (uint32_t)(g * 64 * 128);
+      const uint32_t b_addr = ring0 + (uint32_t)(s * kStage) + kATileBytes;
+      const uint64_t ad = make_sw128_desc(a_addr), bd = make_sw128_desc(b_addr);
+      const uint32_t acc = (q == 0) ? 0u : 1u;
+      wg_fence();
+      if (p.terms == 3) {
+        wgmma_f16<NT>(d1, ad, bd, acc);              // hi * hi
+        wgmma_f16<NT>(d1, ad + 2, bd + 2, 1u);
+        wgmma_f16<NT>(d2, ad, bd + 4, acc);          // hi * lo
+        wgmma_f16<NT>(d2, ad + 2, bd + 6, 1u);
+        wgmma_f16<NT>(d2, ad + 4, bd, 1u);           // lo * hi
+        wgmma_f16<NT>(d2, ad + 6, bd + 2, 1u);
+      } else if (p.terms == 1) {
+        wgmma_f16<NT>(d1, ad, bd, acc);              // high parts only
+        wgmma_f16<NT>(d1, ad + 2, bd + 2, 1u);
+      } else {
+        // plain fp16 rows (self test): 4 slices of 16
+        wgmma_f16<NT>(d1, ad, bd, acc);
+        wgmma_f16<NT>(d1, ad + 2, bd + 2, 1u);
+        wgmma_f16<NT>(d1, ad + 4, bd + 4, 1u);
+        wgmma_f16<NT>(d1, ad + 6, bd + 6, 1u);
       }
-      __syncwarp();
+      wg_commit();
+      wg_wait<1>();                                   // the MMAs of chunk q - 1 have completed: release its stage
+      if (prev >= 0 && (threadIdx.x & 127) == 0) mbar_arrive_local(&empty[prev]);
+      prev = s;
       if (++s == p.stages) { s = 0; ph ^= 1u; }
     }
-  } else {
-    // ================= epilogue (warps 2..9: two per TMEM lane quadrant, 16 channels of each block each) =================
-    const int quad = warp & 3;               // TMEM lane quadrant this warp may access
-    const int half = (warp - 2) >> 2;        // which 16 channels of every 32-channel block
-    const int row = quad * 32 + lane;
+    wg_wait<0>();
+    wg_fence_regs(d1);
+    wg_fence_regs(d2);
+  }
+
+  // ---- epilogue: this thread holds rows r0 and r0 + 8, columns 8i + c2 (+1) of the 64 x NT warpgroup tile ----
+  const int r0 = g * 64 + ((threadIdx.x >> 5) & 3) * 16 + (lane >> 2);
+  const int c2 = 2 * (lane & 3);
+#pragma unroll
+  for (int h = 0; h < 2; ++h) {
+    const int row = r0 + 8 * h;
+    if (p.splits > 1) {
+      // ---- split-K: raw accumulators to the workspace, epilogue deferred to splitk_reduce_kernel ----
+      float* wrow = p.ws + (((size_t)blockIdx.z * gridDim.x + blockIdx.x) * 128 + row) * p.ws_ld + n0;
+#pragma unroll
+      for (int i = 0; i < NT / 8; ++i) {
+        const int k = 4 * i + 2 * h;
+        const float v0 = (p.terms == 3) ? fmaf(d2[k], kLoInv, d1[k]) : d1[k];
+        const float v1 = (p.terms == 3) ? fmaf(d2[k + 1], kLoInv, d1[k + 1]) : d1[k + 1];
+        *reinterpret_cast<float2*>(wrow + 8 * i + c2) = make_float2(v0, v1);
+      }
+      continue;
+    }
     int r_ = row;
     const int dw = r_ % p.bw; r_ /= p.bw;
     const int dh = r_ % p.bh; r_ /= p.bh;
     const int dd = r_ % p.bd; r_ /= p.bd;
-    const int dn = r_;
-    const int ow = ow0 + dw, oh = oh0 + dh, od = od0 + dd, nb = nb0 + dn;
-    const bool valid = ow < p.OW && oh < p.OH && od < p.OD && nb < p.N;
+    const int ow = ow0 + dw, oh = oh0 + dh, od = od0 + dd, nb = nb0 + r_;
+    if (!(ow < p.OW && oh < p.OH && od < p.OD && nb < p.N)) continue;
     const long opix = (((long)nb * p.FD + (od * p.osd + p.ood)) * p.FH + (oh * p.osh + p.ooh)) * p.FW + (ow * p.osw + p.oow);
-    const uint32_t tlane = tmem_base + ((uint32_t)(quad * 32) << 16);
-
-    mbar_wait(tmem_full, 0);
-    tc_fence_after();
-    if (p.splits > 1) {
-      // ---- split-K: raw accumulators to the workspace, epilogue deferred to splitk_reduce_kernel ----
-      float* wrow = p.ws + (((size_t)blockIdx.z * gridDim.x + blockIdx.x) * 128 + row) * p.ws_ld + n0;
-      for (int c0 = half * 16; c0 < p.Nt; c0 += 32) {
-        uint32_t v[16], v2[16];
-        tmem_ld16_nowait(tlane + (uint32_t)c0, v);
-        if (p.terms == 3) tmem_ld16_nowait(tlane + (uint32_t)(p.Nt + c0), v2);
-        tmem_wait_ld();
 #pragma unroll
-        for (int j = 0; j < 16; j += 4) {
-          float4 o;
-          if (p.terms == 3)
-            o = make_float4(fmaf(__uint_as_float(v2[j]), kLoInv, __uint_as_float(v[j])), fmaf(__uint_as_float(v2[j + 1]), kLoInv, __uint_as_float(v[j + 1])),
-                            fmaf(__uint_as_float(v2[j + 2]), kLoInv, __uint_as_float(v[j + 2])), fmaf(__uint_as_float(v2[j + 3]), kLoInv, __uint_as_float(v[j + 3])));
-          else
-            o = make_float4(__uint_as_float(v[j]), __uint_as_float(v[j + 1]), __uint_as_float(v[j + 2]), __uint_as_float(v[j + 3]));
-          *reinterpret_cast<float4*>(wrow + c0 + j) = o;
+    for (int i = 0; i < NT / 8; ++i) {
+      const int k = 4 * i + 2 * h;
+      const int co = n0 + 8 * i + c2;
+      int ch = co;
+      long pix = opix;
+      if (p.n_maps > 1) {   // grouped output: channel block of group mi goes to output phase (mi / (gh gw), (mi / gw) % gh, mi % gw)
+        const int mi = ch / p.oc;
+        ch -= mi * p.oc;
+        pix += ((long)(mi / (p.gh * p.gw)) * p.FH + (mi / p.gw) % p.gh) * p.FW + mi % p.gw;
+      }
+      if (ch >= p.FC) continue;
+      float v0 = (p.terms == 3) ? fmaf(d2[k], kLoInv, d1[k]) : d1[k];
+      float v1 = (p.terms == 3) ? fmaf(d2[k + 1], kLoInv, d1[k + 1]) : d1[k + 1];
+      const float2 sc = __ldg(reinterpret_cast<const float2*>(p.scale + co));
+      const float2 sh = __ldg(reinterpret_cast<const float2*>(p.shift + co));
+      v0 = fmaf(v0, sc.x, sh.x);
+      v1 = fmaf(v1, sc.y, sh.y);
+      float2 rr = make_float2(0.f, 0.f);
+      if (p.residual != LT_RES_NONE) {
+        if (p.out_format == LT_FMT_F32) {
+          rr = *reinterpret_cast<const float2*>(reinterpret_cast<const float*>(p.res) + pix * p.FC + ch);
+        } else {
+          const sh_t* rp = reinterpret_cast<const sh_t*>(p.res) + pix * 2 * p.FC + s32_off(ch);
+          const float2 a = __half22float2(*reinterpret_cast<const __half2*>(rp));
+          const float2 b = __half22float2(*reinterpret_cast<const __half2*>(rp + 32));
+          rr = make_float2(fmaf(b.x, kLoInv, a.x), fmaf(b.y, kLoInv, a.y));
         }
       }
-    } else if (p.tma_epi) {
-      // ---- staged epilogue: 32-channel blocks -> swizzled smem tile -> TMA store; residual tiles arrive by TMA ----
-      // All MMAs have completed (tmem_full), so the operand ring is free: reuse its first 64 KB.
-      uint8_t* out_stage = smem;              // 2 x 16 KB
-      uint8_t* res_stage = smem + 32768;      // 2 x 16 KB
-      const bool leader = threadIdx.x == 64;
-      const int nblk = p.Nt >> 5;
-      const int esz = (p.out_format == LT_FMT_F32) ? 1 : 2;   // tensor-map elements per channel
-      // 32-channel block i of this N tile -> (output map, channel inside it): grouped outputs put block g*oc.. into map g
-      auto blk_map = [&](int i, int& mi, int& ch) {
-        ch = n0 + i * 32; mi = 0;
-        if (p.n_maps > 1) { mi = ch / p.oc; ch -= mi * p.oc; }
-      };
-      if (leader && p.residual != LT_RES_NONE) {
-        for (int i = 0; i < 2 && i < nblk; ++i) {
-          int mi, ch;
-          blk_map(i, mi, ch);
-          mbar_expect_tx(&res_full[i], 16384u);
-          tma_load_5d(res_stage + i * 16384, &tmRes.m[mi], &res_full[i], ch * esz, ow0, oh0, od0, nb0);
-        }
-      }
-      for (int i = 0; i < nblk; ++i) {
-        const int buf = i & 1;
-        float v[16], r[16];
-        {
-          uint32_t t1[16], t2[16];
-          tmem_ld16_nowait(tlane + (uint32_t)(i * 32 + half * 16), t1);
-          if (p.terms == 3) tmem_ld16_nowait(tlane + (uint32_t)(p.Nt + i * 32 + half * 16), t2);
-          tmem_wait_ld();
-#pragma unroll
-          for (int j = 0; j < 16; ++j)
-            v[j] = (p.terms == 3) ? fmaf(__uint_as_float(t2[j]), kLoInv, __uint_as_float(t1[j])) : __uint_as_float(t1[j]);
-        }
-        epi_affine16(v, p.scale, p.shift, n0 + i * 32 + half * 16);
-        if (p.residual != LT_RES_NONE) {
-          mbar_wait(&res_full[buf], (uint32_t)((i >> 1) & 1));
-          epi_load16(smem_u32(res_stage + buf * 16384), row, half, p.out_format, r);
-        }
-        epi_activate16(v, r, p.residual, p.relu);
-        if (leader) bulk_wait_read<1>();      // the store that last read out_stage[buf] (block i-2) is done with it
-        epi_bar_sync();
-        epi_store16(smem_u32(out_stage + buf * 16384), row, half, p.out_format, v);
-        fence_proxy_async();
-        epi_bar_sync();
-        if (leader) {
-          int mi, ch;
-          blk_map(i, mi, ch);
-          tma_store_5d(&tmOut.m[mi], out_stage + buf * 16384, ch * esz, ow0, oh0, od0, nb0);
-          bulk_commit();
-          if (p.residual != LT_RES_NONE && i + 2 < nblk) {
-            blk_map(i + 2, mi, ch);
-            mbar_expect_tx(&res_full[buf], 16384u);
-            tma_load_5d(res_stage + buf * 16384, &tmRes.m[mi], &res_full[buf], ch * esz, ow0, oh0, od0, nb0);
-          }
-        }
-      }
-      if (leader) bulk_wait<0>();
-    } else
-    for (int c0 = half * 16; c0 < p.Nt; c0 += 32) {
-      uint32_t v[16];
-      tmem_ld16(tlane + (uint32_t)c0, v);   // whole warp (sync.aligned)
-      if (p.terms == 3) {
-        uint32_t v2[16];
-        tmem_ld16(tlane + (uint32_t)(p.Nt + c0), v2);
-#pragma unroll
-        for (int j = 0; j < 16; ++j) v[j] = __float_as_uint(fmaf(__uint_as_float(v2[j]), kLoInv, __uint_as_float(v[j])));
-      }
-      if (!valid) continue;
-      const int co0 = n0 + c0;
-#pragma unroll
-      for (int j = 0; j < 16; j += 4) {
-        const int co = co0 + j;
-        if (co >= p.FC) break;
-        const float4 sc = __ldg(reinterpret_cast<const float4*>(p.scale + co));
-        const float4 sh = __ldg(reinterpret_cast<const float4*>(p.shift + co));
-        float4 o = make_float4(fmaf(__uint_as_float(v[j]), sc.x, sh.x), fmaf(__uint_as_float(v[j + 1]), sc.y, sh.y),
-                               fmaf(__uint_as_float(v[j + 2]), sc.z, sh.z), fmaf(__uint_as_float(v[j + 3]), sc.w, sh.w));
-        float4 rr = make_float4(0.f, 0.f, 0.f, 0.f);
-        if (p.residual != LT_RES_NONE) {
-          if (p.out_format == LT_FMT_F32) rr = *reinterpret_cast<const float4*>(reinterpret_cast<const float*>(p.res) + opix * p.FC + co);
-          else rr = load_s32x4(reinterpret_cast<const sh_t*>(p.res) + opix * 2 * p.FC, co);
-        }
-        if (p.residual == LT_RES_BEFORE_RELU) { o.x += rr.x; o.y += rr.y; o.z += rr.z; o.w += rr.w; }
-        if (p.relu) { o.x = fmaxf(o.x, 0.f); o.y = fmaxf(o.y, 0.f); o.z = fmaxf(o.z, 0.f); o.w = fmaxf(o.w, 0.f); }
-        if (p.residual == LT_RES_AFTER_RELU) { o.x += rr.x; o.y += rr.y; o.z += rr.z; o.w += rr.w; }
-        if (p.out_format == LT_FMT_F32) *reinterpret_cast<float4*>(reinterpret_cast<float*>(p.out) + opix * p.FC + co) = o;
-        else store_s32x4(reinterpret_cast<sh_t*>(p.out) + opix * 2 * p.FC, co, o);
+      if (p.residual == LT_RES_BEFORE_RELU) { v0 += rr.x; v1 += rr.y; }
+      if (p.relu) { v0 = fmaxf(v0, 0.f); v1 = fmaxf(v1, 0.f); }
+      if (p.residual == LT_RES_AFTER_RELU) { v0 += rr.x; v1 += rr.y; }
+      if (p.out_format == LT_FMT_F32) {
+        *reinterpret_cast<float2*>(reinterpret_cast<float*>(p.out) + pix * p.FC + ch) = make_float2(v0, v1);
+      } else {
+        uint32_t hi2, lo2;
+        split_s32x2(v0, v1, hi2, lo2);
+        sh_t* op = reinterpret_cast<sh_t*>(p.out) + pix * 2 * p.FC + s32_off(ch);
+        *reinterpret_cast<uint32_t*>(op) = hi2;
+        *reinterpret_cast<uint32_t*>(op + 32) = lo2;
       }
     }
-  }
-
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, (uint32_t)p.tmem_cols);
-  }
-}
-
-// ------------------------------------------------------------------------------------------------
-// Persistent variant: one CTA per SM loops over (M tile, N tile) pairs.  Two TMEM accumulator stages let the
-// epilogue of tile i (8 warps) overlap the MMAs of tile i+1, the operand ring runs continuously across tiles,
-// and the residual tiles of the NEXT epilogue are prefetched by TMA into dedicated staging while the main loop
-// of the current tile is still running (the non-persistent kernel exposes that DRAM latency in every CTA).
-// ------------------------------------------------------------------------------------------------
-struct TcPersistExtra {
-  int n_tiles;        // N tiles
-  long total_tiles;   // M tiles * N tiles
-  int off_out, off_res, off_bar;   // smem offsets
-  // B-resident mode (1x1 convs with K * Nt * 128 B of weights <= ~64 KB): CTA = (N tile, M stream); the CTA's weight
-  // tile is loaded ONCE into shared memory (off_b) and only A tiles stream through the ring -- the per-SM L2 ingest
-  // (64 B/clk, tools/cta2_probe.cu) then carries 16 KB instead of 16 KB + Nt * 128 B per K chunk
-  int b_resident, off_b, m_streams;
-  long m_tiles;
-};
-
-__device__ __forceinline__ void mbar_arrive_cta(uint64_t* bar) {
-  asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(bar)) : "memory");
-}
-
-__global__ void __launch_bounds__(320, 1) conv_tc_persist_kernel(const __grid_constant__ CUtensorMap tmA,
-                                                                 const __grid_constant__ CUtensorMap tmB,
-                                                                 const __grid_constant__ CUtensorMap tmOut,
-                                                                 const __grid_constant__ CUtensorMap tmRes, const TcParams p,
-                                                                 const TcPersistExtra x) {
-  extern __shared__ uint8_t smem_raw[];
-  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
-  const int b_bytes = p.Nt * 128;
-  const int stage_bytes = x.b_resident ? kATileBytes : kATileBytes + b_bytes;
-  uint8_t* out_stage = smem + x.off_out;   // 2 x 16 KB
-  uint8_t* res_stage = smem + x.off_res;   // 2 x 16 KB
-  uint8_t* b_smem = smem + x.off_b;        // resident weights (b_resident): nchunks x b_bytes
-  uint64_t* full = reinterpret_cast<uint64_t*>(smem + x.off_bar);
-  uint64_t* empty = full + p.stages;
-  uint64_t* acc_full = empty + p.stages;   // [2]
-  uint64_t* acc_empty = acc_full + 2;      // [2]
-  uint64_t* res_full = acc_empty + 2;      // [2]
-  uint64_t* b_full = res_full + 2;         // [1]
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(b_full + 1);
-
-  const int warp = uniform_warp_idx(), lane = threadIdx.x & 31;
-  const int nchunks = p.KD * p.KH * p.KW * p.CB;
-  const int acc_cols = (p.terms == 3 ? 2 : 1) * p.Nt;
-
-  if (threadIdx.x == 0) {
-    for (int s = 0; s < p.stages; ++s) { mbar_init(&full[s], 1); mbar_init(&empty[s], 1); }
-    for (int i = 0; i < 2; ++i) { mbar_init(&acc_full[i], 1); mbar_init(&acc_empty[i], kEpiThreads); mbar_init(&res_full[i], 1); }
-    mbar_init(b_full, 1);
-    fence_barrier_init();
-  }
-  if (warp == 0 && lane == 0) { prefetch_tmap(&tmA); prefetch_tmap(&tmB); prefetch_tmap(&tmOut); }
-  if (warp == 1) tmem_alloc(tmem_slot, 512u);
-  tc_fence_before();
-  __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
-
-  // tile -> coordinates (N tile fastest: CTAs running side by side share the A tile in L2)
-  // B-resident mode: `tile` is this CTA's k-th M tile (k * m_streams + stream), the N tile is fixed per CTA
-  const int my_nt = x.b_resident ? (int)(blockIdx.x % x.n_tiles) : 0;
-  const long tile_first = x.b_resident ? (long)(blockIdx.x / x.n_tiles) : (long)blockIdx.x;
-  const long tile_step = x.b_resident ? (long)x.m_streams : (long)gridDim.x;
-  const long tile_end = x.b_resident ? x.m_tiles : x.total_tiles;
-  auto decode = [&](long tile, int& ow0, int& oh0, int& od0, int& nb0, int& n0) {
-    long t;
-    if (x.b_resident) { n0 = my_nt * p.Nt; t = tile; }
-    else { n0 = (int)(tile % x.n_tiles) * p.Nt; t = tile / x.n_tiles; }
-    ow0 = (int)(t % p.tw) * p.bw; t /= p.tw;
-    oh0 = (int)(t % p.th) * p.bh; t /= p.th;
-    od0 = (int)(t % p.td) * p.bd; t /= p.td;
-    nb0 = (int)t * p.bn;
-  };
-
-  if (warp == 0) {
-    // ================= TMA producer =================
-    uint32_t rs = 0, rph = 0;   // ring slot / phase, running across tiles
-    if (x.b_resident) {
-      if (elect_one()) {
-        mbar_expect_tx(b_full, (uint32_t)(nchunks * b_bytes));
-        // weights are packed in 128-wide N tiles [128 hi rows ; 128 lo rows]; this CTA's 64-wide sub-tile = two 64-row boxes
-        const int n0r = my_nt * p.Nt;
-        for (int q = 0; q < nchunks; ++q) {
-          const int row = q * p.b_step1 + (n0r >> 7) * 256 + (n0r & 127);
-          tma_load_2d(b_smem + (size_t)q * b_bytes, &tmB, b_full, q * p.b_step0, row);
-          tma_load_2d(b_smem + (size_t)q * b_bytes + b_bytes / 2, &tmB, b_full, q * p.b_step0, row + 128);
-        }
-      }
-      __syncwarp();
-    }
-    for (long tile = tile_first; tile < tile_end; tile += tile_step) {
-      int ow0, oh0, od0, nb0, n0;
-      decode(tile, ow0, oh0, od0, nb0, n0);
-      const int ax = ow0 * p.sw - p.pw, ay = oh0 * p.sh - p.ph, az = od0 * p.sd - p.pd, bn0 = n0 * p.b_nmul;
-      int cb = 0, kw = 0, kh = 0, kd = 0;     // incremental chunk -> (tap, channel block); ring slot / phase likewise
-      for (int q = 0; q < nchunks; ++q) {
-        mbar_wait(&empty[rs], rph ^ 1u);
-        uint8_t* a_dst = smem + (size_t)rs * stage_bytes;
-        if (elect_one()) {
-          mbar_expect_tx(&full[rs], (uint32_t)stage_bytes);
-          tma_load_5d(a_dst, &tmA, &full[rs], cb * 64, ax + kw, ay + kh, az + kd, nb0);
-          if (!x.b_resident) tma_load_2d(a_dst + kATileBytes, &tmB, &full[rs], q * p.b_step0, q * p.b_step1 + bn0);
-        }
-        __syncwarp();
-        if (++cb == p.CB) { cb = 0; if (++kw == p.KW) { kw = 0; if (++kh == p.KH) { kh = 0; ++kd; } } }
-        if (++rs == (uint32_t)p.stages) { rs = 0; rph ^= 1u; }
-      }
-    }
-  } else if (warp == 1) {
-    // ================= MMA issuer =================
-    const uint32_t idesc = make_idesc_f16(p.Nt), idesc2 = make_idesc_f16(2 * p.Nt);
-    uint32_t rs = 0, rph = 0, it = 0;
-    const uint32_t ring0 = smem_u32(smem), bres0 = smem_u32(b_smem);
-    if (x.b_resident) { mbar_wait(b_full, 0); tc_fence_after(); }
-    for (long tile = tile_first; tile < tile_end; tile += tile_step, ++it) {
-      const uint32_t as = it & 1u;
-      mbar_wait(&acc_empty[as], ((it >> 1) & 1u) ^ 1u);
-      tc_fence_after();
-      const uint32_t d1 = tmem_base + as * (uint32_t)acc_cols, d2 = d1 + (uint32_t)p.Nt;
-      for (int q = 0; q < nchunks; ++q) {
-        const uint32_t s = rs;
-        mbar_wait(&full[s], rph);
-        tc_fence_after();
-        const uint32_t a_addr = ring0 + s * (uint32_t)stage_bytes;
-        const uint64_t ad = make_sw128_desc(a_addr);
-        const uint64_t bd = make_sw64_desc(x.b_resident ? bres0 + (uint32_t)(q * b_bytes) : a_addr + kATileBytes);
-        const uint32_t first = (q == 0) ? 0u : 1u;
-        if (elect_one()) {
-          if (p.terms == 3) {
-            umma_f16(d1, ad, bd, idesc2, first);
-            umma_f16(d2, ad + 4, bd, idesc, 1);
-            umma_f16(d1, ad + 2, bd + 2, idesc2, 1);
-            umma_f16(d2, ad + 6, bd + 2, idesc, 1);
-          } else {
-            umma_f16(d1, ad, bd, idesc, first);
-            umma_f16(d1, ad + 2, bd + 2, idesc, 1);
-          }
-          umma_commit(&empty[s]);
-          if (q == nchunks - 1) umma_commit(&acc_full[as]);
-        }
-        __syncwarp();
-        if (++rs == (uint32_t)p.stages) { rs = 0; rph ^= 1u; }
-      }
-    }
-  } else {
-    // ================= epilogue (warps 2..9) =================
-    const int quad = warp & 3;
-    const int half = (warp - 2) >> 2;
-    const int row = quad * 32 + lane;
-    const bool leader = threadIdx.x == 64;
-    const int nblk = p.Nt >> 5;
-    const int esz = (p.out_format == LT_FMT_F32) ? 1 : 2;
-    const bool has_res = p.residual != LT_RES_NONE;
-    // Residual tiles stream through two 16 KB buffers indexed by a block counter that runs across tiles: global block
-    // c = (k-th tile of this CTA, block c % nblk) lives in buffer c & 1 and is requested two blocks ahead, so the blocks of
-    // the NEXT tile are already in flight while the main loop of that tile runs.
-    const long my_tiles = (tile_end > tile_first) ? (tile_end - 1 - tile_first) / tile_step + 1 : 0;
-    const long total_blocks = my_tiles * nblk;
-    auto issue_res = [&](long c) {   // leader only
-      const long tile_c = tile_first + (c / nblk) * tile_step;
-      const int blk = (int)(c % nblk);
-      int a0, a1, a2, a3, an;
-      decode(tile_c, a0, a1, a2, a3, an);
-      const int buf = (int)(c & 1);
-      mbar_expect_tx(&res_full[buf], 16384u);
-      tma_load_5d(res_stage + buf * 16384, &tmRes, &res_full[buf], an * esz + blk * 32 * esz, a0, a1, a2, a3);
-    };
-    if (leader && has_res)
-      for (long c = 0; c < 2 && c < total_blocks; ++c) issue_res(c);
-    uint32_t it = 0;
-    long c = 0;   // global block counter
-    for (long tile = tile_first; tile < tile_end; tile += tile_step, ++it) {
-      int ow0, oh0, od0, nb0, n0;
-      decode(tile, ow0, oh0, od0, nb0, n0);
-      const uint32_t as = it & 1u;
-      const int cbase = n0 * esz;
-      mbar_wait(&acc_full[as], (it >> 1) & 1u);
-      tc_fence_after();
-      const uint32_t tlane = tmem_base + ((uint32_t)(quad * 32) << 16) + as * (uint32_t)acc_cols;
-      for (int i = 0; i < nblk; ++i, ++c) {
-        const int buf = (int)(c & 1);
-        float v[16], r[16];
-        {
-          uint32_t t1[16], t2[16];
-          tmem_ld16_nowait(tlane + (uint32_t)(i * 32 + half * 16), t1);
-          if (p.terms == 3) tmem_ld16_nowait(tlane + (uint32_t)(p.Nt + i * 32 + half * 16), t2);
-          tmem_wait_ld();
-#pragma unroll
-          for (int j = 0; j < 16; ++j)
-            v[j] = (p.terms == 3) ? fmaf(__uint_as_float(t2[j]), kLoInv, __uint_as_float(t1[j])) : __uint_as_float(t1[j]);
-        }
-        if (i == nblk - 1) {               // accumulator stage fully read: release it to the MMA warp
-          tc_fence_before();
-          mbar_arrive_cta(&acc_empty[as]);
-        }
-        epi_affine16(v, p.scale, p.shift, n0 + i * 32 + half * 16);
-        if (has_res) {
-          mbar_wait(&res_full[buf], (uint32_t)((c >> 1) & 1));
-          epi_load16(smem_u32(res_stage + buf * 16384), row, half, p.out_format, r);
-        }
-        epi_activate16(v, r, p.residual, p.relu);
-        if (leader) bulk_wait_read<1>();      // the store that last read out_stage[buf] (two blocks ago) is done with it
-        epi_bar_sync();                       // also: every thread has finished reading res_stage[buf]
-        epi_store16(smem_u32(out_stage + buf * 16384), row, half, p.out_format, v);
-        fence_proxy_async();
-        epi_bar_sync();
-        if (leader) {
-          tma_store_5d(&tmOut, out_stage + buf * 16384, cbase + i * 32 * esz, ow0, oh0, od0, nb0);
-          bulk_commit();
-          if (has_res && c + 2 < total_blocks) issue_res(c + 2);
-        }
-      }
-    }
-    if (leader) bulk_wait<0>();
-  }
-
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, 512u);
   }
 }
 
@@ -616,100 +333,47 @@ __global__ void __launch_bounds__(256) splitk_reduce_kernel(const TcParams p, lo
   }
 }
 
-// Tensor map over the output (or residual) tensor as seen by this launch: the stride-phase mapping
-// (out coordinate = o * os + oo) becomes a base offset plus scaled strides; box = one 32-channel block of an M tile.
-static int make_out_map(CUtensorMap* map, const void* base, const lt_conv_desc* d, const TcParams& p);
-// one map per output group: group g = (a * ogh + b) * ogw + c adds (a, b, c) to the output offset (ood, ooh, oow)
-static int make_out_maps(OutMaps* maps, const void* base, const lt_conv_desc* d, const TcParams& p) {
-  const int gh = d->ogh > 1 ? d->ogh : 1, gw = d->ogw > 1 ? d->ogw : 1;
-  for (int g = 0; g < p.n_maps; ++g) {
-    lt_conv_desc dg = *d;
-    dg.ood += g / (gh * gw); dg.ooh += (g / gw) % gh; dg.oow += g % gw;
-    int rc = make_out_map(&maps->m[g], base, &dg, p);
-    if (rc) return rc;
-  }
-  return LT_OK;
-}
-static int make_out_map(CUtensorMap* map, const void* base, const lt_conv_desc* d, const TcParams& p) {
-  const uint64_t rowb = (uint64_t)d->FC * 4;   // 4 bytes per channel in both formats
-  const uint8_t* b0 = reinterpret_cast<const uint8_t*>(base) +
-                      (((uint64_t)d->ood * d->FH + d->ooh) * d->FW + d->oow) * rowb;
-  const int f32 = d->out_format == LT_FMT_F32;
-  const uint64_t dims[5] = {(uint64_t)d->FC * (f32 ? 1 : 2), (uint64_t)d->OW, (uint64_t)d->OH, (uint64_t)d->OD, (uint64_t)d->N};
-  const uint64_t str[4] = {rowb * d->osw, rowb * d->FW * d->osh, rowb * d->FW * d->FH * d->osd, rowb * d->FW * d->FH * d->FD};
-  const uint32_t bx[5] = {(uint32_t)(f32 ? 32 : 64), (uint32_t)p.bw, (uint32_t)p.bh, (uint32_t)p.bd, (uint32_t)p.bn};
-  return make_map(map, b0, 5, dims, str, bx, nullptr, 1, f32);
+static int out_groups(const lt_conv_desc* d) {
+  const int g = (d->ogd > 1 ? d->ogd : 1) * (d->ogh > 1 ? d->ogh : 1) * (d->ogw > 1 ? d->ogw : 1);
+  return g;
 }
 
-static int launch_tc(const CUtensorMap& tmA, const CUtensorMap& tmB, const OutMaps& tmOut, const OutMaps& tmRes,
-                     TcParams& p, int n_tiles, cudaStream_t st, void* ws = nullptr, size_t ws_bytes = 0) {
-  p.splits = 1; p.ws = nullptr; p.ws_ld = 0;
-  const int stage_bytes = kATileBytes + p.Nt * 128;
-  const long ctas = (long)p.tw * p.th * p.td * p.tn * n_tiles;
-  // two resident CTAs per SM when the grid fills the chip; small grids (deep V2V levels) are latency-bound on the
-  // K loop instead, so give each CTA the whole shared memory as pipeline depth
-  int stages = ((ctas > (long)sm_count() ? 96 : 200) * 1024) / stage_bytes;
-  if (stages < 2) stages = 2;
-  if (stages > 10) stages = 10;
-  p.stages = stages;
-  const int acc_cols = (p.terms == 3 ? 2 : 1) * p.Nt;
-  p.tmem_cols = pow2_ceil(acc_cols) < 32 ? 32 : pow2_ceil(acc_cols);
-  const size_t smem = (size_t)stages * stage_bytes + (2 * stages + 3) * 8 + 16 + 1024;
-  if (p.tma_epi && (size_t)stages * stage_bytes < 65536) return fail(LT_ERR_INVALID, "conv_tc: operand ring too small for the staged epilogue");
+// largest N tile of {128, 64, 32, 16} that divides the padded channel count (a multiple of 16)
+static int pick_nt(int CoutP) {
+  for (int nt = 128; nt > 16; nt >>= 1)
+    if (CoutP % nt == 0) return nt;
+  return 16;
+}
+
+template <int NT>
+static int launch_nt(const CUtensorMap& tmA, const CUtensorMap& tmB, const TcParams& p, dim3 grid, size_t smem, cudaStream_t st) {
   static DeviceOnce configured;
   if (configured.first()) {
-    cudaError_t e = cudaFuncSetAttribute(conv_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(227 * 1024));
+    cudaError_t e = cudaFuncSetAttribute(conv_tc_kernel<NT>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(227 * 1024));
     if (e != cudaSuccess) return fail(LT_ERR_CUDA, "conv_tc: cudaFuncSetAttribute: %s", cudaGetErrorString(e));
   }
+  conv_tc_kernel<NT><<<grid, kTcThreads, smem, st>>>(tmA, tmB, p);
+  cudaError_t e = cudaGetLastError();
+  if (e != cudaSuccess) return fail(LT_ERR_CUDA, "conv_tc_kernel: %s", cudaGetErrorString(e));
+  return LT_OK;
+}
+
+static int launch_tc(const CUtensorMap& tmA, const CUtensorMap& tmB, TcParams& p, int n_tiles, cudaStream_t st, void* ws = nullptr,
+                     size_t ws_bytes = 0) {
+  const int stage_bytes = kATileBytes + p.Nt * 128;
+  // one CTA per SM (the two consumer warpgroups hold up to 128 fp32 accumulators per thread): the whole shared memory is
+  // pipeline depth
+  int stages = (200 * 1024) / stage_bytes;
+  if (stages > 8) stages = 8;
+  p.stages = stages;
+  const size_t smem = (size_t)stages * stage_bytes + 2 * stages * 8 + 1024;
   const long m_tiles = (long)p.tw * p.th * p.td * p.tn;
-  const int persist_mode = opts().tc_persist;
-  // Measured on B200 (profiles/): two co-resident non-persistent CTAs already overlap epilogue and main loop for the
-  // MMA-heavy layers and win there; the persistent variant wins when a tile carries almost no work (1x1x1 convs at 64^3:
-  // 0.73 -> 0.41 ms for three launches), where CTA setup (TMEM alloc, barrier init, descriptor fetch) dominates.
   const int nchunks_total = p.KD * p.KH * p.KW * p.CB;
-  const bool tiny_tiles = nchunks_total * (p.Nt / 32) <= 2 && m_tiles * n_tiles > 4L * sm_count();
-  // B-resident persistent variant (requested by conv_tc_fwd_terms through p.bres): K-short 1x1 layers whose N tiles re-read
-  // the same A tiles -- the per-SM L2 ingest, not the tensor pipe, bounds them (DESIGN.md section 4)
-  const long bres_bytes = (long)nchunks_total * p.Nt * 128;
-  const bool bres = p.bres != 0;
-  if (p.n_maps == 1 && (bres || ((persist_mode == 2 || (persist_mode == 1 && tiny_tiles)) && p.tma_epi && p.terms != 0 && m_tiles * n_tiles > (long)sm_count()))) {
-    // persistent variant: one CTA per SM, deep operand ring + dedicated epilogue staging, two TMEM accumulator stages
-    TcPersistExtra x;
-    x.n_tiles = n_tiles;
-    x.total_tiles = m_tiles * n_tiles;
-    x.b_resident = bres ? 1 : 0;
-    x.m_tiles = m_tiles;
-    x.m_streams = bres ? sm_count() / n_tiles : 0;
-    const int ring_stage = bres ? kATileBytes : stage_bytes;
-    int pst = ((bres ? 96 : 128) * 1024) / ring_stage;
-    if (pst > 8) pst = 8;
-    if (pst < 2) pst = 2;
-    if (bres && pst > 6) pst = 6;
-    p.stages = pst;
-    const int ring = pst * ring_stage;
-    x.off_b = (ring + 1023) & ~1023;
-    x.off_out = bres ? (int)((x.off_b + bres_bytes + 1023) & ~1023L) : x.off_b;
-    x.off_res = x.off_out + 32768;
-    x.off_bar = x.off_res + 32768;
-    const size_t psmem = (size_t)x.off_bar + (2 * pst + 7) * 8 + 16 + 1024;
-    if (psmem > 227 * 1024) return fail(LT_ERR_INVALID, "conv_tc_persist: shared memory budget exceeded (%zu)", psmem);
-    static DeviceOnce pconf;
-    if (pconf.first()) {
-      cudaError_t e2 = cudaFuncSetAttribute(conv_tc_persist_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(227 * 1024));
-      if (e2 != cudaSuccess) return fail(LT_ERR_CUDA, "conv_tc_persist: cudaFuncSetAttribute: %s", cudaGetErrorString(e2));
-    }
-    const unsigned pgrid = bres ? (unsigned)(x.m_streams * n_tiles) : (unsigned)sm_count();
-    conv_tc_persist_kernel<<<pgrid, 320, psmem, st>>>(tmA, tmB, tmOut.m[0], tmRes.m[0], p, x);
-    cudaError_t e3 = cudaGetLastError();
-    if (e3 != cudaSuccess) return fail(LT_ERR_CUDA, "conv_tc_persist_kernel: %s", cudaGetErrorString(e3));
-    return LT_OK;
-  }
   // split-K: a grid that cannot fill half the SMs is bound by the serial K loop of each CTA (27 taps x Cin/32 chunks of
   // weights streamed from HBM by ONE SM); spread the chunks over blockIdx.z instead
-  const int splitk_mode = opts().tc_splitk;
   int splits = 1;
   const long grid_ctas = m_tiles * n_tiles;
-  if (splitk_mode && ws && p.terms != 0 && p.n_maps == 1 && grid_ctas * 2 <= (long)sm_count() && nchunks_total >= 16) {
+  if (opts().tc_splitk && ws && p.terms != 0 && p.n_maps == 1 && grid_ctas * 2 <= (long)sm_count() && nchunks_total >= 16) {
     splits = (int)((long)sm_count() / grid_ctas);
     if (splits > nchunks_total / 4) splits = nchunks_total / 4;
     const size_t per_split = (size_t)m_tiles * 128 * (size_t)n_tiles * p.Nt * sizeof(float);
@@ -720,29 +384,29 @@ static int launch_tc(const CUtensorMap& tmA, const CUtensorMap& tmB, const OutMa
   p.ws = reinterpret_cast<float*>(ws);
   p.ws_ld = n_tiles * p.Nt;
   dim3 grid((unsigned)m_tiles, (unsigned)n_tiles, (unsigned)splits);
-  conv_tc_kernel<<<grid, 320, smem, st>>>(tmA, tmB, tmOut, tmRes, p);
-  cudaError_t e = cudaGetLastError();
-  if (e != cudaSuccess) return fail(LT_ERR_CUDA, "conv_tc_kernel: %s", cudaGetErrorString(e));
+  int rc;
+  switch (p.Nt) {
+    case 128: rc = launch_nt<128>(tmA, tmB, p, grid, smem, st); break;
+    case 64: rc = launch_nt<64>(tmA, tmB, p, grid, smem, st); break;
+    case 32: rc = launch_nt<32>(tmA, tmB, p, grid, smem, st); break;
+    case 16: rc = launch_nt<16>(tmA, tmB, p, grid, smem, st); break;
+    default: return fail(LT_ERR_INVALID, "conv_tc: unsupported N tile %d", p.Nt);
+  }
+  if (rc) return rc;
   if (splits > 1) {
     const long total = m_tiles * 128 * (p.ws_ld / 4);
     long blocks = (total + 255) / 256;
     if (blocks > 4L * sm_count()) blocks = 4L * sm_count();
     splitk_reduce_kernel<<<(unsigned)blocks, 256, 0, st>>>(p, m_tiles, p.ws_ld);
-    e = cudaGetLastError();
+    cudaError_t e = cudaGetLastError();
     if (e != cudaSuccess) return fail(LT_ERR_CUDA, "splitk_reduce_kernel: %s", cudaGetErrorString(e));
   }
   return LT_OK;
 }
 
-static int out_groups(const lt_conv_desc* d) {
-  const int g = (d->ogd > 1 ? d->ogd : 1) * (d->ogh > 1 ? d->ogh : 1) * (d->ogw > 1 ? d->ogw : 1);
-  return g;
-}
-
 // fills the geometry / epilogue part of the launch parameters (M-tile box, taps, output mapping)
 static void fill_params(const lt_conv_desc* d, TcParams& p, int CB, int CoutP, int Nt, int terms, const float* scale, const float* shift,
                         const void* residual, void* out) {
-  p.bres = 0;
   p.OW = d->OW; p.OH = d->OH; p.OD = d->OD; p.N = d->N;
   int box[4];
   pick_box(d->OW, d->OH, d->OD, d->N, box);
@@ -750,12 +414,12 @@ static void fill_params(const lt_conv_desc* d, TcParams& p, int CB, int CoutP, i
   p.tw = ceil_div(d->OW, p.bw); p.th = ceil_div(d->OH, p.bh); p.td = ceil_div(d->OD, p.bd); p.tn = ceil_div(d->N, p.bn);
   p.KW = d->KW; p.KH = d->KH; p.KD = d->KD; p.pw = d->pw; p.ph = d->ph; p.pd = d->pd;
   p.sw = d->sw; p.sh = d->sh; p.sd = d->sd;
-  p.CB = CB; p.b_step0 = 0; p.b_step1 = 2 * CoutP; p.b_nmul = 2; p.Nt = Nt; p.terms = terms;
+  p.CB = CB; p.b_step0 = 0; p.b_step1 = CoutP; p.b_nmul = 1; p.Nt = Nt; p.terms = terms;
   p.FC = d->FC; p.FD = d->FD; p.FH = d->FH; p.FW = d->FW;
   p.osd = d->osd; p.osh = d->osh; p.osw = d->osw; p.ood = d->ood; p.ooh = d->ooh; p.oow = d->oow;
   p.relu = d->relu; p.residual = d->residual; p.out_format = d->out_format;
   p.scale = scale; p.shift = shift; p.res = residual; p.out = out;
-  p.splits = 1; p.ws = nullptr; p.ws_ld = 0; p.stages = 0; p.tmem_cols = 0; p.tma_epi = 0;
+  p.splits = 1; p.ws = nullptr; p.ws_ld = 0; p.stages = 0;
   p.n_maps = out_groups(d);
   p.oc = p.n_maps > 1 ? d->Cout / p.n_maps : CoutP;
   p.gh = d->ogh > 1 ? d->ogh : 1; p.gw = d->ogw > 1 ? d->ogw : 1;
@@ -773,147 +437,79 @@ static int make_in_map(CUtensorMap* tmA, const lt_conv_desc* d, const TcParams& 
   return make_map(tmA, in, 5, dims, str, bx, es, 1);
 }
 
-static bool staged_epilogue_ok(const lt_conv_desc* d, int CoutP, int Nt) {
+// grouped output (k2 s2 transposed conv as one GEMM): every channel of the GEMM belongs to exactly one group, and a group fills the
+// output's channels exactly
+static bool groups_ok(const lt_conv_desc* d, int CoutP) {
   const int G = out_groups(d);
-  if (G > 1)    // grouped output: every 32-channel block must fall into one group, and fill the group's channels exactly
-    return Nt % 32 == 0 && d->Cout % G == 0 && (d->Cout / G) % 32 == 0 && d->Cout / G == d->FC && CoutP == d->Cout && G <= kMaxOutMaps &&
-           d->out_format == LT_FMT_S32;
-  // float32 outputs may be narrower than the (single) padded N tile: the tensor map then has FC channels and the TMA
-  // store clips the box at the tensor bound (80-byte voxel rows for the 17-joint logits instead of 128)
-  const bool clipped_f32 = d->out_format == LT_FMT_F32 && d->residual == LT_RES_NONE && CoutP == Nt && d->FC % 4 == 0 && d->FC < CoutP;
-  return Nt % 32 == 0 && ((d->FC % 32 == 0 && CoutP <= d->FC) || clipped_f32);
+  return d->Cout % G == 0 && (d->Cout / G) % 32 == 0 && d->Cout / G == d->FC && CoutP == d->Cout && G <= kMaxOutMaps &&
+         d->out_format == LT_FMT_S32;
 }
 
-// CTA-pair kernel (conv_pair.cu): weights packed by lt_conv_pair_pack_weights
-int conv_pair_fwd(const lt_conv_desc* d, const void* in, const void* weight, const float* scale, const float* shift,
-                  const void* residual, void* out, void* stream, int probe_only) {
-  LT_REQUIRE(d->in_format == LT_FMT_S32, "conv_pair: input must be split-fp16");
-  LT_REQUIRE(d->Cin % 32 == 0, "conv_pair: Cin=%d must be a multiple of 32", d->Cin);
-  const int CoutP = (d->Cout + 127) & ~127;
+// Shared by every tensor-core entry point: weights packed as [tap][Cin/32][CoutP rows][32 hi | 32 lo] fp16.
+static int conv_wg_fwd(const lt_conv_desc* d, const void* in, const void* weight, int CoutP, const float* scale, const float* shift,
+                       const void* residual, void* out, int terms, void* stream) {
+  LT_REQUIRE(d->in_format == LT_FMT_S32, "conv_tc: input must be split-fp16");
+  LT_REQUIRE(d->Cin % 32 == 0, "conv_tc: Cin=%d must be a multiple of 32", d->Cin);
+  LT_REQUIRE(d->FC % 4 == 0 && (d->out_format == LT_FMT_F32 || d->FC % 32 == 0), "conv_tc: bad output channel stride %d", d->FC);
   const int CB = d->Cin / 32;
   const int taps = d->KD * d->KH * d->KW;
+  const int Nt = pick_nt(CoutP);
   TcParams p;
-  fill_params(d, p, CB, CoutP, 128, 3, scale, shift, residual, out);
-  p.tma_epi = (d->Cout % 128 == 0 && staged_epilogue_ok(d, CoutP, 128)) ? 1 : 0;
-  PairPlan plan;
-  if (!pair_plan(d, p, CoutP, &plan)) {
-    if (probe_only) return 1;
-    return fail(LT_ERR_INVALID, "conv_pair: shape not covered by the CTA-pair kernel (Cout=%d FC=%d)", d->Cout, d->FC);
-  }
-  if (probe_only) return 0;
-  p.Nt = plan.Nt;
+  fill_params(d, p, CB, CoutP, Nt, terms, scale, shift, residual, out);
+  if (p.n_maps > 1)
+    LT_REQUIRE(groups_ok(d, CoutP), "conv_tc: grouped output needs split-fp16 output, Cout / groups == FC, a multiple of 32");
   CUtensorMap tmA, tmB;
-  OutMaps tmOut, tmRes;
   int rc = make_in_map(&tmA, d, p, in);
   if (rc) return rc;
   {
-    // weights: [tap][cb][CoutP rows][32 hi | 32 lo] fp16, 128-byte rows, 128B swizzle; each CTA of a pair loads Nt/2 rows
     const uint64_t dims[2] = {64, (uint64_t)taps * CB * CoutP};
     const uint64_t str[1] = {128};
-    const uint32_t bx[2] = {64, (uint32_t)(plan.Nt / 2)};
+    const uint32_t bx[2] = {64, (uint32_t)Nt};
     rc = make_map(&tmB, weight, 2, dims, str, bx, nullptr, 1);
     if (rc) return rc;
   }
-  rc = make_out_maps(&tmOut, out, d, p);
-  if (rc) return rc;
-  tmRes = tmOut;
-  if (d->residual != LT_RES_NONE) {
-    rc = make_out_maps(&tmRes, residual, d, p);
-    if (rc) return rc;
-  }
-  return launch_pair(tmA, tmB, tmOut, tmRes, p, plan, CoutP, (cudaStream_t)stream);
+  return launch_tc(tmA, tmB, p, CoutP / Nt, (cudaStream_t)stream, d->workspace, d->workspace_bytes);
+}
+
+// 128-padded weights (lt_conv_pair_pack_weights): the layers with Cout % 128 == 0
+int conv_pair_fwd(const lt_conv_desc* d, const void* in, const void* weight, const float* scale, const float* shift,
+                  const void* residual, void* out, void* stream, int probe_only) {
+  const int CoutP = (d->Cout + 127) & ~127;
+  const int G = out_groups(d);
+  const bool ok = d->in_format == LT_FMT_S32 && d->Cin % 32 == 0 && d->Cout % 128 == 0 &&
+                  (G > 1 ? groups_ok(d, CoutP) : (d->FC % 32 == 0 && CoutP <= d->FC));
+  if (probe_only) return ok ? 0 : 1;
+  if (!ok) return fail(LT_ERR_INVALID, "conv_pair: shape not covered (Cout=%d FC=%d)", d->Cout, d->FC);
+  return conv_wg_fwd(d, in, weight, CoutP, scale, shift, residual, out, 3, stream);
 }
 
 int conv_tc_fwd_terms(const lt_conv_desc* d, const void* in, const void* weight, const float* scale, const float* shift,
                       const void* residual, void* out, int terms, void* stream) {
-  LT_REQUIRE(d->in_format == LT_FMT_S32, "conv_tc: input must be split-fp16");
-  LT_REQUIRE(d->Cin % 32 == 0, "conv_tc: Cin=%d must be a multiple of 32", d->Cin);
-  LT_REQUIRE(d->FC % 4 == 0 && (d->out_format == LT_FMT_F32 || d->FC % 32 == 0), "conv_tc: bad output channel stride %d", d->FC);
-  const int CoutP = (d->Cout + 15) & ~15;
-  const int Nt = CoutP <= 128 ? CoutP : 128;
-  LT_REQUIRE(CoutP % Nt == 0, "conv_tc: Cout=%d (padded %d) not tileable by %d", d->Cout, CoutP, Nt);
-  const int CB = d->Cin / 32;
-  const int taps = d->KD * d->KH * d->KW;
-
-  TcParams p;
-  p.bres = 0;
-  p.OW = d->OW; p.OH = d->OH; p.OD = d->OD; p.N = d->N;
-  int box[4];
-  pick_box(d->OW, d->OH, d->OD, d->N, box);
-  p.bw = box[0]; p.bh = box[1]; p.bd = box[2]; p.bn = box[3];
-  p.tw = ceil_div(d->OW, p.bw); p.th = ceil_div(d->OH, p.bh); p.td = ceil_div(d->OD, p.bd); p.tn = ceil_div(d->N, p.bn);
-  p.KW = d->KW; p.KH = d->KH; p.KD = d->KD; p.pw = d->pw; p.ph = d->ph; p.pd = d->pd;
-  p.sw = d->sw; p.sh = d->sh; p.sd = d->sd;
-  p.CB = CB; p.b_step0 = 0; p.b_step1 = 2 * CoutP; p.b_nmul = 2; p.Nt = Nt; p.terms = terms;
-  p.FC = d->FC; p.FD = d->FD; p.FH = d->FH; p.FW = d->FW;
-  p.osd = d->osd; p.osh = d->osh; p.osw = d->osw; p.ood = d->ood; p.ooh = d->ooh; p.oow = d->oow;
-  p.relu = d->relu; p.residual = d->residual; p.out_format = d->out_format;
-  p.scale = scale; p.shift = shift; p.res = residual; p.out = out;
-  p.n_maps = out_groups(d);
-  p.oc = p.n_maps > 1 ? d->Cout / p.n_maps : CoutP;
-  p.gh = d->ogh > 1 ? d->ogh : 1; p.gw = d->ogw > 1 ? d->ogw : 1;
-
-  CUtensorMap tmA, tmB;
-  {
-    const uint64_t rowb = (uint64_t)d->Cin * 2 * 2;  // 2*Cin fp16 per position
-    const uint64_t dims[5] = {(uint64_t)d->Cin * 2, (uint64_t)d->IW, (uint64_t)d->IH, (uint64_t)d->ID, (uint64_t)d->N};
-    const uint64_t str[4] = {rowb, rowb * d->IW, rowb * d->IW * d->IH, rowb * d->IW * d->IH * d->ID};
-    // strided convs: TMA traversal strides; the box spans (b-1)*s+1 input positions and delivers b of them
-    const uint32_t es[5] = {1, (uint32_t)d->sw, (uint32_t)d->sh, (uint32_t)d->sd, 1};
-    uint32_t bx[5] = {64, (uint32_t)p.bw, (uint32_t)p.bh, (uint32_t)p.bd, (uint32_t)p.bn};
-    for (int i = 1; i <= 3; ++i) bx[i] = (bx[i] - 1) * es[i] + 1;
-    LT_REQUIRE(bx[1] <= 256 && bx[2] <= 256 && bx[3] <= 256, "conv_tc: strided box exceeds 256");
-    int rc = make_map(&tmA, in, 5, dims, str, bx, es, 1);
-    if (rc) return rc;
-  }
-  OutMaps tmOut, tmRes;
-  tmOut.m[0] = tmA; tmRes.m[0] = tmA;
-  const int direct_epi = opts().tc_direct_epilogue;
-  // float32 outputs may be narrower than the (single) padded N tile: the tensor map then has FC channels and the TMA
-  // store clips the box at the tensor bound (80-byte voxel rows for the 17-joint logits instead of 128)
-  const bool clipped_f32 = d->out_format == LT_FMT_F32 && d->residual == LT_RES_NONE && CoutP == Nt && d->FC % 4 == 0 && d->FC < CoutP;
-  p.tma_epi = (!direct_epi && Nt % 32 == 0 && ((d->FC % 32 == 0 && CoutP <= d->FC) || clipped_f32)) ? 1 : 0;
-  if (p.n_maps > 1) {
-    LT_REQUIRE(staged_epilogue_ok(d, CoutP, Nt), "conv_tc: grouped output needs split-fp16 output, Cout / groups == FC, a multiple of 32");
-    p.tma_epi = 1;
-  }
-  // B-resident persistent variant: 1x1-like layers (<= 8 K chunks) with more than one 128-wide N tile and enough M tiles
-  const int bres_mode = opts().tc_bres;
-  const long m_tiles_all = (long)p.tw * p.th * p.td * p.tn;
-  int n_tiles = CoutP / Nt;
-  if (bres_mode && p.n_maps == 1 && terms != 0 && p.tma_epi && taps * CB <= 8 && Nt == 128 && CoutP >= 256 && CoutP / 64 <= sm_count() / 2 &&
-      m_tiles_all >= 2L * (sm_count() / (CoutP / 64))) {
-    p.bres = 1;
-    p.Nt = 64;
-    n_tiles = CoutP / 64;
-  }
-  {
-    // weights: [tap][cb][n tile][hi|lo][Nt rows][32 channels] fp16, 64-byte rows, 64B swizzle
-    const uint64_t dims[2] = {32, (uint64_t)taps * CB * 2 * CoutP};
-    const uint64_t str[1] = {64};
-    const uint32_t bx[2] = {32, (uint32_t)(p.bres ? 64 : 2 * Nt)};
-    int rc = make_map(&tmB, weight, 2, dims, str, bx, nullptr, 2);
-    if (rc) return rc;
-  }
-  if (p.tma_epi) {
-    int rc = make_out_maps(&tmOut, out, d, p);
-    if (rc) return rc;
-    if (d->residual != LT_RES_NONE) {
-      rc = make_out_maps(&tmRes, residual, d, p);
-      if (rc) return rc;
-    }
-  }
-  return launch_tc(tmA, tmB, tmOut, tmRes, p, n_tiles, (cudaStream_t)stream, d->workspace, d->workspace_bytes);
+  return conv_wg_fwd(d, in, weight, (d->Cout + 15) & ~15, scale, shift, residual, out, terms, stream);
 }
 
-int conv_tc_fwd(const lt_conv_desc* d, const void* in, const void* weight, const float* scale, const float* shift,
-                const void* residual, void* out, void* stream) {
-  return conv_tc_fwd_terms(d, in, weight, scale, shift, residual, out, 3, stream);
+// kw-fold entry point (LT_CONV_TC_FOLD: Cin = 32 cubic stride-1 layers): the same kernel over weights packed by
+// lt_conv_fold_pack_weights as [tap][1][32 rows][32 hi | 32 lo], i.e. all 32 output channels (the padding ones are zero)
+int conv_fold_supported(const lt_conv_desc* d) {
+  const bool cubic = d->KD == d->KH && d->KH == d->KW && (d->KW == 3 || d->KW == 7);
+  const int pd = d->KW / 2;
+  return cubic && d->Cin == 32 && d->Cout <= 32 && d->sd == 1 && d->sh == 1 && d->sw == 1 && d->pd == pd && d->ph == pd &&
+         d->pw == pd && d->OD == d->ID && d->OH == d->IH && d->OW == d->IW && d->osd == 1 && d->osh == 1 && d->osw == 1 &&
+         d->ood == 0 && d->ooh == 0 && d->oow == 0 && d->FD == d->OD && d->FH == d->OH && d->FW == d->OW && d->FC == 32 &&
+         d->in_format == LT_FMT_S32 && d->IW >= 16;
 }
 
-// ---- weight packing: fp32 [taps][Cin][Cout] -> fp16 [taps][Cin/32][n tile][hi|lo][Nt][32] (64-byte rows) ----------
+int conv_fold_fwd(const lt_conv_desc* d, const void* in, const void* weight, const float* scale, const float* shift,
+                  const void* residual, void* out, void* stream) {
+  LT_REQUIRE(conv_fold_supported(d), "conv_fold: unsupported layer shape");
+  lt_conv_desc dg = *d;
+  dg.Cout = 32;
+  return conv_wg_fwd(&dg, in, weight, 32, scale, shift, residual, out, 3, stream);
+}
+
+// ---- weight packing: fp32 [taps][Cin][Cout] -> fp16 [taps][Cin/32][CoutP][32 hi | 32 lo] (128-byte rows) ----------
 __global__ void __launch_bounds__(256) pack_weights_kernel(const float* __restrict__ w, sh_t* __restrict__ out,
-                                                           int taps, int Cin, int Cout, int CoutP, int Nt) {
+                                                           int taps, int Cin, int Cout, int CoutP) {
   const int CB = Cin / 32;
   const long total = (long)taps * CB * CoutP * 32;
   for (long i = (long)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (long)gridDim.x * blockDim.x) {
@@ -925,11 +521,19 @@ __global__ void __launch_bounds__(256) pack_weights_kernel(const float* __restri
     const float v = (n < Cout) ? w[((long)tap * Cin + cb * 32 + j) * Cout + n] : 0.0f;
     sh_t hi, lo;
     split_s32(v, hi, lo);
-    const int nt = n / Nt, ni = n % Nt;
-    sh_t* tile = out + ((((long)tap * CB + cb) * (CoutP / Nt) + nt) * 2) * (long)Nt * 32;
-    tile[(long)ni * 32 + j] = hi;
-    tile[((long)Nt + ni) * 32 + j] = lo;
+    sh_t* rowp = out + ((((long)tap * CB + cb) * CoutP + n) << 6);
+    rowp[j] = hi;
+    rowp[32 + j] = lo;
   }
+}
+
+static int pack_weights(const float* w, void* packed, int taps, int Cin, int Cout, int CoutP, void* stream) {
+  const long total = (long)taps * (Cin / 32) * CoutP * 32;
+  long blocks = (total + 255) / 256;
+  if (blocks > 65535) blocks = 65535;
+  pack_weights_kernel<<<(unsigned)blocks, 256, 0, (cudaStream_t)stream>>>(w, reinterpret_cast<sh_t*>(packed), taps, Cin, Cout, CoutP);
+  LT_CHECK_LAUNCH("pack_weights_kernel");
+  return LT_OK;
 }
 
 __global__ void ones_zeros_kernel(float* ones, float* zeros, int n) {
@@ -943,32 +547,45 @@ using namespace lt;
 
 extern "C" size_t lt_conv_tc_weight_bytes(int taps, int Cin, int Cout) {
   const int CoutP = (Cout + 15) & ~15;
-  return (size_t)taps * (Cin / 32) * CoutP * 64 * 2;
+  return (size_t)taps * (Cin / 32) * CoutP * 128;
 }
 
 extern "C" int lt_conv_tc_pack_weights(const float* w, void* packed, int taps, int Cin, int Cout, void* stream) {
   LT_REQUIRE(w && packed, "conv_tc_pack_weights: null pointer");
   LT_REQUIRE(Cin % 32 == 0 && taps > 0 && Cout > 0, "conv_tc_pack_weights: bad sizes");
-  const int CoutP = (Cout + 15) & ~15;
-  const long total = (long)taps * (Cin / 32) * CoutP * 32;
-  long blocks = (total + 255) / 256;
-  if (blocks > 65535) blocks = 65535;
-  const int Nt = CoutP <= 128 ? CoutP : 128;
-  LT_REQUIRE(CoutP % Nt == 0, "conv_tc_pack_weights: Cout not tileable");
-  pack_weights_kernel<<<(unsigned)blocks, 256, 0, (cudaStream_t)stream>>>(w, reinterpret_cast<sh_t*>(packed), taps, Cin, Cout, CoutP, Nt);
-  LT_CHECK_LAUNCH("pack_weights_kernel");
-  return LT_OK;
+  return pack_weights(w, packed, taps, Cin, Cout, (Cout + 15) & ~15, stream);
+}
+
+extern "C" size_t lt_conv_pair_weight_bytes(int taps, int Cin, int Cout) {
+  const int CoutP = (Cout + 127) & ~127;
+  return (size_t)taps * (Cin / 32) * CoutP * 128;
+}
+
+extern "C" int lt_conv_pair_pack_weights(const float* w, void* packed, int taps, int Cin, int Cout, void* stream) {
+  LT_REQUIRE(w && packed, "conv_pair_pack_weights: null pointer");
+  LT_REQUIRE(Cin % 32 == 0 && taps > 0 && Cout > 0, "conv_pair_pack_weights: bad sizes");
+  return pack_weights(w, packed, taps, Cin, Cout, (Cout + 127) & ~127, stream);
+}
+
+extern "C" size_t lt_conv_fold_weight_bytes(int K, int Cout) {
+  (void)Cout;
+  return (size_t)K * K * K * 32 * 128;
+}
+
+// w_tap_ci_co: fp32 [K^3 taps (kd, kh, kw)][32][Cout]
+extern "C" int lt_conv_fold_pack_weights(const float* w_tap_ci_co, void* packed, int K, int Cout, void* stream) {
+  LT_REQUIRE(w_tap_ci_co && packed && (K == 3 || K == 7) && Cout > 0 && Cout <= 32, "conv_fold_pack_weights: bad arguments");
+  return pack_weights(w_tap_ci_co, packed, K * K * K, 32, Cout, 32, stream);
 }
 
 // D[M][N] (fp32) = A[M][K] * B[N][K]^T, plain fp16 row-major operands; exercises the exact TMA /
-// descriptor / tcgen05 / epilogue code of the conv kernel (terms = 0 selects plain rows).
+// descriptor / wgmma / epilogue code of the conv kernel (terms = 0 selects plain rows).
 // `d` must hold M*N floats followed by 2*N floats of scratch (scale/shift).
 extern "C" int lt_tc_gemm_selftest(const void* a, const void* b, float* d, int M, int N, int K, int variant, void* stream) {
   LT_REQUIRE(a && b && d, "tc_gemm_selftest: null pointer");
   LT_REQUIRE(M > 0 && N % 16 == 0 && N >= 16 && K % 64 == 0, "tc_gemm_selftest: need N %% 16 == 0, K %% 64 == 0");
   (void)variant;
-  const int Nt = N <= 128 ? N : 128;
-  LT_REQUIRE(N % Nt == 0, "tc_gemm_selftest: N must be <= 128 or a multiple of 128");
+  const int Nt = pick_nt(N);
   float* ones = d + (size_t)M * N;
   float* zeros = ones + N;
   ones_zeros_kernel<<<ceil_div(N, 256), 256, 0, (cudaStream_t)stream>>>(ones, zeros, N);
@@ -977,10 +594,11 @@ extern "C" int lt_tc_gemm_selftest(const void* a, const void* b, float* d, int M
   p.bw = 128; p.bh = 1; p.bd = 1; p.bn = 1;
   p.tw = ceil_div(M, 128); p.th = 1; p.td = 1; p.tn = 1;
   p.KW = p.KH = p.KD = 1; p.pw = p.ph = p.pd = 0; p.sw = p.sh = p.sd = 1;
-  p.CB = K / 64; p.b_step0 = 64; p.b_step1 = 0; p.b_nmul = 1; p.Nt = Nt; p.terms = 0; p.bres = 0;
+  p.CB = K / 64; p.b_step0 = 64; p.b_step1 = 0; p.b_nmul = 1; p.Nt = Nt; p.terms = 0;
   p.FC = N; p.FD = 1; p.FH = 1; p.FW = M; p.osd = p.osh = p.osw = 1; p.ood = p.ooh = p.oow = 0;
   p.relu = 0; p.residual = LT_RES_NONE; p.out_format = LT_FMT_F32;
   p.scale = ones; p.shift = zeros; p.res = nullptr; p.out = d;
+  p.n_maps = 1; p.oc = N; p.gh = p.gw = 1;
   CUtensorMap tmA, tmB;
   {
     const uint64_t dims[5] = {(uint64_t)K, (uint64_t)M, 1, 1, 1};
@@ -996,9 +614,5 @@ extern "C" int lt_tc_gemm_selftest(const void* a, const void* b, float* d, int M
     int rc = make_map(&tmB, b, 2, dims, str, bx, nullptr, 1);
     if (rc) return rc;
   }
-  p.tma_epi = 0;
-  p.n_maps = 1; p.oc = N; p.gh = p.gw = 1;
-  OutMaps dummy;
-  dummy.m[0] = tmA;
-  return launch_tc(tmA, tmB, dummy, dummy, p, N / Nt, (cudaStream_t)stream);
+  return launch_tc(tmA, tmB, p, N / Nt, (cudaStream_t)stream);
 }

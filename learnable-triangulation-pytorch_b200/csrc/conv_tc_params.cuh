@@ -1,4 +1,4 @@
-// Launch parameters shared by the tcgen05 implicit-GEMM conv kernels (conv_tc.cu: one CTA per tile; conv_pair.cu: CTA pairs).
+// Launch parameters of the wgmma implicit-GEMM conv kernel (conv_tc.cu).
 #pragma once
 #include "tc_common.cuh"
 
@@ -13,9 +13,7 @@ struct TcParams {
   int CB;                  // 64-element K chunks per tap
   int b_step0, b_step1;    // B-map coordinates of chunk q: (q*b_step0, q*b_step1 + n0*b_nmul)
   int b_nmul;
-  int Nt, stages, terms;   // N tile, pipeline depth, 1 or 3 product terms
-  int tmem_cols;
-  int tma_epi;             // 1: epilogue stages 32-channel blocks through smem and uses TMA store / residual load
+  int Nt, stages, terms;   // N tile, pipeline depth, 0 (plain fp16 rows), 1 or 3 product terms
   // epilogue
   int FC, FD, FH, FW, osd, osh, osw, ood, ooh, oow, relu, residual, out_format;
   const float* scale;
@@ -26,34 +24,15 @@ struct TcParams {
   // writes its raw fp32 accumulator tile to ws[z][m tile][128][ws_ld]; splitk_reduce_kernel sums and applies the epilogue
   int splits, ws_ld;
   float* ws;
-  int bres;   // host-side request: B-resident persistent variant (Nt = 64 sub-tiles of the 128-wide packed weight tiles)
   // grouped output (lt_conv_desc.ogd/ogh/ogw): output channel block g of `oc` channels goes to output map g (its own phase offset)
   int oc, n_maps;
   int gh, gw;    // output group grid (group g -> offset (g / (gh*gw), (g / gw) % gh, g % gw)); 1, 1 without groups
 };
 
-// Output / residual tensor maps of a launch: one per output group (k2 s2 transposed conv as ONE GEMM with N = 8 x Cout: group g
-// is the phase (a, b, c) of the output lattice); plain convs use m[0] only.
+// grouped output (lt_conv_desc.ogd/ogh/ogw): a k2 s2 transposed conv as ONE GEMM with N = 8 x Cout, group g = phase (a, b, c) of
+// the output lattice
 constexpr int kMaxOutMaps = 8;
-struct OutMaps { CUtensorMap m[kMaxOutMaps]; };
 
 constexpr int kATileBytes = 128 * 128;  // 128 rows x 64 fp16
-
-// conv_pair.cu: cta_group::2 persistent kernel (M = 256 per CTA pair, N tile up to 256, single fp32 accumulator)
-struct PairPlan {
-  int Nt;            // N tile (128 or 256)
-  int n_tiles;       // CoutP / Nt
-  long m_tiles;      // 128-position M tiles
-  long m_pairs;      // ceil(m_tiles / 2)
-  int stages;        // operand ring depth
-  int res_bufs;      // residual staging tiles (0 without a residual)
-  int direct_out;    // split-fp16 outputs: the epilogue stores rows straight from registers (no staging tile, no TMA store)
-  int two_acc;       // separate accumulator for the cross products (accuracy: see conv_pair.cu); acc_stages = TMEM stages that fit
-  int acc_stages;
-  unsigned grid;     // CTAs (2 per pair)
-};
-bool pair_plan(const lt_conv_desc* d, const TcParams& p, int CoutP, PairPlan* plan);   // false: shape not covered by the pair kernel
-int launch_pair(const CUtensorMap& tmA, const CUtensorMap& tmB, const OutMaps& tmOut, const OutMaps& tmRes, TcParams& p,
-                const PairPlan& plan, int CoutP, cudaStream_t st);
 
 }  // namespace lt

@@ -224,8 +224,8 @@ __global__ void __launch_bounds__(256) gather_weights_kernel(const float* __rest
 
 // y = acc * scale + shift with scale = gamma / sqrt(var + eps), shift = beta - mean * scale (+ conv_bias * scale); double arithmetic,
 // rounded once.  Any of gamma / beta / bias may be null; mean == null means "no BatchNorm" (scale 1, shift = bias).
-// accum_gain = 1 + 0.28 * steps * 2^-24: compensates the expected shrinkage of a sum accumulated by `steps` truncating tcgen05.mma
-// additions (tools/accum_probe.py); 1 for the exact-fp32 kernels.
+// accum_gain = 1 + 0.28 * steps * 2^-24: compensates the expected shrinkage of a sum accumulated by `steps` truncating tensor-core
+// additions (rate measured on the kernels' first target, not re-measured for wgmma); 1 for the exact-fp32 kernels.
 __global__ void fold_bn_kernel(const float* gamma, const float* beta, const float* mean, const float* var, const float* bias, double eps,
                                int C, int CP, const unsigned* absmax_bits, double accum_gain, float* scale, float* shift) {
   const int c = blockIdx.x * blockDim.x + threadIdx.x;

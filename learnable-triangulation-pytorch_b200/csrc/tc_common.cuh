@@ -1,4 +1,4 @@
-// PTX wrappers shared by the tcgen05 kernels (conv_tc.cu, conv_tc_fold.cu): mbarrier, TMA, TMEM, UMMA.
+// PTX wrappers shared by the tensor-core kernels (conv_tc.cu, conv_tail.cu): mbarrier, TMA, wgmma.
 #pragma once
 #include "common.cuh"
 #include <cuda.h>
@@ -17,7 +17,6 @@ __device__ __forceinline__ bool elect_one() {
   asm volatile("{\n\t.reg .pred p;\n\telect.sync _|p, 0xffffffff;\n\tselp.u32 %0, 1, 0, p;\n\t}" : "=r"(pred));
   return pred != 0;
 }
-__device__ __forceinline__ int uniform_warp_idx() { return __shfl_sync(0xffffffffu, (int)(threadIdx.x >> 5), 0); }
 
 __device__ __forceinline__ void mbar_init(uint64_t* bar, uint32_t count) {
   asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(smem_u32(bar)), "r"(count));
@@ -62,82 +61,63 @@ __device__ __forceinline__ void tma_load_2d(void* dst, const CUtensorMap* map, u
       ::"r"(smem_u32(dst)), "l"(map), "r"(smem_u32(bar)), "r"(c0), "r"(c1)
       : "memory");
 }
-__device__ __forceinline__ void tma_store_5d(const CUtensorMap* map, const void* src, int c0, int c1, int c2, int c3, int c4) {
-  asm volatile("cp.async.bulk.tensor.5d.global.shared::cta.bulk_group [%0, {%2, %3, %4, %5, %6}], [%1];"
-               ::"l"(map), "r"(smem_u32(src)), "r"(c0), "r"(c1), "r"(c2), "r"(c3), "r"(c4)
-               : "memory");
-}
-__device__ __forceinline__ void bulk_commit() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
-template <int N>
-__device__ __forceinline__ void bulk_wait_read() { asm volatile("cp.async.bulk.wait_group.read %0;" ::"n"(N) : "memory"); }
-template <int N>
-__device__ __forceinline__ void bulk_wait() { asm volatile("cp.async.bulk.wait_group %0;" ::"n"(N) : "memory"); }
-constexpr int kEpiThreads = 256;   // 8 epilogue warps: two per TMEM lane quadrant, each taking 16 of a block's 32 channels
-__device__ __forceinline__ void epi_bar_sync() { asm volatile("bar.sync 1, 256;" ::: "memory"); }
-// byte offset of 16-byte chunk c16 of row `row` inside a [rows][128 B] tile with the 128-byte swizzle
-__device__ __forceinline__ uint32_t sw128_off(int row, int c16) { return (uint32_t)(row * 128 + ((c16 ^ (row & 7)) << 4)); }
 __device__ __forceinline__ uint4 lds128(uint32_t a) {
   uint4 v;
   asm volatile("ld.shared.v4.u32 {%0, %1, %2, %3}, [%4];" : "=r"(v.x), "=r"(v.y), "=r"(v.z), "=r"(v.w) : "r"(a));
   return v;
 }
-__device__ __forceinline__ void sts128(uint32_t a, uint4 v) {
-  asm volatile("st.shared.v4.u32 [%0], {%1, %2, %3, %4};" ::"r"(a), "r"(v.x), "r"(v.y), "r"(v.z), "r"(v.w) : "memory");
-}
 __device__ __forceinline__ void prefetch_tmap(const CUtensorMap* map) {
   asm volatile("prefetch.tensormap [%0];" ::"l"(map) : "memory");
 }
 
-__device__ __forceinline__ void tmem_alloc(uint32_t* slot, uint32_t ncols) {
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(slot)), "r"(ncols) : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
+// ---- wgmma (sm_90a warpgroup MMA): A and B from shared memory, fp32 accumulators in registers ----
+// m64nNk16, fp16 operands, both K-major.  The accumulator of a warpgroup is the 64 x N tile; thread t (warp w = t / 32 of the
+// warpgroup, lane l) holds d[4i + {0,1,2,3}] = rows 16w + l/4 (+0, +0, +8, +8), columns 8i + 2(l%4) (+0, +1, +0, +1).
+__device__ __forceinline__ void wg_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wg_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wg_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
+// the accumulator registers must not be touched by other instructions while an MMA that writes them is in flight
+template <int R>
+__device__ __forceinline__ void wg_fence_regs(float (&d)[R]) {
+#pragma unroll
+  for (int i = 0; i < R; ++i) asm volatile("" : "+f"(d[i])::"memory");
 }
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t ncols) {
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-
-__device__ __forceinline__ void umma_f16(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t accumulate) {
+template <int N>
+__device__ __forceinline__ void wgmma_f16(float (&d)[N / 2], uint64_t ad, uint64_t bd, uint32_t scale_d);
+template <>
+__device__ __forceinline__ void wgmma_f16<16>(float (&d)[8], uint64_t ad, uint64_t bd, uint32_t scale_d) {
   asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}"
-      ::"r"(tmem_d), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-      : "memory");
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %10, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n16k16.f32.f16.f16 {%0,%1,%2,%3,%4,%5,%6,%7}, %8, %9, p, 1, 1, 0, 0;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7])
+      : "l"(ad), "l"(bd), "r"(scale_d));
 }
-__device__ __forceinline__ void umma_commit(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar)) : "memory");
-}
-__device__ __forceinline__ void tmem_ld16(uint32_t taddr, uint32_t (&r)[16]) {
+template <>
+__device__ __forceinline__ void wgmma_f16<32>(float (&d)[16], uint64_t ad, uint64_t bd, uint32_t scale_d) {
   asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-        "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-      : "r"(taddr));
-  asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %18, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n32k16.f32.f16.f16 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, %16, %17, p, 1, 1, 0, 0;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
+      : "l"(ad), "l"(bd), "r"(scale_d));
 }
-
-__device__ __forceinline__ void tmem_ld16_nowait(uint32_t taddr, uint32_t (&r)[16]) {
+template <>
+__device__ __forceinline__ void wgmma_f16<64>(float (&d)[32], uint64_t ad, uint64_t bd, uint32_t scale_d) {
   asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-        "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-      : "r"(taddr));
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %34, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n64k16.f32.f16.f16 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31}, %32, %33, p, 1, 1, 0, 0;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+      : "l"(ad), "l"(bd), "r"(scale_d));
 }
-__device__ __forceinline__ void tmem_wait_ld() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
+template <>
+__device__ __forceinline__ void wgmma_f16<128>(float (&d)[64], uint64_t ad, uint64_t bd, uint32_t scale_d) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %66, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n128k16.f32.f16.f16 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31,%32,%33,%34,%35,%36,%37,%38,%39,%40,%41,%42,%43,%44,%45,%46,%47,%48,%49,%50,%51,%52,%53,%54,%55,%56,%57,%58,%59,%60,%61,%62,%63}, %64, %65, p, 1, 1, 0, 0;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+      : "l"(ad), "l"(bd), "r"(scale_d));
+}
 
-// 32 contiguous bytes (16 fp16 values of one voxel row) in one request
-__device__ __forceinline__ void stg256(void* p, const uint32_t (&v)[8]) {
-  asm volatile("st.global.v8.b32 [%0], {%1, %2, %3, %4, %5, %6, %7, %8};"
-               ::"l"(p), "r"(v[0]), "r"(v[1]), "r"(v[2]), "r"(v[3]), "r"(v[4]), "r"(v[5]), "r"(v[6]), "r"(v[7]) : "memory");
-}
-
-// 32 contiguous bytes through the read-only path (two 16-byte requests)
-__device__ __forceinline__ void ldg256(const void* p, uint32_t (&v)[8]) {
-  const uint4 a = __ldg(reinterpret_cast<const uint4*>(p)), b = __ldg(reinterpret_cast<const uint4*>(p) + 1);
-  v[0] = a.x; v[1] = a.y; v[2] = a.z; v[3] = a.w; v[4] = b.x; v[5] = b.y; v[6] = b.z; v[7] = b.w;
-}
 // two floats -> packed split-fp16 (hi pair, lo pair); element `a` lands in the low half-word (lower address)
 __device__ __forceinline__ void split_s32x2(float a, float b, uint32_t& hi2, uint32_t& lo2) {
   asm("cvt.rn.satfinite.f16x2.f32 %0, %1, %2;" : "=r"(hi2) : "f"(b), "f"(a));
@@ -146,89 +126,12 @@ __device__ __forceinline__ void split_s32x2(float a, float b, uint32_t& hi2, uin
   asm("cvt.rn.satfinite.f16x2.f32 %0, %1, %2;" : "=r"(lo2) : "f"(rb), "f"(ra));
 }
 
-// 16 channels (half `half` of a 32-channel block) of staged row `srow`: [rows][128 B] tile, 128B swizzle.
-// split-fp16: hi halves in chunks 0..3, lo halves in chunks 4..7 (8 channels per chunk); fp32: 4 channels per chunk.
-__device__ __forceinline__ void epi_load16(uint32_t base, int srow, int half, int out_format, float (&r)[16]) {
-  if (out_format == LT_FMT_F32) {
-#pragma unroll
-    for (int c = 0; c < 4; ++c) {
-      const uint4 q = lds128(base + sw128_off(srow, half * 4 + c));
-      r[c * 4] = __uint_as_float(q.x); r[c * 4 + 1] = __uint_as_float(q.y);
-      r[c * 4 + 2] = __uint_as_float(q.z); r[c * 4 + 3] = __uint_as_float(q.w);
-    }
-  } else {
-#pragma unroll
-    for (int c = 0; c < 2; ++c) {
-      const uint4 qh = lds128(base + sw128_off(srow, half * 2 + c)), ql = lds128(base + sw128_off(srow, 4 + half * 2 + c));
-      const __half2* hh = reinterpret_cast<const __half2*>(&qh);
-      const __half2* ll = reinterpret_cast<const __half2*>(&ql);
-#pragma unroll
-      for (int e = 0; e < 4; ++e) {
-        const float2 a = __half22float2(hh[e]), b = __half22float2(ll[e]);
-        r[c * 8 + e * 2] = fmaf(b.x, kLoInv, a.x);
-        r[c * 8 + e * 2 + 1] = fmaf(b.y, kLoInv, a.y);
-      }
-    }
-  }
-}
-__device__ __forceinline__ void epi_store16(uint32_t base, int srow, int half, int out_format, const float (&v)[16]) {
-  if (out_format == LT_FMT_F32) {
-#pragma unroll
-    for (int c = 0; c < 4; ++c)
-      sts128(base + sw128_off(srow, half * 4 + c), make_uint4(__float_as_uint(v[c * 4]), __float_as_uint(v[c * 4 + 1]),
-                                                               __float_as_uint(v[c * 4 + 2]), __float_as_uint(v[c * 4 + 3])));
-  } else {
-#pragma unroll
-    for (int c = 0; c < 2; ++c) {
-      uint4 qh, ql;
-      split_s32x2(v[c * 8], v[c * 8 + 1], qh.x, ql.x);
-      split_s32x2(v[c * 8 + 2], v[c * 8 + 3], qh.y, ql.y);
-      split_s32x2(v[c * 8 + 4], v[c * 8 + 5], qh.z, ql.z);
-      split_s32x2(v[c * 8 + 6], v[c * 8 + 7], qh.w, ql.w);
-      sts128(base + sw128_off(srow, half * 2 + c), qh);
-      sts128(base + sw128_off(srow, 4 + half * 2 + c), ql);
-    }
-  }
-}
-// scale/shift, residual, ReLU on 16 channels starting at channel index co
-__device__ __forceinline__ void epi_affine16(float (&v)[16], const float* __restrict__ scale, const float* __restrict__ shift, int co) {
-#pragma unroll
-  for (int j = 0; j < 16; j += 4) {
-    const float4 sc = __ldg(reinterpret_cast<const float4*>(scale + co + j));
-    const float4 sh = __ldg(reinterpret_cast<const float4*>(shift + co + j));
-    v[j] = fmaf(v[j], sc.x, sh.x); v[j + 1] = fmaf(v[j + 1], sc.y, sh.y);
-    v[j + 2] = fmaf(v[j + 2], sc.z, sh.z); v[j + 3] = fmaf(v[j + 3], sc.w, sh.w);
-  }
-}
-__device__ __forceinline__ void epi_activate16(float (&v)[16], const float (&r)[16], int residual, int relu) {
-  if (residual == LT_RES_BEFORE_RELU) {
-#pragma unroll
-    for (int j = 0; j < 16; ++j) v[j] += r[j];
-  }
-  if (relu) {
-#pragma unroll
-    for (int j = 0; j < 16; ++j) v[j] = fmaxf(v[j], 0.f);
-  }
-  if (residual == LT_RES_AFTER_RELU) {
-#pragma unroll
-    for (int j = 0; j < 16; ++j) v[j] += r[j];
-  }
-}
-
-// K-major, 128-byte-swizzled shared-memory matrix descriptor (rows of 128 bytes, 8-row atoms
-// 1024 bytes apart): start address >> 4 | LBO=1 | SBO=1024>>4 | version=1 | layout=SWIZZLE_128B
+// wgmma shared-memory matrix descriptor, K-major, 128-byte swizzle (rows of 128 bytes, 8-row atoms 1024 bytes apart):
+// start address >> 4 | LBO = 1 (unused for swizzled K-major) | SBO = 1024 >> 4 | layout SWIZZLE_128B (1 << 62).
+// A 16-wide K slice at byte offset 32 j of the row is the same descriptor plus 2 j.
 __device__ __forceinline__ uint64_t make_sw128_desc(uint32_t saddr) {
-  return (uint64_t)((saddr & 0x3FFFFu) >> 4) | (1ull << 16) | ((uint64_t)(1024 >> 4) << 32) | (1ull << 46) | (2ull << 61);
+  return (uint64_t)((saddr & 0x3FFFFu) >> 4) | (1ull << 16) | ((uint64_t)(1024 >> 4) << 32) | (1ull << 62);
 }
-// K-major, 64-byte-swizzled descriptor (rows of 64 bytes, 8-row atoms 512 bytes apart): layout = SWIZZLE_64B (4)
-__device__ __forceinline__ uint64_t make_sw64_desc(uint32_t saddr) {
-  return (uint64_t)((saddr & 0x3FFFFu) >> 4) | (1ull << 16) | ((uint64_t)(512 >> 4) << 32) | (1ull << 46) | (4ull << 61);
-}
-// kind::f16 instruction descriptor: D=f32 (bit 4), A=B=fp16 (format 0), both K-major, M=128, N=n
-__host__ __device__ inline uint32_t make_idesc_f16(int n) {
-  return (1u << 4) | ((uint32_t)(n >> 3) << 17) | ((uint32_t)(128 >> 4) << 24);
-}
-
 
 // ---- host helpers (conv_tc.cu) ----
 int make_map(CUtensorMap* map, const void* base, int rank, const uint64_t* dims, const uint64_t* strides_bytes,

@@ -478,12 +478,10 @@ __device__ __forceinline__ const float4* q_at(const float4* base, unsigned idx) 
   return reinterpret_cast<const float4*>(r);
 }
 
-// 256-bit read-only load (sm_100): two adjacent float4 of a channels-last pixel row in ONE request, so that four lanes cover a
-// voxel's 128-byte tap with one L1 wavefront (two 128-bit loads per lane would touch every line twice)
+// two adjacent float4 of a channels-last pixel row through the read-only path (sm_90 has no 256-bit load: two 128-bit requests)
 __device__ __forceinline__ void ldg256(const float4* p, float4& a, float4& b) {
-  asm volatile("ld.global.nc.v8.f32 {%0,%1,%2,%3,%4,%5,%6,%7}, [%8];"
-               : "=f"(a.x), "=f"(a.y), "=f"(a.z), "=f"(a.w), "=f"(b.x), "=f"(b.y), "=f"(b.z), "=f"(b.w)
-               : "l"(p));
+  a = __ldg(p);
+  b = __ldg(p + 1);
 }
 
 template <int MAXV, int FMT, bool EXACT, int MINB, int CPL>   // EXACT: V == MAXV (no per-view predicates); MINB: min CTAs / SM; CPL: channels per lane (4 or 8)
@@ -698,8 +696,8 @@ static int launch_unproject(const float* features, const float* proj, const floa
   const bool pow2q = (units & (units - 1)) == 0;
   const int v2_mode = opts().unproject_v2;
   if (v2_mode && C == 32 && agg == LT_AGG_SOFTMAX && partial == 0 && V <= 8 && (long)V * h * w * C < (1L << 30)) {
-    // variants (measured on B200 at config #2 shapes, see profiles/): 8 lanes x 4 channels per voxel at 4 CTAs/SM was the
-    // round-1 default (0.29-0.31 ms); 4 lanes x 8 channels halves the per-voxel ray / shuffle / address overhead
+    // variants: 8 lanes x 4 channels per voxel at 4 CTAs/SM (default); 4 lanes x 8 channels halves the per-voxel ray / shuffle /
+    // address overhead
     const int cpl = opts().unproject_cpl, lb = opts().unproject_lb;
     {
       // brick walk for cubic volumes (the coordinate volume of the reference is n x n x n, triangulation.py:306-311)

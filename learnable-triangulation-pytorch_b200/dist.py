@@ -76,14 +76,14 @@ def complete_partials(partial, plan, pg, collective="all_reduce", reduce_op="sum
     per = B // plan.group_size
     if collective == "reduce_scatter":
         if partial.numel() * partial.element_size() >= (1 << 31):
-            # see below: a single 2 GiB collective on this buffer gave wrong sums on B200 x4; the all-reduce is sliced, the
+            # see below: a single 2 GiB collective on this buffer gave wrong sums on a 4-GPU node; the all-reduce is sliced, the
             # reduce-scatter (one output block per rank) is not
             raise NotImplementedError("reduce_scatter of a packed buffer >= 2 GiB is not validated; use collective='all_reduce' or 'features'")
         if out is None:
             out = torch.empty((per,) + tuple(partial.shape[1:]), dtype=partial.dtype, device=partial.device)
         dist.reduce_scatter_tensor(out, partial.contiguous(), op=op, group=pg)
         return out
-    # Issued in slices of at most 512 MiB (whole samples).  Measured on B200 x4 / x8 (profiles/r02_bench_tc_n4*.json): with the
+    # Issued in slices of at most 512 MiB (whole samples).  Measured on the kernels' first 4- and 8-GPU target: with the
     # 2 GiB buffer of a 32-sample group as ONE call the key points came out wrong by a run-dependent 2-84 mm, while the 1 GiB buffer
     # of a 16-sample group (N = 2) and every smaller case agree with the single-GPU forward to 0.02-0.07 mm.
     per_sample = partial[0].numel() * partial.element_size()
@@ -104,7 +104,7 @@ class PeerExchange:
         import torch.distributed._symmetric_memory as symm_mem
         if plan.n_groups > 1:
             # measured on 8 GPUs (2 groups x 4): the symmetric-memory exchanges give wrong key points as soon as two view groups
-            # rendezvous side by side, while one group of 2 / 4 / 8 ranks is exact (tools/dist_probe.py, profiles/r02_dist_probe_*.log)
+            # rendezvous side by side, while one group of 2 / 4 / 8 ranks is exact
             raise NotImplementedError("the peer-memory exchange is validated for ONE view group spanning all ranks; "
                                       "use collective='all_reduce' / 'reduce_scatter' / 'features' with several groups")
         self.plan, self.pg = plan, pg
@@ -130,8 +130,7 @@ class FeatureExchange:
         self.shape = (self.per, n_views, h, w, channels)
         self.n_views = n_views
         # One view group spanning all ranks: symmetric memory + our own store kernel.  Several groups side by side (world 8, 4 views):
-        # the symmetric-memory path returned wrong key points on the B200 box (2 groups x 4 ranks; one group of 2 / 4 ranks is exact,
-        # tools/dist_probe.py), so the groups then exchange the same maps with one NCCL all-gather each and assemble locally.
+        # the symmetric-memory path returned wrong key points on an 8-GPU node (2 groups x 4 ranks; one group of 2 / 4 ranks is exact), so the groups then exchange the same maps with one NCCL all-gather each and assemble locally.
         self.nccl = plan.n_groups > 1
         if self.nccl:
             self.buf = torch.empty(self.shape, dtype=torch.float32, device=device)

@@ -8,8 +8,8 @@ C-ABI launches on the current CUDA stream -- optionally captured into one CUDA g
 
 Data layout in HBM: every activation is channels-last ([N][D][H][W][C]); 2-D maps use D = 1.
   mode "simt": float32 activations, exact-fp32 FFMA convs (parity mode / checker)
-  mode "tc"  : split-fp16 activations, tcgen05 convs with 3-term products (fp32-grade)
-  mode "tc1" : split-fp16 activations, tcgen05 convs with high parts only (bf16-grade, fast)
+  mode "tc"  : split-fp16 activations, wgmma convs with 3-term products (fp32-grade)
+  mode "tc1" : split-fp16 activations, wgmma convs with high parts only (bf16-grade, fast)
 Layers the tensor-core kernel does not cover (the 3-channel stem and the six stride-2 convs of
 the trunk) run on the FFMA kernel in every mode.
 """
@@ -151,7 +151,7 @@ class NativeEngine:
             packed = torch.empty(capi.conv_tc_weight_bytes(taps, cin_p, cout_p) // 2, dtype=torch.float16, device=dev)
             capi.conv_tc_pack_weights(wp, packed, taps, cin_p, cout_p)
             pk.w, pk.cin, pk.cout_p, pk.impl, pk.in_fmt = packed, cin_p, cout_p, self.tc_impl, FMT_S32
-            # wide layers: also pack for the CTA-pair kernel (cta_group::2, 256 x {128,256} tiles; csrc/conv_pair.cu)
+            # wide layers: also pack with the 128-channel padding of LT_CONV_TC_PAIR
             if self.mode == "tc" and ((self.use_pair and cout_p % 128 == 0) or force_pair):
                 wq = torch.empty(capi.conv_pair_weight_bytes(taps, cin_p, cout_p) // 2, dtype=torch.float16, device=dev)
                 capi.conv_pair_pack_weights(wp, wq, taps, cin_p, cout_p)
@@ -167,7 +167,7 @@ class NativeEngine:
             pk.w, pk.cin, pk.cout_p, pk.impl, pk.in_fmt = wp, cin_p, cout_p, CONV_SIMT, FMT_F32
         pk.scale = torch.empty(cout_p, dtype=torch.float32, device=dev)
         pk.shift = torch.empty(cout_p, dtype=torch.float32, device=dev)
-        # tcgen05 accumulation steps on the main fp32 accumulator (one hi*hi MMA per 16 input channels and tap; the kw-folded kernel keeps
+        # tensor-core accumulation steps on the main fp32 accumulator (one hi*hi MMA per 16 input channels and tap; the kw-folded kernel keeps
         # the kw taps in separate accumulator columns): lt_fold_bn_fwd compensates the expected truncation shrinkage (include/lt_b200.h)
         steps = 0
         if use_tc and self.accum_compensation:

@@ -1,4 +1,4 @@
-"""Host-side batch contract on either side of the forward path, B200-first (SURVEY.md 8(f) row 3).
+"""Host-side batch contract on either side of the forward path, GPU-first (SURVEY.md 8(f) row 3).
 
 Mirrors `/root/reference/mvn/datasets/utils.py`: `make_collate_fn` (:6-39), `worker_init_fn`
 (:42-43) and `prepare_batch` (:45-65) with the same names, arguments and return values, but:

@@ -9,7 +9,7 @@ optional {alg,vol}_confidences heads), so reference checkpoints load unchanged.
 
 These modules only *hold parameters* and provide an autograd-capable torch
 forward (backend="torch": training / CPU plumbing).  The product inference
-path walks this tree once (see engine.py) and runs hand-written sm_100a
+path walks this tree once (see engine.py) and runs hand-written sm_90a
 kernels instead.
 """
 import torch

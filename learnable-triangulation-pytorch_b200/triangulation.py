@@ -7,7 +7,7 @@ wrap in DDP and call it unchanged.
 
 backend="native" (default; eval/no-grad on a CUDA device): host geometry is vectorised numpy
 (float64, cast last, like the reference) and everything on the device runs in the hand-written
-sm_100a kernels through engine.NativeEngine.  backend="torch": autograd-capable torch ops
+sm_90a kernels through engine.NativeEngine.  backend="torch": autograd-capable torch ops
 (training, CPU plumbing).  Nothing switches backend silently.
 """
 import os

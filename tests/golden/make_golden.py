@@ -1,7 +1,7 @@
 """Generate the golden fixtures in this directory from the UNMODIFIED reference.
 
-Run in the authoring container only (needs /root/reference; the GPU box does not have it):
-    python tests/golden/make_golden.py
+Needs a checkout of the reference (karfly/learnable-triangulation-pytorch); the tests only read the stored fixtures:
+    LT_REFERENCE=<path to the reference checkout> python tests/golden/make_golden.py [fixture ...]
 It imports karfly/learnable-triangulation-pytorch read-only, feeds it seeded synthetic inputs and the
 seeded weight recipe of lt_b200.testing (loaded with strict=True -- which also proves state_dict
 compatibility), and stores small input/output vectors as .npz.  Nothing is copied from the reference.
@@ -15,7 +15,8 @@ import torch
 HERE = os.path.dirname(os.path.abspath(__file__))
 ROOT = os.path.dirname(os.path.dirname(HERE))
 sys.path.insert(0, ROOT)
-sys.path.insert(0, "/root/reference")
+REFERENCE = os.environ["LT_REFERENCE"]
+sys.path.insert(0, REFERENCE)
 
 import lt_b200  # noqa: E402
 from lt_b200 import testing  # noqa: E402
@@ -134,11 +135,73 @@ def gen_state_dict_keys():
         json.dump({k: list(v.shape) for k, v in ref.state_dict().items()}, f)
 
 
+PIN_SAMPLES = 4096
+
+
+def _sample(a, seed):
+    """Fixed, seeded sample of a large output: (flat indices, values)."""
+    a = np.asarray(a).ravel()
+    idx = np.sort(np.random.RandomState(seed).choice(a.size, min(PIN_SAMPLES, a.size), replace=False))
+    return idx, a[idx]
+
+
+def gen_reference_pins():
+    """Outputs of the reference functions on the seeded inputs of tests/test_oracle_vs_reference.py and
+    tests/test_pipeline_cpu.py (the tests regenerate the inputs from the same seeds)."""
+    sys.path.insert(0, os.path.dirname(HERE))
+    from test_oracle_vs_reference import UNPROJECT_SHAPES, unproject_inputs, v2v_and_backbone_inputs
+    from test_pipeline_cpu import collate_inputs, _items
+    from mvn.models import v2v as ref_v2v, pose_resnet as ref_pr
+    from mvn.datasets import utils as ref_utils
+    from mvn.utils import img as ref_img
+    out = {}
+    for i, shape in enumerate(UNPROJECT_SHAPES):
+        heat, proj, coord, conf = unproject_inputs(shape)
+        for agg in ("sum", "max", "softmax", "conf"):
+            out["unproject_%d_%s" % (i, agg)] = ref_op.unproject_heatmaps(
+                torch.from_numpy(heat), torch.from_numpy(proj), torch.from_numpy(coord), agg, torch.from_numpy(conf)).numpy()
+    # coordinate volume of the reference forward and the projection of a resized camera
+    base = np.array([123.4, -56.7, 910.1])
+    net = RefNet(testing.make_config(num_layers=18, volume_size=32), device="cpu").eval()
+    images, batch = testing.make_batch(1, 2, image_size=64, seed=5, camera_cls=ref_multiview.Camera)
+    batch["keypoints_3d"][0][6, :3] = base
+    with torch.no_grad():
+        coords = net(images, None, batch)[5].numpy()[0]
+    out["coord_idx"], out["coord_val"] = _sample(coords, 1)
+    cam = batch["cameras"][1][0]
+    c2 = ref_multiview.Camera(cam.R, cam.t, cam.K)
+    c2.update_after_resize((64, 64), (16, 16))
+    out["projection"] = c2.projection.astype(np.float32)
+    # V2V and ResNet-34 backbone on seeded weights (the package's modules draw the same initial weights from the same seed)
+    v, x, bb, xi = v2v_and_backbone_inputs(ref_v2v.V2VModel, ref_pr.get_pose_net)
+    with torch.no_grad():
+        vo = v(x)
+        hm, feats, _, _ = bb(xi)
+    out["v2v_idx"], out["v2v_val"] = _sample(vo.numpy(), 2)
+    out["feats_idx"], out["feats_val"] = _sample(feats.numpy(), 3)
+    out["heat_idx"], out["heat_val"] = _sample(hm.numpy(), 4)
+    # collate + prepare_batch + uint8 normalisation
+    for randomize in (False, True):
+        items, kw = collate_inputs(randomize, camera_cls=ref_multiview.Camera)
+        np.random.seed(11)
+        want = ref_utils.make_collate_fn(**kw)(list(items))
+        tag = "collate_%d_" % randomize
+        out[tag + "images"], out[tag + "detections"] = want["images"], want["detections"]
+        out[tag + "pred_keypoints_3d"] = want["pred_keypoints_3d"]
+        cams = items[0]["cameras"]
+        out[tag + "camera_index"] = np.array([[[c is k for k in cams].index(True) for c in row] for row in want["cameras"]])
+        for j, t in enumerate(ref_utils.prepare_batch(want, "cpu", None)):
+            out[tag + "prepared_%d" % j] = t.numpy()
+    u8 = np.random.RandomState(1).randint(0, 256, size=(2, 2, 6, 7, 3)).astype(np.uint8)
+    ref_norm = np.stack([np.stack([ref_img.normalize_image(im) for im in row]) for row in u8])
+    out["normalized_u8"] = torch.stack([ref_img.image_batch_to_torch(x) for x in ref_norm]).numpy()
+    np.savez_compressed(os.path.join(HERE, "reference_pins.npz"), **out)
+
+
 if __name__ == "__main__":
-    gen_state_dict_keys()
-    gen_unproject()
-    gen_softargmax()
-    gen_forward()
-    gen_algebraic()
+    fixtures = {"state_dict_keys": gen_state_dict_keys, "unproject": gen_unproject, "softargmax": gen_softargmax,
+                "forward": gen_forward, "algebraic": gen_algebraic, "reference_pins": gen_reference_pins}
+    for name in sys.argv[1:] or list(fixtures):
+        fixtures[name]()
     for f in sorted(os.listdir(HERE)):
         print(f, os.path.getsize(os.path.join(HERE, f)))

@@ -19,7 +19,7 @@ class Recorder:
             return f
         monkeypatch.setattr(capi, "conv_fold_weight_bytes", lambda k, co: k * k * k * ((co + 15) // 16 * 16) * 64 * 2)
         monkeypatch.setattr(capi, "conv_pair_weight_bytes", lambda t, ci, co: t * (ci // 32) * ((co + 127) // 128 * 128) * 128)
-        # same shape rule as csrc/conv_pair.cu pair_plan (without its wave-count heuristics): staged epilogue + Cout % 128 == 0
+        # stand-in for lt_conv_pair_eligible (Cout % 128 == 0, output wide enough): the dry run loads no library
         monkeypatch.setattr(capi, "conv_pair_eligible", lambda d: d.Cout % 128 == 0 and d.FC % 32 == 0 and d.Cout <= d.FC and
                             d.N * d.OD * d.OH * d.OW >= 128 * 40)
         for name in ("v2v_tail", "absmax", "conv_gather_weights", "fold_bn", "conv_pair_pack_weights", "conv_fold_pack_weights", "stem_s2d", "coord_volume", "unproject_aggregate", "softargmax3d", "maxpool", "nchw_to_nhwc", "f32_to_s32",

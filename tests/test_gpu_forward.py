@@ -90,7 +90,7 @@ def test_stages_match_oracle(r50_case, mode):
 
 
 def test_config2_sizes_tensor_core_vs_exact_fp32():
-    """ResNet-152, 4 views 384x384, 64^3 grid (BASELINE config #2 shapes, B=2): tcgen05 path vs exact-fp32 path."""
+    """ResNet-152, 4 views 384x384, 64^3 grid (BASELINE config #2 shapes, B=2): tensor-core path vs exact-fp32 path."""
     B, V, S, n = 2, 4, 384, 64
     cfg = testing.make_config(num_layers=152, volume_size=n)
     ref = lt_b200.VolumetricTriangulationNet(cfg, device="cpu", backend="torch")

@@ -1,4 +1,4 @@
-"""GPU parity tests of the tcgen05/TMA convolution path (through the C ABI): GEMM core self-test, conv vs the
+"""GPU parity tests of the wgmma/TMA convolution path (through the C ABI): GEMM core self-test, conv vs the
 fp32 torch reference of the same op, transposed-conv phases, and tensor-core vs FFMA kernels at larger sizes."""
 import numpy as np
 import pytest
@@ -196,8 +196,7 @@ FOLD_CASES = [
 @pytest.mark.parametrize("with_res", [False, True])
 @pytest.mark.parametrize("variant", ["pair", "one_cta", "staged", "windowed", "default"])
 def test_conv_fold_vs_torch(case, with_res, variant):
-    # pair: cta_group::2 CTA pairs, register -> global epilogue (default); one_cta: the single-CTA kernel; staged: pairs with the
-    # shared-memory staging tile + TMA store / residual load; windowed: one CTA with 16/32-row x windows instead of full lines
+    # the variants set the kw-fold options of lt_options, which the sm_90a kernel accepts and ignores: every variant must agree
     if variant != "default":
         capi.set_options(fold_pair=2 * int(variant in ("pair", "staged")), fold_fullw=int(variant != "windowed"), fold_direct=int(variant != "staged"))
     try:
@@ -258,8 +257,7 @@ PAIR_CASES = [
 @pytest.mark.parametrize("acc", ["single", "two"])
 @pytest.mark.parametrize("case", PAIR_CASES)
 def test_conv_pair_vs_torch(case, acc):
-    """CTA-pair kernel (cta_group::2, M = 256 per pair) against the fp32 torch op, with one fp32 accumulator for the three products
-    and with the cross products in a second accumulator (one or two TMEM stages depending on the N tile)."""
+    """LT_CONV_TC_PAIR (weights padded to 128 channels) against the fp32 torch op, under both settings of lt_options.pair_two_acc."""
     capi.set_options(pair_two_acc=int(acc == "two"))
     try:
         _pair_case(case)

@@ -1,13 +1,13 @@
 """Host batch contract (lt_b200.pipeline): collate, normalisation table, prepare_batch (torch backend on CPU).
-Reference behaviours mirrored: mvn/datasets/utils.py:6-65, mvn/utils/img.py:96-110.  Where /root/reference is mounted
-(the authoring container) the same inputs also run through the reference functions."""
-import sys
+Reference behaviours mirrored: mvn/datasets/utils.py:6-65, mvn/utils/img.py:96-110.  The reference functions' outputs on the
+seeded inputs of test_collate_and_prepare_batch_equal_reference are stored in tests/golden/reference_pins.npz."""
+import os
 
 import numpy as np
 import pytest
 import torch
 
-from conftest import REFERENCE, has_reference
+from conftest import GOLDEN
 from lt_b200 import pipeline, testing
 
 
@@ -90,29 +90,27 @@ def test_native_backend_refuses_cpu_device():
         pipeline.prepare_batch(batch, "cpu", None)          # default backend is the CUDA path: no silent CPU route
 
 
-@pytest.mark.skipif(not has_reference(), reason="reference checkout not mounted")
+def collate_inputs(randomize, camera_cls=None):
+    return _items(3, 5, seed=9, camera_cls=camera_cls), dict(randomize_n_views=randomize, min_n_views=2, max_n_views=4)
+
+
 @pytest.mark.parametrize("randomize", [False, True])
 def test_collate_and_prepare_batch_equal_reference(randomize):
-    sys.path.insert(0, REFERENCE)
-    from mvn.datasets import utils as ref_utils
-    from mvn.utils import img as ref_img
-    from mvn.utils.multiview import Camera as RefCamera
-    items = _items(3, 5, seed=9, camera_cls=RefCamera)
-    kw = dict(randomize_n_views=randomize, min_n_views=2, max_n_views=4)
-    np.random.seed(11)
-    want = ref_utils.make_collate_fn(**kw)(list(items))
+    pins = np.load(os.path.join(GOLDEN, "reference_pins.npz"))
+    tag = "collate_%d_" % randomize
+    items, kw = collate_inputs(randomize)
     np.random.seed(11)
     got = pipeline.make_collate_fn(**kw)(list(items))
-    assert np.array_equal(got["images"], want["images"]) and np.array_equal(got["detections"], want["detections"])
-    assert np.array_equal(got["pred_keypoints_3d"], want["pred_keypoints_3d"])
-    assert [[id(c) for c in row] for row in got["cameras"]] == [[id(c) for c in row] for row in want["cameras"]]
-    r = ref_utils.prepare_batch(want, "cpu", None)
+    assert np.array_equal(got["images"], pins[tag + "images"]) and np.array_equal(got["detections"], pins[tag + "detections"])
+    assert np.array_equal(got["pred_keypoints_3d"], pins[tag + "pred_keypoints_3d"])
+    cams = items[0]["cameras"]
+    assert np.array_equal([[[c is k for k in cams].index(True) for c in row] for row in got["cameras"]], pins[tag + "camera_index"])
     m = pipeline.prepare_batch(got, "cpu", None, backend="torch")
-    for a, b in zip(m, r):
+    assert len(m) == sum(1 for k in pins.files if k.startswith(tag + "prepared_"))
+    for j, a in enumerate(m):
+        b = torch.from_numpy(pins[tag + "prepared_%d" % j])
         assert a.dtype == b.dtype and torch.equal(a, b)
     # uint8 crops normalised through the table == normalize_image on the CPU, then the reference upload path
     u8 = np.random.RandomState(1).randint(0, 256, size=(2, 2, 6, 7, 3)).astype(np.uint8)
-    ref_norm = np.stack([np.stack([ref_img.normalize_image(im) for im in row]) for row in u8])
-    want_t = torch.stack([ref_img.image_batch_to_torch(x) for x in ref_norm])
     got_t = pipeline.images_to_device(u8, "cpu", normalize_u8=True, backend="torch")
-    assert torch.equal(got_t, want_t)
+    assert torch.equal(got_t, torch.from_numpy(pins["normalized_u8"]))
