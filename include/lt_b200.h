@@ -46,8 +46,9 @@ enum lt_conv_impl {
   LT_CONV_SIMT = 0, /* fp32 FFMA implicit GEMM (exact, any shape) */
   LT_CONV_TC = 1,   /* wgmma, split-fp16 3-term products (fp32-grade) */
   LT_CONV_TC1 = 2,  /* wgmma, high parts only (plain fp16 precision, fast mode) */
-  LT_CONV_TC_FOLD = 3, /* wgmma over all 32 output channels (Cin = 32 cubic 3^3 / 7^3 stride-1 layers; weights from
-                         lt_conv_fold_pack_weights; desc->Cout = real channel count <= 32, FC = 32) */
+  LT_CONV_TC_FOLD = 3, /* wgmma, 3-term products, one input halo box per pipeline stage serving all kh (and kd) taps of a kw
+                         (Cin = 32 cubic 3^3 / 7^3 stride-1 "same" layers; weights from lt_conv_fold_pack_weights; desc->Cout = real
+                         channel count <= 32, N tile round_up(Cout, 16), FC = 32 with channels Cout .. 31 written as zeros) */
   LT_CONV_TC_PAIR = 4  /* wgmma, 3-term products, weights padded to 128 output channels (layers with Cout % 128 == 0 that
                          lt_conv_pair_eligible accepts; weights from lt_conv_pair_pack_weights) */
 };
@@ -270,7 +271,8 @@ int lt_v2v_tail_stats_fwd(const void* x, const void* w1, const void* w2, const v
                           long nvox, int FC, const float* coord, int J, float multiplier, int softmax, void* workspace,
                           size_t workspace_bytes, int* n_partials, void* stream);
 
-/* kw-folded weight packing: float32 [K^3][32][Cout] (DEVICE) -> split-fp16 [kd][kh][kw*NC + co][64], NC = round_up(Cout, 16). */
+/* LT_CONV_TC_FOLD weight packing: float32 [K^3 taps (kd, kh, kw)][32][Cout] (DEVICE) -> split-fp16 [kw][kd][kh][NC][32 hi | 32 lo]
+ * (128-byte rows), NC = round_up(Cout, 16), rows Cout .. NC-1 zero; lt_conv_fold_weight_bytes = K^3 * NC * 128. */
 size_t lt_conv_fold_weight_bytes(int K, int Cout);
 int lt_conv_fold_pack_weights(const float* w_tap_ci_co, void* packed, int K, int Cout, void* stream);
 

@@ -31,9 +31,6 @@ namespace lt {
 // ------------------------------------------------------------------------------------------------
 constexpr int kTcThreads = 384;
 
-__device__ __forceinline__ void regs_release_producer() { asm volatile("setmaxnreg.dec.sync.aligned.u32 40;"); }
-__device__ __forceinline__ void regs_claim_consumer() { asm volatile("setmaxnreg.inc.sync.aligned.u32 232;"); }
-
 template <int NT>
 __global__ void __launch_bounds__(kTcThreads, 1) conv_tc_kernel(const __grid_constant__ CUtensorMap tmA,
                                                                 const __grid_constant__ CUtensorMap tmB, const TcParams p) {
@@ -162,48 +159,7 @@ __global__ void __launch_bounds__(kTcThreads, 1) conv_tc_kernel(const __grid_con
     const int ow = ow0 + dw, oh = oh0 + dh, od = od0 + dd, nb = nb0 + r_;
     if (!(ow < p.OW && oh < p.OH && od < p.OD && nb < p.N)) continue;
     const long opix = (((long)nb * p.FD + (od * p.osd + p.ood)) * p.FH + (oh * p.osh + p.ooh)) * p.FW + (ow * p.osw + p.oow);
-#pragma unroll
-    for (int i = 0; i < NT / 8; ++i) {
-      const int k = 4 * i + 2 * h;
-      const int co = n0 + 8 * i + c2;
-      int ch = co;
-      long pix = opix;
-      if (p.n_maps > 1) {   // grouped output: channel block of group mi goes to output phase (mi / (gh gw), (mi / gw) % gh, mi % gw)
-        const int mi = ch / p.oc;
-        ch -= mi * p.oc;
-        pix += ((long)(mi / (p.gh * p.gw)) * p.FH + (mi / p.gw) % p.gh) * p.FW + mi % p.gw;
-      }
-      if (ch >= p.FC) continue;
-      float v0 = (p.terms == 3) ? fmaf(d2[k], kLoInv, d1[k]) : d1[k];
-      float v1 = (p.terms == 3) ? fmaf(d2[k + 1], kLoInv, d1[k + 1]) : d1[k + 1];
-      const float2 sc = __ldg(reinterpret_cast<const float2*>(p.scale + co));
-      const float2 sh = __ldg(reinterpret_cast<const float2*>(p.shift + co));
-      v0 = fmaf(v0, sc.x, sh.x);
-      v1 = fmaf(v1, sc.y, sh.y);
-      float2 rr = make_float2(0.f, 0.f);
-      if (p.residual != LT_RES_NONE) {
-        if (p.out_format == LT_FMT_F32) {
-          rr = *reinterpret_cast<const float2*>(reinterpret_cast<const float*>(p.res) + pix * p.FC + ch);
-        } else {
-          const sh_t* rp = reinterpret_cast<const sh_t*>(p.res) + pix * 2 * p.FC + s32_off(ch);
-          const float2 a = __half22float2(*reinterpret_cast<const __half2*>(rp));
-          const float2 b = __half22float2(*reinterpret_cast<const __half2*>(rp + 32));
-          rr = make_float2(fmaf(b.x, kLoInv, a.x), fmaf(b.y, kLoInv, a.y));
-        }
-      }
-      if (p.residual == LT_RES_BEFORE_RELU) { v0 += rr.x; v1 += rr.y; }
-      if (p.relu) { v0 = fmaxf(v0, 0.f); v1 = fmaxf(v1, 0.f); }
-      if (p.residual == LT_RES_AFTER_RELU) { v0 += rr.x; v1 += rr.y; }
-      if (p.out_format == LT_FMT_F32) {
-        *reinterpret_cast<float2*>(reinterpret_cast<float*>(p.out) + pix * p.FC + ch) = make_float2(v0, v1);
-      } else {
-        uint32_t hi2, lo2;
-        split_s32x2(v0, v1, hi2, lo2);
-        sh_t* op = reinterpret_cast<sh_t*>(p.out) + pix * 2 * p.FC + s32_off(ch);
-        *reinterpret_cast<uint32_t*>(op) = hi2;
-        *reinterpret_cast<uint32_t*>(op + 32) = lo2;
-      }
-    }
+    conv_epilogue_row<NT>(p, d1, d2, h, opix, n0, c2);
   }
 }
 
@@ -405,7 +361,7 @@ static int launch_tc(const CUtensorMap& tmA, const CUtensorMap& tmB, TcParams& p
 }
 
 // fills the geometry / epilogue part of the launch parameters (M-tile box, taps, output mapping)
-static void fill_params(const lt_conv_desc* d, TcParams& p, int CB, int CoutP, int Nt, int terms, const float* scale, const float* shift,
+void fill_params(const lt_conv_desc* d, TcParams& p, int CB, int CoutP, int Nt, int terms, const float* scale, const float* shift,
                         const void* residual, void* out) {
   p.OW = d->OW; p.OH = d->OH; p.OD = d->OD; p.N = d->N;
   int box[4];
@@ -425,13 +381,13 @@ static void fill_params(const lt_conv_desc* d, TcParams& p, int CB, int CoutP, i
   p.gh = d->ogh > 1 ? d->ogh : 1; p.gw = d->ogw > 1 ? d->ogw : 1;
 }
 
-static int make_in_map(CUtensorMap* tmA, const lt_conv_desc* d, const TcParams& p, const void* in) {
+int make_in_map(CUtensorMap* tmA, const lt_conv_desc* d, int bw, int bh, int bd, int bn, const void* in) {
   const uint64_t rowb = (uint64_t)d->Cin * 2 * 2;  // 2*Cin fp16 per position
   const uint64_t dims[5] = {(uint64_t)d->Cin * 2, (uint64_t)d->IW, (uint64_t)d->IH, (uint64_t)d->ID, (uint64_t)d->N};
   const uint64_t str[4] = {rowb, rowb * d->IW, rowb * d->IW * d->IH, rowb * d->IW * d->IH * d->ID};
   // strided convs: TMA traversal strides; the box spans (b-1)*s+1 input positions and delivers b of them
   const uint32_t es[5] = {1, (uint32_t)d->sw, (uint32_t)d->sh, (uint32_t)d->sd, 1};
-  uint32_t bx[5] = {64, (uint32_t)p.bw, (uint32_t)p.bh, (uint32_t)p.bd, (uint32_t)p.bn};
+  uint32_t bx[5] = {64, (uint32_t)bw, (uint32_t)bh, (uint32_t)bd, (uint32_t)bn};
   for (int i = 1; i <= 3; ++i) bx[i] = (bx[i] - 1) * es[i] + 1;
   LT_REQUIRE(bx[1] <= 256 && bx[2] <= 256 && bx[3] <= 256, "conv_tc: strided box exceeds 256");
   return make_map(tmA, in, 5, dims, str, bx, es, 1);
@@ -459,7 +415,7 @@ static int conv_wg_fwd(const lt_conv_desc* d, const void* in, const void* weight
   if (p.n_maps > 1)
     LT_REQUIRE(groups_ok(d, CoutP), "conv_tc: grouped output needs split-fp16 output, Cout / groups == FC, a multiple of 32");
   CUtensorMap tmA, tmB;
-  int rc = make_in_map(&tmA, d, p, in);
+  int rc = make_in_map(&tmA, d, p.bw, p.bh, p.bd, p.bn, in);
   if (rc) return rc;
   {
     const uint64_t dims[2] = {64, (uint64_t)taps * CB * CoutP};
@@ -486,25 +442,6 @@ int conv_pair_fwd(const lt_conv_desc* d, const void* in, const void* weight, con
 int conv_tc_fwd_terms(const lt_conv_desc* d, const void* in, const void* weight, const float* scale, const float* shift,
                       const void* residual, void* out, int terms, void* stream) {
   return conv_wg_fwd(d, in, weight, (d->Cout + 15) & ~15, scale, shift, residual, out, terms, stream);
-}
-
-// kw-fold entry point (LT_CONV_TC_FOLD: Cin = 32 cubic stride-1 layers): the same kernel over weights packed by
-// lt_conv_fold_pack_weights as [tap][1][32 rows][32 hi | 32 lo], i.e. all 32 output channels (the padding ones are zero)
-int conv_fold_supported(const lt_conv_desc* d) {
-  const bool cubic = d->KD == d->KH && d->KH == d->KW && (d->KW == 3 || d->KW == 7);
-  const int pd = d->KW / 2;
-  return cubic && d->Cin == 32 && d->Cout <= 32 && d->sd == 1 && d->sh == 1 && d->sw == 1 && d->pd == pd && d->ph == pd &&
-         d->pw == pd && d->OD == d->ID && d->OH == d->IH && d->OW == d->IW && d->osd == 1 && d->osh == 1 && d->osw == 1 &&
-         d->ood == 0 && d->ooh == 0 && d->oow == 0 && d->FD == d->OD && d->FH == d->OH && d->FW == d->OW && d->FC == 32 &&
-         d->in_format == LT_FMT_S32 && d->IW >= 16;
-}
-
-int conv_fold_fwd(const lt_conv_desc* d, const void* in, const void* weight, const float* scale, const float* shift,
-                  const void* residual, void* out, void* stream) {
-  LT_REQUIRE(conv_fold_supported(d), "conv_fold: unsupported layer shape");
-  lt_conv_desc dg = *d;
-  dg.Cout = 32;
-  return conv_wg_fwd(&dg, in, weight, 32, scale, shift, residual, out, 3, stream);
 }
 
 // ---- weight packing: fp32 [taps][Cin][Cout] -> fp16 [taps][Cin/32][CoutP][32 hi | 32 lo] (128-byte rows) ----------
@@ -565,17 +502,6 @@ extern "C" int lt_conv_pair_pack_weights(const float* w, void* packed, int taps,
   LT_REQUIRE(w && packed, "conv_pair_pack_weights: null pointer");
   LT_REQUIRE(Cin % 32 == 0 && taps > 0 && Cout > 0, "conv_pair_pack_weights: bad sizes");
   return pack_weights(w, packed, taps, Cin, Cout, (Cout + 127) & ~127, stream);
-}
-
-extern "C" size_t lt_conv_fold_weight_bytes(int K, int Cout) {
-  (void)Cout;
-  return (size_t)K * K * K * 32 * 128;
-}
-
-// w_tap_ci_co: fp32 [K^3 taps (kd, kh, kw)][32][Cout]
-extern "C" int lt_conv_fold_pack_weights(const float* w_tap_ci_co, void* packed, int K, int Cout, void* stream) {
-  LT_REQUIRE(w_tap_ci_co && packed && (K == 3 || K == 7) && Cout > 0 && Cout <= 32, "conv_fold_pack_weights: bad arguments");
-  return pack_weights(w_tap_ci_co, packed, K * K * K, 32, Cout, 32, stream);
 }
 
 // D[M][N] (fp32) = A[M][K] * B[N][K]^T, plain fp16 row-major operands; exercises the exact TMA /

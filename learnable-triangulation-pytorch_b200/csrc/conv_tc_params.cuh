@@ -35,4 +35,62 @@ constexpr int kMaxOutMaps = 8;
 
 constexpr int kATileBytes = 128 * 128;  // 128 rows x 64 fp16
 
+// Fused epilogue of one row of a 64 x NT wgmma accumulator tile (conv_tc.cu, conv_fold.cu): this thread holds columns 8i + c2 (+1)
+// of row 16 w + l / 4 (h = 0) or the row 8 below it (h = 1), which belongs to output pixel `opix`; n0 is the tile's first output
+// channel.  Forms D1 + D2 / S (3-term products) and applies the folded scale / shift, the residual, ReLU and the store (float32 or
+// split-fp16; grouped outputs go to their phase of the output lattice).
+template <int NT>
+__device__ __forceinline__ void conv_epilogue_row(const TcParams& p, const float (&d1)[NT / 2], const float (&d2)[NT / 2], int h,
+                                                  long opix, int n0, int c2) {
+#pragma unroll
+  for (int i = 0; i < NT / 8; ++i) {
+    const int k = 4 * i + 2 * h;
+    const int co = n0 + 8 * i + c2;
+    int ch = co;
+    long pix = opix;
+    if (p.n_maps > 1) {   // grouped output: channel block of group mi goes to output phase (mi / (gh gw), (mi / gw) % gh, mi % gw)
+      const int mi = ch / p.oc;
+      ch -= mi * p.oc;
+      pix += ((long)(mi / (p.gh * p.gw)) * p.FH + (mi / p.gw) % p.gh) * p.FW + mi % p.gw;
+    }
+    if (ch >= p.FC) continue;
+    float v0 = (p.terms == 3) ? fmaf(d2[k], kLoInv, d1[k]) : d1[k];
+    float v1 = (p.terms == 3) ? fmaf(d2[k + 1], kLoInv, d1[k + 1]) : d1[k + 1];
+    const float2 sc = __ldg(reinterpret_cast<const float2*>(p.scale + co));
+    const float2 sh = __ldg(reinterpret_cast<const float2*>(p.shift + co));
+    v0 = fmaf(v0, sc.x, sh.x);
+    v1 = fmaf(v1, sc.y, sh.y);
+    float2 rr = make_float2(0.f, 0.f);
+    if (p.residual != LT_RES_NONE) {
+      if (p.out_format == LT_FMT_F32) {
+        rr = *reinterpret_cast<const float2*>(reinterpret_cast<const float*>(p.res) + pix * p.FC + ch);
+      } else {
+        const sh_t* rp = reinterpret_cast<const sh_t*>(p.res) + pix * 2 * p.FC + s32_off(ch);
+        const float2 a = __half22float2(*reinterpret_cast<const __half2*>(rp));
+        const float2 b = __half22float2(*reinterpret_cast<const __half2*>(rp + 32));
+        rr = make_float2(fmaf(b.x, kLoInv, a.x), fmaf(b.y, kLoInv, a.y));
+      }
+    }
+    if (p.residual == LT_RES_BEFORE_RELU) { v0 += rr.x; v1 += rr.y; }
+    if (p.relu) { v0 = fmaxf(v0, 0.f); v1 = fmaxf(v1, 0.f); }
+    if (p.residual == LT_RES_AFTER_RELU) { v0 += rr.x; v1 += rr.y; }
+    if (p.out_format == LT_FMT_F32) {
+      *reinterpret_cast<float2*>(reinterpret_cast<float*>(p.out) + pix * p.FC + ch) = make_float2(v0, v1);
+    } else {
+      uint32_t hi2, lo2;
+      split_s32x2(v0, v1, hi2, lo2);
+      sh_t* op = reinterpret_cast<sh_t*>(p.out) + pix * 2 * p.FC + s32_off(ch);
+      *reinterpret_cast<uint32_t*>(op) = hi2;
+      *reinterpret_cast<uint32_t*>(op + 32) = lo2;
+    }
+  }
+}
+
+// ---- host helpers (conv_tc.cu) ----
+// geometry / epilogue part of the launch parameters for `CB` 32-channel input blocks, CoutP padded output channels and N tile Nt
+void fill_params(const lt_conv_desc* d, TcParams& p, int CB, int CoutP, int Nt, int terms, const float* scale, const float* shift,
+                 const void* residual, void* out);
+// input tensor map: split-fp16 channels-last rows [64 fp16], box of bw x bh x bd x bn positions (before the traversal strides)
+int make_in_map(CUtensorMap* tmA, const lt_conv_desc* d, int bw, int bh, int bd, int bn, const void* in);
+
 }  // namespace lt

@@ -1,4 +1,4 @@
-// PTX wrappers shared by the tensor-core kernels (conv_tc.cu, conv_tail.cu): mbarrier, TMA, wgmma.
+// PTX wrappers shared by the tensor-core kernels (conv_tc.cu, conv_fold.cu, conv_tail.cu): mbarrier, TMA, wgmma.
 #pragma once
 #include "common.cuh"
 #include <cuda.h>
@@ -55,6 +55,12 @@ __device__ __forceinline__ void tma_load_5d(void* dst, const CUtensorMap* map, u
       ::"r"(smem_u32(dst)), "l"(map), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "r"(c2), "r"(c3), "r"(c4)
       : "memory");
 }
+__device__ __forceinline__ void tma_load_3d(void* dst, const CUtensorMap* map, uint64_t* bar, int c0, int c1, int c2) {
+  asm volatile(
+      "cp.async.bulk.tensor.3d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5}], [%2];"
+      ::"r"(smem_u32(dst)), "l"(map), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "r"(c2)
+      : "memory");
+}
 __device__ __forceinline__ void tma_load_2d(void* dst, const CUtensorMap* map, uint64_t* bar, int c0, int c1) {
   asm volatile(
       "cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], [%2];"
@@ -69,6 +75,10 @@ __device__ __forceinline__ uint4 lds128(uint32_t a) {
 __device__ __forceinline__ void prefetch_tmap(const CUtensorMap* map) {
   asm volatile("prefetch.tensormap [%0];" ::"l"(map) : "memory");
 }
+
+// register split of the 384-thread producer / 2-consumer-warpgroup kernels: 128 x 40 + 256 x 232 <= 64 K registers
+__device__ __forceinline__ void regs_release_producer() { asm volatile("setmaxnreg.dec.sync.aligned.u32 40;"); }
+__device__ __forceinline__ void regs_claim_consumer() { asm volatile("setmaxnreg.inc.sync.aligned.u32 232;"); }
 
 // ---- wgmma (sm_90a warpgroup MMA): A and B from shared memory, fp32 accumulators in registers ----
 // m64nNk16, fp16 operands, both K-major.  The accumulator of a warpgroup is the 64 x N tile; thread t (warp w = t / 32 of the

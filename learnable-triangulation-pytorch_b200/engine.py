@@ -87,7 +87,7 @@ class NativeEngine:
         self._epoch = 0
         self._graphs = {}
         self.launches = 0          # kernels launched by the last eager forward (our own kernels only)
-        self.use_fold = os.environ.get("LT_TC_FOLD", "1") == "1"          # kw-folded kernel for Cin=32 cubic layers
+        self.use_fold = os.environ.get("LT_TC_FOLD", "1") == "1"          # halo-reusing kernel for Cin=32 cubic layers (0: generic kernel)
         self.use_pair = os.environ.get("LT_TC_PAIR", "1") == "1"          # CTA-pair kernel for Cout % 128 == 0 layers
         self.use_tail = os.environ.get("LT_TC_TAIL", "1") == "1"          # fused back1 + back2 + output kernel
         self.weight_prescale = os.environ.get("LT_TC_WSCALE", "1") == "1"   # power-of-two filter pre-scale (common.cuh)
@@ -156,7 +156,7 @@ class NativeEngine:
                 wq = torch.empty(capi.conv_pair_weight_bytes(taps, cin_p, cout_p) // 2, dtype=torch.float16, device=dev)
                 capi.conv_pair_pack_weights(wp, wq, taps, cin_p, cout_p)
                 pk.w_pair = wq
-            # narrow cubic stride-1 layers (V2V at full resolution): also pack for the kw-folded persistent kernel
+            # narrow cubic stride-1 layers (V2V at full resolution): also pack for the halo-reusing persistent kernel (csrc/conv_fold.cu)
             if (self.use_fold and self.mode == "tc" and cin_p == 32 and cout <= 32 and k[0] == k[1] == k[2] and k[0] in (3, 7)
                     and tuple(pad) == (k[0] // 2,) * 3 and max(stride) == 1):
                 wf = torch.empty(capi.conv_fold_weight_bytes(k[0], cout) // 2, dtype=torch.float16, device=dev)
@@ -167,11 +167,11 @@ class NativeEngine:
             pk.w, pk.cin, pk.cout_p, pk.impl, pk.in_fmt = wp, cin_p, cout_p, CONV_SIMT, FMT_F32
         pk.scale = torch.empty(cout_p, dtype=torch.float32, device=dev)
         pk.shift = torch.empty(cout_p, dtype=torch.float32, device=dev)
-        # tensor-core accumulation steps on the main fp32 accumulator (one hi*hi MMA per 16 input channels and tap; the kw-folded kernel keeps
-        # the kw taps in separate accumulator columns): lt_fold_bn_fwd compensates the expected truncation shrinkage (include/lt_b200.h)
+        # tensor-core accumulation steps on the main fp32 accumulator (one hi*hi MMA per 16 input channels and tap, in conv_tc_kernel and in
+        # conv_fold_kernel alike): lt_fold_bn_fwd compensates the expected truncation shrinkage (include/lt_b200.h)
         steps = 0
         if use_tc and self.accum_compensation:
-            steps = (taps // k[2] if pk.w_fold is not None else taps) * (cin_p // 16)
+            steps = taps * (cin_p // 16)
         for g in range(G):     # the per-channel affine repeats for every column block
             sc, sh = pk.scale[g * cout:g * cout + blk_p], pk.shift[g * cout:g * cout + blk_p]
             if bn is not None:
