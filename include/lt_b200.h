@@ -170,7 +170,10 @@ int lt_unproject_aggregate_bwd(const float* features, const float* proj, const f
  *   volumes_out = relu(logits), keypoints = sum(relu * coord) / sum(relu)).
  * ---------------------------------------------------------------------------------------- */
 /* Backward of the soft-argmax in the op-level (NCDHW) layout: probs = the forward's volumes_out [B][J][nvox],
- * grad_keypoints [B][J][3], grad_volumes [B][J][nvox] or NULL, scratch >= B*J floats -> grad_logits [B][J][nvox]. */
+ * grad_keypoints [B][J][3], grad_volumes [B][J][nvox] or NULL -> grad_logits [B][J][nvox] (written).  softmax = the forward's
+ * mode: 0 and 1 are op.py:84-96; 2 is the ReLU branch of the 2-D op (op.py:11-47, run with the pixel grid (x, y, 0) as coord):
+ * d logit_i = multiplier * [probs_i > 0] * (grad_volumes_i + (<g_kp, x_i> - <g_kp, kp>) / sum probs).  Other modes are rejected.
+ * scratch: >= B*J floats in mode 1, >= 2*B*J floats in mode 2, unused in mode 0. */
 int lt_softargmax3d_bwd(const float* probs, const float* coord, const float* grad_keypoints, const float* grad_volumes,
                         float* grad_logits, float* scratch, int B, int J, long nvox, float multiplier, int softmax, void* stream);
 size_t lt_softargmax3d_workspace_bytes(int B, int J, long nvox);
@@ -297,6 +300,15 @@ int lt_view_normalize_fwd(float* conf, int B, int V, int C, float eps, void* str
  * NULL -> out [B][J][3]; float64 A^T A + Jacobi eigen-solve per (sample, joint). */
 int lt_triangulate_dlt_fwd(const float* proj, const float* keypoints_2d, const float* confidences, float* out, int B,
                            int V, int J, void* stream);
+/* Backward of lt_triangulate_dlt_fwd for the training loop: what autograd derives through the reference's per-(sample, joint)
+ * torch.svd (multiview.py:141-183).  grad_out [B][J][3] -> grad_keypoints_2d [B][V][J][2] and grad_confidences [B][V][J] (may
+ * be NULL; confidences NULL means all ones).  Both are WRITTEN, not accumulated into (unlike lt_unproject_aggregate_bwd).
+ * Projection matrices get no gradient (they come from numpy camera data in the reference too).  One thread per (sample, joint)
+ * redoes the forward's float64 eigen-solve (same code, same order of operations) and applies the first-order eigenvector
+ * perturbation.  Where the smallest eigenvalue of A^T A is tied with another (gap <= 1e-12 of the largest eigenvalue) the
+ * derivative does not exist; the tied term is dropped, so the gradient stays finite (torch's SVD backward is not finite there). */
+int lt_triangulate_dlt_bwd(const float* proj, const float* keypoints_2d, const float* confidences, const float* grad_out,
+                           float* grad_keypoints_2d, float* grad_confidences, int B, int V, int J, void* stream);
 
 /* ------------------------------------------------------------------------------------------
  * Layout / format helpers.
@@ -327,15 +339,17 @@ int lt_tc_gemm_selftest(const void* a_fp16, const void* b_fp16, float* d, int M,
                         int variant, void* stream);
 
 /* ------------------------------------------------------------------------------------------
- * Test hooks (NOT part of the product path): the per-item code of the two backward kernels executed on the CPU with HOST
+ * Test hooks (NOT part of the product path): the per-item code of the backward kernels executed on the CPU with HOST
  * pointers, so that the `-m "not gpu"` suite can check the gradient arithmetic against torch autograd without a GPU.
- * Same arguments as the device entry points minus scratch / stream.
+ * Same arguments as the device entry points minus scratch / stream (softmax: modes 0, 1 and 2 as in lt_softargmax3d_bwd).
  * ---------------------------------------------------------------------------------------- */
 int lt_test_unproject_aggregate_bwd_host(const float* features, const float* proj, const float* coord, const float* conf,
                                          const float* grad_out, float* grad_features, float* grad_conf, int B, int V, int C, int h, int w,
                                          long nvox, int agg);
 int lt_test_softargmax3d_bwd_host(const float* probs, const float* coord, const float* grad_keypoints, const float* grad_volumes,
                                   float* grad_logits, int B, int J, long nvox, float multiplier, int softmax);
+int lt_test_triangulate_dlt_bwd_host(const float* proj, const float* keypoints_2d, const float* confidences, const float* grad_out,
+                                     float* grad_keypoints_2d, float* grad_confidences, int B, int V, int J);
 
 #ifdef __cplusplus
 }

@@ -1,11 +1,15 @@
-"""Differentiable wrappers of the two native custom ops (`backend="hybrid"`): the forward is the same hand-written kernel
-the inference path uses, the backward is `csrc/backward.cu` (lt_unproject_aggregate_bwd, lt_softargmax3d_bwd).
+"""Differentiable wrappers of the native custom ops (`backend="hybrid"`): the forward is the same hand-written kernel the
+inference path uses, the backward is `csrc/backward.cu` (lt_unproject_aggregate_bwd, lt_softargmax3d_bwd) and
+`csrc/algebraic.cu` (lt_triangulate_dlt_bwd).
 
 This is the first stage of SURVEY section 8f row 1: with it the reference training loop (`train.py:159-243`,
-`total_loss.backward()` at :236) runs the unprojection + aggregation and the soft-argmax -- the ops the reference implements
-as Python loops over (sample, view) pairs with ~10 passes over a (V, C, N^3) staging tensor -- on the native kernels while
-the convolutions stay on torch/cuDNN autograd.  Gradients: feature maps, `conf` confidences, V2V logits; projection matrices
-and coordinate volumes carry none (they do not in the reference either: they come from numpy camera data).
+`total_loss.backward()` at :236) runs the custom ops on the native kernels while the convolutions stay on torch/cuDNN
+autograd.  Volumetric model: the unprojection + aggregation and the 3-D soft-argmax -- the ops the reference implements as
+Python loops over (sample, view) pairs with ~10 passes over a (V, C, N^3) staging tensor.  Algebraic model: the 2-D
+soft-argmax (op.py:11-47, both branches) and the confidence-weighted DLT, which the reference runs as one torch.svd per
+(sample, joint) (multiview.py:171-183).  Gradients: feature maps / heat-maps, `conf` and algebraic confidences, V2V logits,
+2-D key points; projection matrices and coordinate volumes carry none (they do not in the reference either: they come from
+numpy camera data).
 """
 import torch
 
@@ -77,6 +81,81 @@ class IntegrateTensor3dFn(torch.autograd.Function):
         scratch = torch.empty(B * J, dtype=torch.float32, device=dev)
         capi.softargmax3d_bwd(probs, coord, g_kp, g_vol, grad_logits, scratch, B, J, nvox, 1.0, ctx.softmax)
         return grad_logits, None, None
+
+
+def pixel_grid(B, h, w, device):
+    """(B, h*w, 3) float32 coordinates (x, y, 0) of the pixels of an h x w map: the 2-D soft-argmax runs on the 3-D kernels."""
+    ys, xs = torch.meshgrid(torch.arange(h, device=device, dtype=torch.float32), torch.arange(w, device=device, dtype=torch.float32),
+                            indexing="ij")
+    return torch.stack([xs, ys, torch.zeros_like(xs)], dim=-1).reshape(1, h * w, 3).expand(B, h * w, 3).contiguous()
+
+
+class IntegrateTensor2dFn(torch.autograd.Function):
+    """op.integrate_tensor_2d (reference op.py:11-47): (B, J, h, w) -> (coordinates (B, J, 2) [x, y in pixels], heat-maps)."""
+
+    @staticmethod
+    def forward(ctx, heatmaps, softmax):
+        B, J, h, w = heatmaps.shape
+        dev = heatmaps.device
+        logits = heatmaps.detach().float().contiguous()
+        grid = pixel_grid(B, h, w, dev)
+        out = torch.empty_like(logits)
+        kp = torch.empty((B, J, 3), dtype=torch.float32, device=dev)
+        ws = torch.empty(capi.softargmax3d_workspace_bytes(B, J, h * w) // 4 + 1, dtype=torch.float32, device=dev)
+        mode = 1 if softmax else 2          # 2: ReLU heat-maps, centre of mass divided by the mass (op.py:25-41)
+        capi.softargmax3d(logits, J * h * w, 1, h * w, grid, out, kp, ws, B, J, h * w, 1.0, mode)
+        ctx.save_for_backward(out, grid)
+        ctx.mode = mode
+        return kp[:, :, :2].contiguous(), out
+
+    @staticmethod
+    def backward(ctx, grad_kp, grad_heat):
+        probs, grid = ctx.saved_tensors
+        B, J, h, w = probs.shape
+        dev = probs.device
+        g_kp = torch.zeros((B, J, 3), dtype=torch.float32, device=dev)
+        if grad_kp is not None:
+            g_kp[:, :, :2] = grad_kp
+        g_heat = None if grad_heat is None else grad_heat.float().contiguous()
+        grad_logits = torch.empty_like(probs)
+        scratch = torch.empty(2 * B * J, dtype=torch.float32, device=dev)
+        capi.softargmax3d_bwd(probs, grid, g_kp, g_heat, grad_logits, scratch, B, J, h * w, 1.0, ctx.mode)
+        return grad_logits, None
+
+
+class TriangulateDltFn(torch.autograd.Function):
+    """multiview.triangulate_batch_of_points (reference multiview.py:141-183): (B, V, 3, 4), (B, V, J, 2), (B, V, J) or None
+    -> (B, J, 3).  Gradients reach the key points and the confidences, not the projection matrices."""
+
+    @staticmethod
+    def forward(ctx, proj_matricies, points, confidences):
+        B, V, J = points.shape[:3]
+        proj = proj_matricies.detach().float().contiguous()
+        kp = points.detach().float().contiguous()
+        conf = None if confidences is None else confidences.detach().float().contiguous()
+        out = torch.empty((B, J, 3), dtype=torch.float32, device=points.device)
+        capi.triangulate_dlt(proj, kp, conf, out)
+        ctx.save_for_backward(proj, kp, conf if conf is not None else torch.empty(0, device=points.device))
+        ctx.has_conf = conf is not None
+        return out
+
+    @staticmethod
+    def backward(ctx, grad_out):
+        proj, kp, conf = ctx.saved_tensors
+        conf = conf if ctx.has_conf else None
+        need_conf = ctx.has_conf and ctx.needs_input_grad[2]
+        grad_kp = torch.empty_like(kp)
+        grad_conf = torch.empty_like(conf) if need_conf else None
+        capi.triangulate_dlt_bwd(proj, kp, conf, grad_out.float().contiguous(), grad_kp, grad_conf)
+        return None, (grad_kp if ctx.needs_input_grad[1] else None), grad_conf
+
+
+def integrate_tensor_2d(heatmaps, softmax=True):
+    return IntegrateTensor2dFn.apply(heatmaps, softmax)
+
+
+def triangulate_batch_of_points(proj_matricies_batch, points_batch, confidences_batch=None):
+    return TriangulateDltFn.apply(proj_matricies_batch, points_batch, confidences_batch)
 
 
 def unproject_heatmaps(heatmaps, proj_matricies, coord_volumes, volume_aggregation_method="sum", vol_confidences=None):

@@ -87,6 +87,8 @@ SIGNATURES = {
     "lt_gap_mlp3_fwd": (c_int, [c_void_p] + [c_int] * 7 + [c_void_p] * 7 + [c_void_p]),
     "lt_view_normalize_fwd": (c_int, [c_void_p, c_int, c_int, c_int, c_float, c_void_p]),
     "lt_triangulate_dlt_fwd": (c_int, [c_void_p] * 4 + [c_int] * 3 + [c_void_p]),
+    "lt_triangulate_dlt_bwd": (c_int, [c_void_p] * 6 + [c_int] * 3 + [c_void_p]),
+    "lt_test_triangulate_dlt_bwd_host": (c_int, [c_void_p] * 6 + [c_int] * 3),
     "lt_nchw_to_nhwc_f32": (c_int, [c_void_p, c_void_p] + [c_int] * 5 + [c_void_p]),
     "lt_images_hwc_to_nchw_fwd": (c_int, [c_void_p, c_int, c_void_p, c_void_p] + [c_int] * 4 + [c_void_p]),
     "lt_stem_s2d_fwd": (c_int, [c_void_p, c_void_p] + [c_int] * 4 + [c_void_p]),
@@ -336,6 +338,34 @@ def view_normalize(conf, B, V, C, eps):
 def triangulate_dlt(proj, kp2d, conf, out):
     B, V, J = kp2d.shape[:3]
     _check(lib().lt_triangulate_dlt_fwd(_ptr(proj), _ptr(kp2d), _ptr(conf), _ptr(out), B, V, J, _stream()), "lt_triangulate_dlt_fwd")
+
+
+def triangulate_dlt_bwd(proj, kp2d, conf, grad_out, grad_kp2d, grad_conf):
+    """grad_kp2d (B, V, J, 2) and grad_conf (B, V, J) or None are written, not accumulated into."""
+    B, V, J = kp2d.shape[:3]
+    _check(lib().lt_triangulate_dlt_bwd(_ptr(proj), _ptr(kp2d), _ptr(conf), _ptr(grad_out), _ptr(grad_kp2d), _ptr(grad_conf), B, V, J,
+                                        _stream()), "lt_triangulate_dlt_bwd")
+
+
+def _host_ptr(t):
+    if t is None:
+        return None
+    assert not t.is_cuda and t.is_contiguous() and t.dtype == torch.float32, "test hooks need contiguous float32 CPU tensors"
+    return t.data_ptr()
+
+
+def triangulate_dlt_bwd_host(proj, kp2d, conf, grad_out, grad_kp2d, grad_conf):
+    """lt_test_triangulate_dlt_bwd_host: the backward kernel's per-item code run on CPU tensors (test hook, no GPU needed)."""
+    B, V, J = kp2d.shape[:3]
+    _check(lib().lt_test_triangulate_dlt_bwd_host(_host_ptr(proj), _host_ptr(kp2d), _host_ptr(conf), _host_ptr(grad_out),
+                                                  _host_ptr(grad_kp2d), _host_ptr(grad_conf), B, V, J), "lt_test_triangulate_dlt_bwd_host")
+
+
+def softargmax3d_bwd_host(probs, coord, grad_keypoints, grad_volumes, grad_logits, B, J, nvox, multiplier, mode):
+    """lt_test_softargmax3d_bwd_host: the soft-argmax backward's per-item code run on CPU tensors (test hook, no GPU needed)."""
+    _check(lib().lt_test_softargmax3d_bwd_host(_host_ptr(probs), _host_ptr(coord), _host_ptr(grad_keypoints), _host_ptr(grad_volumes),
+                                               _host_ptr(grad_logits), B, J, nvox, float(multiplier), int(mode)),
+           "lt_test_softargmax3d_bwd_host")
 
 
 def nchw_to_nhwc(inp, out, N, C, H, W, Cp):

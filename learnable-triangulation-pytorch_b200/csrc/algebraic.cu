@@ -1,8 +1,9 @@
 // Small kernels of the algebraic-triangulation path and the confidence heads (SURVEY section 8f rows 2 and 4):
 //   - global-average-pool + 3-layer MLP + sigmoid tail of GlobalAveragePoolingHead (pose_resnet.py:163-174)
 //   - normalisation of per-view confidences (triangulation.py:173-174, :268-269)
-//   - confidence-weighted DLT triangulation (multiview.py:141-183), one thread per (sample, joint)
+//   - confidence-weighted DLT triangulation (multiview.py:141-183) and its backward, one thread per (sample, joint)
 #include "common.cuh"
+#include <math.h>
 
 namespace lt {
 
@@ -64,12 +65,23 @@ __global__ void view_normalize_kernel(float* __restrict__ conf, int B, int V, in
 // vector of the smallest singular value of A (2V x 4) = eigenvector of A^T A for its smallest eigenvalue.  A^T A and a cyclic
 // Jacobi eigen-solve run in float64 (forming A^T A squares the condition number, fp32 would not do); the reference's
 // `-vh[:, 3]` sign cancels in the dehomogenisation.
-__global__ void __launch_bounds__(128) triangulate_dlt_kernel(const float* __restrict__ proj, const float* __restrict__ kp2d,
-                                                              const float* __restrict__ conf, float* __restrict__ out, int B, int V, int J) {
-  const int idx = blockIdx.x * blockDim.x + threadIdx.x;
-  if (idx >= B * J) return;
-  const int b = idx / J, j = idx % J;
-  double M[4][4];
+
+// the two DLT rows of view v, as the forward rounds them: formed in float32 like the reference (multiview.py:159-161), then
+// widened.  cf = 1 gives the unweighted rows x*P[2] - P[0], y*P[2] - P[1].
+__host__ __device__ __forceinline__ void dlt_rows(const float* P, float x, float y, float cf, double r0[4], double r1[4]) {
+#pragma unroll
+  for (int c = 0; c < 4; ++c) {
+    r0[c] = (double)((P[8 + c] * x - P[c]) * cf);
+    r1[c] = (double)((P[8 + c] * y - P[4 + c]) * cf);
+  }
+}
+
+// A^T A of item (b, j) accumulated in float64, then diagonalised by cyclic Jacobi rotations: on return M's diagonal holds the
+// eigenvalues, the columns of E the eigenvectors, and the result is the index of the smallest eigenvalue (the first one on a
+// tie).  Shared by the forward and the backward kernel (and the host test hook): one sequence of operations.
+__host__ __device__ __forceinline__ int dlt_eigen(const float* __restrict__ proj, const float* __restrict__ kp2d,
+                                                  const float* __restrict__ conf, int b, int j, int V, int J, double M[4][4],
+                                                  double E[4][4]) {
 #pragma unroll
   for (int r = 0; r < 4; ++r)
 #pragma unroll
@@ -79,18 +91,16 @@ __global__ void __launch_bounds__(128) triangulate_dlt_kernel(const float* __res
     const float x = kp2d[(((long)b * V + v) * J + j) * 2], y = kp2d[(((long)b * V + v) * J + j) * 2 + 1];
     const float cf = conf ? conf[((long)b * V + v) * J + j] : 1.0f;
     double r0[4], r1[4];
-#pragma unroll
-    for (int c = 0; c < 4; ++c) {
-      // the reference forms these rows in float32 (multiview.py:159-161); keep that rounding, accumulate in float64
-      r0[c] = (double)((P[8 + c] * x - P[c]) * cf);
-      r1[c] = (double)((P[8 + c] * y - P[4 + c]) * cf);
-    }
+    dlt_rows(P, x, y, cf, r0, r1);
 #pragma unroll
     for (int r = 0; r < 4; ++r)
 #pragma unroll
       for (int c = 0; c < 4; ++c) M[r][c] += r0[r] * r0[c] + r1[r] * r1[c];
   }
-  double E[4][4] = {{1, 0, 0, 0}, {0, 1, 0, 0}, {0, 0, 1, 0}, {0, 0, 0, 1}};
+#pragma unroll
+  for (int r = 0; r < 4; ++r)
+#pragma unroll
+    for (int c = 0; c < 4; ++c) E[r][c] = r == c ? 1.0 : 0.0;
   for (int sweep = 0; sweep < 16; ++sweep) {
     double off = 0.0;
 #pragma unroll
@@ -115,13 +125,116 @@ __global__ void __launch_bounds__(128) triangulate_dlt_kernel(const float* __res
       }
     }
   }
+  // compile-time indices only (the select loops below too): M and E stay in registers
   int m = 0;
+  double lm = M[0][0];
 #pragma unroll
-  for (int k = 1; k < 4; ++k) if (M[k][k] < M[m][m]) m = k;
-  const double w = E[3][m];
-  out[(long)idx * 3 + 0] = (float)(E[0][m] / w);
-  out[(long)idx * 3 + 1] = (float)(E[1][m] / w);
-  out[(long)idx * 3 + 2] = (float)(E[2][m] / w);
+  for (int k = 1; k < 4; ++k)
+    if (M[k][k] < lm) { lm = M[k][k]; m = k; }
+  return m;
+}
+
+// u = column m of E
+__host__ __device__ __forceinline__ void dlt_column(const double E[4][4], int m, double u[4]) {
+#pragma unroll
+  for (int r = 0; r < 4; ++r) {
+    u[r] = E[r][0];
+#pragma unroll
+    for (int k = 1; k < 4; ++k)
+      if (k == m) u[r] = E[r][k];
+  }
+}
+
+__global__ void __launch_bounds__(128) triangulate_dlt_kernel(const float* __restrict__ proj, const float* __restrict__ kp2d,
+                                                              const float* __restrict__ conf, float* __restrict__ out, int B, int V, int J) {
+  const int idx = blockIdx.x * blockDim.x + threadIdx.x;
+  if (idx >= B * J) return;
+  const int b = idx / J, j = idx % J;
+  double M[4][4], E[4][4], u[4];
+  dlt_column(E, dlt_eigen(proj, kp2d, conf, b, j, V, J, M, E), u);
+  const double w = u[3];
+  out[(long)idx * 3 + 0] = (float)(u[0] / w);
+  out[(long)idx * 3 + 1] = (float)(u[1] / w);
+  out[(long)idx * 3 + 2] = (float)(u[2] / w);
+}
+
+// Eigenvalue gaps at or below this fraction of the largest eigenvalue count as ties (see dlt_bwd_item).
+constexpr double kDltTieTol = 1e-12;
+
+// Backward of the weighted DLT for item (b, j).  With (lambda_k, e_k) the eigenpairs of M = A^T A, u = e_0 the smallest:
+//   X = u[0:3] / u[3]  ->  g_u = [g_X / u[3], -(g_X . u[0:3]) / u[3]^2]
+//   w = sum_{k != 0} (g_u . e_k) / (lambda_0 - lambda_k) e_k          (first-order perturbation of the eigenvector)
+//   G_A = A (w u^T + u w^T): row r of A gets (a_r . w) u + (a_r . u) w
+//   d x = c (G_A[r0] . P[2]),  d y = c (G_A[r1] . P[2]),  d c = G_A[r0] . (x P[2] - P[0]) + G_A[r1] . (y P[2] - P[1]).
+// Independent of the sign of u.  A term whose gap |lambda_0 - lambda_k| is at most kDltTieTol * max |lambda| is dropped: on an
+// exact tie the derivative does not exist (torch's SVD backward returns non-finite values there); dropping keeps it finite.
+// grad_kp / grad_conf are WRITTEN (every (v, j) of the item), grad_conf may be null.
+__host__ __device__ __forceinline__ void dlt_bwd_item(const float* __restrict__ proj, const float* __restrict__ kp2d,
+                                                      const float* __restrict__ conf, const float* __restrict__ grad_out,
+                                                      float* __restrict__ grad_kp, float* __restrict__ grad_conf, int b, int j,
+                                                      int V, int J) {
+  double M[4][4], E[4][4], u[4];
+  const int m = dlt_eigen(proj, kp2d, conf, b, j, V, J, M, E);
+  dlt_column(E, m, u);
+  double lam0 = M[0][0], lmax = fabs(M[0][0]);
+#pragma unroll
+  for (int k = 1; k < 4; ++k) {
+    if (k == m) lam0 = M[k][k];
+    lmax = fmax(lmax, fabs(M[k][k]));
+  }
+  const long bj = (long)b * J + j;
+  const double gx = grad_out[bj * 3], gy = grad_out[bj * 3 + 1], gz = grad_out[bj * 3 + 2];
+  const double iw = 1.0 / u[3];
+  const double gu[4] = {gx * iw, gy * iw, gz * iw, -(gx * u[0] + gy * u[1] + gz * u[2]) * iw * iw};
+  double w[4] = {0.0, 0.0, 0.0, 0.0};
+#pragma unroll
+  for (int k = 0; k < 4; ++k) {
+    const double gap = lam0 - M[k][k];
+    if (k == m || !(fabs(gap) > kDltTieTol * lmax)) continue;
+    const double s = (gu[0] * E[0][k] + gu[1] * E[1][k] + gu[2] * E[2][k] + gu[3] * E[3][k]) / gap;
+#pragma unroll
+    for (int r = 0; r < 4; ++r) w[r] += s * E[r][k];
+  }
+  for (int v = 0; v < V; ++v) {
+    const float* P = proj + ((long)b * V + v) * 12;
+    const long vj = ((long)b * V + v) * J + j;
+    const float x = kp2d[vj * 2], y = kp2d[vj * 2 + 1];
+    const float cf = conf ? conf[vj] : 1.0f;
+    double a0[4], a1[4];
+    dlt_rows(P, x, y, cf, a0, a1);
+    double aw0 = 0.0, au0 = 0.0, aw1 = 0.0, au1 = 0.0;
+#pragma unroll
+    for (int c = 0; c < 4; ++c) {
+      aw0 += a0[c] * w[c]; au0 += a0[c] * u[c];
+      aw1 += a1[c] * w[c]; au1 += a1[c] * u[c];
+    }
+    double g0[4], g1[4], dx = 0.0, dy = 0.0;
+#pragma unroll
+    for (int c = 0; c < 4; ++c) {
+      g0[c] = aw0 * u[c] + au0 * w[c];
+      g1[c] = aw1 * u[c] + au1 * w[c];
+      dx += g0[c] * (double)P[8 + c];
+      dy += g1[c] * (double)P[8 + c];
+    }
+    grad_kp[vj * 2] = (float)(cf * dx);
+    grad_kp[vj * 2 + 1] = (float)(cf * dy);
+    if (grad_conf) {
+      dlt_rows(P, x, y, 1.0f, a0, a1);
+      double dc = 0.0;
+#pragma unroll
+      for (int c = 0; c < 4; ++c) dc += g0[c] * a0[c] + g1[c] * a1[c];
+      grad_conf[vj] = (float)dc;
+    }
+  }
+}
+
+__global__ void __launch_bounds__(128) triangulate_dlt_bwd_kernel(const float* __restrict__ proj, const float* __restrict__ kp2d,
+                                                                  const float* __restrict__ conf, const float* __restrict__ grad_out,
+                                                                  float* __restrict__ grad_kp, float* __restrict__ grad_conf, int B,
+                                                                  int V, int J) {
+  const int idx = blockIdx.x * blockDim.x + threadIdx.x;
+  if (idx >= B * J) return;
+  dlt_bwd_item(proj, kp2d, conf, grad_out, grad_kp, grad_conf, idx / J, idx % J, V, J);
 }
 
 }  // namespace lt
@@ -153,5 +266,25 @@ extern "C" int lt_triangulate_dlt_fwd(const float* proj, const float* keypoints_
   LT_REQUIRE(proj && keypoints_2d && out && B > 0 && V > 0 && J > 0, "triangulate_dlt: bad arguments");
   triangulate_dlt_kernel<<<ceil_div((long)B * J, 128), 128, 0, (cudaStream_t)stream>>>(proj, keypoints_2d, confidences, out, B, V, J);
   LT_CHECK_LAUNCH("triangulate_dlt_kernel");
+  return LT_OK;
+}
+
+extern "C" int lt_triangulate_dlt_bwd(const float* proj, const float* keypoints_2d, const float* confidences, const float* grad_out,
+                                      float* grad_keypoints_2d, float* grad_confidences, int B, int V, int J, void* stream) {
+  LT_REQUIRE(proj && keypoints_2d && grad_out && grad_keypoints_2d && B > 0 && V > 0 && J > 0, "triangulate_dlt_bwd: bad arguments");
+  triangulate_dlt_bwd_kernel<<<ceil_div((long)B * J, 128), 128, 0, (cudaStream_t)stream>>>(proj, keypoints_2d, confidences, grad_out,
+                                                                                           grad_keypoints_2d, grad_confidences, B, V, J);
+  LT_CHECK_LAUNCH("triangulate_dlt_bwd_kernel");
+  return LT_OK;
+}
+
+// test hook: the backward's per-item code on the CPU (host pointers), for the `-m "not gpu"` gradient tests
+extern "C" int lt_test_triangulate_dlt_bwd_host(const float* proj, const float* keypoints_2d, const float* confidences,
+                                                const float* grad_out, float* grad_keypoints_2d, float* grad_confidences, int B, int V,
+                                                int J) {
+  LT_REQUIRE(proj && keypoints_2d && grad_out && grad_keypoints_2d && B > 0 && V > 0 && J > 0,
+             "test_triangulate_dlt_bwd_host: bad arguments");
+  for (int b = 0; b < B; ++b)
+    for (int j = 0; j < J; ++j) dlt_bwd_item(proj, keypoints_2d, confidences, grad_out, grad_keypoints_2d, grad_confidences, b, j, V, J);
   return LT_OK;
 }

@@ -1,4 +1,5 @@
-// Backward passes of the two custom ops of the volumetric path (SURVEY section 8f row 1, first stage): what
+// Backward passes of the two custom ops of the volumetric path (SURVEY section 8f row 1, first stage), the soft-argmax one
+// also serving the 2-D soft-argmax of the algebraic model: what
 // `total_loss.backward()` (train.py:236) needs from op.unproject_heatmaps (op.py:99-166) and
 // op.integrate_tensor_3d_with_coordinates (op.py:84-96) when they run on the native kernels inside the torch training
 // graph (`backend="hybrid"`: torch convolutions, native custom ops).  Gradients flow to the feature maps (and to the
@@ -12,6 +13,10 @@
 // and scatters it with 16-byte vector atomics (red.global.add.v4.f32) into the channels-last feature gradient.
 // Soft-argmax backward (HBM bound, NCDHW like the op-level API): with t_i = g_vol_i + <g_kp, x_i>,
 //     softmax: d logit_i = mult * p_i * (t_i - sum_k p_k t_k)      ReLU: d logit_i = mult * [mult * logit_i > 0] * t_i
+// and for mode 2, the ReLU branch of the 2-D op (op.integrate_tensor_2d, op.py:25-41: kp = sum p_i x_i / M, M = sum p_i), which
+// the algebraic model (triangulation.py:131-200) trains through with the pixel grid (x, y, 0) as coordinates:
+//     mass:    d logit_i = mult * [p_i > 0] * (g_vol_i + (<g_kp, x_i> - <g_kp, kp>) / M)
+// The DLT backward of the algebraic model is in algebraic.cu (it shares the forward's eigen-solve).
 #include "common.cuh"
 #include <math.h>
 
@@ -205,48 +210,84 @@ struct SoftBwdParams {
   const float* coord;      // [B][nvox][3]
   const float* g_kp;       // [B][J][3]
   const float* g_vol;      // [B][J][nvox] or null
-  float* dots;             // [B][J] scratch: sum_k p_k t_k
+  float* dots;             // scratch: mode 1 [B][J] sum_k p_k t_k; mode 2 [2][B][J] (S, M) below
   float* grad_logits;      // [B][J][nvox]
-  int B, J, softmax;
+  int B, J, softmax;       // mode: 0 ReLU, 1 softmax, 2 ReLU with mass-normalised coordinates
   long nvox;
   float mult;
 };
 
-__host__ __device__ __forceinline__ float soft_t(const SoftBwdParams& p, int b, int j, long i, float gx, float gy, float gz) {
+// <g_kp, x_i>
+__host__ __device__ __forceinline__ float soft_tk(const SoftBwdParams& p, int b, long i, float gx, float gy, float gz) {
   const float* c = p.coord + ((long)b * p.nvox + i) * 3;
-  float t = fmaf(gx, LT_LD(c), fmaf(gy, LT_LD(c + 1), gz * LT_LD(c + 2)));
-  if (p.g_vol) t += LT_LD(p.g_vol + ((long)b * p.J + j) * p.nvox + i);
+  return fmaf(gx, LT_LD(c), fmaf(gy, LT_LD(c + 1), gz * LT_LD(c + 2)));
+}
+__host__ __device__ __forceinline__ float soft_gvol(const SoftBwdParams& p, int b, int j, long i) {
+  return p.g_vol ? LT_LD(p.g_vol + ((long)b * p.J + j) * p.nvox + i) : 0.0f;
+}
+// t_i = g_vol_i + <g_kp, x_i>
+__host__ __device__ __forceinline__ float soft_t(const SoftBwdParams& p, int b, int j, long i, float gx, float gy, float gz) {
+  float t = soft_tk(p, b, i, gx, gy, gz);
+  if (p.g_vol) t += soft_gvol(p, b, j, i);
   return t;
 }
+// modes 0 and 1; ReLU: probs = relu(mult * logit) > 0 exactly where the gradient passes
 __host__ __device__ __forceinline__ float soft_grad(const SoftBwdParams& p, float pi, float t, float S) {
-  // ReLU: probs = relu(mult * logit) > 0 exactly where the gradient passes
   return p.softmax ? p.mult * pi * (t - S) : (pi > 0.0f ? p.mult * t : 0.0f);
 }
+// mode 2: kp = sum p_i x_i / M with M = sum p_i, S = <g_kp, kp>:  d logit_i = mult [p_i > 0] (g_vol_i + (<g_kp, x_i> - S) / M)
+__host__ __device__ __forceinline__ float soft_grad_mass(const SoftBwdParams& p, float pi, float tk, float gv, float S, float M) {
+  return pi > 0.0f ? p.mult * (gv + (tk - S) / M) : 0.0f;
+}
 
-// one CTA per (b, j): S = sum_i p_i t_i
+// one CTA per (b, j), one pass over the voxels.  Mode 1: dots[bj] = sum_i p_i t_i.  Mode 2: dots[bj] = S = sum_i p_i tk_i / M and
+// dots[B*J + bj] = M = sum_i p_i.
 __global__ void __launch_bounds__(512) softargmax_bwd_dot_kernel(const SoftBwdParams p) {
   const int bj = blockIdx.x, b = bj / p.J, j = bj % p.J;
+  const bool mass = p.softmax == 2;
   const float gx = p.g_kp[bj * 3], gy = p.g_kp[bj * 3 + 1], gz = p.g_kp[bj * 3 + 2];
   const float* pr = p.probs + (long)bj * p.nvox;
-  float acc = 0.f;
-  for (long i = threadIdx.x; i < p.nvox; i += blockDim.x) acc = fmaf(__ldg(pr + i), soft_t(p, b, j, i, gx, gy, gz), acc);
+  float acc = 0.f, m = 0.f;
+  if (mass) {
+    for (long i = threadIdx.x; i < p.nvox; i += blockDim.x) {
+      const float pi = __ldg(pr + i);
+      acc = fmaf(pi, soft_tk(p, b, i, gx, gy, gz), acc);
+      m += pi;
+    }
+  } else {
+    for (long i = threadIdx.x; i < p.nvox; i += blockDim.x) acc = fmaf(__ldg(pr + i), soft_t(p, b, j, i, gx, gy, gz), acc);
+  }
   acc = warp_sum(acc);
-  __shared__ float sh[16];
-  if ((threadIdx.x & 31) == 0) sh[threadIdx.x >> 5] = acc;
+  if (mass) m = warp_sum(m);
+  __shared__ float sh[2][16];
+  if ((threadIdx.x & 31) == 0) { sh[0][threadIdx.x >> 5] = acc; sh[1][threadIdx.x >> 5] = m; }
   __syncthreads();
   if (threadIdx.x < 32) {
-    float v = threadIdx.x < (blockDim.x >> 5) ? sh[threadIdx.x] : 0.f;
+    const bool lane_ok = threadIdx.x < (blockDim.x >> 5);
+    float v = lane_ok ? sh[0][threadIdx.x] : 0.f;
     v = warp_sum(v);
-    if (threadIdx.x == 0) p.dots[bj] = v;
+    if (mass) {
+      float mv = lane_ok ? sh[1][threadIdx.x] : 0.f;
+      mv = warp_sum(mv);
+      if (threadIdx.x == 0) { p.dots[bj] = v / mv; p.dots[p.B * p.J + bj] = mv; }
+    } else if (threadIdx.x == 0) {
+      p.dots[bj] = v;
+    }
   }
 }
 
 __global__ void __launch_bounds__(256) softargmax_bwd_apply_kernel(const SoftBwdParams p) {
   const int bj = blockIdx.y, b = bj / p.J, j = bj % p.J;
   const float gx = p.g_kp[bj * 3], gy = p.g_kp[bj * 3 + 1], gz = p.g_kp[bj * 3 + 2];
-  const float S = p.softmax ? p.dots[bj] : 0.f;
   const float* pr = p.probs + (long)bj * p.nvox;
   float* out = p.grad_logits + (long)bj * p.nvox;
+  if (p.softmax == 2) {
+    const float S = p.dots[bj], M = p.dots[p.B * p.J + bj];
+    for (long i = (long)blockIdx.x * blockDim.x + threadIdx.x; i < p.nvox; i += (long)gridDim.x * blockDim.x)
+      out[i] = soft_grad_mass(p, __ldg(pr + i), soft_tk(p, b, i, gx, gy, gz), soft_gvol(p, b, j, i), S, M);
+    return;
+  }
+  const float S = p.softmax ? p.dots[bj] : 0.f;
   for (long i = (long)blockIdx.x * blockDim.x + threadIdx.x; i < p.nvox; i += (long)gridDim.x * blockDim.x) {
     out[i] = soft_grad(p, __ldg(pr + i), soft_t(p, b, j, i, gx, gy, gz), S);
   }
@@ -281,6 +322,8 @@ extern "C" int lt_softargmax3d_bwd(const float* probs, const float* coord, const
                                    float* grad_logits, float* scratch, int B, int J, long nvox, float multiplier, int softmax, void* stream) {
   LT_REQUIRE(probs && coord && grad_keypoints && grad_logits && scratch, "softargmax3d_bwd: null pointer");
   LT_REQUIRE(B > 0 && J > 0 && nvox > 0 && (long)B * J <= 65535, "softargmax3d_bwd: bad sizes");
+  LT_REQUIRE(softmax >= 0 && softmax <= 2, "softargmax3d_bwd: mode must be 0 (ReLU), 1 (softmax) or 2 (ReLU, mass-normalised coordinates), got %d",
+             softmax);
   SoftBwdParams p{probs, coord, grad_keypoints, grad_volumes, scratch, grad_logits, B, J, softmax, nvox, multiplier};
   cudaStream_t st = (cudaStream_t)stream;
   if (softmax) {
@@ -311,11 +354,23 @@ extern "C" int lt_test_unproject_aggregate_bwd_host(const float* features, const
 extern "C" int lt_test_softargmax3d_bwd_host(const float* probs, const float* coord, const float* grad_keypoints, const float* grad_volumes,
                                              float* grad_logits, int B, int J, long nvox, float multiplier, int softmax) {
   LT_REQUIRE(probs && coord && grad_keypoints && grad_logits, "test_softargmax3d_bwd_host: null pointer");
+  LT_REQUIRE(softmax >= 0 && softmax <= 2, "test_softargmax3d_bwd_host: mode must be 0, 1 or 2, got %d", softmax);
   SoftBwdParams p{probs, coord, grad_keypoints, grad_volumes, nullptr, grad_logits, B, J, softmax, nvox, multiplier};
   for (int bj = 0; bj < B * J; ++bj) {
     const int b = bj / J, j = bj % J;
     const float gx = grad_keypoints[bj * 3], gy = grad_keypoints[bj * 3 + 1], gz = grad_keypoints[bj * 3 + 2];
     const float* pr = probs + (long)bj * nvox;
+    if (softmax == 2) {
+      double num = 0.0, M = 0.0;
+      for (long i = 0; i < nvox; ++i) {
+        num += (double)pr[i] * soft_tk(p, b, i, gx, gy, gz);
+        M += pr[i];
+      }
+      const float S = (float)(num / M);
+      for (long i = 0; i < nvox; ++i)
+        grad_logits[(long)bj * nvox + i] = soft_grad_mass(p, pr[i], soft_tk(p, b, i, gx, gy, gz), soft_gvol(p, b, j, i), S, (float)M);
+      continue;
+    }
     double S = 0.0;
     if (softmax)
       for (long i = 0; i < nvox; ++i) S += (double)pr[i] * soft_t(p, b, j, i, gx, gy, gz);

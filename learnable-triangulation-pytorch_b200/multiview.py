@@ -96,9 +96,13 @@ def project_3d_points_to_image_plane_without_distortion(proj_matrix, points_3d, 
 
 def triangulate_batch_of_points(proj_matricies_batch, points_batch, confidences_batch=None, backend=None):
     """Drop-in for reference multiview.py:171-183: (B, V, 3, 4), (B, V, J, 2), (B, V, J) -> (B, J, 3)."""
-    from . import capi, op as _op, torch_ops
-    if _op._resolve_backend(backend, proj_matricies_batch, points_batch, confidences_batch) == "torch":
+    from . import autograd_ops, capi, op as _op, torch_ops
+    which = _op._resolve_backend(backend, proj_matricies_batch, points_batch, confidences_batch)
+    if which == "torch":
         return torch_ops.triangulate_batch_of_points(proj_matricies_batch, points_batch, confidences_batch)
+    if which == "hybrid":
+        # native forward and backward kernels in the autograd graph (gradients to the points and the confidences)
+        return autograd_ops.triangulate_batch_of_points(proj_matricies_batch, points_batch, confidences_batch)
     B, V, J = points_batch.shape[:3]
     out = torch.empty((B, J, 3), dtype=torch.float32, device=points_batch.device)
     conf = None if confidences_batch is None else confidences_batch.float().contiguous()

@@ -78,12 +78,14 @@ def integrate_tensor_3d_with_coordinates(volumes, coord_volumes, softmax=True, b
 
 def integrate_tensor_2d(heatmaps, softmax=True, backend=None):
     """Drop-in for reference op.py:11-47: (B, J, h, w) -> coordinates (B, J, 2) [x, y in pixels], normalised heatmaps."""
-    if _resolve_backend(backend, heatmaps) in ("torch", "hybrid"):
+    which = _resolve_backend(backend, heatmaps)
+    if which == "torch":
         return torch_ops.integrate_tensor_2d(heatmaps, softmax)
+    if which == "hybrid":
+        return autograd_ops.integrate_tensor_2d(heatmaps, softmax)
     B, J, h, w = heatmaps.shape
     dev = heatmaps.device
-    ys, xs = torch.meshgrid(torch.arange(h, device=dev, dtype=torch.float32), torch.arange(w, device=dev, dtype=torch.float32), indexing="ij")
-    grid = torch.stack([xs, ys, torch.zeros_like(xs)], dim=-1).reshape(1, h * w, 3).expand(B, h * w, 3).contiguous()
+    grid = autograd_ops.pixel_grid(B, h, w, dev)
     logits = heatmaps.float().contiguous()
     out = torch.empty_like(logits)
     kp = torch.empty((B, J, 3), dtype=torch.float32, device=dev)

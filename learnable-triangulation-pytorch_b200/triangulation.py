@@ -198,7 +198,9 @@ class VolumetricTriangulationNet(_EngineOwner):
 class AlgebraicTriangulationNet(_EngineOwner):
     """Drop-in for reference mvn/models/triangulation.py:131-200 (BASELINE config #5): backbone heatmaps -> 2-D
     soft-argmax -> confidence-weighted DLT.  Same ctor keys (`config.model.use_confidences`, `heatmap_softmax`,
-    `heatmap_multiplier`, `backbone.*`), same config side effects, same 4-tuple."""
+    `heatmap_multiplier`, `backbone.*`), same config side effects, same 4-tuple.  backend="native": eval / no-grad on the
+    kernels (engine.algebraic_forward); "torch": autograd torch ops; "hybrid": torch backbone, native 2-D soft-argmax and DLT
+    with their backward kernels (trains, any mode)."""
 
     def __init__(self, config, device="cuda:0", backend=None, conv_mode=None):
         super().__init__()
@@ -223,6 +225,11 @@ class AlgebraicTriangulationNet(_EngineOwner):
     def forward(self, images, proj_matricies, batch):
         if self.backend == "torch":
             return self._forward_torch(images, proj_matricies)
+        if self.backend == "hybrid":
+            # torch/cuDNN backbone with the native 2-D soft-argmax and DLT (forward + backward kernels) in the autograd graph
+            if not images.is_cuda:
+                raise RuntimeError("lt_b200 hybrid backend needs CUDA tensors (native custom ops); use backend='torch' on CPU")
+            return self._forward_torch(images, proj_matricies, ops_backend="hybrid")
         if not images.is_cuda:
             raise RuntimeError("lt_b200 native backend needs CUDA tensors; construct the model with backend='torch' for CPU/autograd")
         if self.training or torch.is_grad_enabled():
@@ -231,12 +238,13 @@ class AlgebraicTriangulationNet(_EngineOwner):
             return self.engine().algebraic_forward(images.float().contiguous(), proj_matricies.float().contiguous(),
                                                    self.heatmap_multiplier, self.use_confidences, self.heatmap_softmax)
 
-    def _forward_torch(self, images, proj_matricies):
+    def _forward_torch(self, images, proj_matricies, ops_backend="torch"):
+        """The reference forward on torch autograd; ops_backend="hybrid" runs its 2-D soft-argmax and DLT on the native kernels."""
         B, V = images.shape[:2]
         heatmaps, _, alg_conf, _ = self.backbone(images.reshape(-1, *images.shape[2:]))
         if not self.use_confidences:
             alg_conf = torch.ones(B * V, heatmaps.shape[1], dtype=torch.float, device=images.device)
-        kp2d, heatmaps = op.integrate_tensor_2d(heatmaps * self.heatmap_multiplier, self.heatmap_softmax, backend="torch")
+        kp2d, heatmaps = op.integrate_tensor_2d(heatmaps * self.heatmap_multiplier, self.heatmap_softmax, backend=ops_backend)
         heatmaps = heatmaps.view(B, V, *heatmaps.shape[1:])
         kp2d = kp2d.view(B, V, *kp2d.shape[1:])
         alg_conf = alg_conf.view(B, V, -1)
@@ -244,5 +252,5 @@ class AlgebraicTriangulationNet(_EngineOwner):
         h, w = heatmaps.shape[3:]
         H, W = images.shape[3:]
         kp2d = kp2d * torch.tensor([W / w, H / h], device=images.device, dtype=kp2d.dtype)
-        kp3d = multiview.triangulate_batch_of_points(proj_matricies, kp2d, confidences_batch=alg_conf, backend="torch")
+        kp3d = multiview.triangulate_batch_of_points(proj_matricies, kp2d, confidences_batch=alg_conf, backend=ops_backend)
         return kp3d, kp2d, heatmaps, alg_conf
