@@ -49,8 +49,6 @@ enum lt_conv_impl {
   LT_CONV_TC_FOLD = 3, /* wgmma, 3-term products, one input halo box per pipeline stage serving all kh (and kd) taps of a kw
                          (Cin = 32 cubic 3^3 / 7^3 stride-1 "same" layers; weights from lt_conv_fold_pack_weights; desc->Cout = real
                          channel count <= 32, N tile round_up(Cout, 16), FC = 32 with channels Cout .. 31 written as zeros) */
-  LT_CONV_TC_PAIR = 4  /* wgmma, 3-term products, weights padded to 128 output channels (layers with Cout % 128 == 0 that
-                         lt_conv_pair_eligible accepts; weights from lt_conv_pair_pack_weights) */
 };
 
 /* residual placement in the conv epilogue */
@@ -212,7 +210,7 @@ typedef struct lt_conv_desc {
                                 Cout/G channels, block g = (a*ogh + b)*ogw + c being written (and its residual read) at the output
                                 offset (ood + a, ooh + b, oow + c) with channel index 0..Cout/G-1 (FC == Cout/G).  A k2 s2
                                 transposed conv (v2v.py:54-66) is ONE 1x1x1 GEMM this way: N = 8 x Cout, osd=osh=osw=2, ogd=ogh=ogw=2;
-                                scale/shift carry Cout entries (the per-channel values repeated G times).  LT_CONV_TC / _PAIR only */
+                                scale/shift carry Cout entries (the per-channel values repeated G times).  LT_CONV_TC / TC1 only */
   int reserved0;             /* set to 0 (keeps the pointer below 8-byte aligned without implicit padding) */
   void* workspace;           /* optional device scratch for split-K (layers with fewer M x N tiles than half the SMs:
                                 the K loop is spread over more CTAs and summed in a fixed order); NULL = never split */
@@ -249,18 +247,12 @@ int lt_conv_gather_weights_fwd(const float* w, long base, long s_td, long s_th, 
 int lt_fold_bn_fwd(const float* gamma, const float* beta, const float* mean, const float* var, const float* conv_bias, float eps,
                    int C, int CP, const unsigned int* absmax_bits, int accum_steps, float* scale, float* shift, void* stream);
 
-/* CTA-pair weight packing: float32 [taps][Cin][Cout] (DEVICE) -> fp16 [taps][Cin/32][CoutP][32 hi | 32 lo] (128-byte rows),
- * CoutP = round_up(Cout, 128).  lt_conv_pair_eligible: 1 if LT_CONV_TC_PAIR covers this launch (shape / tiling heuristics),
- * else 0 (use LT_CONV_TC). */
-size_t lt_conv_pair_weight_bytes(int taps, int Cin, int Cout);
-int lt_conv_pair_pack_weights(const float* w_tap_ci_co, void* packed, int taps, int Cin, int Cout, void* stream);
-int lt_conv_pair_eligible(const lt_conv_desc* desc);
-
 /* Fused tail of the V2V network (v2v.py:154-160,168-169): back_layers[1], back_layers[2] (1x1x1 conv 32->32 + BN + ReLU each) and
  * output_layer (1x1x1 conv 32->J + bias) as one kernel: x split-fp16 [rows][32 hi | 32 lo] -> logits float32 [rows][FC]
- * (J <= FC <= 32, FC % 4 == 0; channels J..FC-1 are written as bias3 = 0).  w1/w2/w3: lt_conv_pair_pack_weights(taps 1, Cin 32)
- * buffers; scale/shift: folded BatchNorm ([32] each); scale3 / bias3 [32]: output affine (lt_fold_bn_fwd without BatchNorm: the
- * inverse filter pre-scale and the bias, zero padded). */
+ * (J <= FC <= 32, FC % 4 == 0; channels J..FC-1 are written as bias3 = 0).  w1/w2/w3: lt_conv_tc_pack_weights(taps 1, Cin 32)
+ * buffers with Cout = 32, 32 and J; w3 must hold round_up(FC, 16) rows (it does for FC = round_up(J, 4)).  scale/shift: folded
+ * BatchNorm ([32] each); scale3 / bias3 [FC]: output affine (lt_fold_bn_fwd without BatchNorm: the inverse filter pre-scale and
+ * the bias, zero padded). */
 int lt_v2v_tail_fwd(const void* x, const void* w1, const void* w2, const void* w3, const float* scale1, const float* shift1,
                     const float* scale2, const float* shift2, const float* scale3, const float* bias3, float* logits, long rows, int FC,
                     void* stream);

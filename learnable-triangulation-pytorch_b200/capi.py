@@ -16,7 +16,7 @@ LIB_PATH = os.path.join(_HERE, "liblt_b200.so")
 
 FMT_F32, FMT_S32 = 0, 1
 AGG = {"sum": 0, "max": 1, "softmax": 2, "conf": 3, "conf_norm": 3}
-CONV_SIMT, CONV_TC, CONV_TC1, CONV_TC_FOLD, CONV_TC_PAIR = 0, 1, 2, 3, 4
+CONV_SIMT, CONV_TC, CONV_TC1, CONV_TC_FOLD = 0, 1, 2, 3
 RES_NONE, RES_BEFORE_RELU, RES_AFTER_RELU = 0, 1, 2
 
 c_int, c_long, c_float, c_void_p, c_size_t = ctypes.c_int, ctypes.c_long, ctypes.c_float, ctypes.c_void_p, ctypes.c_size_t
@@ -73,9 +73,6 @@ SIGNATURES = {
     "lt_absmax_fwd": (c_int, [c_void_p, c_long, c_void_p, c_void_p]),
     "lt_conv_gather_weights_fwd": (c_int, [c_void_p] + [c_long] * 6 + [c_int] * 7 + [c_void_p, c_void_p, c_int, c_int, c_void_p]),
     "lt_fold_bn_fwd": (c_int, [c_void_p] * 5 + [c_float, c_int, c_int, c_void_p, c_int, c_void_p, c_void_p, c_void_p]),
-    "lt_conv_pair_weight_bytes": (c_size_t, [c_int, c_int, c_int]),
-    "lt_conv_pair_pack_weights": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_void_p]),
-    "lt_conv_pair_eligible": (c_int, [ctypes.POINTER(ConvDesc)]),
     "lt_v2v_tail_fwd": (c_int, [c_void_p] * 11 + [c_long, c_int, c_void_p]),
     "lt_v2v_tail_stats_fwd": (c_int, [c_void_p] * 11 + [c_int, c_long, c_int, c_void_p, c_int, c_float, c_int, c_void_p, c_size_t,
                                       ctypes.POINTER(c_int), c_void_p]),
@@ -278,18 +275,6 @@ def conv_gather_weights(w, base, strides, k, cin, cin_p, cout, cout_p, out, absm
 def fold_bn(gamma, beta, mean, var, bias, eps, c, cp, scale, shift, absmax_bits=None, accum_steps=0):
     _check(lib().lt_fold_bn_fwd(_ptr(gamma), _ptr(beta), _ptr(mean), _ptr(var), _ptr(bias), float(eps), c, cp, _ptr(absmax_bits),
                                 int(accum_steps), _ptr(scale), _ptr(shift), _stream()), "lt_fold_bn_fwd")
-
-
-def conv_pair_weight_bytes(taps, cin, cout):
-    return lib().lt_conv_pair_weight_bytes(taps, cin, cout)
-
-
-def conv_pair_pack_weights(w_tap_ci_co, packed, taps, cin, cout):
-    _check(lib().lt_conv_pair_pack_weights(_ptr(w_tap_ci_co), _ptr(packed), taps, cin, cout, _stream()), "lt_conv_pair_pack_weights")
-
-
-def conv_pair_eligible(desc):
-    return bool(lib().lt_conv_pair_eligible(ctypes.byref(desc)))
 
 
 def v2v_tail(x, w1, w2, w3, scale1, shift1, scale2, shift2, scale3, bias3, logits, rows, fc):

@@ -55,15 +55,12 @@ int conv_simt_fwd(const lt_conv_desc* d, const void* in, const void* weight, con
 int conv_tc_fwd_terms(const lt_conv_desc* d, const void* in, const void* weight, const float* scale, const float* shift,
                       const void* residual, void* out, int terms, void* stream);
 
-int conv_pair_fwd(const lt_conv_desc* d, const void* in, const void* weight, const float* scale, const float* shift,
-                  const void* residual, void* out, void* stream, int probe_only);
-
 int conv_fold_fwd(const lt_conv_desc* d, const void* in, const void* weight, const float* scale, const float* shift,
                   const void* residual, void* out, void* stream);
 
 }  // namespace lt
 
-extern "C" int lt_version(void) { return 200; }
+extern "C" int lt_version(void) { return 201; }
 
 extern "C" void lt_default_options(lt_options* o) {
   if (o) *o = lt::make_default_options();
@@ -107,7 +104,7 @@ extern "C" int lt_conv_nd_fwd(const lt_conv_desc* d, const void* in, const void*
   LT_REQUIRE((d->OD - 1) * d->osd + d->ood + gd - 1 < d->FD && (d->OH - 1) * d->osh + d->ooh + gh - 1 < d->FH &&
                  (d->OW - 1) * d->osw + d->oow + gw - 1 < d->FW && d->ood >= 0 && d->ooh >= 0 && d->oow >= 0,
              "conv_nd: output mapping exceeds the output tensor");
-  LT_REQUIRE(gd * gh * gw == 1 || impl == LT_CONV_TC || impl == LT_CONV_TC1 || impl == LT_CONV_TC_PAIR,
+  LT_REQUIRE(gd * gh * gw == 1 || impl == LT_CONV_TC || impl == LT_CONV_TC1,
              "conv_nd: grouped output (ogd/ogh/ogw) is only implemented by the tensor-core kernels");
   LT_REQUIRE(d->residual == LT_RES_NONE || residual, "conv_nd: residual requested but pointer is null");
   LT_REQUIRE(d->residual >= LT_RES_NONE && d->residual <= LT_RES_AFTER_RELU, "conv_nd: bad residual mode");
@@ -115,11 +112,5 @@ extern "C" int lt_conv_nd_fwd(const lt_conv_desc* d, const void* in, const void*
   if (impl == LT_CONV_TC) return conv_tc_fwd_terms(d, in, weight, scale, shift, residual, out, 3, stream);
   if (impl == LT_CONV_TC_FOLD) return conv_fold_fwd(d, in, weight, scale, shift, residual, out, stream);
   if (impl == LT_CONV_TC1) return conv_tc_fwd_terms(d, in, weight, scale, shift, residual, out, 1, stream);
-  if (impl == LT_CONV_TC_PAIR) return conv_pair_fwd(d, in, weight, scale, shift, residual, out, stream, 0);
   return fail(LT_ERR_INVALID, "conv_nd: unknown impl %d", impl);
-}
-
-extern "C" int lt_conv_pair_eligible(const lt_conv_desc* d) {
-  if (!d || d->in_format != LT_FMT_S32 || d->Cin % 32 != 0) return 0;
-  return lt::conv_pair_fwd(d, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, 1) == 0 ? 1 : 0;
 }

@@ -19,7 +19,7 @@ namespace lt {
 struct TailParams {
   const float* scale1; const float* shift1;   // [32] folded BN of back_layers[1]
   const float* scale2; const float* shift2;   // [32] back_layers[2]
-  const float* scale3; const float* bias3;    // [32] output layer: 1 / (filter pre-scale) and bias (zero padded)
+  const float* scale3; const float* bias3;    // [FC] output layer: 1 / (filter pre-scale) and bias (zero padded)
   float* logits;                              // [rows][FC]
   long rows;
   long tiles;
@@ -272,9 +272,11 @@ static int launch_tail(const void* x, const void* w1, const void* w2, const void
     int rc = make_map(&tmX, x, 2, dims, str, bx, nullptr, 1);
     if (rc) return rc;
   }
+  // each map spans the rows the buffer holds; the 32-row box reads past the 16 rows of a w3 with J <= 16 as zeros (TMA fill)
   const void* ws[3] = {w1, w2, w3};
+  const uint64_t wrows[3] = {32, 32, (uint64_t)((p.FC + 15) & ~15)};
   for (int i = 0; i < 3; ++i) {
-    const uint64_t dims[2] = {64, 128};
+    const uint64_t dims[2] = {64, wrows[i]};
     const uint64_t str[1] = {128};
     const uint32_t bx[2] = {64, 32};
     int rc = make_map(&tmW[i], ws[i], 2, dims, str, bx, nullptr, 1);
@@ -299,8 +301,8 @@ static int launch_tail(const void* x, const void* w1, const void* w2, const void
   return LT_OK;
 }
 
-// x: split-fp16 rows [rows][32 hi | 32 lo]; w1/w2/w3: lt_conv_pair_pack_weights(taps = 1, Cin = 32, Cout = 32 / 32 / J) buffers
-// (rows padded to 128; the first 32 are used); scale/shift: folded BN of the two hidden layers; scale3 / bias3 [32]: output affine
+// x: split-fp16 rows [rows][32 hi | 32 lo]; w1/w2/w3: lt_conv_tc_pack_weights(taps = 1, Cin = 32, Cout = 32 / 32 / J) buffers
+// (32, 32 and round_up(FC, 16) rows); scale/shift: folded BN of the two hidden layers; scale3 / bias3 [FC]: output affine
 // (scale3 = 1 / filter pre-scale, bias zero padded);
 // logits float32 [rows][FC], FC % 4 == 0, J <= FC <= 32.
 extern "C" int lt_v2v_tail_fwd(const void* x, const void* w1, const void* w2, const void* w3, const float* scale1, const float* shift1,

@@ -401,12 +401,14 @@ static bool groups_ok(const lt_conv_desc* d, int CoutP) {
          d->out_format == LT_FMT_S32;
 }
 
-// Shared by every tensor-core entry point: weights packed as [tap][Cin/32][CoutP rows][32 hi | 32 lo] fp16.
-static int conv_wg_fwd(const lt_conv_desc* d, const void* in, const void* weight, int CoutP, const float* scale, const float* shift,
-                       const void* residual, void* out, int terms, void* stream) {
+// LT_CONV_TC (terms = 3) and LT_CONV_TC1 (terms = 1): weights packed as [tap][Cin/32][CoutP rows][32 hi | 32 lo] fp16,
+// CoutP = round_up(Cout, 16) (lt_conv_tc_pack_weights).
+int conv_tc_fwd_terms(const lt_conv_desc* d, const void* in, const void* weight, const float* scale, const float* shift,
+                      const void* residual, void* out, int terms, void* stream) {
   LT_REQUIRE(d->in_format == LT_FMT_S32, "conv_tc: input must be split-fp16");
   LT_REQUIRE(d->Cin % 32 == 0, "conv_tc: Cin=%d must be a multiple of 32", d->Cin);
   LT_REQUIRE(d->FC % 4 == 0 && (d->out_format == LT_FMT_F32 || d->FC % 32 == 0), "conv_tc: bad output channel stride %d", d->FC);
+  const int CoutP = (d->Cout + 15) & ~15;
   const int CB = d->Cin / 32;
   const int taps = d->KD * d->KH * d->KW;
   const int Nt = pick_nt(CoutP);
@@ -425,23 +427,6 @@ static int conv_wg_fwd(const lt_conv_desc* d, const void* in, const void* weight
     if (rc) return rc;
   }
   return launch_tc(tmA, tmB, p, CoutP / Nt, (cudaStream_t)stream, d->workspace, d->workspace_bytes);
-}
-
-// 128-padded weights (lt_conv_pair_pack_weights): the layers with Cout % 128 == 0
-int conv_pair_fwd(const lt_conv_desc* d, const void* in, const void* weight, const float* scale, const float* shift,
-                  const void* residual, void* out, void* stream, int probe_only) {
-  const int CoutP = (d->Cout + 127) & ~127;
-  const int G = out_groups(d);
-  const bool ok = d->in_format == LT_FMT_S32 && d->Cin % 32 == 0 && d->Cout % 128 == 0 &&
-                  (G > 1 ? groups_ok(d, CoutP) : (d->FC % 32 == 0 && CoutP <= d->FC));
-  if (probe_only) return ok ? 0 : 1;
-  if (!ok) return fail(LT_ERR_INVALID, "conv_pair: shape not covered (Cout=%d FC=%d)", d->Cout, d->FC);
-  return conv_wg_fwd(d, in, weight, CoutP, scale, shift, residual, out, 3, stream);
-}
-
-int conv_tc_fwd_terms(const lt_conv_desc* d, const void* in, const void* weight, const float* scale, const float* shift,
-                      const void* residual, void* out, int terms, void* stream) {
-  return conv_wg_fwd(d, in, weight, (d->Cout + 15) & ~15, scale, shift, residual, out, terms, stream);
 }
 
 // ---- weight packing: fp32 [taps][Cin][Cout] -> fp16 [taps][Cin/32][CoutP][32 hi | 32 lo] (128-byte rows) ----------
@@ -464,15 +449,6 @@ __global__ void __launch_bounds__(256) pack_weights_kernel(const float* __restri
   }
 }
 
-static int pack_weights(const float* w, void* packed, int taps, int Cin, int Cout, int CoutP, void* stream) {
-  const long total = (long)taps * (Cin / 32) * CoutP * 32;
-  long blocks = (total + 255) / 256;
-  if (blocks > 65535) blocks = 65535;
-  pack_weights_kernel<<<(unsigned)blocks, 256, 0, (cudaStream_t)stream>>>(w, reinterpret_cast<sh_t*>(packed), taps, Cin, Cout, CoutP);
-  LT_CHECK_LAUNCH("pack_weights_kernel");
-  return LT_OK;
-}
-
 __global__ void ones_zeros_kernel(float* ones, float* zeros, int n) {
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i < n) { ones[i] = 1.0f; zeros[i] = 0.0f; }
@@ -490,18 +466,13 @@ extern "C" size_t lt_conv_tc_weight_bytes(int taps, int Cin, int Cout) {
 extern "C" int lt_conv_tc_pack_weights(const float* w, void* packed, int taps, int Cin, int Cout, void* stream) {
   LT_REQUIRE(w && packed, "conv_tc_pack_weights: null pointer");
   LT_REQUIRE(Cin % 32 == 0 && taps > 0 && Cout > 0, "conv_tc_pack_weights: bad sizes");
-  return pack_weights(w, packed, taps, Cin, Cout, (Cout + 15) & ~15, stream);
-}
-
-extern "C" size_t lt_conv_pair_weight_bytes(int taps, int Cin, int Cout) {
-  const int CoutP = (Cout + 127) & ~127;
-  return (size_t)taps * (Cin / 32) * CoutP * 128;
-}
-
-extern "C" int lt_conv_pair_pack_weights(const float* w, void* packed, int taps, int Cin, int Cout, void* stream) {
-  LT_REQUIRE(w && packed, "conv_pair_pack_weights: null pointer");
-  LT_REQUIRE(Cin % 32 == 0 && taps > 0 && Cout > 0, "conv_pair_pack_weights: bad sizes");
-  return pack_weights(w, packed, taps, Cin, Cout, (Cout + 127) & ~127, stream);
+  const int CoutP = (Cout + 15) & ~15;
+  const long total = (long)taps * (Cin / 32) * CoutP * 32;
+  long blocks = (total + 255) / 256;
+  if (blocks > 65535) blocks = 65535;
+  pack_weights_kernel<<<(unsigned)blocks, 256, 0, (cudaStream_t)stream>>>(w, reinterpret_cast<sh_t*>(packed), taps, Cin, Cout, CoutP);
+  LT_CHECK_LAUNCH("pack_weights_kernel");
+  return LT_OK;
 }
 
 // D[M][N] (fp32) = A[M][K] * B[N][K]^T, plain fp16 row-major operands; exercises the exact TMA /

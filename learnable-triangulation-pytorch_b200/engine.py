@@ -10,8 +10,8 @@ Data layout in HBM: every activation is channels-last ([N][D][H][W][C]); 2-D map
   mode "simt": float32 activations, exact-fp32 FFMA convs (parity mode / checker)
   mode "tc"  : split-fp16 activations, wgmma convs with 3-term products (fp32-grade)
   mode "tc1" : split-fp16 activations, wgmma convs with high parts only (bf16-grade, fast)
-Layers the tensor-core kernel does not cover (the 3-channel stem and the six stride-2 convs of
-the trunk) run on the FFMA kernel in every mode.
+In the tensor-core modes every conv runs on the tensor cores: the 3-channel 7x7 stride-2 stem as a
+4x4 stride-1 conv over the 2x2 space-to-depth image, the stride-2 convs through TMA traversal strides.
 """
 import math
 import os
@@ -20,7 +20,7 @@ import torch
 from torch import nn
 
 from . import capi
-from .capi import FMT_F32, FMT_S32, CONV_SIMT, CONV_TC, CONV_TC1, CONV_TC_FOLD, CONV_TC_PAIR, RES_NONE, RES_BEFORE_RELU, RES_AFTER_RELU
+from .capi import FMT_F32, FMT_S32, CONV_SIMT, CONV_TC, CONV_TC1, CONV_TC_FOLD, RES_NONE, RES_BEFORE_RELU, RES_AFTER_RELU
 
 
 def _round_up(v, m):
@@ -48,7 +48,7 @@ class Act:
 
 class ConvPack:
     """One (phase of a) convolution, ready to launch: packed filter + folded scale/shift + geometry."""
-    __slots__ = ("w", "scale", "shift", "taps", "k", "stride", "pad", "cin", "cout", "cout_p", "impl", "in_fmt", "kmacs", "w_fold", "w_pair", "groups")
+    __slots__ = ("w", "scale", "shift", "taps", "k", "stride", "pad", "cin", "cout", "cout_p", "impl", "in_fmt", "kmacs", "w_fold", "groups")
 
 
 def _f32(t):
@@ -87,16 +87,6 @@ class NativeEngine:
         self._epoch = 0
         self._graphs = {}
         self.launches = 0          # kernels launched by the last eager forward (our own kernels only)
-        self.use_fold = os.environ.get("LT_TC_FOLD", "1") == "1"          # halo-reusing kernel for Cin=32 cubic layers (0: generic kernel)
-        self.use_pair = os.environ.get("LT_TC_PAIR", "1") == "1"          # CTA-pair kernel for Cout % 128 == 0 layers
-        self.use_tail = os.environ.get("LT_TC_TAIL", "1") == "1"          # fused back1 + back2 + output kernel
-        self.weight_prescale = os.environ.get("LT_TC_WSCALE", "1") == "1"   # power-of-two filter pre-scale (common.cuh)
-        self.merge_deconv3d = os.environ.get("LT_TC_MERGE_DECONV", "1") == "1"   # k2 s2 transposed conv as one GEMM
-        self.tc_stem = os.environ.get("LT_TC_STEM", "1") == "1"          # stem conv on the tensor-core kernel (space-to-depth)
-        self.tc_strided = os.environ.get("LT_TC_STRIDED", "1") == "1"   # stride-2 convs on the tensor-core kernel
-        self.compact_logits = os.environ.get("LT_LOGITS_COMPACT", "1") == "1"
-        self.accum_compensation = os.environ.get("LT_TC_ACCUM_COMP", "1") == "1"   # truncation-shrinkage factor in the folded scale
-        self.fuse_stats = os.environ.get("LT_TAIL_STATS", "1") == "1"      # soft-argmax statistics inside the fused tail kernel
         self.timeline = None       # set to [] to record (label, flops, bytes, start_evt, end_evt) per launch
         capi.lib()                 # fail loudly if the extension is missing
 
@@ -114,7 +104,7 @@ class NativeEngine:
         self._packs = None
         self._graphs = {}
 
-    def _pack(self, src, k, stride, pad, cin, cout, bias, bn, cin_pad=None, force_simt=False, out_fmt=None, force_pair=False):
+    def _pack(self, src, k, stride, pad, cin, cout, bias, bn, cin_pad=None, force_simt=False, out_fmt=None):
         """src = (filter tensor, base, (s_td, s_th, s_tw, s_ci, s_co)): where element (td, th, tw, ci, co) of this (phase of a)
         convolution sits inside the module's own weight tensor.  Everything below is our own kernels: gather to the canonical
         [tap][Cin][Cout] layout (lt_conv_gather_weights_fwd), operand packing, BatchNorm folding (lt_fold_bn_fwd)."""
@@ -129,8 +119,7 @@ class NativeEngine:
         pk.taps, pk.k, pk.stride, pk.pad, pk.cout, pk.groups = taps, k, stride, pad, G * cout, G
         pk.kmacs = taps * cin * cout * G   # algorithmic MACs per output position
         pk.w_fold = None
-        pk.w_pair = None
-        use_tc = (self.mode != "simt") and not force_simt and (max(stride) == 1 or self.tc_strided)
+        use_tc = (self.mode != "simt") and not force_simt
         assert G == 1 or (use_tc and cout % 32 == 0), "column blocks need the tensor-core path and 32-channel multiples"
         if use_tc:
             cin_p = _round_up(max(cin, cin_pad or 0), 32)
@@ -141,7 +130,7 @@ class NativeEngine:
         blk_p = cout if G > 1 else cout_p
         wp = torch.empty((taps, cin_p, cout_p), dtype=torch.float32, device=dev)
         amax = None
-        if use_tc and self.weight_prescale:
+        if use_tc:
             # power-of-two pre-scale of the whole filter tensor (all phases of a transposed conv share it): common.cuh
             amax = torch.empty(1, dtype=torch.int32, device=dev)
             capi.absmax(w, amax)
@@ -151,13 +140,8 @@ class NativeEngine:
             packed = torch.empty(capi.conv_tc_weight_bytes(taps, cin_p, cout_p) // 2, dtype=torch.float16, device=dev)
             capi.conv_tc_pack_weights(wp, packed, taps, cin_p, cout_p)
             pk.w, pk.cin, pk.cout_p, pk.impl, pk.in_fmt = packed, cin_p, cout_p, self.tc_impl, FMT_S32
-            # wide layers: also pack with the 128-channel padding of LT_CONV_TC_PAIR
-            if self.mode == "tc" and ((self.use_pair and cout_p % 128 == 0) or force_pair):
-                wq = torch.empty(capi.conv_pair_weight_bytes(taps, cin_p, cout_p) // 2, dtype=torch.float16, device=dev)
-                capi.conv_pair_pack_weights(wp, wq, taps, cin_p, cout_p)
-                pk.w_pair = wq
             # narrow cubic stride-1 layers (V2V at full resolution): also pack for the halo-reusing persistent kernel (csrc/conv_fold.cu)
-            if (self.use_fold and self.mode == "tc" and cin_p == 32 and cout <= 32 and k[0] == k[1] == k[2] and k[0] in (3, 7)
+            if (self.mode == "tc" and cin_p == 32 and cout <= 32 and k[0] == k[1] == k[2] and k[0] in (3, 7)
                     and tuple(pad) == (k[0] // 2,) * 3 and max(stride) == 1):
                 wf = torch.empty(capi.conv_fold_weight_bytes(k[0], cout) // 2, dtype=torch.float16, device=dev)
                 wsrc = wp if cout_p == cout else wp[:, :, :cout].contiguous()
@@ -169,9 +153,7 @@ class NativeEngine:
         pk.shift = torch.empty(cout_p, dtype=torch.float32, device=dev)
         # tensor-core accumulation steps on the main fp32 accumulator (one hi*hi MMA per 16 input channels and tap, in conv_tc_kernel and in
         # conv_fold_kernel alike): lt_fold_bn_fwd compensates the expected truncation shrinkage (include/lt_b200.h)
-        steps = 0
-        if use_tc and self.accum_compensation:
-            steps = taps * (cin_p // 16)
+        steps = taps * (cin_p // 16) if use_tc else 0
         for g in range(G):     # the per-channel affine repeats for every column block
             sc, sh = pk.scale[g * cout:g * cout + blk_p], pk.shift[g * cout:g * cout + blk_p]
             if bn is not None:
@@ -241,7 +223,7 @@ class NativeEngine:
         instead of eight times and a level costs one launch instead of eight."""
         w = _f32(deconv.weight)  # (Cin, Cout, 2, 2, 2)
         cin, cout = w.shape[:2]
-        if self.mode != "simt" and cout % 32 == 0 and self.merge_deconv3d:
+        if self.mode != "simt" and cout % 32 == 0:
             srcs = [(w, a * 4 + b * 2 + c, (0, 0, 0, cout * 8, 8)) for a in (0, 1) for b in (0, 1) for c in (0, 1)]
             return self._pack(srcs, (1, 1, 1), (1, 1, 1), (0, 0, 0), cin, cout, deconv.bias, bn)
         phases = {}
@@ -261,7 +243,7 @@ class NativeEngine:
         with torch.no_grad():
             # stem: exact-fp32 mode pads 3 -> 4 channels (float4 per pixel) for the FFMA kernel; the tensor-core modes
             # rewrite the 7x7 stride-2 conv as a 4x4 stride-1 conv over the 2x2 space-to-depth image (12 -> 32 channels)
-            if self.mode == "simt" or not self.tc_stem:
+            if self.mode == "simt":
                 P["stem"] = self._pack_conv(bb.conv1, bb.bn1, cin_pad=4, force_simt=True)
             else:
                 P["stem_s2d"] = self._pack_stem_s2d(bb.conv1, bb.bn1)
@@ -310,11 +292,9 @@ class NativeEngine:
                 P["up%d" % lvl] = self._pack_deconv3d_k2s2(up.block[0], up.block[1])
             pack_res("mid", ed.mid_res)
             pack_res("back0", v.back_layers[0])
-            # the three point-wise layers of the tail are also packed for the fused tail kernel (csrc/conv_tail.cu)
-            tail = self.use_tail and self.mode == "tc"
-            P["back1"] = self._pack_conv(v.back_layers[1].block[0], v.back_layers[1].block[1], force_pair=tail)
-            P["back2"] = self._pack_conv(v.back_layers[2].block[0], v.back_layers[2].block[1], force_pair=tail)
-            P["output"] = self._pack_conv(v.output_layer, None, out_fmt=FMT_F32, force_pair=tail)
+            P["back1"] = self._pack_conv(v.back_layers[1].block[0], v.back_layers[1].block[1])
+            P["back2"] = self._pack_conv(v.back_layers[2].block[0], v.back_layers[2].block[1])
+            P["output"] = self._pack_conv(v.output_layer, None, out_fmt=FMT_F32)
         self._packs, self._packs_version = P, ver
         self._graphs = {}
 
@@ -364,9 +344,7 @@ class NativeEngine:
         if (pk.w_fold is not None and x.W >= 16 and out.C == 32 and out_scale == (1, 1, 1) and (od, oh, ow) == (x.D, x.H, x.W)):
             impl, weight = CONV_TC_FOLD, pk.w_fold
             d.Cout = pk.cout
-        elif pk.w_pair is not None and capi.conv_pair_eligible(d):
-            impl, weight = CONV_TC_PAIR, pk.w_pair
-        label = {CONV_TC_FOLD: "conv_fold", CONV_TC_PAIR: "conv_pair", CONV_SIMT: "conv_ffma"}.get(impl, "conv_tc")
+        label = {CONV_TC_FOLD: "conv_fold", CONV_SIMT: "conv_ffma"}.get(impl, "conv_tc")
         with self._timed(label, flops=2.0 * x.N * od * oh * ow * pk.kmacs,
                          desc="N%d %dx%dx%d Cin%d Cout%d k%d%d%d s%d" % (x.N, od, oh, ow, pk.cin, pk.cout, kd, kh, kw, sw)):
             capi.conv_nd(d, x.data, weight, pk.scale, pk.shift, None if residual is None else residual.data, out.data, impl)
@@ -512,26 +490,27 @@ class NativeEngine:
             x = self._res3d(x, "dec%d" % lvl)
             x = self._deconv3d(x, P["up%d" % lvl], skips.pop(lvl))
         x = self._res3d(x, "back0")
-        out_c = _round_up(P["output"].cout, 4) if self.compact_logits else None
+        out_c = _round_up(P["output"].cout, 4)
         b1, b2, b3 = P["back1"], P["back2"], P["output"]
-        if (b1.w_pair is not None and b2.w_pair is not None and b3.w_pair is not None and x.fmt == FMT_S32 and x.C == 32 and out_c is not None
-                and b1.cin == b2.cin == b3.cin == 32 and b1.cout == b2.cout == 32 and b3.cout <= out_c <= 32):
+        # the tail kernel reads b1.w / b2.w as 32 rows and b3.w as round_up(out_c, 16) rows of lt_conv_tc_pack_weights
+        if (b1.impl == b2.impl == b3.impl == CONV_TC and x.fmt == FMT_S32 and x.C == 32 and b1.cin == b2.cin == b3.cin == 32
+                and b1.cout == b2.cout == b1.cout_p == b2.cout_p == 32 and b3.cout <= out_c <= 32 and b3.cout_p == _round_up(out_c, 16)):
             # v2v.py:154-160,168-169 in one kernel: the two hidden activations never leave the SM
             logits = Act(x.N, x.D, x.H, x.W, out_c, FMT_F32, x.data.device)
             rows = x.pixels
             nvox = x.D * x.H * x.W
-            fuse = (self.fuse_stats and softargmax_args is not None and nvox % 128 == 0 and nvox >= 16384 and out_c <= 20
+            fuse = (softargmax_args is not None and nvox % 128 == 0 and nvox >= 16384 and out_c <= 20
                     and softargmax_args[3] in (0, 1, False, True))
             with self._timed("conv_tail", flops=2.0 * rows * (b1.kmacs + b2.kmacs + b3.kmacs), nbytes=rows * (128 + 4 * out_c + (12 if fuse else 0)),
                              desc="N%d %dx%dx%d 32->32->32->%d k111 fused%s" % (x.N, x.D, x.H, x.W, b3.cout, " + soft-argmax statistics" if fuse else "")):
                 if fuse:
                     coord, J, mult, softmax = softargmax_args
                     ws = torch.empty(capi.softargmax3d_workspace_bytes(x.N, J, nvox) // 4 + 1, dtype=torch.float32, device=x.data.device)
-                    G = capi.v2v_tail_stats(x.data, b1.w_pair, b2.w_pair, b3.w_pair, b1.scale, b1.shift, b2.scale, b2.shift, b3.scale, b3.shift,
+                    G = capi.v2v_tail_stats(x.data, b1.w, b2.w, b3.w, b1.scale, b1.shift, b2.scale, b2.shift, b3.scale, b3.shift,
                                             logits.data, x.N, nvox, out_c, coord, J, mult, int(softmax), ws)
                     logits.stats = (ws, G)
                 else:
-                    capi.v2v_tail(x.data, b1.w_pair, b2.w_pair, b3.w_pair, b1.scale, b1.shift, b2.scale, b2.shift, b3.scale, b3.shift, logits.data, rows, out_c)
+                    capi.v2v_tail(x.data, b1.w, b2.w, b3.w, b1.scale, b1.shift, b2.scale, b2.shift, b3.scale, b3.shift, logits.data, rows, out_c)
             self.launches += 1
             return logits
         x = self._conv(x, P["back1"], relu=True)

@@ -18,11 +18,7 @@ class Recorder:
                 self.calls.append((name, a))
             return f
         monkeypatch.setattr(capi, "conv_fold_weight_bytes", lambda k, co: k * k * k * ((co + 15) // 16 * 16) * 64 * 2)
-        monkeypatch.setattr(capi, "conv_pair_weight_bytes", lambda t, ci, co: t * (ci // 32) * ((co + 127) // 128 * 128) * 128)
-        # stand-in for lt_conv_pair_eligible (Cout % 128 == 0, output wide enough): the dry run loads no library
-        monkeypatch.setattr(capi, "conv_pair_eligible", lambda d: d.Cout % 128 == 0 and d.FC % 32 == 0 and d.Cout <= d.FC and
-                            d.N * d.OD * d.OH * d.OW >= 128 * 40)
-        for name in ("v2v_tail", "absmax", "conv_gather_weights", "fold_bn", "conv_pair_pack_weights", "conv_fold_pack_weights", "stem_s2d", "coord_volume", "unproject_aggregate", "softargmax3d", "maxpool", "nchw_to_nhwc", "f32_to_s32",
+        for name in ("v2v_tail", "absmax", "conv_gather_weights", "fold_bn", "conv_fold_pack_weights", "stem_s2d", "coord_volume", "unproject_aggregate", "softargmax3d", "maxpool", "nchw_to_nhwc", "f32_to_s32",
                      "s32_to_f32", "cl_to_cf", "conv_tc_pack_weights"):
             monkeypatch.setattr(capi, name, rec(name))
         def tail_stats(*a, **k):
@@ -48,10 +44,6 @@ class Recorder:
         if impl == capi.CONV_TC_FOLD:
             assert d.Cin == 32 and d.FC == 32 and d.Cout <= 32 and d.IW >= 16 and d.KD == d.KH == d.KW and d.KW in (3, 7)
             assert w.numel() == d.KW ** 3 * ((d.Cout + 15) // 16 * 16) * 64
-        elif impl == capi.CONV_TC_PAIR:
-            assert d.in_format == capi.FMT_S32 and x.dtype == torch.float16 and d.Cin % 32 == 0 and d.Cout % 128 == 0
-            assert w.numel() == d.KD * d.KH * d.KW * (d.Cin // 32) * d.Cout * 64 and scale.numel() >= d.Cout
-            assert d.FC % 32 == 0 and d.Cout >= d.FC
         elif impl == capi.CONV_SIMT:
             assert d.in_format == capi.FMT_F32 and x.dtype == torch.float32
             cw = (d.Cout + 3) // 4 * 4
@@ -95,7 +87,23 @@ def test_engine_plan_is_consistent(monkeypatch, mode, layers):
     assert tail == (1 if mode == "tc" else 0)
     up = 5 * (1 if mode == "tc" else 8)     # tc: each k2 s2 transposed conv is one grouped-output GEMM; simt: eight phase convs
     assert v2v == 1 + 20 * 2 + 3 + up + (0 if tail else 2 + 1), v2v
-    assert e.launches == len(rec.calls) - sum(1 for c in rec.calls if c[0] in ("conv_tc_pack_weights", "conv_fold_pack_weights", "conv_pair_pack_weights", "conv_gather_weights", "fold_bn", "absmax")) + (1 if tail else 2)   # softargmax = 3 launches (2 behind the fused tail)
+    assert e.launches == len(rec.calls) - sum(1 for c in rec.calls if c[0] in ("conv_tc_pack_weights", "conv_fold_pack_weights", "conv_gather_weights", "fold_bn", "absmax")) + (1 if tail else 2)   # softargmax = 3 launches (2 behind the fused tail)
     if mode == "tc":
         simt = [c for c in convs if c[1][0] == capi.CONV_SIMT]
         assert len(simt) == 0, "every conv runs on the tensor-core kernels"
+        # the fused tail reads the same packed filters as the three separate convs would
+        P = e._packs
+        for name, a in rec.calls:
+            if name in ("v2v_tail", "v2v_tail_stats"):
+                assert a[1] is P["back1"].w and a[2] is P["back2"].w and a[3] is P["output"].w
+        # each filter is packed once: one lt_conv_tc_pack_weights per ConvPack, one lt_conv_fold_pack_weights per fold layer
+        packs = []
+        for v in P.values():          # a ConvPack, a dict of transposed-conv phases, or a confidence head's MLP weights
+            if isinstance(v, dict):
+                packs += v.values()
+            elif isinstance(v, eng_mod.ConvPack):
+                packs.append(v)
+        packed = [a[1] for name, a in rec.calls if name == "conv_tc_pack_weights"]
+        assert sorted(map(id, packed)) == sorted(id(pk.w) for pk in packs)
+        folded = [a[1] for name, a in rec.calls if name == "conv_fold_pack_weights"]
+        assert sorted(map(id, folded)) == sorted(id(pk.w_fold) for pk in packs if pk.w_fold is not None)

@@ -165,9 +165,7 @@ def _engine(mode):
     e.model, e.mode, e.use_graph = _Holder(), mode, False
     e.act_fmt = capi.FMT_F32 if mode == "simt" else capi.FMT_S32
     e.tc_impl = {"simt": capi.CONV_SIMT, "tc": capi.CONV_TC, "tc1": capi.CONV_TC1}[mode]
-    e._packs, e._graphs, e.launches, e.timeline, e.tc_strided, e.use_fold, e.tc_stem = {}, {}, 0, None, True, True, True
-    e.use_pair, e.use_tail, e.weight_prescale, e.merge_deconv3d, e._epoch = True, True, True, True, 0
-    e.accum_compensation, e.fuse_stats, e.compact_logits = True, True, True
+    e._packs, e._graphs, e.launches, e.timeline, e._epoch = {}, {}, 0, None, 0
     return e
 
 

@@ -237,14 +237,14 @@ def _fold_case(case, with_res):
         assert float(full[:, cout:].abs().max()) == 0.0
 
 
-PAIR_CASES = [
-    # (dims, cin, cout, k, stride, pad, spatial, batch, res_mode)  -- layers with Cout % 128 == 0 (csrc/conv_pair.cu)
-    (2, 256, 1024, 1, 1, 0, (24, 24), 9, "before"),     # 1x1 expand of a bottleneck: Nt = 256, 4 N tiles, odd M-tile count (41)
-    (2, 1024, 256, 1, 1, 0, (24, 24), 8, "none"),       # 1x1 reduce: 32 K chunks, one N tile
-    (2, 256, 256, 3, 1, 1, (24, 24), 32, "none"),       # 3x3: padding through TMA zero fill in both CTAs of a pair
+WIDE_CASES = [
+    # (dims, cin, cout, k, stride, pad, spatial, batch, res_mode)  -- layers with Cout % 128 == 0 (Nt = 128)
+    (2, 256, 1024, 1, 1, 0, (24, 24), 9, "before"),     # 1x1 expand of a bottleneck: 8 N tiles, odd M-tile count (41)
+    (2, 1024, 256, 1, 1, 0, (24, 24), 8, "none"),       # 1x1 reduce: 32 K chunks
+    (2, 256, 256, 3, 1, 1, (24, 24), 32, "none"),       # 3x3: padding through TMA zero fill
     (2, 128, 128, 3, 1, 1, (48, 48), 3, "none"),        # Nt = 128
     (2, 128, 512, 1, 1, 0, (48, 48), 3, "before"),
-    (2, 64, 256, 1, 1, 0, (96, 96), 2, "before"),       # 2 K chunks per tile: epilogue-bound, many tiles per pair
+    (2, 64, 256, 1, 1, 0, (96, 96), 2, "before"),       # 2 K chunks per tile: epilogue-bound
     (2, 256, 512, 1, 2, 0, (48, 48), 4, "none"),        # stride-2 downsample through TMA traversal strides
     (2, 128, 128, 3, 2, 1, (48, 48), 16, "none"),
     (2, 512, 2048, 1, 1, 0, (12, 12), 6, "before"),
@@ -255,17 +255,18 @@ PAIR_CASES = [
 
 
 @pytest.mark.parametrize("acc", ["single", "two"])
-@pytest.mark.parametrize("case", PAIR_CASES)
-def test_conv_pair_vs_torch(case, acc):
-    """LT_CONV_TC_PAIR (weights padded to 128 channels) against the fp32 torch op, under both settings of lt_options.pair_two_acc."""
+@pytest.mark.parametrize("case", WIDE_CASES)
+def test_conv_tc_wide_vs_torch(case, acc):
+    """LT_CONV_TC on the wide layers (Cout % 128 == 0) against the fp32 torch op, under both settings of lt_options.pair_two_acc (which
+    has no effect)."""
     capi.set_options(pair_two_acc=int(acc == "two"))
     try:
-        _pair_case(case)
+        _wide_case(case)
     finally:
         capi.set_options(pair_two_acc=1)
 
 
-def _pair_case(case):
+def _wide_case(case):
     dims, cin, cout, k, stride, pad, spatial, N, res_mode = case
     torch.manual_seed(cin + cout + k + N)
     conv = (torch.nn.Conv2d if dims == 2 else torch.nn.Conv3d)(cin, cout, k, stride, pad, bias=(dims == 3)).eval()
@@ -278,7 +279,7 @@ def _pair_case(case):
         want = {"none": F.relu(y0), "before": F.relu(y0 + res), "after": F.relu(y0) + res}[res_mode]
     e = _engine("tc")
     pk = e._pack_conv(conv.to(DEV), bn.to(DEV))
-    assert pk.w_pair is not None
+    assert pk.impl == capi.CONV_TC
     ra = act_from_nchw(res, capi.FMT_S32) if res_mode != "none" else None
     launched = []
     orig = capi.conv_nd
@@ -288,17 +289,17 @@ def _pair_case(case):
     finally:
         capi.conv_nd = orig
     torch.cuda.synchronize()
-    assert launched == [capi.CONV_TC_PAIR], "the CTA-pair kernel must have been selected"
+    assert launched == [capi.CONV_TC], "the generic tensor-core kernel must have been selected"
     got = act_to_nchw(ya, cout).cpu()
     if dims == 2:
         got = got.squeeze(2)
     err = rel_err(got.numpy(), want.numpy())
-    print("conv_pair %s rel err %.2e" % (case, err))
+    print("conv_tc wide %s rel err %.2e" % (case, err))
     assert err < TOL["tc"]
 
 
-def test_conv_pair_deconv_phases_vs_torch():
-    """k4 s2 p1 transposed conv 256 -> 256 (pose_resnet.py:266-291) as four stride-phase 2x2 convs on the CTA-pair kernel."""
+def test_conv_tc_wide_deconv_phases_vs_torch():
+    """k4 s2 p1 transposed conv 256 -> 256 (pose_resnet.py:266-291) as four stride-phase 2x2 convs on the tensor-core kernel."""
     torch.manual_seed(14)
     e = _engine("tc")
     dc = torch.nn.ConvTranspose2d(256, 256, 4, 2, 1, 0, bias=False).eval()
@@ -313,14 +314,14 @@ def test_conv_pair_deconv_phases_vs_torch():
         got = act_to_nchw(e._deconv2d(act_from_nchw(x, capi.FMT_S32), e._pack_deconv2d_k4s2(dc.to(DEV), bn.to(DEV)))).squeeze(2).cpu()
     finally:
         capi.conv_nd = orig
-    assert launched == [capi.CONV_TC_PAIR] * 4
+    assert launched == [capi.CONV_TC] * 4
     assert rel_err(got.numpy(), want.numpy()) < TOL["tc"]
 
 
 @pytest.mark.parametrize("cin,cout,spatial,N", [(64, 32, (32, 32, 32), 2), (128, 64, (16, 16, 16), 4), (128, 128, (8, 8, 8), 2), (128, 128, (2, 2, 2), 8)])
 def test_deconv3d_merged_single_gemm_vs_torch(cin, cout, spatial, N):
     """ConvTranspose3d(k=2, s=2) + BN + ReLU + skip (v2v.py:54-66, :118-137) as ONE GEMM with N = 8 x Cout and grouped output
-    (lt_conv_desc.ogd/ogh/ogw): large levels on the CTA-pair kernel, small ones on the one-CTA kernel."""
+    (lt_conv_desc.ogd/ogh/ogw) on the tensor-core kernel, from a 32^3 input level down to 2^3."""
     torch.manual_seed(cin + cout + spatial[0])
     e = _engine("tc")
     dc = torch.nn.ConvTranspose3d(cin, cout, 2, 2).eval()
@@ -396,31 +397,32 @@ def test_conv_tc_vs_ffma_at_config2_sizes(case):
     assert err < TOL["tc"]
 
 
+@pytest.mark.parametrize("J,FC", [(17, 20), (15, 16)])
 @pytest.mark.parametrize("spatial,N", [((16, 16, 16), 2), ((5, 6, 7), 3), ((64, 64, 16), 1)])
-def test_v2v_tail_fused_vs_torch(spatial, N):
+def test_v2v_tail_fused_vs_torch(spatial, N, J, FC):
     """back_layers[1], back_layers[2], output_layer (v2v.py:154-160,168-169) as one kernel (csrc/conv_tail.cu) vs the three torch ops;
-    row counts that are not a multiple of the 128-voxel tile included."""
+    row counts that are not a multiple of the 128-voxel tile included.  J = 15 packs the output filter as 16 rows, which the kernel's
+    32-row weight load extends with zeros."""
     torch.manual_seed(21)
-    c1, c2, c3 = torch.nn.Conv3d(32, 32, 1).eval(), torch.nn.Conv3d(32, 32, 1).eval(), torch.nn.Conv3d(32, 17, 1).eval()
+    c1, c2, c3 = torch.nn.Conv3d(32, 32, 1).eval(), torch.nn.Conv3d(32, 32, 1).eval(), torch.nn.Conv3d(32, J, 1).eval()
     bn1, bn2 = _bn_for(c1, 5), _bn_for(c2, 6)
     x = torch.randn(N, 32, *spatial)
     with torch.no_grad():
         want = c3(F.relu(bn2(c2(F.relu(bn1(c1(x)))))))
     e = _engine("tc")
-    e.use_tail = True
-    b1 = e._pack_conv(c1.to(DEV), bn1.to(DEV), force_pair=True)
-    b2 = e._pack_conv(c2.to(DEV), bn2.to(DEV), force_pair=True)
-    b3 = e._pack_conv(c3.to(DEV), None, out_fmt=capi.FMT_F32, force_pair=True)
+    b1 = e._pack_conv(c1.to(DEV), bn1.to(DEV))
+    b2 = e._pack_conv(c2.to(DEV), bn2.to(DEV))
+    b3 = e._pack_conv(c3.to(DEV), None, out_fmt=capi.FMT_F32)
     xa = act_from_nchw(x, capi.FMT_S32)
     rows = xa.pixels
-    logits = torch.full((rows, 20), 7.0, dtype=torch.float32, device=DEV)
-    capi.v2v_tail(xa.data, b1.w_pair, b2.w_pair, b3.w_pair, b1.scale, b1.shift, b2.scale, b2.shift, b3.scale, b3.shift, logits, rows, 20)
+    logits = torch.full((rows, FC), 7.0, dtype=torch.float32, device=DEV)
+    capi.v2v_tail(xa.data, b1.w, b2.w, b3.w, b1.scale, b1.shift, b2.scale, b2.shift, b3.scale, b3.shift, logits, rows, FC)
     torch.cuda.synchronize()
-    got = logits.view(N, *spatial, 20).permute(0, 4, 1, 2, 3).cpu()
-    err = rel_err(got[:, :17].numpy(), want.numpy())
-    print("v2v tail %s N=%d rel err %.2e" % (spatial, N, err))
+    got = logits.view(N, *spatial, FC).permute(0, 4, 1, 2, 3).cpu()
+    err = rel_err(got[:, :J].numpy(), want.numpy())
+    print("v2v tail %s N=%d J=%d rel err %.2e" % (spatial, N, J, err))
     assert err < TOL["tc"] * 2          # three chained layers
-    assert float(got[:, 17:].abs().max()) == 0.0
+    assert float(got[:, J:].abs().max()) == 0.0
 
 
 @pytest.mark.parametrize("softmax", [True, False])
@@ -437,13 +439,13 @@ def test_v2v_tail_with_softargmax_statistics(spatial, N, softmax):
     bn1, bn2 = _bn_for(c1, 5), _bn_for(c2, 6)
     x = torch.randn(N, 32, *spatial)
     e = _engine("tc")
-    b1 = e._pack_conv(c1.to(DEV), bn1.to(DEV), force_pair=True)
-    b2 = e._pack_conv(c2.to(DEV), bn2.to(DEV), force_pair=True)
-    b3 = e._pack_conv(c3.to(DEV), None, out_fmt=capi.FMT_F32, force_pair=True)
+    b1 = e._pack_conv(c1.to(DEV), bn1.to(DEV))
+    b2 = e._pack_conv(c2.to(DEV), bn2.to(DEV))
+    b3 = e._pack_conv(c3.to(DEV), None, out_fmt=capi.FMT_F32)
     xa = act_from_nchw(x, capi.FMT_S32)
     nvox, J, FC, mult = spatial[0] * spatial[1] * spatial[2], 17, 20, 1.7
     coord = (torch.randn(N, nvox, 3) * 600).to(DEV)
-    args = (xa.data, b1.w_pair, b2.w_pair, b3.w_pair, b1.scale, b1.shift, b2.scale, b2.shift, b3.scale, b3.shift)
+    args = (xa.data, b1.w, b2.w, b3.w, b1.scale, b1.shift, b2.scale, b2.shift, b3.scale, b3.shift)
     ws_bytes = capi.softargmax3d_workspace_bytes(N, J, nvox)
     # unfused
     lg0 = torch.empty((N * nvox, FC), dtype=torch.float32, device=DEV)
