@@ -61,7 +61,7 @@ typedef struct lt_options {
   /* sm_90a: the variants of the first (tensor-memory) kernels that these fields selected are one wgmma kernel; the fields
      marked "no effect" are kept for ABI compatibility and ignored */
   int tc_persist;          /* no effect */
-  int tc_splitk;           /* conv_tc: split-K for grids below half the SMs (default 1) */
+  int tc_splitk;           /* conv_tc: split the K loop where the launch model says it pays (lt_conv_tc_plan; default 1) */
   int tc_bres;             /* no effect */
   int tc_direct_epilogue;  /* no effect */
   int fold_fast_issue;     /* no effect */
@@ -212,8 +212,9 @@ typedef struct lt_conv_desc {
                                 transposed conv (v2v.py:54-66) is ONE 1x1x1 GEMM this way: N = 8 x Cout, osd=osh=osw=2, ogd=ogh=ogw=2;
                                 scale/shift carry Cout entries (the per-channel values repeated G times).  LT_CONV_TC / TC1 only */
   int reserved0;             /* set to 0 (keeps the pointer below 8-byte aligned without implicit padding) */
-  void* workspace;           /* optional device scratch for split-K (layers with fewer M x N tiles than half the SMs:
-                                the K loop is spread over more CTAs and summed in a fixed order); NULL = never split */
+  void* workspace;           /* optional device scratch for split-K (LT_CONV_TC / TC1 layers whose tiles fill the SMs
+                                unevenly: the K loop is spread over more CTAs and summed in a fixed order, see
+                                lt_conv_tc_plan); NULL = never split */
   size_t workspace_bytes;    /* size of workspace; a split is only used when its partial tiles fit */
 } lt_conv_desc;
 
@@ -226,6 +227,20 @@ int lt_conv_nd_fwd(const lt_conv_desc* desc, const void* in, const void* weight,
  * to fp16 [taps][Cin/32][n tile][hi|lo][Nt][32] (64-byte rows; Nt = min(CoutP, 128), CoutP = round_up(Cout, 16));
  * Cin % 32 == 0. */
 size_t lt_conv_tc_weight_bytes(int taps, int Cin, int Cout);
+
+/* Work decomposition of one LT_CONV_TC / TC1 launch of lt_conv_nd_fwd on a GPU with `sm_count` SMs, computed on the host without
+ * touching the device.  The persistent kernel runs `grid` CTAs (one per SM at most) over m_tiles x n_tiles x splits work units.
+ * splits > 1 spreads each tile's K chunks over that many units whose fp32 partial tiles are summed in a fixed order by a second
+ * launch; it is chosen by a model of the launch time (waves x per-unit K work + epilogue, plus the reduce pass) when `splitk` is
+ * non-zero, desc->workspace is not NULL and the partial tiles fit desc->workspace_bytes.  Grouped outputs never split. */
+typedef struct lt_conv_tc_launch_plan {
+  int nt;                    /* N tile: 16, 32, 64 or 128 output channels */
+  int m_tiles, n_tiles;      /* output tiles: 128 positions x nt channels */
+  int chunks;                /* K chunks of a tile: taps x Cin / 32 */
+  int splits;                /* K split count, 1 = none */
+  int grid;                  /* CTAs launched: min(m_tiles x n_tiles x splits, sm_count) */
+} lt_conv_tc_launch_plan;
+int lt_conv_tc_plan(const lt_conv_desc* desc, int sm_count, int splitk, lt_conv_tc_launch_plan* plan);
 int lt_conv_tc_pack_weights(const float* w_tap_ci_co, void* packed, int taps, int Cin, int Cout, void* stream);
 
 /* Weight preparation (once per parameter version, engine.prepare()).

@@ -36,6 +36,11 @@ class ConvDesc(ctypes.Structure):
         "relu", "residual", "in_format", "out_format", "ogd", "ogh", "ogw", "reserved0")] + [("workspace", c_void_p), ("workspace_bytes", c_size_t)]
 
 
+class ConvTcPlan(ctypes.Structure):
+    """Mirror of `struct lt_conv_tc_launch_plan` (include/lt_b200.h)."""
+    _fields_ = [(n, c_int) for n in ("nt", "m_tiles", "n_tiles", "chunks", "splits", "grid")]
+
+
 class Options(ctypes.Structure):
     """Mirror of `struct lt_options` (include/lt_b200.h): kernel-selection switches, all defaulting to the measured-best path."""
     _fields_ = [(n, c_int) for n in ("tc_persist", "tc_splitk", "tc_bres", "tc_direct_epilogue", "fold_fast_issue", "fold_debug",
@@ -69,6 +74,7 @@ SIGNATURES = {
                                     c_int, c_int, c_long, c_float, c_int, c_void_p]),
     "lt_conv_nd_fwd": (c_int, [ctypes.POINTER(ConvDesc)] + [c_void_p] * 6 + [c_int, c_void_p]),
     "lt_conv_tc_weight_bytes": (c_size_t, [c_int, c_int, c_int]),
+    "lt_conv_tc_plan": (c_int, [ctypes.POINTER(ConvDesc), c_int, c_int, ctypes.POINTER(ConvTcPlan)]),
     "lt_conv_tc_pack_weights": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_void_p]),
     "lt_absmax_fwd": (c_int, [c_void_p, c_long, c_void_p, c_void_p]),
     "lt_conv_gather_weights_fwd": (c_int, [c_void_p] + [c_long] * 6 + [c_int] * 7 + [c_void_p, c_void_p, c_int, c_int, c_void_p]),
@@ -250,6 +256,13 @@ def softargmax3d_workspace_bytes(B, J, nvox):
 def conv_nd(desc, inp, weight, scale, shift, residual, out, impl):
     _check(lib().lt_conv_nd_fwd(ctypes.byref(desc), _ptr(inp), _ptr(weight), _ptr(scale), _ptr(shift), _ptr(residual),
                                 _ptr(out), impl, _stream()), "lt_conv_nd_fwd")
+
+
+def conv_tc_plan(desc, sm_count, splitk=1):
+    """Host-only work decomposition of an LT_CONV_TC launch (lt_conv_tc_plan): dict of nt, m_tiles, n_tiles, chunks, splits, grid."""
+    plan = ConvTcPlan()
+    _check(lib().lt_conv_tc_plan(ctypes.byref(desc), sm_count, splitk, ctypes.byref(plan)), "lt_conv_tc_plan")
+    return {name: getattr(plan, name) for name, _ in ConvTcPlan._fields_}
 
 
 def conv_tc_weight_bytes(taps, cin, cout):

@@ -19,6 +19,12 @@
 // Warp roles (384 threads): warpgroup 0 = TMA producer (one warp issues), warpgroups 1 and 2 = MMA + epilogue for rows 0-63 and
 // 64-127 of the M tile.  The operand ring is released per stage by one arrival of each consumer warpgroup once its MMAs that read
 // the stage have completed (wgmma.wait_group 1 keeps one chunk of MMAs in flight behind the issue).
+//
+// Persistent grid: min(work units, SMs) CTAs stride over the work units (M tile x N tile x K split, N tile fastest).  Producer and
+// consumers keep one ring across unit boundaries, so the next unit's first boxes load while the consumers run the epilogue; on the
+// 1x1 layers of the backbone (2-8 K chunks per tile) the fill was most of a one-tile CTA's time.  The K split count comes from a
+// launch-time model (tc_plan, exported as lt_conv_tc_plan); split units write fp32 partial tiles that splitk_reduce_kernel sums in
+// a fixed order.
 #include "tc_common.cuh"
 #include "conv_tc_params.cuh"
 #include <stdlib.h>
@@ -31,6 +37,29 @@ namespace lt {
 // ------------------------------------------------------------------------------------------------
 constexpr int kTcThreads = 384;
 
+// Work unit u of the persistent grid: N tile fastest, so the N tiles of one M tile (which read the same A boxes) run side by side
+// in time and the A boxes are L2 hits for all but the first; then M tile; the K split z outermost.
+struct TcUnit {
+  int m, n0, z, q_begin, nchunks;
+};
+__device__ __forceinline__ TcUnit tc_unit(const TcParams& p, int u, int m_tiles, int nchunks_all) {
+  TcUnit w;
+  const int n = u % p.n_tiles;
+  u /= p.n_tiles;
+  w.m = u % m_tiles;
+  w.z = u / m_tiles;
+  w.n0 = n * p.Nt;
+  w.q_begin = (int)(((long)w.z * nchunks_all) / p.splits);
+  w.nchunks = (int)(((long)(w.z + 1) * nchunks_all) / p.splits) - w.q_begin;
+  return w;
+}
+__device__ __forceinline__ void tc_tile_origin(const TcParams& p, int t, int& ow0, int& oh0, int& od0, int& nb0) {
+  ow0 = (t % p.tw) * p.bw; t /= p.tw;
+  oh0 = (t % p.th) * p.bh; t /= p.th;
+  od0 = (t % p.td) * p.bd;
+  nb0 = (t / p.td) * p.bn;
+}
+
 template <int NT>
 __global__ void __launch_bounds__(kTcThreads, 1) conv_tc_kernel(const __grid_constant__ CUtensorMap tmA,
                                                                 const __grid_constant__ CUtensorMap tmB, const TcParams p) {
@@ -42,18 +71,9 @@ __global__ void __launch_bounds__(kTcThreads, 1) conv_tc_kernel(const __grid_con
 
   const int wg = __shfl_sync(0xffffffffu, (int)(threadIdx.x >> 7), 0);
   const int lane = threadIdx.x & 31;
-
-  // tile coordinates
-  int t = blockIdx.x;
-  const int twi = t % p.tw; t /= p.tw;
-  const int thi = t % p.th; t /= p.th;
-  const int tdi = t % p.td; t /= p.td;
-  const int tni = t;
-  const int ow0 = twi * p.bw, oh0 = thi * p.bh, od0 = tdi * p.bd, nb0 = tni * p.bn;
-  const int n0 = blockIdx.y * NT;
+  const int m_tiles = p.tw * p.th * p.td * p.tn;
+  const int units = m_tiles * p.n_tiles * p.splits;
   const int nchunks_all = p.KD * p.KH * p.KW * p.CB;
-  const int q_begin = (int)(((long)blockIdx.z * nchunks_all) / p.splits);
-  const int nchunks = (int)(((long)(blockIdx.z + 1) * nchunks_all) / p.splits) - q_begin;   // chunks of this split
 
   if (threadIdx.x == 0) {
     for (int s = 0; s < p.stages; ++s) { mbar_init(&full[s], 1); mbar_init(&empty[s], 2); }
@@ -65,25 +85,31 @@ __global__ void __launch_bounds__(kTcThreads, 1) conv_tc_kernel(const __grid_con
 
   if (wg == 0) {
     // ================= TMA producer (warp 0 runs the loop; one elected lane issues) =================
+    // The ring slot / phase run on across units: the next unit's boxes load while the consumers run the previous epilogue.
     regs_release_producer();
     if (threadIdx.x < 32) {
-      // chunk -> (tap, channel block) and ring slot / phase are advanced incrementally: no integer division in the loop
-      int tap = q_begin / p.CB, cb = q_begin - tap * p.CB;
-      int kw = tap % p.KW, kh = (tap / p.KW) % p.KH, kd = tap / (p.KW * p.KH);
       int s = 0;
       uint32_t ph = 0;
-      const int ax = ow0 * p.sw - p.pw, ay = oh0 * p.sh - p.ph, az = od0 * p.sd - p.pd, bn0 = n0 * p.b_nmul;
-      for (int q = 0, qa = q_begin; q < nchunks; ++q, ++qa) {
-        mbar_wait(&empty[s], ph ^ 1u);
-        uint8_t* a_dst = smem + (size_t)s * kStage;
-        if (elect_one()) {
-          mbar_expect_tx(&full[s], (uint32_t)kStage);
-          tma_load_5d(a_dst, &tmA, &full[s], cb * 64, ax + kw, ay + kh, az + kd, nb0);
-          tma_load_2d(a_dst + kATileBytes, &tmB, &full[s], qa * p.b_step0, qa * p.b_step1 + bn0);
+      for (int u = blockIdx.x; u < units; u += gridDim.x) {
+        const TcUnit w = tc_unit(p, u, m_tiles, nchunks_all);
+        int ow0, oh0, od0, nb0;
+        tc_tile_origin(p, w.m, ow0, oh0, od0, nb0);
+        // chunk -> (tap, channel block) advanced incrementally: no integer division in the loop
+        int tap = w.q_begin / p.CB, cb = w.q_begin - tap * p.CB;
+        int kw = tap % p.KW, kh = (tap / p.KW) % p.KH, kd = tap / (p.KW * p.KH);
+        const int ax = ow0 * p.sw - p.pw, ay = oh0 * p.sh - p.ph, az = od0 * p.sd - p.pd, bn0 = w.n0 * p.b_nmul;
+        for (int q = 0, qa = w.q_begin; q < w.nchunks; ++q, ++qa) {
+          mbar_wait(&empty[s], ph ^ 1u);
+          uint8_t* a_dst = smem + (size_t)s * kStage;
+          if (elect_one()) {
+            mbar_expect_tx(&full[s], (uint32_t)kStage);
+            tma_load_5d(a_dst, &tmA, &full[s], cb * 64, ax + kw, ay + kh, az + kd, nb0);
+            tma_load_2d(a_dst + kATileBytes, &tmB, &full[s], qa * p.b_step0, qa * p.b_step1 + bn0);
+          }
+          __syncwarp();
+          if (++cb == p.CB) { cb = 0; if (++kw == p.KW) { kw = 0; if (++kh == p.KH) { kh = 0; ++kd; } } }
+          if (++s == p.stages) { s = 0; ph ^= 1u; }
         }
-        __syncwarp();
-        if (++cb == p.CB) { cb = 0; if (++kw == p.KW) { kw = 0; if (++kh == p.KH) { kh = 0; ++kd; } } }
-        if (++s == p.stages) { s = 0; ph ^= 1u; }
       }
     }
     return;
@@ -95,11 +121,16 @@ __global__ void __launch_bounds__(kTcThreads, 1) conv_tc_kernel(const __grid_con
   float d1[NT / 2], d2[NT / 2];
 #pragma unroll
   for (int i = 0; i < NT / 2; ++i) { d1[i] = 0.f; d2[i] = 0.f; }
-  {
-    int s = 0, prev = -1;
-    uint32_t ph = 0;
-    const uint32_t ring0 = smem_u32(smem);
-    for (int q = 0; q < nchunks; ++q) {
+  // this thread holds rows r0 and r0 + 8, columns 8i + c2 (+1) of the 64 x NT warpgroup tile
+  const int r0 = g * 64 + ((threadIdx.x >> 5) & 3) * 16 + (lane >> 2);
+  const int c2 = 2 * (lane & 3);
+  const uint32_t ring0 = smem_u32(smem);
+  int s = 0;
+  uint32_t ph = 0;
+  for (int u = blockIdx.x; u < units; u += gridDim.x) {
+    const TcUnit w = tc_unit(p, u, m_tiles, nchunks_all);
+    int prev = -1;
+    for (int q = 0; q < w.nchunks; ++q) {
       mbar_wait(&full[s], ph);
       const uint32_t a_addr = ring0 + (uint32_t)(s * kStage) + (uint32_t)(g * 64 * 128);
       const uint32_t b_addr = ring0 + (uint32_t)(s * kStage) + kATileBytes;
@@ -130,36 +161,37 @@ __global__ void __launch_bounds__(kTcThreads, 1) conv_tc_kernel(const __grid_con
       if (++s == p.stages) { s = 0; ph ^= 1u; }
     }
     wg_wait<0>();
+    if (prev >= 0 && (threadIdx.x & 127) == 0) mbar_arrive_local(&empty[prev]);   // the producer refills it during the epilogue
     wg_fence_regs(d1);
     wg_fence_regs(d2);
-  }
 
-  // ---- epilogue: this thread holds rows r0 and r0 + 8, columns 8i + c2 (+1) of the 64 x NT warpgroup tile ----
-  const int r0 = g * 64 + ((threadIdx.x >> 5) & 3) * 16 + (lane >> 2);
-  const int c2 = 2 * (lane & 3);
+    // ---- epilogue ----
+    int ow0, oh0, od0, nb0;
+    tc_tile_origin(p, w.m, ow0, oh0, od0, nb0);
 #pragma unroll
-  for (int h = 0; h < 2; ++h) {
-    const int row = r0 + 8 * h;
-    if (p.splits > 1) {
-      // ---- split-K: raw accumulators to the workspace, epilogue deferred to splitk_reduce_kernel ----
-      float* wrow = p.ws + (((size_t)blockIdx.z * gridDim.x + blockIdx.x) * 128 + row) * p.ws_ld + n0;
+    for (int h = 0; h < 2; ++h) {
+      const int row = r0 + 8 * h;
+      if (p.splits > 1) {
+        // ---- split-K: raw accumulators to the workspace, epilogue deferred to splitk_reduce_kernel ----
+        float* wrow = p.ws + (((size_t)w.z * m_tiles + w.m) * 128 + row) * p.ws_ld + w.n0;
 #pragma unroll
-      for (int i = 0; i < NT / 8; ++i) {
-        const int k = 4 * i + 2 * h;
-        const float v0 = (p.terms == 3) ? fmaf(d2[k], kLoInv, d1[k]) : d1[k];
-        const float v1 = (p.terms == 3) ? fmaf(d2[k + 1], kLoInv, d1[k + 1]) : d1[k + 1];
-        *reinterpret_cast<float2*>(wrow + 8 * i + c2) = make_float2(v0, v1);
+        for (int i = 0; i < NT / 8; ++i) {
+          const int k = 4 * i + 2 * h;
+          const float v0 = (p.terms == 3) ? fmaf(d2[k], kLoInv, d1[k]) : d1[k];
+          const float v1 = (p.terms == 3) ? fmaf(d2[k + 1], kLoInv, d1[k + 1]) : d1[k + 1];
+          *reinterpret_cast<float2*>(wrow + 8 * i + c2) = make_float2(v0, v1);
+        }
+        continue;
       }
-      continue;
+      int r_ = row;
+      const int dw = r_ % p.bw; r_ /= p.bw;
+      const int dh = r_ % p.bh; r_ /= p.bh;
+      const int dd = r_ % p.bd; r_ /= p.bd;
+      const int ow = ow0 + dw, oh = oh0 + dh, od = od0 + dd, nb = nb0 + r_;
+      if (!(ow < p.OW && oh < p.OH && od < p.OD && nb < p.N)) continue;
+      const long opix = (((long)nb * p.FD + (od * p.osd + p.ood)) * p.FH + (oh * p.osh + p.ooh)) * p.FW + (ow * p.osw + p.oow);
+      conv_epilogue_row<NT>(p, d1, d2, h, opix, w.n0, c2);
     }
-    int r_ = row;
-    const int dw = r_ % p.bw; r_ /= p.bw;
-    const int dh = r_ % p.bh; r_ /= p.bh;
-    const int dd = r_ % p.bd; r_ /= p.bd;
-    const int ow = ow0 + dw, oh = oh0 + dh, od = od0 + dd, nb = nb0 + r_;
-    if (!(ow < p.OW && oh < p.OH && od < p.OD && nb < p.N)) continue;
-    const long opix = (((long)nb * p.FD + (od * p.osd + p.ood)) * p.FH + (oh * p.osh + p.ooh)) * p.FW + (ow * p.osw + p.oow);
-    conv_epilogue_row<NT>(p, d1, d2, h, opix, n0, c2);
   }
 }
 
@@ -314,6 +346,43 @@ static int launch_nt(const CUtensorMap& tmA, const CUtensorMap& tmB, const TcPar
   return LT_OK;
 }
 
+// Modelled time of one conv_tc launch (SM clocks) with the K loop split `splits` ways: every CTA of the persistent grid runs
+// ceil(units / grid) work units, each its share of the K chunks plus one epilogue; a split adds the fp32 partial tiles, which
+// splitk_reduce_kernel reads back.  Per K chunk the SM takes the larger of its MMA time (3 products: 12 m64 x Nt x k16 wgmma of
+// 64 * Nt / 128 clocks) and its operand feed from L2 (16 KB of A and Nt * 128 bytes of B at ~30 B/clk per SM).  The epilogue
+// moves 128 x Nt x 4 bytes from one SM at the same rate; the reduce pass streams its bytes over the whole GPU at ~1.5 KB/clk
+// (2.5 TB/s at 1.7 GHz) after a ~7000-clock launch.  Only the ranking of split counts matters, not the absolute values.
+static double tc_model_clocks(long tiles, int chunks, int nt, int splits, int sm) {
+  const long units = tiles * splits;
+  const long grid = units < sm ? units : sm;
+  const long waves = (units + grid - 1) / grid;
+  const double chunk = fmax(12.0 * 64.0 * nt / 128.0, (kATileBytes + nt * 128.0) / 30.0);
+  const double epilogue = 128.0 * nt * 4.0 / 30.0;
+  double t = (double)waves * ((double)ceil_div(chunks, splits) * chunk + epilogue);
+  if (splits > 1) t += 7000.0 + (double)tiles * 128 * nt * 4.0 * (splits + 2) / 1500.0;
+  return t;
+}
+
+// Work decomposition of one conv_tc launch: tiles, K split and persistent grid size (host only, no device access).  A split is
+// taken when the model above says it is faster and its partial tiles fit the workspace; `terms` 0 (plain-fp16 self test) and
+// grouped outputs never split.
+static void tc_plan(long m_tiles, int n_tiles, int nt, int chunks, int terms, int n_maps, int splitk, size_t ws_bytes, int sm,
+                    int* splits_out, int* grid_out) {
+  const long tiles = m_tiles * n_tiles;
+  int best = 1;
+  if (splitk && terms != 0 && n_maps == 1) {
+    const size_t per_split = (size_t)tiles * 128 * nt * sizeof(float);
+    double best_t = tc_model_clocks(tiles, chunks, nt, 1, sm);
+    for (int s = 2; s <= chunks / 4 && (size_t)s * per_split <= ws_bytes; ++s) {
+      const double t = tc_model_clocks(tiles, chunks, nt, s, sm);
+      if (t < best_t) { best_t = t; best = s; }
+    }
+  }
+  const long units = tiles * best;
+  *splits_out = best;
+  *grid_out = (int)(units < sm ? units : sm);
+}
+
 static int launch_tc(const CUtensorMap& tmA, const CUtensorMap& tmB, TcParams& p, int n_tiles, cudaStream_t st, void* ws = nullptr,
                      size_t ws_bytes = 0) {
   const int stage_bytes = kATileBytes + p.Nt * 128;
@@ -324,28 +393,19 @@ static int launch_tc(const CUtensorMap& tmA, const CUtensorMap& tmB, TcParams& p
   p.stages = stages;
   const size_t smem = (size_t)stages * stage_bytes + 2 * stages * 8 + 1024;
   const long m_tiles = (long)p.tw * p.th * p.td * p.tn;
-  const int nchunks_total = p.KD * p.KH * p.KW * p.CB;
-  // split-K: a grid that cannot fill half the SMs is bound by the serial K loop of each CTA (27 taps x Cin/32 chunks of
-  // weights streamed from HBM by ONE SM); spread the chunks over blockIdx.z instead
-  int splits = 1;
-  const long grid_ctas = m_tiles * n_tiles;
-  if (opts().tc_splitk && ws && p.terms != 0 && p.n_maps == 1 && grid_ctas * 2 <= (long)sm_count() && nchunks_total >= 16) {
-    splits = (int)((long)sm_count() / grid_ctas);
-    if (splits > nchunks_total / 4) splits = nchunks_total / 4;
-    const size_t per_split = (size_t)m_tiles * 128 * (size_t)n_tiles * p.Nt * sizeof(float);
-    if ((size_t)splits * per_split > ws_bytes) splits = (int)(ws_bytes / per_split);
-    if (splits < 2) splits = 1;
-  }
+  int splits, grid;
+  tc_plan(m_tiles, n_tiles, p.Nt, p.KD * p.KH * p.KW * p.CB, p.terms, p.n_maps, ws ? opts().tc_splitk : 0, ws_bytes, sm_count(),
+          &splits, &grid);
   p.splits = splits;
   p.ws = reinterpret_cast<float*>(ws);
   p.ws_ld = n_tiles * p.Nt;
-  dim3 grid((unsigned)m_tiles, (unsigned)n_tiles, (unsigned)splits);
+  p.n_tiles = n_tiles;
   int rc;
   switch (p.Nt) {
-    case 128: rc = launch_nt<128>(tmA, tmB, p, grid, smem, st); break;
-    case 64: rc = launch_nt<64>(tmA, tmB, p, grid, smem, st); break;
-    case 32: rc = launch_nt<32>(tmA, tmB, p, grid, smem, st); break;
-    case 16: rc = launch_nt<16>(tmA, tmB, p, grid, smem, st); break;
+    case 128: rc = launch_nt<128>(tmA, tmB, p, dim3(grid), smem, st); break;
+    case 64: rc = launch_nt<64>(tmA, tmB, p, dim3(grid), smem, st); break;
+    case 32: rc = launch_nt<32>(tmA, tmB, p, dim3(grid), smem, st); break;
+    case 16: rc = launch_nt<16>(tmA, tmB, p, dim3(grid), smem, st); break;
     default: return fail(LT_ERR_INVALID, "conv_tc: unsupported N tile %d", p.Nt);
   }
   if (rc) return rc;
@@ -375,7 +435,7 @@ void fill_params(const lt_conv_desc* d, TcParams& p, int CB, int CoutP, int Nt, 
   p.osd = d->osd; p.osh = d->osh; p.osw = d->osw; p.ood = d->ood; p.ooh = d->ooh; p.oow = d->oow;
   p.relu = d->relu; p.residual = d->residual; p.out_format = d->out_format;
   p.scale = scale; p.shift = shift; p.res = residual; p.out = out;
-  p.splits = 1; p.ws = nullptr; p.ws_ld = 0; p.stages = 0;
+  p.splits = 1; p.ws = nullptr; p.ws_ld = 0; p.stages = 0; p.n_tiles = 1;
   p.n_maps = out_groups(d);
   p.oc = p.n_maps > 1 ? d->Cout / p.n_maps : CoutP;
   p.gh = d->ogh > 1 ? d->ogh : 1; p.gw = d->ogw > 1 ? d->ogw : 1;
@@ -458,6 +518,21 @@ __global__ void ones_zeros_kernel(float* ones, float* zeros, int n) {
 
 using namespace lt;
 
+extern "C" int lt_conv_tc_plan(const lt_conv_desc* d, int sm_count, int splitk, lt_conv_tc_launch_plan* plan) {
+  LT_REQUIRE(d && plan && sm_count > 0, "conv_tc_plan: bad arguments");
+  LT_REQUIRE(d->Cin % 32 == 0 && d->Cout > 0, "conv_tc_plan: Cin=%d must be a multiple of 32", d->Cin);
+  const int CoutP = (d->Cout + 15) & ~15;
+  int box[4];
+  pick_box(d->OW, d->OH, d->OD, d->N, box);
+  plan->nt = pick_nt(CoutP);
+  plan->m_tiles = ceil_div(d->OW, box[0]) * ceil_div(d->OH, box[1]) * ceil_div(d->OD, box[2]) * ceil_div(d->N, box[3]);
+  plan->n_tiles = CoutP / plan->nt;
+  plan->chunks = d->KD * d->KH * d->KW * (d->Cin / 32);
+  tc_plan(plan->m_tiles, plan->n_tiles, plan->nt, plan->chunks, 3, out_groups(d), d->workspace ? splitk : 0, d->workspace_bytes,
+          sm_count, &plan->splits, &plan->grid);
+  return LT_OK;
+}
+
 extern "C" size_t lt_conv_tc_weight_bytes(int taps, int Cin, int Cout) {
   const int CoutP = (Cout + 15) & ~15;
   return (size_t)taps * (Cin / 32) * CoutP * 128;
@@ -496,6 +571,7 @@ extern "C" int lt_tc_gemm_selftest(const void* a, const void* b, float* d, int M
   p.relu = 0; p.residual = LT_RES_NONE; p.out_format = LT_FMT_F32;
   p.scale = ones; p.shift = zeros; p.res = nullptr; p.out = d;
   p.n_maps = 1; p.oc = N; p.gh = p.gw = 1;
+  p.splits = 1; p.ws = nullptr; p.ws_ld = 0; p.n_tiles = 1;
   CUtensorMap tmA, tmB;
   {
     const uint64_t dims[5] = {(uint64_t)K, (uint64_t)M, 1, 1, 1};

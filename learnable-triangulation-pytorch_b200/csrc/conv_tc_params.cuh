@@ -24,6 +24,7 @@ struct TcParams {
   // writes its raw fp32 accumulator tile to ws[z][m tile][128][ws_ld]; splitk_reduce_kernel sums and applies the epilogue
   int splits, ws_ld;
   float* ws;
+  int n_tiles;   // N tiles of Nt channels (conv_tc_kernel work units: n_tiles x M tiles x splits)
   // grouped output (lt_conv_desc.ogd/ogh/ogw): output channel block g of `oc` channels goes to output map g (its own phase offset)
   int oc, n_maps;
   int gh, gw;    // output group grid (group g -> offset (g / (gh*gw), (g / gw) % gh, g % gw)); 1, 1 without groups
@@ -35,24 +36,56 @@ constexpr int kMaxOutMaps = 8;
 
 constexpr int kATileBytes = 128 * 128;  // 128 rows x 64 fp16
 
+// Output pixel and channel of accumulator column 8i + c2 of a tile whose first output channel is n0: grouped outputs send channel
+// block mi to output phase (mi / (gh gw), (mi / gw) % gh, mi % gw).
+__device__ __forceinline__ void epilogue_target(const TcParams& p, int co, long opix, int& ch, long& pix) {
+  ch = co;
+  pix = opix;
+  if (p.n_maps > 1) {
+    const int mi = ch / p.oc;
+    ch -= mi * p.oc;
+    pix += ((long)(mi / (p.gh * p.gw)) * p.FH + (mi / p.gw) % p.gh) * p.FW + mi % p.gw;
+  }
+}
+
 // Fused epilogue of one row of a 64 x NT wgmma accumulator tile (conv_tc.cu, conv_fold.cu): this thread holds columns 8i + c2 (+1)
 // of row 16 w + l / 4 (h = 0) or the row 8 below it (h = 1), which belongs to output pixel `opix`; n0 is the tile's first output
 // channel.  Forms D1 + D2 / S (3-term products) and applies the folded scale / shift, the residual, ReLU and the store (float32 or
 // split-fp16; grouped outputs go to their phase of the output lattice).
 template <int NT>
+__device__ __forceinline__ float2 epilogue_residual(const TcParams& p, int ch, long pix) {
+  if (p.residual == LT_RES_NONE || ch >= p.FC) return make_float2(0.f, 0.f);
+  if (p.out_format == LT_FMT_F32) return *reinterpret_cast<const float2*>(reinterpret_cast<const float*>(p.res) + pix * p.FC + ch);
+  const sh_t* rp = reinterpret_cast<const sh_t*>(p.res) + pix * 2 * p.FC + s32_off(ch);
+  const float2 a = __half22float2(*reinterpret_cast<const __half2*>(rp));
+  const float2 b = __half22float2(*reinterpret_cast<const __half2*>(rp + 32));
+  return make_float2(fmaf(b.x, kLoInv, a.x), fmaf(b.y, kLoInv, a.y));
+}
+
+// Up to NT = 64 the residual of the whole row is loaded before the first store: the output may alias the residual as far as the
+// compiler knows, so loads interleaved with the stores each wait for a full memory round trip.  At NT = 128 the 32 extra registers
+// do not fit beside the 128 accumulators (measured slower on the H100), and each load stays next to its store.
+template <int NT>
 __device__ __forceinline__ void conv_epilogue_row(const TcParams& p, const float (&d1)[NT / 2], const float (&d2)[NT / 2], int h,
                                                   long opix, int n0, int c2) {
+  constexpr bool kHoist = NT <= 64;
+  float2 rr[kHoist ? NT / 8 : 1];
+  if constexpr (kHoist) {
+#pragma unroll
+    for (int i = 0; i < NT / 8; ++i) {
+      int ch;
+      long pix;
+      epilogue_target(p, n0 + 8 * i + c2, opix, ch, pix);
+      rr[i] = epilogue_residual<NT>(p, ch, pix);
+    }
+  }
 #pragma unroll
   for (int i = 0; i < NT / 8; ++i) {
     const int k = 4 * i + 2 * h;
     const int co = n0 + 8 * i + c2;
-    int ch = co;
-    long pix = opix;
-    if (p.n_maps > 1) {   // grouped output: channel block of group mi goes to output phase (mi / (gh gw), (mi / gw) % gh, mi % gw)
-      const int mi = ch / p.oc;
-      ch -= mi * p.oc;
-      pix += ((long)(mi / (p.gh * p.gw)) * p.FH + (mi / p.gw) % p.gh) * p.FW + mi % p.gw;
-    }
+    int ch;
+    long pix;
+    epilogue_target(p, co, opix, ch, pix);
     if (ch >= p.FC) continue;
     float v0 = (p.terms == 3) ? fmaf(d2[k], kLoInv, d1[k]) : d1[k];
     float v1 = (p.terms == 3) ? fmaf(d2[k + 1], kLoInv, d1[k + 1]) : d1[k + 1];
@@ -60,20 +93,10 @@ __device__ __forceinline__ void conv_epilogue_row(const TcParams& p, const float
     const float2 sh = __ldg(reinterpret_cast<const float2*>(p.shift + co));
     v0 = fmaf(v0, sc.x, sh.x);
     v1 = fmaf(v1, sc.y, sh.y);
-    float2 rr = make_float2(0.f, 0.f);
-    if (p.residual != LT_RES_NONE) {
-      if (p.out_format == LT_FMT_F32) {
-        rr = *reinterpret_cast<const float2*>(reinterpret_cast<const float*>(p.res) + pix * p.FC + ch);
-      } else {
-        const sh_t* rp = reinterpret_cast<const sh_t*>(p.res) + pix * 2 * p.FC + s32_off(ch);
-        const float2 a = __half22float2(*reinterpret_cast<const __half2*>(rp));
-        const float2 b = __half22float2(*reinterpret_cast<const __half2*>(rp + 32));
-        rr = make_float2(fmaf(b.x, kLoInv, a.x), fmaf(b.y, kLoInv, a.y));
-      }
-    }
-    if (p.residual == LT_RES_BEFORE_RELU) { v0 += rr.x; v1 += rr.y; }
+    const float2 r = kHoist ? rr[kHoist ? i : 0] : epilogue_residual<NT>(p, ch, pix);
+    if (p.residual == LT_RES_BEFORE_RELU) { v0 += r.x; v1 += r.y; }
     if (p.relu) { v0 = fmaxf(v0, 0.f); v1 = fmaxf(v1, 0.f); }
-    if (p.residual == LT_RES_AFTER_RELU) { v0 += rr.x; v1 += rr.y; }
+    if (p.residual == LT_RES_AFTER_RELU) { v0 += r.x; v1 += r.y; }
     if (p.out_format == LT_FMT_F32) {
       *reinterpret_cast<float2*>(reinterpret_cast<float*>(p.out) + pix * p.FC + ch) = make_float2(v0, v1);
     } else {
