@@ -318,6 +318,29 @@ int lt_triangulate_dlt_bwd(const float* proj, const float* keypoints_2d, const f
                            float* grad_keypoints_2d, float* grad_confidences, int B, int V, int J, void* stream);
 
 /* ------------------------------------------------------------------------------------------
+ * Volumetric cross-entropy loss of the volumetric training recipe.  Replaces VolumetricCELoss (mvn/models/loss.py:52-80, called
+ * from train.py:222-230): per (sample, joint) the voxel nearest to the ground-truth point, loss.py:68-72 (per-sample difference
+ * and distance tensors, torch.argmin, copy of the indices to the host), and v * -log(p + 1e-6) there, loss.py:74-77 (one chain
+ * of selects per (sample, joint), each of whose backward zero-fills a volume-sized gradient).
+ *   probs [B][J][nvox] (the softmaxed volumes), coord [B][nvox][3], keypoints_gt [B][J][3], validity [B][J] (element 0 of the
+ *   reference's validity vector)
+ *   loss: one float; index [B][J]: flat voxel index chosen; picked [B][J]: probs at that index (kept for the backward)
+ *   workspace: lt_volumetric_ce_workspace_bytes(B, J, nvox) bytes
+ * Exactly the reference's choice: the distance is sqrt((dx*dx + dy*dy) + dz*dz) rounded per fp32 operation (no FMA), and the
+ * rounded square roots are compared over every voxel (any coordinate volume: rotated, permuted, flipped); ties go to the smallest
+ * index, a NaN distance wins and the first NaN wins (torch.argmin).  loss = (sum over b, then j, of v * -log(p + 1e-6)) / (B * J),
+ * summed from 0 in fp32 in that order; the term is computed when v == 0 as well (a NaN propagates as in the reference).
+ * Deterministic, no host synchronisation.  nvox < 2^31. */
+size_t lt_volumetric_ce_workspace_bytes(int B, int J, long nvox);
+int lt_volumetric_ce_fwd(const float* probs, const float* coord, const float* keypoints_gt, const float* validity, float* loss,
+                         int* index, float* picked, void* workspace, size_t workspace_bytes, int B, int J, long nvox, void* stream);
+/* Backward of lt_volumetric_ce_fwd, what autograd derives through loss.py:76,80: grad_loss is a DEVICE pointer to dL/dloss;
+ * grad_probs [B][J][nvox] is WRITTEN in full: -((g / (B * J)) * v) / (p + 1e-6) at index[b][j], 0 everywhere else.  Coordinates,
+ * ground truth and validity get no gradient (the reference's argmin is detached; they are data). */
+int lt_volumetric_ce_bwd(const float* grad_loss, const int* index, const float* picked, const float* validity, float* grad_probs,
+                         int B, int J, long nvox, void* stream);
+
+/* ------------------------------------------------------------------------------------------
  * Layout / format helpers.
  * ---------------------------------------------------------------------------------------- */
 /* images [N][C][H][W] float32 -> [N][H][W][Cp] float32, channels >= C zero filled */
@@ -357,6 +380,10 @@ int lt_test_softargmax3d_bwd_host(const float* probs, const float* coord, const 
                                   float* grad_logits, int B, int J, long nvox, float multiplier, int softmax);
 int lt_test_triangulate_dlt_bwd_host(const float* proj, const float* keypoints_2d, const float* confidences, const float* grad_out,
                                      float* grad_keypoints_2d, float* grad_confidences, int B, int V, int J);
+/* lt_volumetric_ce_fwd (+ lt_volumetric_ce_bwd when grad_probs is not NULL, grad_loss then a HOST pointer) on host pointers, with
+ * the kernels' distance, argmin key, term and gradient code: loss.py:52-80. */
+int lt_test_volumetric_ce_host(const float* probs, const float* coord, const float* keypoints_gt, const float* validity, float* loss,
+                               int* index, float* picked, const float* grad_loss, float* grad_probs, int B, int J, long nvox);
 
 #ifdef __cplusplus
 }

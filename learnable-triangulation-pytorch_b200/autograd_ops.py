@@ -150,6 +150,41 @@ class TriangulateDltFn(torch.autograd.Function):
         return None, (grad_kp if ctx.needs_input_grad[1] else None), grad_conf
 
 
+class VolumetricCEFn(torch.autograd.Function):
+    """VolumetricCELoss (reference loss.py:52-80) on csrc/loss.cu: probs (B, J, nvox), coord (B, nvox, 3), keypoints_gt (B, J, 3),
+    validity (B, J), all float32 CUDA -> 0-dim loss.  Only the volumes get a gradient: the reference's argmin is detached, and the
+    coordinates, ground truth and validity are data."""
+
+    @staticmethod
+    def forward(ctx, probs, coord, keypoints_gt, validity):
+        B, J, nvox = probs.shape
+        dev = probs.device
+        p = probs.detach().contiguous()
+        v = validity.detach().contiguous()
+        loss = torch.empty(1, dtype=torch.float32, device=dev)
+        index = torch.empty((B, J), dtype=torch.int32, device=dev)
+        picked = torch.empty((B, J), dtype=torch.float32, device=dev)
+        ws = torch.empty(capi.volumetric_ce_workspace_bytes(B, J, nvox), dtype=torch.uint8, device=dev)
+        capi.volumetric_ce(p, coord.detach().contiguous(), keypoints_gt.detach().contiguous(), v, loss, index, picked, ws)
+        ctx.save_for_backward(index, picked, v)
+        ctx.nvox = nvox
+        ctx.mark_non_differentiable(index, picked)
+        return loss.reshape(()), index, picked
+
+    @staticmethod
+    def backward(ctx, grad_loss, grad_index, grad_picked):
+        index, picked, v = ctx.saved_tensors
+        B, J = index.shape
+        grad = torch.empty((B, J, ctx.nvox), dtype=torch.float32, device=index.device)
+        capi.volumetric_ce_bwd(grad_loss.float().reshape(1).contiguous(), index, picked, v, grad)
+        return grad, None, None, None
+
+
+def volumetric_ce_loss(probs, coord, keypoints_gt, validity):
+    """-> (0-dim loss, index (B, J) int32, picked (B, J)); probs etc. as VolumetricCEFn."""
+    return VolumetricCEFn.apply(probs, coord, keypoints_gt, validity)
+
+
 def integrate_tensor_2d(heatmaps, softmax=True):
     return IntegrateTensor2dFn.apply(heatmaps, softmax)
 

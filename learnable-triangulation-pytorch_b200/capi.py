@@ -92,6 +92,10 @@ SIGNATURES = {
     "lt_triangulate_dlt_fwd": (c_int, [c_void_p] * 4 + [c_int] * 3 + [c_void_p]),
     "lt_triangulate_dlt_bwd": (c_int, [c_void_p] * 6 + [c_int] * 3 + [c_void_p]),
     "lt_test_triangulate_dlt_bwd_host": (c_int, [c_void_p] * 6 + [c_int] * 3),
+    "lt_volumetric_ce_workspace_bytes": (c_size_t, [c_int, c_int, c_long]),
+    "lt_volumetric_ce_fwd": (c_int, [c_void_p] * 8 + [c_size_t, c_int, c_int, c_long, c_void_p]),
+    "lt_volumetric_ce_bwd": (c_int, [c_void_p] * 5 + [c_int, c_int, c_long, c_void_p]),
+    "lt_test_volumetric_ce_host": (c_int, [c_void_p] * 9 + [c_int, c_int, c_long]),
     "lt_nchw_to_nhwc_f32": (c_int, [c_void_p, c_void_p] + [c_int] * 5 + [c_void_p]),
     "lt_images_hwc_to_nchw_fwd": (c_int, [c_void_p, c_int, c_void_p, c_void_p] + [c_int] * 4 + [c_void_p]),
     "lt_stem_s2d_fwd": (c_int, [c_void_p, c_void_p] + [c_int] * 4 + [c_void_p]),
@@ -345,11 +349,45 @@ def triangulate_dlt_bwd(proj, kp2d, conf, grad_out, grad_kp2d, grad_conf):
                                         _stream()), "lt_triangulate_dlt_bwd")
 
 
+def volumetric_ce_workspace_bytes(B, J, nvox):
+    return lib().lt_volumetric_ce_workspace_bytes(B, J, nvox)
+
+
+def volumetric_ce(probs, coord, keypoints_gt, validity, loss, index, picked, workspace):
+    """probs (B, J, nvox), coord (B, nvox, 3), keypoints_gt (B, J, 3), validity (B, J) float32 -> loss (1,) float32,
+    index (B, J) int32, picked (B, J) float32."""
+    B, J, nvox = probs.shape
+    _check(lib().lt_volumetric_ce_fwd(_ptr(probs), _ptr(coord), _ptr(keypoints_gt), _ptr(validity), _ptr(loss), _ptr(index), _ptr(picked),
+                                      _ptr(workspace), workspace.numel() * workspace.element_size(), B, J, nvox, _stream()),
+           "lt_volumetric_ce_fwd")
+
+
+def volumetric_ce_bwd(grad_loss, index, picked, validity, grad_probs):
+    """grad_loss: one float32 on the device; grad_probs (B, J, nvox) is written in full."""
+    B, J, nvox = grad_probs.shape
+    _check(lib().lt_volumetric_ce_bwd(_ptr(grad_loss), _ptr(index), _ptr(picked), _ptr(validity), _ptr(grad_probs), B, J, nvox, _stream()),
+           "lt_volumetric_ce_bwd")
+
+
 def _host_ptr(t):
     if t is None:
         return None
     assert not t.is_cuda and t.is_contiguous() and t.dtype == torch.float32, "test hooks need contiguous float32 CPU tensors"
     return t.data_ptr()
+
+
+def volumetric_ce_host(probs, coord, keypoints_gt, validity, grad_loss=None, grad_probs=None):
+    """lt_test_volumetric_ce_host: the loss kernels' per-voxel, per-term and gradient code run on CPU tensors (test hook, no GPU
+    needed).  Returns (loss float, index (B, J) int32, picked (B, J)); grad_probs (B, J, nvox), if given, is written."""
+    B, J, nvox = probs.shape
+    loss = torch.empty(1, dtype=torch.float32)
+    index = torch.empty((B, J), dtype=torch.int32)
+    picked = torch.empty((B, J), dtype=torch.float32)
+    g = None if grad_loss is None else torch.tensor([float(grad_loss)], dtype=torch.float32)
+    _check(lib().lt_test_volumetric_ce_host(_host_ptr(probs), _host_ptr(coord), _host_ptr(keypoints_gt), _host_ptr(validity),
+                                            _host_ptr(loss), index.data_ptr(), _host_ptr(picked), _host_ptr(g), _host_ptr(grad_probs),
+                                            B, J, nvox), "lt_test_volumetric_ce_host")
+    return float(loss[0]), index, picked
 
 
 def triangulate_dlt_bwd_host(proj, kp2d, conf, grad_out, grad_kp2d, grad_conf):

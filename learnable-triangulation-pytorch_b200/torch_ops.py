@@ -87,6 +87,24 @@ def integrate_tensor_2d(heatmaps, softmax=True):
     return torch.cat((x, y), dim=2), hm
 
 
+def volumetric_ce_index(coord_volumes, keypoints_gt):
+    """(B, J) flat index of the voxel nearest to each ground-truth point: the distances and torch.argmin of loss.py:68-71, for all
+    samples at once and without copying the indices to the host."""
+    B = coord_volumes.shape[0]
+    dists = torch.sqrt(((coord_volumes.reshape(B, 1, -1, 3) - keypoints_gt.unsqueeze(2)) ** 2).sum(-1))   # (B, J, nvox)
+    return torch.argmin(dists, dim=-1)
+
+
+def volumetric_ce_loss(coord_volumes_batch, volumes_batch_pred, keypoints_gt, keypoints_binary_validity):
+    """Same contract as reference loss.py:52-80 (VolumetricCELoss.forward), vectorised: one argmin over (B, J, nvox), one gather,
+    one sum; no host synchronisation."""
+    B, J = volumes_batch_pred.shape[:2]
+    index = volumetric_ce_index(coord_volumes_batch.detach(), keypoints_gt.detach())
+    p = volumes_batch_pred.reshape(B, J, -1).gather(2, index.unsqueeze(-1)).squeeze(-1)
+    terms = keypoints_binary_validity[..., 0] * (-torch.log(p + 1e-6))
+    return terms.sum() / (B * J)
+
+
 def triangulate_batch_of_points(proj_matricies_batch, points_batch, confidences_batch=None):
     """Weighted DLT, batched (reference multiview.py:141-183 loops over samples and joints and calls torch.svd each time)."""
     B, V, J = points_batch.shape[:3]
