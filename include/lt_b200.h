@@ -219,7 +219,9 @@ typedef struct lt_conv_desc {
 } lt_conv_desc;
 
 /* SIMT weights: float32 [KD*KH*KW][Cin][CoutW], CoutW = round_up(Cout, 4), zero padded.
- * TC weights: see lt_conv_tc_pack_weights. */
+ * TC weights: see lt_conv_tc_pack_weights.
+ * LT_CONV_TC / TC1: `out` and `residual` must be 16-byte aligned and FC % 4 == 0 (the epilogue reads and writes them with TMA);
+ * LT_ERR_INVALID otherwise. */
 int lt_conv_nd_fwd(const lt_conv_desc* desc, const void* in, const void* weight, const float* scale,
                    const float* shift, const void* residual, void* out, int impl, void* stream);
 

@@ -1,7 +1,7 @@
 // Tensor-core implicit-GEMM convolution for sm_90a: TMA-staged channels-last tiles -> shared memory (128B swizzle) ->
 // wgmma (m64 x Nt x k16 per warpgroup, fp16 in, fp32 accumulators in registers) -> epilogue with folded-BN scale/shift,
-// residual, ReLU and strided channels-last store straight from the accumulator registers (plain conv, stride-phase
-// transposed conv, grouped outputs).
+// residual and ReLU staged in shared memory: the residual tile arrives and the output tile leaves by TMA (plain conv,
+// stride-phase transposed conv, grouped outputs).
 //
 // GEMM view:  M = output positions (tile = a bw x bh x bd x bn box of 128 positions),
 //             N = output channels (tile Nt = 16 / 32 / 64 / 128), K = taps x Cin.
@@ -16,9 +16,16 @@
 // Weights: [tap][Cin/32][CoutP rows][32 hi | 32 lo] fp16 (128-byte rows), so the K slices of both operands are descriptor offsets
 // (+0, +2 hi; +4, +6 lo, in 16-byte units).
 //
-// Warp roles (384 threads): warpgroup 0 = TMA producer (one warp issues), warpgroups 1 and 2 = MMA + epilogue for rows 0-63 and
-// 64-127 of the M tile.  The operand ring is released per stage by one arrival of each consumer warpgroup once its MMAs that read
-// the stage have completed (wgmma.wait_group 1 keeps one chunk of MMAs in flight behind the issue).
+// Warp roles (384 threads): warpgroup 0 = TMA producers (warp 0 fills the operand ring, warp 1 owns the epilogue buffer),
+// warpgroups 1 and 2 = MMA + epilogue for rows 0-63 and 64-127 of the M tile.  The operand ring is released per stage by one
+// arrival of each consumer warpgroup once its MMAs that read the stage have completed (wgmma.wait_group 1 keeps one chunk of MMAs
+// in flight behind the issue).
+//
+// Epilogue: stored straight from the accumulators, each residual load of a 128-channel tile would wait behind the previous store
+// (the output may alias the residual): 32 dependent memory round trips per unit with the tensor cores idle.  So warp 1 TMA-loads
+// the unit's residual tile into a shared-memory buffer while the K loop runs, the consumers turn it into the output tile in place
+// with shared-memory accesses only, and warp 1 TMA-stores it while the next unit's K loop runs.  Warp 0 never waits on that
+// buffer.  16-channel tiles (half a 32-channel slab) keep the register store.
 //
 // Persistent grid: min(work units, SMs) CTAs stride over the work units (M tile x N tile x K split, N tile fastest).  Producer and
 // consumers keep one ring across unit boundaries, so the next unit's first boxes load while the consumers run the epilogue; on the
@@ -60,14 +67,37 @@ __device__ __forceinline__ void tc_tile_origin(const TcParams& p, int t, int& ow
   nb0 = (t / p.td) * p.bn;
 }
 
+// The epilogue tile buffer: per 32 output channels one 16 KB slab of 128 rows (M-tile positions) x 128 bytes, [32 hi | 32 lo]
+// fp16 or 32 fp32, 128-byte swizzled like the A box.  Units of a launch without K split and with whole slabs use it.
+constexpr int kSlabBytes = 128 * 128;
+__host__ __device__ constexpr int tc_epi_bytes(int nt, int splits) { return (nt >= 32 && splits == 1) ? nt / 32 * kSlabBytes : 0; }
+
+// map index and box channel coordinate of the slab that starts at GEMM column co (a multiple of 32)
+__device__ __forceinline__ void epi_slab(const TcParams& p, int co, int& g, int& c) {
+  g = p.n_maps > 1 ? co / p.oc : 0;
+  const int ch = co - g * p.oc;
+  c = p.out_format == LT_FMT_F32 ? ch : 2 * ch;
+}
+
+// byte offset of byte b of row `row` in a 128-byte-swizzled slab (16-byte chunk j of row r sits at chunk j ^ (r % 8))
+__device__ __forceinline__ uint32_t sw128(int row, int b) {
+  return (uint32_t)(row * 128 + ((((b >> 4) ^ row) & 7) << 4) + (b & 15));
+}
+
 template <int NT>
 __global__ void __launch_bounds__(kTcThreads, 1) conv_tc_kernel(const __grid_constant__ CUtensorMap tmA,
-                                                                const __grid_constant__ CUtensorMap tmB, const TcParams p) {
+                                                                const __grid_constant__ CUtensorMap tmB,
+                                                                const __grid_constant__ TcEpiMaps tmE, const TcParams p) {
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
   constexpr int kStage = kATileBytes + NT * 128;
-  uint64_t* full = reinterpret_cast<uint64_t*>(smem + (size_t)p.stages * kStage);
+  const int epi_bytes = tc_epi_bytes(NT, p.splits);
+  const bool staged = epi_bytes > 0;
+  uint8_t* ebuf = smem + (size_t)p.stages * kStage;
+  uint64_t* full = reinterpret_cast<uint64_t*>(ebuf + epi_bytes);
   uint64_t* empty = full + p.stages;
+  uint64_t* efull = empty + p.stages;   // the epilogue buffer is free and holds the unit's residual
+  uint64_t* edone = efull + 1;          // both consumer warpgroups wrote the unit's output into it
 
   const int wg = __shfl_sync(0xffffffffu, (int)(threadIdx.x >> 7), 0);
   const int lane = threadIdx.x & 31;
@@ -77,6 +107,8 @@ __global__ void __launch_bounds__(kTcThreads, 1) conv_tc_kernel(const __grid_con
 
   if (threadIdx.x == 0) {
     for (int s = 0; s < p.stages; ++s) { mbar_init(&full[s], 1); mbar_init(&empty[s], 2); }
+    mbar_init(efull, 1);
+    mbar_init(edone, 256);
     fence_barrier_init();
     prefetch_tmap(&tmA);
     prefetch_tmap(&tmB);
@@ -84,9 +116,39 @@ __global__ void __launch_bounds__(kTcThreads, 1) conv_tc_kernel(const __grid_con
   __syncthreads();
 
   if (wg == 0) {
+    regs_release_producer();
+    if (staged && threadIdx.x == 32) {
+      // ================= epilogue buffer (warp 1, one lane): residual tile in, output tile out =================
+      // The residual load of unit u overlaps its K loop; its store overlaps the K loop of the next unit.
+      uint32_t eph = 0;
+      for (int u = blockIdx.x; u < units; u += gridDim.x) {
+        const TcUnit w = tc_unit(p, u, m_tiles, nchunks_all);
+        int ow0, oh0, od0, nb0;
+        tc_tile_origin(p, w.m, ow0, oh0, od0, nb0);
+        bulk_wait_read0();                      // the previous unit's store has read the buffer
+        if (p.residual != LT_RES_NONE) {
+          mbar_expect_tx(efull, (uint32_t)epi_bytes);   // out-of-range positions and channels arrive as zeros
+          for (int sl = 0; sl < NT / 32; ++sl) {
+            int g, c;
+            epi_slab(p, w.n0 + 32 * sl, g, c);
+            tma_load_5d(ebuf + sl * kSlabBytes, &tmE.res[g], efull, c, ow0, oh0, od0, nb0);
+          }
+        } else {
+          mbar_arrive_local(efull);
+        }
+        mbar_wait(edone, eph);
+        eph ^= 1u;
+        for (int sl = 0; sl < NT / 32; ++sl) {  // clipped at the edges of the output grid and at FC
+          int g, c;
+          epi_slab(p, w.n0 + 32 * sl, g, c);
+          tma_store_5d(&tmE.out[g], ebuf + sl * kSlabBytes, c, ow0, oh0, od0, nb0);
+        }
+        bulk_commit();
+      }
+      bulk_wait0();
+    }
     // ================= TMA producer (warp 0 runs the loop; one elected lane issues) =================
     // The ring slot / phase run on across units: the next unit's boxes load while the consumers run the previous epilogue.
-    regs_release_producer();
     if (threadIdx.x < 32) {
       int s = 0;
       uint32_t ph = 0;
@@ -126,7 +188,7 @@ __global__ void __launch_bounds__(kTcThreads, 1) conv_tc_kernel(const __grid_con
   const int c2 = 2 * (lane & 3);
   const uint32_t ring0 = smem_u32(smem);
   int s = 0;
-  uint32_t ph = 0;
+  uint32_t ph = 0, eph = 0;
   for (int u = blockIdx.x; u < units; u += gridDim.x) {
     const TcUnit w = tc_unit(p, u, m_tiles, nchunks_all);
     int prev = -1;
@@ -166,14 +228,11 @@ __global__ void __launch_bounds__(kTcThreads, 1) conv_tc_kernel(const __grid_con
     wg_fence_regs(d2);
 
     // ---- epilogue ----
-    int ow0, oh0, od0, nb0;
-    tc_tile_origin(p, w.m, ow0, oh0, od0, nb0);
+    if (p.splits > 1) {
+      // ---- split-K: raw accumulators to the workspace, epilogue deferred to splitk_reduce_kernel ----
 #pragma unroll
-    for (int h = 0; h < 2; ++h) {
-      const int row = r0 + 8 * h;
-      if (p.splits > 1) {
-        // ---- split-K: raw accumulators to the workspace, epilogue deferred to splitk_reduce_kernel ----
-        float* wrow = p.ws + (((size_t)w.z * m_tiles + w.m) * 128 + row) * p.ws_ld + w.n0;
+      for (int h = 0; h < 2; ++h) {
+        float* wrow = p.ws + (((size_t)w.z * m_tiles + w.m) * 128 + r0 + 8 * h) * p.ws_ld + w.n0;
 #pragma unroll
         for (int i = 0; i < NT / 8; ++i) {
           const int k = 4 * i + 2 * h;
@@ -181,16 +240,93 @@ __global__ void __launch_bounds__(kTcThreads, 1) conv_tc_kernel(const __grid_con
           const float v1 = (p.terms == 3) ? fmaf(d2[k + 1], kLoInv, d1[k + 1]) : d1[k + 1];
           *reinterpret_cast<float2*>(wrow + 8 * i + c2) = make_float2(v0, v1);
         }
-        continue;
       }
-      int r_ = row;
-      const int dw = r_ % p.bw; r_ /= p.bw;
-      const int dh = r_ % p.bh; r_ /= p.bh;
-      const int dd = r_ % p.bd; r_ /= p.bd;
-      const int ow = ow0 + dw, oh = oh0 + dh, od = od0 + dd, nb = nb0 + r_;
-      if (!(ow < p.OW && oh < p.OH && od < p.OD && nb < p.N)) continue;
-      const long opix = (((long)nb * p.FD + (od * p.osd + p.ood)) * p.FH + (oh * p.osh + p.ooh)) * p.FW + (ow * p.osw + p.oow);
-      conv_epilogue_row<NT>(p, d1, d2, h, opix, w.n0, c2);
+      continue;
+    }
+    if constexpr (NT >= 32) {
+      // ---- staged: the residual comes from and the output goes to the epilogue buffer; warp 1 moves both with TMA ----
+      // The arithmetic is conv_epilogue_row's.  A thread's residual and output elements share their addresses.
+      mbar_wait(efull, eph);
+      eph ^= 1u;
+      const uint32_t e0 = smem_u32(ebuf);
+      // Column group i + 1's scale and shift load while group i is processed: the compiler does not move loads across the
+      // shared-memory accesses (volatile asm), so a load issued in its own iteration would wait a full L1 round trip.
+      auto fc_ok = [&](int co) {
+        int ch;
+        long pix;
+        epilogue_target(p, co, 0, ch, pix);
+        return ch < p.FC;
+      };
+      float2 sc = make_float2(0.f, 0.f), sh = sc;
+      if (fc_ok(w.n0 + c2)) {
+        sc = __ldg(reinterpret_cast<const float2*>(p.scale + w.n0 + c2));
+        sh = __ldg(reinterpret_cast<const float2*>(p.shift + w.n0 + c2));
+      }
+#pragma unroll
+      for (int i = 0; i < NT / 8; ++i) {
+        const int co = w.n0 + 8 * i + c2;
+        const bool ok = fc_ok(co);
+        float2 sc_next = sc, sh_next = sh;
+        if (i + 1 < NT / 8 && fc_ok(co + 8)) {
+          sc_next = __ldg(reinterpret_cast<const float2*>(p.scale + co + 8));
+          sh_next = __ldg(reinterpret_cast<const float2*>(p.shift + co + 8));
+        }
+        const uint32_t slab = e0 + (uint32_t)((i >> 2) * kSlabBytes);
+        const int cc = 8 * (i & 3) + c2;   // column in the slab
+#pragma unroll
+        for (int h = 0; h < 2 && ok; ++h) {
+          const int row = r0 + 8 * h;
+          const int k = 4 * i + 2 * h;
+          float v0 = (p.terms == 3) ? fmaf(d2[k], kLoInv, d1[k]) : d1[k];
+          float v1 = (p.terms == 3) ? fmaf(d2[k + 1], kLoInv, d1[k + 1]) : d1[k + 1];
+          v0 = fmaf(v0, sc.x, sh.x);
+          v1 = fmaf(v1, sc.y, sh.y);
+          if (p.out_format == LT_FMT_F32) {
+            const uint32_t a = slab + sw128(row, 4 * cc);
+            float2 r = make_float2(0.f, 0.f);
+            if (p.residual != LT_RES_NONE) r = lds_f2(a);
+            if (p.residual == LT_RES_BEFORE_RELU) { v0 += r.x; v1 += r.y; }
+            if (p.relu) { v0 = fmaxf(v0, 0.f); v1 = fmaxf(v1, 0.f); }
+            if (p.residual == LT_RES_AFTER_RELU) { v0 += r.x; v1 += r.y; }
+            sts_f2(a, make_float2(v0, v1));
+          } else {
+            const uint32_t ahi = slab + sw128(row, 2 * cc), alo = slab + sw128(row, 64 + 2 * cc);
+            float2 r = make_float2(0.f, 0.f);
+            if (p.residual != LT_RES_NONE) {
+              const uint32_t rh = lds32(ahi), rl = lds32(alo);
+              const float2 a = __half22float2(*reinterpret_cast<const __half2*>(&rh));
+              const float2 b = __half22float2(*reinterpret_cast<const __half2*>(&rl));
+              r = make_float2(fmaf(b.x, kLoInv, a.x), fmaf(b.y, kLoInv, a.y));
+            }
+            if (p.residual == LT_RES_BEFORE_RELU) { v0 += r.x; v1 += r.y; }
+            if (p.relu) { v0 = fmaxf(v0, 0.f); v1 = fmaxf(v1, 0.f); }
+            if (p.residual == LT_RES_AFTER_RELU) { v0 += r.x; v1 += r.y; }
+            uint32_t hi2, lo2;
+            split_s32x2(v0, v1, hi2, lo2);
+            sts32(ahi, hi2);
+            sts32(alo, lo2);
+          }
+        }
+        sc = sc_next;
+        sh = sh_next;
+      }
+      fence_proxy_async();   // the generic-proxy writes become visible to the TMA store
+      mbar_arrive_local(edone);
+    } else {
+      // ---- 16-channel tiles (half a slab): fused epilogue straight from the accumulator registers ----
+      int ow0, oh0, od0, nb0;
+      tc_tile_origin(p, w.m, ow0, oh0, od0, nb0);
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        int r_ = r0 + 8 * h;
+        const int dw = r_ % p.bw; r_ /= p.bw;
+        const int dh = r_ % p.bh; r_ /= p.bh;
+        const int dd = r_ % p.bd; r_ /= p.bd;
+        const int ow = ow0 + dw, oh = oh0 + dh, od = od0 + dd, nb = nb0 + r_;
+        if (!(ow < p.OW && oh < p.OH && od < p.OD && nb < p.N)) continue;
+        const long opix = (((long)nb * p.FD + (od * p.osd + p.ood)) * p.FH + (oh * p.osh + p.ooh)) * p.FW + (ow * p.osw + p.oow);
+        conv_epilogue_row<NT>(p, d1, d2, h, opix, w.n0, c2);
+      }
     }
   }
 }
@@ -334,13 +470,14 @@ static int pick_nt(int CoutP) {
 }
 
 template <int NT>
-static int launch_nt(const CUtensorMap& tmA, const CUtensorMap& tmB, const TcParams& p, dim3 grid, size_t smem, cudaStream_t st) {
+static int launch_nt(const CUtensorMap& tmA, const CUtensorMap& tmB, const TcEpiMaps& tmE, const TcParams& p, dim3 grid, size_t smem,
+                     cudaStream_t st) {
   static DeviceOnce configured;
   if (configured.first()) {
     cudaError_t e = cudaFuncSetAttribute(conv_tc_kernel<NT>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(227 * 1024));
     if (e != cudaSuccess) return fail(LT_ERR_CUDA, "conv_tc: cudaFuncSetAttribute: %s", cudaGetErrorString(e));
   }
-  conv_tc_kernel<NT><<<grid, kTcThreads, smem, st>>>(tmA, tmB, p);
+  conv_tc_kernel<NT><<<grid, kTcThreads, smem, st>>>(tmA, tmB, tmE, p);
   cudaError_t e = cudaGetLastError();
   if (e != cudaSuccess) return fail(LT_ERR_CUDA, "conv_tc_kernel: %s", cudaGetErrorString(e));
   return LT_OK;
@@ -383,15 +520,33 @@ static void tc_plan(long m_tiles, int n_tiles, int nt, int chunks, int terms, in
   *grid_out = (int)(units < sm ? units : sm);
 }
 
+// Tensor maps of the staged epilogue.  Output position (ow, oh, od, nb) of group g is row ((nb FD + od osd + ood) FH + oh osh + ooh)
+// FW + ow osw + oow of the channels-last tensor plus the group's phase offset, so every output is a plain map over the launch's
+// OW x OH x OD x N grid: base at the (phase) origin, position strides scaled by osw / osh / osd.  Rows are FC x 4 bytes in both
+// formats (the C ABI requires FC % 4 == 0, so they are 16-byte multiples).
+static int make_epi_maps(const TcParams& p, TcEpiMaps* m) {
+  const int f32 = p.out_format == LT_FMT_F32;
+  const uint64_t rowb = (uint64_t)p.FC * 4;
+  const uint64_t dims[5] = {(uint64_t)(f32 ? p.FC : 2 * p.FC), (uint64_t)p.OW, (uint64_t)p.OH, (uint64_t)p.OD, (uint64_t)p.N};
+  const uint64_t str[4] = {rowb * p.osw, rowb * p.FW * p.osh, rowb * p.FW * p.FH * p.osd, rowb * p.FW * p.FH * p.FD};
+  const uint32_t bx[5] = {f32 ? 32u : 64u, (uint32_t)p.bw, (uint32_t)p.bh, (uint32_t)p.bd, (uint32_t)p.bn};
+  for (int g = 0; g < p.n_maps; ++g) {
+    const long pix0 = ((long)(p.ood + g / (p.gh * p.gw)) * p.FH + p.ooh + (g / p.gw) % p.gh) * p.FW + p.oow + g % p.gw;
+    int rc = make_map(&m->out[g], static_cast<const uint8_t*>(p.out) + pix0 * rowb, 5, dims, str, bx, nullptr, 1, f32);
+    if (rc) return rc;
+    if (p.residual == LT_RES_NONE) continue;
+    rc = make_map(&m->res[g], static_cast<const uint8_t*>(p.res) + pix0 * rowb, 5, dims, str, bx, nullptr, 1, f32);
+    if (rc) return rc;
+  }
+  return LT_OK;
+}
+
+// one CTA per SM (the two consumer warpgroups hold up to 128 fp32 accumulators per thread): the shared memory beside the epilogue
+// buffer is pipeline depth (N tile 128: 5 stages beside the 64 KB buffer)
+constexpr int kTcSmemBudget = 224 * 1024;
+
 static int launch_tc(const CUtensorMap& tmA, const CUtensorMap& tmB, TcParams& p, int n_tiles, cudaStream_t st, void* ws = nullptr,
                      size_t ws_bytes = 0) {
-  const int stage_bytes = kATileBytes + p.Nt * 128;
-  // one CTA per SM (the two consumer warpgroups hold up to 128 fp32 accumulators per thread): the whole shared memory is
-  // pipeline depth
-  int stages = (200 * 1024) / stage_bytes;
-  if (stages > 8) stages = 8;
-  p.stages = stages;
-  const size_t smem = (size_t)stages * stage_bytes + 2 * stages * 8 + 1024;
   const long m_tiles = (long)p.tw * p.th * p.td * p.tn;
   int splits, grid;
   tc_plan(m_tiles, n_tiles, p.Nt, p.KD * p.KH * p.KW * p.CB, p.terms, p.n_maps, ws ? opts().tc_splitk : 0, ws_bytes, sm_count(),
@@ -400,12 +555,23 @@ static int launch_tc(const CUtensorMap& tmA, const CUtensorMap& tmB, TcParams& p
   p.ws = reinterpret_cast<float*>(ws);
   p.ws_ld = n_tiles * p.Nt;
   p.n_tiles = n_tiles;
+  const int stage_bytes = kATileBytes + p.Nt * 128;
+  const int epi_bytes = tc_epi_bytes(p.Nt, splits);
+  int stages = (kTcSmemBudget - epi_bytes) / stage_bytes;
+  if (stages > 8) stages = 8;
+  p.stages = stages;
+  const size_t smem = (size_t)stages * stage_bytes + epi_bytes + (2 * stages + 2) * 8 + 1024;
+  TcEpiMaps tmE{};
   int rc;
+  if (epi_bytes) {
+    rc = make_epi_maps(p, &tmE);
+    if (rc) return rc;
+  }
   switch (p.Nt) {
-    case 128: rc = launch_nt<128>(tmA, tmB, p, dim3(grid), smem, st); break;
-    case 64: rc = launch_nt<64>(tmA, tmB, p, dim3(grid), smem, st); break;
-    case 32: rc = launch_nt<32>(tmA, tmB, p, dim3(grid), smem, st); break;
-    case 16: rc = launch_nt<16>(tmA, tmB, p, dim3(grid), smem, st); break;
+    case 128: rc = launch_nt<128>(tmA, tmB, tmE, p, dim3(grid), smem, st); break;
+    case 64: rc = launch_nt<64>(tmA, tmB, tmE, p, dim3(grid), smem, st); break;
+    case 32: rc = launch_nt<32>(tmA, tmB, tmE, p, dim3(grid), smem, st); break;
+    case 16: rc = launch_nt<16>(tmA, tmB, tmE, p, dim3(grid), smem, st); break;
     default: return fail(LT_ERR_INVALID, "conv_tc: unsupported N tile %d", p.Nt);
   }
   if (rc) return rc;
@@ -468,6 +634,8 @@ int conv_tc_fwd_terms(const lt_conv_desc* d, const void* in, const void* weight,
   LT_REQUIRE(d->in_format == LT_FMT_S32, "conv_tc: input must be split-fp16");
   LT_REQUIRE(d->Cin % 32 == 0, "conv_tc: Cin=%d must be a multiple of 32", d->Cin);
   LT_REQUIRE(d->FC % 4 == 0 && (d->out_format == LT_FMT_F32 || d->FC % 32 == 0), "conv_tc: bad output channel stride %d", d->FC);
+  LT_REQUIRE((reinterpret_cast<uintptr_t>(out) | reinterpret_cast<uintptr_t>(residual)) % 16 == 0,
+             "conv_tc: out and residual must be 16-byte aligned (TMA global addresses)");
   const int CoutP = (d->Cout + 15) & ~15;
   const int CB = d->Cin / 32;
   const int taps = d->KD * d->KH * d->KW;

@@ -34,6 +34,13 @@ struct TcParams {
 // the output lattice
 constexpr int kMaxOutMaps = 8;
 
+// Tensor maps of conv_tc_kernel's staged epilogue, one per output group (only [0] without groups): the output and the residual
+// over the launch's OW x OH x OD x N output grid (stride-phase outputs: the phase's sub-lattice), boxes of 32 channels x the M tile.
+struct TcEpiMaps {
+  CUtensorMap out[kMaxOutMaps];
+  CUtensorMap res[kMaxOutMaps];
+};
+
 constexpr int kATileBytes = 128 * 128;  // 128 rows x 64 fp16
 
 // Output pixel and channel of accumulator column 8i + c2 of a tile whose first output channel is n0: grouped outputs send channel
@@ -62,22 +69,20 @@ __device__ __forceinline__ float2 epilogue_residual(const TcParams& p, int ch, l
   return make_float2(fmaf(b.x, kLoInv, a.x), fmaf(b.y, kLoInv, a.y));
 }
 
-// Up to NT = 64 the residual of the whole row is loaded before the first store: the output may alias the residual as far as the
-// compiler knows, so loads interleaved with the stores each wait for a full memory round trip.  At NT = 128 the 32 extra registers
-// do not fit beside the 128 accumulators (measured slower on the H100), and each load stays next to its store.
+// The residual of the whole row is loaded before the first store: the output may alias the residual as far as the compiler knows,
+// so loads interleaved with the stores would each wait for a full memory round trip.  Used for tiles of up to 32 channels only
+// (conv_fold_kernel, and conv_tc_kernel's 16-channel tiles); wider conv_tc tiles stage their epilogue in shared memory.
 template <int NT>
 __device__ __forceinline__ void conv_epilogue_row(const TcParams& p, const float (&d1)[NT / 2], const float (&d2)[NT / 2], int h,
                                                   long opix, int n0, int c2) {
-  constexpr bool kHoist = NT <= 64;
-  float2 rr[kHoist ? NT / 8 : 1];
-  if constexpr (kHoist) {
+  static_assert(NT <= 32, "wider tiles would not hold the hoisted residual beside their accumulators");
+  float2 rr[NT / 8];
 #pragma unroll
-    for (int i = 0; i < NT / 8; ++i) {
-      int ch;
-      long pix;
-      epilogue_target(p, n0 + 8 * i + c2, opix, ch, pix);
-      rr[i] = epilogue_residual<NT>(p, ch, pix);
-    }
+  for (int i = 0; i < NT / 8; ++i) {
+    int ch;
+    long pix;
+    epilogue_target(p, n0 + 8 * i + c2, opix, ch, pix);
+    rr[i] = epilogue_residual<NT>(p, ch, pix);
   }
 #pragma unroll
   for (int i = 0; i < NT / 8; ++i) {
@@ -93,7 +98,7 @@ __device__ __forceinline__ void conv_epilogue_row(const TcParams& p, const float
     const float2 sh = __ldg(reinterpret_cast<const float2*>(p.shift + co));
     v0 = fmaf(v0, sc.x, sh.x);
     v1 = fmaf(v1, sc.y, sh.y);
-    const float2 r = kHoist ? rr[kHoist ? i : 0] : epilogue_residual<NT>(p, ch, pix);
+    const float2 r = rr[i];
     if (p.residual == LT_RES_BEFORE_RELU) { v0 += r.x; v1 += r.y; }
     if (p.relu) { v0 = fmaxf(v0, 0.f); v1 = fmaxf(v1, 0.f); }
     if (p.residual == LT_RES_AFTER_RELU) { v0 += r.x; v1 += r.y; }
