@@ -152,6 +152,36 @@ __device__ __forceinline__ void wgmma_f16<128>(float (&d)[64], uint64_t ad, uint
       : "l"(ad), "l"(bd), "r"(scale_d));
 }
 
+// ---- wgmma with A from registers (RS): B from shared memory as above, A the m16k16 fragment of each warp's 16 rows, laid out as
+// the A operand of mma.m16n8k16 (a0: rows 0-7 k 0-7, a1: rows 8-15 k 0-7, a2: rows 0-7 k 8-15, a3: rows 8-15 k 8-15).  The
+// A registers, like the accumulators, must not be rewritten before a wgmma.wait_group that covers the MMA reading them.
+template <int N>
+__device__ __forceinline__ void wgmma_f16_rs(float (&d)[N / 2], const uint32_t (&a)[4], uint64_t bd, uint32_t scale_d);
+template <>
+__device__ __forceinline__ void wgmma_f16_rs<16>(float (&d)[8], const uint32_t (&a)[4], uint64_t bd, uint32_t scale_d) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %13, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n16k16.f32.f16.f16 {%0,%1,%2,%3,%4,%5,%6,%7}, {%8,%9,%10,%11}, %12, p, 1, 1, 0;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7])
+      : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(bd), "r"(scale_d));
+}
+template <>
+__device__ __forceinline__ void wgmma_f16_rs<32>(float (&d)[16], const uint32_t (&a)[4], uint64_t bd, uint32_t scale_d) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %21, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n32k16.f32.f16.f16 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, {%16,%17,%18,%19}, %20, p, 1, 1, 0;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
+      : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(bd), "r"(scale_d));
+}
+
+// four 8x8 b16 matrices: lanes 8 m .. 8 m + 7 give the row addresses of matrix m, which lands in r[m] (lane l: row l / 4,
+// elements 2 (l % 4), +1)
+__device__ __forceinline__ void ldmatrix_x4(uint32_t (&r)[4], uint32_t addr) {
+  asm volatile("ldmatrix.sync.aligned.m8n8.x4.shared.b16 {%0, %1, %2, %3}, [%4];"
+               : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3])
+               : "r"(addr));
+}
+
 // two floats -> packed split-fp16 (hi pair, lo pair); element `a` lands in the low half-word (lower address)
 __device__ __forceinline__ void split_s32x2(float a, float b, uint32_t& hi2, uint32_t& lo2) {
   asm("cvt.rn.satfinite.f16x2.f32 %0, %1, %2;" : "=r"(hi2) : "f"(b), "f"(a));

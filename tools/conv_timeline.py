@@ -1,12 +1,12 @@
 #!/usr/bin/env python
-"""Per-class time of the generic tensor-core convolutions (conv_tc_kernel) in one eager bench.py step.
+"""Per-class time of the tensor-core convolutions (conv_tc_kernel, conv_fold_kernel) in one eager bench.py step.
 
     python tools/conv_timeline.py [--timeline FILE] [--bench PATH] [--json OUT] [-- <bench.py arguments>]
 
 Runs `bench.py` with LT_BENCH_TIMELINE pointing at a temporary file (bench.py records one CUDA-event pair per launch
-of one eager, graph-free step: label, desc, ms, GFLOP, MB), or reads such a file with --timeline.  The `conv_tc`
-launches are grouped by their layer description (batch, output grid, Cin, Cout, kernel, stride), so every class below
-is one set of layers of identical shape.  Printed per class: launches, ms per step, useful GFLOP and the issued
+of one eager, graph-free step: label, desc, ms, GFLOP, MB), or reads such a file with --timeline.  The `conv_tc` and
+`conv_fold` launches are grouped by kernel and layer description (batch, output grid, Cin, Cout, kernel, stride), so every
+class below is one set of layers of identical shape run by one kernel.  Printed per class: launches, ms per step, useful GFLOP and the issued
 tensor rate (3 fp16 products per term in the default `tc` mode, 1 in `tc1`).  The other kernels are summed per label.
 """
 import argparse
@@ -34,11 +34,15 @@ def run_bench(bench, bench_args):
     return launches, (json.loads(lines[-1]) if lines else None)
 
 
+CONV_KERNELS = ("conv_tc", "conv_fold")
+
+
 def classify(launches, products):
     classes, others = {}, {}
     for r in launches:
-        if r["kernel"] == "conv_tc":
-            c = classes.setdefault(r["desc"], {"desc": r["desc"], "launches": 0, "ms": 0.0, "gflop": 0.0})
+        if r["kernel"] in CONV_KERNELS:
+            c = classes.setdefault((r["kernel"], r["desc"]), {"kernel": r["kernel"], "desc": r["desc"], "launches": 0, "ms": 0.0,
+                                                              "gflop": 0.0})
             c["launches"] += 1
             c["ms"] += r["ms"]
             c["gflop"] += r["gflop"]
@@ -71,12 +75,16 @@ def main():
     rows, others = classify(launches, products)
     total_ms = sum(c["ms"] for c in rows)
     total_gf = sum(c["gflop"] for c in rows)
-    print("| conv_tc class (desc) | launches | ms | GFLOP | issued TFLOP/s |")
-    print("|---|---|---|---|---|")
+    print("| kernel | class (desc) | launches | ms | GFLOP | issued TFLOP/s |")
+    print("|---|---|---|---|---|---|")
     for c in rows:
-        print("| %s | %d | %.3f | %.1f | %.0f |" % (c["desc"], c["launches"], c["ms"], c["gflop"], c["issued_tflops"]))
-    print("| **all conv_tc** | %d | %.3f | %.1f | %.0f |" % (sum(c["launches"] for c in rows), total_ms, total_gf,
-                                                           products * total_gf / total_ms if total_ms > 0 else 0.0))
+        print("| %s | %s | %d | %.3f | %.1f | %.0f |" % (c["kernel"], c["desc"], c["launches"], c["ms"], c["gflop"], c["issued_tflops"]))
+    for k in CONV_KERNELS:
+        sel = [c for c in rows if c["kernel"] == k]
+        ms, gf = sum(c["ms"] for c in sel), sum(c["gflop"] for c in sel)
+        print("| **all %s** | | %d | %.3f | %.1f | %.0f |" % (k, sum(c["launches"] for c in sel), ms, gf, products * gf / ms if ms > 0 else 0.0))
+    print("| **all** | | %d | %.3f | %.1f | %.0f |" % (sum(c["launches"] for c in rows), total_ms, total_gf,
+                                                     products * total_gf / total_ms if total_ms > 0 else 0.0))
     print()
     print("| other kernel | launches | ms |")
     print("|---|---|---|")
@@ -87,7 +95,7 @@ def main():
         print("bench.py: %.1f %s, gpu_launches %s" % (line.get("value", 0.0), line.get("unit", ""), line.get("gpu_launches")))
     if args.json:
         with open(args.json, "w") as f:
-            json.dump({"conv_tc": rows, "other": others, "products": products}, f, indent=1)
+            json.dump({"conv": rows, "other": others, "products": products}, f, indent=1)
 
 
 if __name__ == "__main__":
