@@ -283,6 +283,18 @@ int lt_v2v_tail_stats_fwd(const void* x, const void* w1, const void* w2, const v
                           long nvox, int FC, const float* coord, int J, float multiplier, int softmax, void* workspace,
                           size_t workspace_bytes, int* n_partials, void* stream);
 
+/* Weight gradient of the lt_conv_nd_fwd call that `desc` describes (training backward of nn.Conv3d / nn.ConvTranspose3d, v2v.py):
+ *   grad_w[t][ci][g*Cout + co] = sum_{n,o} in[n, o*s - p + t][ci] * grad_out[n, o*os + oo (+ group g's offset)][g*(desc->Cout/G) + co]
+ * for ci < Cin, co < Cout (the real channel counts; padded channels never reach grad_w), with the output-mapping fields
+ * (osd/ood, ogd/ogh/ogw) read as the forward reads them: a k2 s2 transposed conv is the one 1x1x1 grouped GEMM of the forward.
+ * `in` and `grad_out` are split-fp16 (in_format = out_format = LT_FMT_S32) with desc->Cin and desc->Cout multiples of 32 and
+ * FC == desc->Cout / G.  grad_out carries the power-of-two scale of lt_f32_to_s32_scaled with the same grad_absmax_bits (NULL: none),
+ * which is divided out exactly.  wgmma with four-term products (fp32-grade).  Deterministic: the K split over positions writes
+ * fp32 partial tiles into `workspace` (lt_conv_wgrad_workspace_bytes(desc) bytes) that a second pass sums in a fixed order. */
+size_t lt_conv_wgrad_workspace_bytes(const lt_conv_desc* desc);
+int lt_conv_wgrad_fwd(const lt_conv_desc* desc, const void* in, const void* grad_out, const unsigned int* grad_absmax_bits, int Cin,
+                      int Cout, float* grad_w, void* workspace, size_t workspace_bytes, void* stream);
+
 /* LT_CONV_TC_FOLD weight packing: float32 [K^3 taps (kd, kh, kw)][32][Cout] (DEVICE) -> split-fp16 [kw][kd][kh][NC][32 hi | 32 lo]
  * (128-byte rows), NC = round_up(Cout, 16), rows Cout .. NC-1 zero; lt_conv_fold_weight_bytes = K^3 * NC * 128. */
 size_t lt_conv_fold_weight_bytes(int K, int Cout);
@@ -361,6 +373,11 @@ int lt_stem_s2d_fwd(const float* in, void* out, int N, int C, int H, int W, void
 /* channels-last [P][C] float32 <-> split-fp16 (C % 32 == 0) */
 int lt_f32_to_s32(const float* in, void* out, long pixels, int C, void* stream);
 int lt_s32_to_f32(const void* in, float* out, long pixels, int C, void* stream);
+/* [P][C] float32 (any C) -> [P][CP] split-fp16 of S * x (CP % 32 == 0, channels C .. CP-1 zero), S the power-of-two pre-scale
+ * that lt_absmax_fwd bits select (the filters' rule: max|S x| in [512, 1024)), 1 for absmax_bits NULL; inv_scale (NULL or one
+ * float) receives 1 / S.  Output gradients lie far below fp16's normal range; scaled, they keep ~22 significand bits. */
+int lt_f32_to_s32_scaled(const float* in, void* out, long pixels, int C, int CP, const unsigned int* absmax_bits, float* inv_scale,
+                         void* stream);
 /* channels-last [N][P][Cs] (first C channels) -> channels-first [N][C][P] float32 */
 int lt_cl_to_cf_f32(const float* in, float* out, int N, long P, int Cs, int C, void* stream);
 
@@ -386,6 +403,10 @@ int lt_test_triangulate_dlt_bwd_host(const float* proj, const float* keypoints_2
  * the kernels' distance, argmin key, term and gradient code: loss.py:52-80. */
 int lt_test_volumetric_ce_host(const float* probs, const float* coord, const float* keypoints_gt, const float* validity, float* loss,
                                int* index, float* picked, const float* grad_loss, float* grad_probs, int B, int J, long nvox);
+/* lt_conv_wgrad_fwd's index mapping (which input row and which output-gradient row meet for a tap, M tile, row and output group) on
+ * host pointers, summed in double over plain float32 channels-last tensors: in [N][ID][IH][IW][desc->Cin], grad_out [N][FD][FH][FW][FC]
+ * -> grad_w [taps][Cin][G * Cout]. */
+int lt_test_conv_wgrad_host(const lt_conv_desc* desc, const float* in, const float* grad_out, int Cin, int Cout, float* grad_w);
 
 #ifdef __cplusplus
 }

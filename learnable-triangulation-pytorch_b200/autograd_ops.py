@@ -200,3 +200,231 @@ def unproject_heatmaps(heatmaps, proj_matricies, coord_volumes, volume_aggregati
 
 def integrate_tensor_3d_with_coordinates(volumes, coord_volumes, softmax=True):
     return IntegrateTensor3dFn.apply(volumes, coord_volumes, softmax)
+
+
+# ---- V2V convolutions for training (v2v_backend="native"): forward and data gradient on the forward conv kernels, weight gradient on
+# csrc/conv_wgrad.cu.  Activations are float32 channels_last_3d tensors, so the kernels read and write them in place of a transpose
+# and torch's BatchNorm / ReLU / pooling / adds run on them unchanged.
+
+class _Filter:
+    """The nn.Conv attributes engine.pack_conv reads, for a filter that is not (or not only) a module's own."""
+
+    def __init__(self, weight, bias, stride, padding):
+        self.weight, self.bias = weight, bias
+        self.kernel_size, self.stride, self.padding = tuple(weight.shape[2:]), tuple(stride), tuple(padding)
+
+
+_WORKSPACE = {}
+
+
+def _workspace(device, nbytes):
+    """Scratch shared by the split-K conv launches and the weight gradient of one device (launches on one stream are ordered)."""
+    ws = _WORKSPACE.get(device)
+    if ws is None or ws.numel() < nbytes:
+        ws = torch.empty(max(nbytes, 32 << 20), dtype=torch.uint8, device=device)
+        _WORKSPACE[device] = ws
+    return ws
+
+
+def _round_up(v, m):
+    return (v + m - 1) // m * m
+
+
+def _cl(x):
+    """(N, C, D, H, W) -> contiguous float32 (N, D, H, W, C) (a view for channels_last_3d input)."""
+    if not x.is_cuda:
+        raise RuntimeError("lt_b200 native V2V convolutions need CUDA tensors (got %s)" % x.device)
+    return x.float().contiguous(memory_format=torch.channels_last_3d).permute(0, 2, 3, 4, 1)
+
+
+def _to_s32(x_cl, cp, absmax_bits=None, inv_scale=None):
+    """(N, D, H, W, C) float32 -> split-fp16 (N, D, H, W, 2 cp), scaled by the power of two that absmax_bits selects."""
+    out = torch.empty(x_cl.shape[:4] + (2 * cp,), dtype=torch.float16, device=x_cl.device)
+    capi.f32_to_s32_scaled(x_cl, out, x_cl[..., 0].numel(), x_cl.shape[4], cp, absmax_bits, inv_scale)
+    return out
+
+
+def conv_desc(N, in_dims, cin_p, cout_p, k, stride, pad, out_dims, out_c, out_fmt, out_scale=(1, 1, 1), out_full=None, groups=(1, 1, 1)):
+    """lt_conv_desc of a split-fp16-input launch without ReLU or residual; out_full: the output tensor's grid (default out_dims)."""
+    fd, fh, fw = out_full or out_dims
+    return capi.ConvDesc(N=N, ID=in_dims[0], IH=in_dims[1], IW=in_dims[2], Cin=cin_p, OD=out_dims[0], OH=out_dims[1], OW=out_dims[2],
+                         Cout=cout_p, KD=k[0], KH=k[1], KW=k[2], sd=stride[0], sh=stride[1], sw=stride[2], pd=pad[0], ph=pad[1], pw=pad[2],
+                         FD=fd, FH=fh, FW=fw, FC=out_c, osd=out_scale[0], osh=out_scale[1], osw=out_scale[2], relu=0, residual=capi.RES_NONE,
+                         in_format=capi.FMT_S32, out_format=out_fmt, ogd=groups[0], ogh=groups[1], ogw=groups[2])
+
+
+def conv3d_wgrad_desc(N, dims, cin, cout, k, padding):
+    """The forward launch of a stride-1 Conv3d as lt_conv_wgrad_fwd reads it: split-fp16 input and output gradient, 32-channel padded."""
+    return conv_desc(N, dims, _round_up(cin, 32), _round_up(cout, 32), k, (1, 1, 1), padding, dims, _round_up(cout, 32), capi.FMT_S32)
+
+
+def conv_transpose3d_desc(N, dims, cin, cout):
+    """ConvTranspose3d(k=2, s=2) as the engine's one grouped 1x1x1 GEMM: N = 8 cout, block g = a 4 + b 2 + c to output phase (a, b, c)."""
+    D, H, W = dims
+    return conv_desc(N, dims, cin, 8 * cout, (1, 1, 1), (1, 1, 1), (0, 0, 0), dims, cout, capi.FMT_S32, out_scale=(2, 2, 2),
+                     out_full=(2 * D, 2 * H, 2 * W), groups=(2, 2, 2))
+
+
+def conv3d_dgrad_filter(weight_shape, padding):
+    """Data gradient of a stride-1 'same' Conv3d (Cout, Cin, kd, kh, kw) as a forward conv of dY: lt_conv_gather_weights_fwd source
+    (base, (s_td, s_th, s_tw, s_ci, s_co)) of the filter flipped in space with Cin and Cout swapped -- element (td, th, tw, ci' = co,
+    co' = ci) = w[co][ci][kd-1-td][kh-1-th][kw-1-tw] -- and the conv's (k, stride, pad, cin', cout')."""
+    cout, cin, kd, kh, kw = weight_shape
+    T = kd * kh * kw
+    return (T - 1, (-kh * kw, -kw, -1, cin * T, T)), (kd, kh, kw), (1, 1, 1), tuple(padding), cout, cin
+
+
+def conv_transpose3d_dgrad_filter(weight_shape):
+    """Data gradient of ConvTranspose3d(k=2, s=2) (Cin, Cout, 2, 2, 2): dX[o][ci] = sum_{t, co} dY[2 o + t][co] w[ci][co][t], a 2^3
+    stride-2 pad-0 conv of dY with element (td, th, tw, ci' = co, co' = ci) = w[ci][co][td][th][tw]."""
+    cin, cout = weight_shape[:2]
+    return (0, (4, 2, 1, 8, cout * 8)), (2, 2, 2), (2, 2, 2), (0, 0, 0), cout, cin
+
+
+def _launch(x_s, cin_p, pk, out_dims, out_c, scale, shift, out_fmt=capi.FMT_F32, out_scale=(1, 1, 1), out_full=None, groups=(1, 1, 1)):
+    """One lt_conv_nd_fwd of packed filter `pk` over split-fp16 x_s; the full-resolution 3^3 / 7^3 layers take LT_CONV_TC_FOLD as in
+    the inference engine."""
+    N, D, H, W = x_s.shape[:4]
+    fd, fh, fw = out_full or out_dims
+    c_store = out_c if out_fmt == capi.FMT_F32 else 2 * out_c
+    out = torch.empty((N, fd, fh, fw, c_store), dtype=torch.float32 if out_fmt == capi.FMT_F32 else torch.float16, device=x_s.device)
+    d = conv_desc(N, (D, H, W), cin_p, pk.cout_p, pk.k, pk.stride, pk.pad, out_dims, out_c, out_fmt, out_scale, out_full, groups)
+    ws = _workspace(x_s.device, 0)
+    d.workspace, d.workspace_bytes = ws.data_ptr(), ws.numel()
+    impl, weight = capi.CONV_TC, pk.w
+    if pk.w_fold is not None and W >= 16 and out_c == 32 and out_fmt == capi.FMT_F32:
+        impl, weight = capi.CONV_TC_FOLD, pk.w_fold
+        d.Cout = pk.cout
+    capi.conv_nd(d, x_s, weight, scale, shift, None, out, impl)
+    return out, d
+
+
+def _grad_s32(grad_out, cp):
+    """dL/dy -> (split-fp16 of S dL/dy, (N, D, H, W, C) float32 view, absmax bits, 1 / S on the device): S = 2^(9 - floor(log2 max|g|))."""
+    g = _cl(grad_out)
+    amax = torch.empty(1, dtype=torch.int32, device=g.device)
+    capi.absmax(g, amax)
+    inv = torch.empty(1, dtype=torch.float32, device=g.device)
+    return _to_s32(g, cp, amax, inv), g, amax, inv
+
+
+def _wgrad(desc, x_s, g_s, amax, cin, cout, taps, groups=1):
+    """lt_conv_wgrad_fwd of the forward call `desc` -> float32 [taps][cin][groups cout]."""
+    gw = torch.empty((taps, cin, groups * cout), dtype=torch.float32, device=x_s.device)
+    ws = _workspace(x_s.device, capi.conv_wgrad_workspace_bytes(desc))
+    capi.conv_wgrad(desc, x_s, g_s, amax, cin, cout, gw, ws)
+    return gw
+
+
+class Conv3dFn(torch.autograd.Function):
+    """nn.Conv3d with stride 1 and "same" padding (every Conv3d of v2v.py) on the tensor-core kernels, fp32-grade in all three passes.
+    forward: lt_conv_nd_fwd (scale 1 / S, shift = bias); data gradient: the same kernels over the output gradient with the filter
+    flipped in space and Cin / Cout swapped (re-gathered by lt_conv_gather_weights_fwd with negated tap strides); weight gradient:
+    lt_conv_wgrad_fwd; bias gradient: torch's sum of the output gradient."""
+
+    @staticmethod
+    def forward(ctx, x, weight, bias, padding):
+        from .engine import pack_conv
+        cout, cin, kd, kh, kw = weight.shape
+        if tuple(padding) != (kd // 2, kh // 2, kw // 2) or not (kd % 2 and kh % 2 and kw % 2):
+            raise ValueError("native Conv3d: stride 1 'same' convolutions only (odd kernel, padding k // 2), got k=%s padding=%s"
+                             % ((kd, kh, kw), tuple(padding)))
+        x_cl = _cl(x)
+        cin_p = _round_up(cin, 32)
+        x_s = _to_s32(x_cl, cin_p)
+        pk = pack_conv(_Filter(weight.detach(), None if bias is None else bias.detach(), (1, 1, 1), padding), None, cin_pad=cin_p,
+                       out_fmt=capi.FMT_F32)
+        out, _ = _launch(x_s, cin_p, pk, x_cl.shape[1:4], _round_up(cout, 4), pk.scale, pk.shift)
+        ctx.save_for_backward(x_s, weight)
+        ctx.padding = tuple(padding)
+        return out[..., :cout].permute(0, 4, 1, 2, 3)
+
+    @staticmethod
+    def backward(ctx, grad_out):
+        from .engine import pack_filter
+        x_s, weight = ctx.saved_tensors
+        cout, cin, kd, kh, kw = weight.shape
+        T = kd * kh * kw
+        cout_p = _round_up(cout, 32)
+        g_s, g, amax, inv = _grad_s32(grad_out, cout_p)
+        N, D, H, W = g.shape[:4]
+        gx = gw = gb = None
+        if ctx.needs_input_grad[0]:
+            w = weight.detach().float().contiguous()
+            (base, strides), k, stride, pad, ci, co = conv3d_dgrad_filter(weight.shape, ctx.padding)
+            pk = pack_filter((w, base, strides), k, stride, pad, ci, co, None, None, out_fmt=capi.FMT_F32)
+            out, _ = _launch(g_s, cout_p, pk, (D, H, W), _round_up(cin, 4), pk.scale * inv, pk.shift)
+            gx = out[..., :cin].permute(0, 4, 1, 2, 3)
+        if ctx.needs_input_grad[1]:
+            d = conv3d_wgrad_desc(N, (D, H, W), cin, cout, (kd, kh, kw), ctx.padding)
+            gw = _wgrad(d, x_s, g_s, amax, cin, cout, T).reshape(kd, kh, kw, cin, cout).permute(4, 3, 0, 1, 2).contiguous()
+        if ctx.needs_input_grad[2]:
+            gb = g.sum(dim=(0, 1, 2, 3))
+        return gx, gw, gb, None
+
+
+class ConvTranspose3dFn(torch.autograd.Function):
+    """nn.ConvTranspose3d(k=2, s=2, p=0) (v2v.py Upsample3DBlock) with Cout % 32 == 0: the forward is the engine's one grouped 1x1x1
+    GEMM (N = 8 Cout, each 32-channel block written to its phase of the output lattice); the data gradient is a 2^3 stride-2
+    convolution of the output gradient (Cin' = Cout, Cout' = Cin) on conv_tc_kernel; the weight gradient is lt_conv_wgrad_fwd over
+    the forward's grouped GEMM."""
+
+    @staticmethod
+    def forward(ctx, x, weight, bias):
+        from .engine import pack_deconv3d_k2s2
+        cin, cout = weight.shape[:2]
+        if tuple(weight.shape[2:]) != (2, 2, 2) or cout % 32 or cin % 32:
+            raise ValueError("native ConvTranspose3d: kernel 2, stride 2 and channel counts that are multiples of 32 only, got %s"
+                             % (tuple(weight.shape),))
+        x_cl = _cl(x)
+        N, D, H, W = x_cl.shape[:4]
+        x_s = _to_s32(x_cl, cin)
+        pk = pack_deconv3d_k2s2(_Filter(weight.detach(), None if bias is None else bias.detach(), (2, 2, 2), (0, 0, 0)), None)
+        y_s, _ = _launch(x_s, cin, pk, (D, H, W), cout, pk.scale, pk.shift, out_fmt=capi.FMT_S32, out_scale=(2, 2, 2),
+                         out_full=(2 * D, 2 * H, 2 * W), groups=(2, 2, 2))
+        out = torch.empty((N, 2 * D, 2 * H, 2 * W, cout), dtype=torch.float32, device=x.device)
+        capi.s32_to_f32(y_s, out, out[..., 0].numel(), cout)
+        ctx.save_for_backward(x_s, weight)
+        return out.permute(0, 4, 1, 2, 3)
+
+    @staticmethod
+    def backward(ctx, grad_out):
+        from .engine import pack_filter
+        x_s, weight = ctx.saved_tensors
+        cin, cout = weight.shape[:2]
+        g_s, g, amax, inv = _grad_s32(grad_out, cout)
+        N, D, H, W = x_s.shape[:4]
+        gx = gw = gb = None
+        if ctx.needs_input_grad[0]:
+            w = weight.detach().float().contiguous()
+            (base, strides), k, stride, pad, ci, co = conv_transpose3d_dgrad_filter(weight.shape)
+            pk = pack_filter((w, base, strides), k, stride, pad, ci, co, None, None, out_fmt=capi.FMT_F32)
+            out, _ = _launch(g_s, cout, pk, (D, H, W), cin, pk.scale * inv, pk.shift)
+            gx = out.permute(0, 4, 1, 2, 3)
+        if ctx.needs_input_grad[1]:
+            gw = _wgrad(conv_transpose3d_desc(N, (D, H, W), cin, cout), x_s, g_s, amax, cin, cout, 1, groups=8)       # [1][ci][g cout + co], g = a 4 + b 2 + c
+            gw = gw.reshape(cin, 8, cout).permute(0, 2, 1).reshape(cin, cout, 2, 2, 2).contiguous()
+        if ctx.needs_input_grad[2]:
+            gb = g.sum(dim=(0, 1, 2, 3))
+        return gx, gw, gb
+
+
+def conv3d(x, weight, bias=None, padding=(0, 0, 0)):
+    """F.conv3d(x, weight, bias, 1, padding) for stride-1 'same' filters on the native training kernels."""
+    return Conv3dFn.apply(x, weight, bias, tuple(padding))
+
+
+def conv_transpose3d(x, weight, bias=None):
+    """F.conv_transpose3d(x, weight, bias, stride=2) for 2^3 filters on the native training kernels."""
+    return ConvTranspose3dFn.apply(x, weight, bias)
+
+
+def v2v_conv(module, x):
+    """A Conv3d / ConvTranspose3d module of the V2V net applied through the native functions (the module's own parameters)."""
+    if isinstance(module, torch.nn.ConvTranspose3d):
+        if tuple(module.stride) != (2, 2, 2) or tuple(module.padding) != (0, 0, 0) or tuple(module.output_padding) != (0, 0, 0):
+            raise ValueError("native ConvTranspose3d: stride 2, no padding only")
+        return conv_transpose3d(x, module.weight, module.bias)
+    if tuple(module.stride) != (1, 1, 1) or module.groups != 1 or tuple(module.dilation) != (1, 1, 1):
+        raise ValueError("native Conv3d: stride 1, no groups, no dilation only")
+    return conv3d(x, module.weight, module.bias, module.padding)

@@ -84,6 +84,10 @@ SIGNATURES = {
                                       ctypes.POINTER(c_int), c_void_p]),
     "lt_softargmax3d_finish_fwd": (c_int, [c_void_p, c_long, c_long, c_void_p, c_void_p, c_void_p, c_void_p, c_size_t, c_int, c_int, c_long, c_int,
                                            c_float, c_int, c_void_p]),
+    "lt_conv_wgrad_workspace_bytes": (c_size_t, [ctypes.POINTER(ConvDesc)]),
+    "lt_conv_wgrad_fwd": (c_int, [ctypes.POINTER(ConvDesc)] + [c_void_p] * 3 + [c_int, c_int, c_void_p, c_void_p, c_size_t, c_void_p]),
+    "lt_test_conv_wgrad_host": (c_int, [ctypes.POINTER(ConvDesc), c_void_p, c_void_p, c_int, c_int, c_void_p]),
+    "lt_f32_to_s32_scaled": (c_int, [c_void_p, c_void_p, c_long, c_int, c_int, c_void_p, c_void_p, c_void_p]),
     "lt_conv_fold_weight_bytes": (c_size_t, [c_int, c_int]),
     "lt_conv_fold_pack_weights": (c_int, [c_void_p, c_void_p, c_int, c_int, c_void_p]),
     "lt_maxpool_fwd": (c_int, [c_void_p, c_void_p] + [c_int] * 18 + [c_void_p]),
@@ -423,6 +427,28 @@ def stem_s2d(inp, out, N, C, H, W):
 
 def f32_to_s32(inp, out, pixels, C):
     _check(lib().lt_f32_to_s32(_ptr(inp), _ptr(out), pixels, C, _stream()), "lt_f32_to_s32")
+
+
+def f32_to_s32_scaled(inp, out, pixels, C, CP, absmax_bits=None, inv_scale=None):
+    """[P][C] float32 -> [P][CP] split-fp16 of S x (S from absmax_bits, 1 without); inv_scale: float32[1] receiving 1 / S, or None."""
+    _check(lib().lt_f32_to_s32_scaled(_ptr(inp), _ptr(out), pixels, C, CP, _ptr(absmax_bits), _ptr(inv_scale), _stream()),
+           "lt_f32_to_s32_scaled")
+
+
+def conv_wgrad_workspace_bytes(desc):
+    return lib().lt_conv_wgrad_workspace_bytes(ctypes.byref(desc))
+
+
+def conv_wgrad(desc, inp, grad_out, grad_absmax_bits, cin, cout, grad_w, workspace):
+    """grad_w float32 [taps][cin][G cout] of the lt_conv_nd_fwd call `desc` describes (both operands split-fp16)."""
+    _check(lib().lt_conv_wgrad_fwd(ctypes.byref(desc), _ptr(inp), _ptr(grad_out), _ptr(grad_absmax_bits), cin, cout, _ptr(grad_w),
+                                   _ptr(workspace), workspace.numel() * workspace.element_size(), _stream()), "lt_conv_wgrad_fwd")
+
+
+def conv_wgrad_host(desc, inp, grad_out, cin, cout, grad_w):
+    """lt_test_conv_wgrad_host: the weight-gradient kernel's index mapping on CPU float32 channels-last tensors (test hook)."""
+    _check(lib().lt_test_conv_wgrad_host(ctypes.byref(desc), _host_ptr(inp), _host_ptr(grad_out), cin, cout, _host_ptr(grad_w)),
+           "lt_test_conv_wgrad_host")
 
 
 def s32_to_f32(inp, out, pixels, C):

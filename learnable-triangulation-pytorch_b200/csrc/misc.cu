@@ -157,6 +157,27 @@ __global__ void __launch_bounds__(256) f32_to_s32_kernel(const float* __restrict
   }
 }
 
+// [P][C] float32 (any C) -> [P][CP] split-fp16 of S * x, S = weight_pow2_scale(absmax_bits) (1 without bits), channels C..CP-1 zero;
+// inv_scale (optional) receives 1 / S
+__global__ void __launch_bounds__(256) f32_to_s32_scaled_kernel(const float* __restrict__ in, sh_t* __restrict__ out, long pixels, int C,
+                                                                int CP, const unsigned* __restrict__ absmax_bits, float* __restrict__ inv_scale) {
+  const float S = weight_pow2_scale(absmax_bits);
+  if (inv_scale && blockIdx.x == 0 && threadIdx.x == 0) *inv_scale = 1.0f / S;
+  const int c4n = CP / 4;
+  const long total = pixels * c4n;
+  for (long i = (long)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (long)gridDim.x * blockDim.x) {
+    const long pix = i / c4n;
+    const int c = (int)(i % c4n) * 4;
+    const float* src = in + pix * C;
+    float4 v;
+    v.x = c < C ? __ldg(src + c) * S : 0.0f;
+    v.y = c + 1 < C ? __ldg(src + c + 1) * S : 0.0f;
+    v.z = c + 2 < C ? __ldg(src + c + 2) * S : 0.0f;
+    v.w = c + 3 < C ? __ldg(src + c + 3) * S : 0.0f;
+    store_s32x4(out + pix * 2 * CP, c, v);
+  }
+}
+
 __global__ void __launch_bounds__(256) s32_to_f32_kernel(const sh_t* __restrict__ in, float* __restrict__ out, long pixels, int C) {
   const int c4n = C / 4;
   const long total = pixels * c4n;
@@ -374,6 +395,15 @@ extern "C" int lt_f32_to_s32(const float* in, void* out, long pixels, int C, voi
   LT_REQUIRE(in && out && C % 32 == 0, "f32_to_s32: C %% 32 != 0");
   f32_to_s32_kernel<<<grid_for(pixels * (C / 4)), 256, 0, (cudaStream_t)stream>>>(in, reinterpret_cast<sh_t*>(out), pixels, C);
   LT_CHECK_LAUNCH("f32_to_s32_kernel");
+  return LT_OK;
+}
+
+extern "C" int lt_f32_to_s32_scaled(const float* in, void* out, long pixels, int C, int CP, const unsigned int* absmax_bits,
+                                    float* inv_scale, void* stream) {
+  LT_REQUIRE(in && out && C > 0 && CP >= C && CP % 32 == 0, "f32_to_s32_scaled: need C <= CP, CP %% 32 == 0");
+  f32_to_s32_scaled_kernel<<<grid_for(pixels * (CP / 4)), 256, 0, (cudaStream_t)stream>>>(in, reinterpret_cast<sh_t*>(out), pixels, C, CP,
+                                                                                         absmax_bits, inv_scale);
+  LT_CHECK_LAUNCH("f32_to_s32_scaled_kernel");
   return LT_OK;
 }
 

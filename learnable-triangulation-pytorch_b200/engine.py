@@ -74,6 +74,106 @@ class _Timed:
         return False
 
 
+_TC_IMPL = {"simt": CONV_SIMT, "tc": CONV_TC, "tc1": CONV_TC1}
+
+
+def pack_filter(src, k, stride, pad, cin, cout, bias, bn, mode="tc", cin_pad=None, force_simt=False, out_fmt=None):
+    """src = (filter tensor, base, (s_td, s_th, s_tw, s_ci, s_co)): where element (td, th, tw, ci, co) of this (phase of a)
+    convolution sits inside the module's own weight tensor.  Everything below is our own kernels: gather to the canonical
+    [tap][Cin][Cout] layout (lt_conv_gather_weights_fwd), operand packing, BatchNorm folding (lt_fold_bn_fwd).  mode: the
+    engine's conv mode; NativeEngine packs once per parameter version, the training convolutions (autograd_ops) on every call."""
+    # a list of sources = column blocks of ONE wider filter (k2 s2 transposed conv: 8 phases side by side along N)
+    srcs = src if isinstance(src, list) else [src]
+    G = len(srcs)
+    w = srcs[0][0]
+    dev = w.device
+    taps = k[0] * k[1] * k[2]
+    act_fmt = FMT_F32 if mode == "simt" else FMT_S32
+    out_fmt = act_fmt if out_fmt is None else out_fmt
+    pk = ConvPack()
+    pk.taps, pk.k, pk.stride, pk.pad, pk.cout, pk.groups = taps, k, stride, pad, G * cout, G
+    pk.kmacs = taps * cin * cout * G   # algorithmic MACs per output position
+    pk.w_fold = None
+    use_tc = (mode != "simt") and not force_simt
+    assert G == 1 or (use_tc and cout % 32 == 0), "column blocks need the tensor-core path and 32-channel multiples"
+    if use_tc:
+        cin_p = _round_up(max(cin, cin_pad or 0), 32)
+        cout_p = _round_up(G * cout, 32 if out_fmt == FMT_S32 else 16)
+    else:
+        cin_p = max(cin, cin_pad or 0)
+        cout_p = _round_up(cout, 4)
+    blk_p = cout if G > 1 else cout_p
+    wp = torch.empty((taps, cin_p, cout_p), dtype=torch.float32, device=dev)
+    amax = None
+    if use_tc:
+        # power-of-two pre-scale of the whole filter tensor (all phases of a transposed conv share it): common.cuh
+        amax = torch.empty(1, dtype=torch.int32, device=dev)
+        capi.absmax(w, amax)
+    for g, (wg, base, strides) in enumerate(srcs):
+        capi.conv_gather_weights(wg, base, strides, k, cin, cin_p, cout, blk_p, wp, amax, out_ld=cout_p, out_col0=g * cout)
+    if use_tc:
+        packed = torch.empty(capi.conv_tc_weight_bytes(taps, cin_p, cout_p) // 2, dtype=torch.float16, device=dev)
+        capi.conv_tc_pack_weights(wp, packed, taps, cin_p, cout_p)
+        pk.w, pk.cin, pk.cout_p, pk.impl, pk.in_fmt = packed, cin_p, cout_p, _TC_IMPL[mode], FMT_S32
+        # narrow cubic stride-1 layers (V2V at full resolution): also pack for the halo-reusing persistent kernel (csrc/conv_fold.cu)
+        if (mode == "tc" and cin_p == 32 and cout <= 32 and k[0] == k[1] == k[2] and k[0] in (3, 7)
+                and tuple(pad) == (k[0] // 2,) * 3 and max(stride) == 1):
+            wf = torch.empty(capi.conv_fold_weight_bytes(k[0], cout) // 2, dtype=torch.float16, device=dev)
+            wsrc = wp if cout_p == cout else wp[:, :, :cout].contiguous()
+            capi.conv_fold_pack_weights(wsrc, wf, k[0], cout)
+            pk.w_fold = wf
+    else:
+        pk.w, pk.cin, pk.cout_p, pk.impl, pk.in_fmt = wp, cin_p, cout_p, CONV_SIMT, FMT_F32
+    pk.scale = torch.empty(cout_p, dtype=torch.float32, device=dev)
+    pk.shift = torch.empty(cout_p, dtype=torch.float32, device=dev)
+    # tensor-core accumulation steps on the main fp32 accumulator (one hi*hi MMA per 16 input channels and tap, in conv_tc_kernel and in
+    # conv_fold_kernel alike): lt_fold_bn_fwd compensates the expected truncation shrinkage (include/lt_b200.h)
+    steps = taps * (cin_p // 16) if use_tc else 0
+    for g in range(G):     # the per-channel affine repeats for every column block
+        sc, sh = pk.scale[g * cout:g * cout + blk_p], pk.shift[g * cout:g * cout + blk_p]
+        if bn is not None:
+            capi.fold_bn(_f32(bn.weight), _f32(bn.bias), _f32(bn.running_mean), _f32(bn.running_var), _f32(bias), bn.eps, cout, blk_p,
+                         sc, sh, amax, accum_steps=steps)
+        else:
+            capi.fold_bn(None, None, None, None, _f32(bias), 0.0, cout, blk_p, sc, sh, amax, accum_steps=steps)
+    return pk
+
+
+def pack_conv(conv, bn, mode="tc", cin_pad=None, **kw):
+    """conv: anything with the nn.Conv2d / nn.Conv3d attributes weight, bias, kernel_size, stride, padding."""
+    w = _f32(conv.weight)
+    cout, cin = w.shape[:2]
+    if w.dim() == 4:   # (Cout, Cin, KH, KW)
+        k = (1,) + tuple(conv.kernel_size)
+        stride = (1,) + tuple(conv.stride)
+        pad = (0,) + tuple(conv.padding)
+    else:              # (Cout, Cin, KD, KH, KW)
+        k, stride, pad = tuple(conv.kernel_size), tuple(conv.stride), tuple(conv.padding)
+    T = k[0] * k[1] * k[2]
+    src = (w, 0, (k[1] * k[2], k[2], 1, T, cin * T))
+    return pack_filter(src, k, stride, pad, cin, cout, conv.bias, bn, mode=mode, cin_pad=cin_pad, **kw)
+
+
+def pack_deconv3d_k2s2(deconv, bn, mode="tc"):
+    """ConvTranspose3d(k=2, s=2): eight independent 1x1x1 convs scattered to the output parities.
+
+    Tensor-core modes with Cout % 32 == 0: ONE 1x1x1 GEMM with N = 8 x Cout (the phases side by side along N, the epilogue
+    writing each 32-channel block to its phase of the output lattice: lt_conv_desc.ogd/ogh/ogw) -- the input is read once
+    instead of eight times and a level costs one launch instead of eight."""
+    w = _f32(deconv.weight)  # (Cin, Cout, 2, 2, 2)
+    cin, cout = w.shape[:2]
+    if mode != "simt" and cout % 32 == 0:
+        srcs = [(w, a * 4 + b * 2 + c, (0, 0, 0, cout * 8, 8)) for a in (0, 1) for b in (0, 1) for c in (0, 1)]
+        return pack_filter(srcs, (1, 1, 1), (1, 1, 1), (0, 0, 0), cin, cout, deconv.bias, bn, mode=mode)
+    phases = {}
+    for a in (0, 1):
+        for b in (0, 1):
+            for c in (0, 1):
+                src = (w, a * 4 + b * 2 + c, (0, 0, 0, cout * 8, 8))
+                phases[(a, b, c)] = pack_filter(src, (1, 1, 1), (1, 1, 1), (0, 0, 0), cin, cout, deconv.bias, bn, mode=mode)
+    return phases
+
+
 class NativeEngine:
     def __init__(self, model, mode="tc", use_graph=True):
         assert mode in ("simt", "tc", "tc1")
@@ -81,7 +181,7 @@ class NativeEngine:
         self.mode = mode
         self.use_graph = use_graph
         self.act_fmt = FMT_F32 if mode == "simt" else FMT_S32
-        self.tc_impl = {"simt": CONV_SIMT, "tc": CONV_TC, "tc1": CONV_TC1}[mode]
+        self.tc_impl = _TC_IMPL[mode]
         self._packs = None
         self._packs_version = None
         self._epoch = 0
@@ -104,77 +204,11 @@ class NativeEngine:
         self._packs = None
         self._graphs = {}
 
-    def _pack(self, src, k, stride, pad, cin, cout, bias, bn, cin_pad=None, force_simt=False, out_fmt=None):
-        """src = (filter tensor, base, (s_td, s_th, s_tw, s_ci, s_co)): where element (td, th, tw, ci, co) of this (phase of a)
-        convolution sits inside the module's own weight tensor.  Everything below is our own kernels: gather to the canonical
-        [tap][Cin][Cout] layout (lt_conv_gather_weights_fwd), operand packing, BatchNorm folding (lt_fold_bn_fwd)."""
-        # a list of sources = column blocks of ONE wider filter (k2 s2 transposed conv: 8 phases side by side along N)
-        srcs = src if isinstance(src, list) else [src]
-        G = len(srcs)
-        w = srcs[0][0]
-        dev = w.device
-        taps = k[0] * k[1] * k[2]
-        out_fmt = self.act_fmt if out_fmt is None else out_fmt
-        pk = ConvPack()
-        pk.taps, pk.k, pk.stride, pk.pad, pk.cout, pk.groups = taps, k, stride, pad, G * cout, G
-        pk.kmacs = taps * cin * cout * G   # algorithmic MACs per output position
-        pk.w_fold = None
-        use_tc = (self.mode != "simt") and not force_simt
-        assert G == 1 or (use_tc and cout % 32 == 0), "column blocks need the tensor-core path and 32-channel multiples"
-        if use_tc:
-            cin_p = _round_up(max(cin, cin_pad or 0), 32)
-            cout_p = _round_up(G * cout, 32 if out_fmt == FMT_S32 else 16)
-        else:
-            cin_p = max(cin, cin_pad or 0)
-            cout_p = _round_up(cout, 4)
-        blk_p = cout if G > 1 else cout_p
-        wp = torch.empty((taps, cin_p, cout_p), dtype=torch.float32, device=dev)
-        amax = None
-        if use_tc:
-            # power-of-two pre-scale of the whole filter tensor (all phases of a transposed conv share it): common.cuh
-            amax = torch.empty(1, dtype=torch.int32, device=dev)
-            capi.absmax(w, amax)
-        for g, (wg, base, strides) in enumerate(srcs):
-            capi.conv_gather_weights(wg, base, strides, k, cin, cin_p, cout, blk_p, wp, amax, out_ld=cout_p, out_col0=g * cout)
-        if use_tc:
-            packed = torch.empty(capi.conv_tc_weight_bytes(taps, cin_p, cout_p) // 2, dtype=torch.float16, device=dev)
-            capi.conv_tc_pack_weights(wp, packed, taps, cin_p, cout_p)
-            pk.w, pk.cin, pk.cout_p, pk.impl, pk.in_fmt = packed, cin_p, cout_p, self.tc_impl, FMT_S32
-            # narrow cubic stride-1 layers (V2V at full resolution): also pack for the halo-reusing persistent kernel (csrc/conv_fold.cu)
-            if (self.mode == "tc" and cin_p == 32 and cout <= 32 and k[0] == k[1] == k[2] and k[0] in (3, 7)
-                    and tuple(pad) == (k[0] // 2,) * 3 and max(stride) == 1):
-                wf = torch.empty(capi.conv_fold_weight_bytes(k[0], cout) // 2, dtype=torch.float16, device=dev)
-                wsrc = wp if cout_p == cout else wp[:, :, :cout].contiguous()
-                capi.conv_fold_pack_weights(wsrc, wf, k[0], cout)
-                pk.w_fold = wf
-        else:
-            pk.w, pk.cin, pk.cout_p, pk.impl, pk.in_fmt = wp, cin_p, cout_p, CONV_SIMT, FMT_F32
-        pk.scale = torch.empty(cout_p, dtype=torch.float32, device=dev)
-        pk.shift = torch.empty(cout_p, dtype=torch.float32, device=dev)
-        # tensor-core accumulation steps on the main fp32 accumulator (one hi*hi MMA per 16 input channels and tap, in conv_tc_kernel and in
-        # conv_fold_kernel alike): lt_fold_bn_fwd compensates the expected truncation shrinkage (include/lt_b200.h)
-        steps = taps * (cin_p // 16) if use_tc else 0
-        for g in range(G):     # the per-channel affine repeats for every column block
-            sc, sh = pk.scale[g * cout:g * cout + blk_p], pk.shift[g * cout:g * cout + blk_p]
-            if bn is not None:
-                capi.fold_bn(_f32(bn.weight), _f32(bn.bias), _f32(bn.running_mean), _f32(bn.running_var), _f32(bias), bn.eps, cout, blk_p,
-                             sc, sh, amax, accum_steps=steps)
-            else:
-                capi.fold_bn(None, None, None, None, _f32(bias), 0.0, cout, blk_p, sc, sh, amax, accum_steps=steps)
-        return pk
+    def _pack(self, *args, **kw):
+        return pack_filter(*args, mode=self.mode, **kw)
 
     def _pack_conv(self, conv, bn, cin_pad=None, **kw):
-        w = _f32(conv.weight)
-        cout, cin = w.shape[:2]
-        if w.dim() == 4:   # (Cout, Cin, KH, KW)
-            k = (1,) + tuple(conv.kernel_size)
-            stride = (1,) + tuple(conv.stride)
-            pad = (0,) + tuple(conv.padding)
-        else:              # (Cout, Cin, KD, KH, KW)
-            k, stride, pad = tuple(conv.kernel_size), tuple(conv.stride), tuple(conv.padding)
-        T = k[0] * k[1] * k[2]
-        src = (w, 0, (k[1] * k[2], k[2], 1, T, cin * T))
-        return self._pack(src, k, stride, pad, cin, cout, conv.bias, bn, cin_pad=cin_pad, **kw)
+        return pack_conv(conv, bn, mode=self.mode, cin_pad=cin_pad, **kw)
 
     def _pack_stem_s2d(self, conv, bn):
         """7x7 stride-2 pad-3 conv == 4x4 stride-1 conv (front pad 2) over the 2x2 space-to-depth input.
@@ -216,23 +250,7 @@ class NativeEngine:
         return phases
 
     def _pack_deconv3d_k2s2(self, deconv, bn):
-        """ConvTranspose3d(k=2, s=2): eight independent 1x1x1 convs scattered to the output parities.
-
-        Tensor-core modes with Cout % 32 == 0: ONE 1x1x1 GEMM with N = 8 x Cout (the phases side by side along N, the epilogue
-        writing each 32-channel block to its phase of the output lattice: lt_conv_desc.ogd/ogh/ogw) -- the input is read once
-        instead of eight times and a level costs one launch instead of eight."""
-        w = _f32(deconv.weight)  # (Cin, Cout, 2, 2, 2)
-        cin, cout = w.shape[:2]
-        if self.mode != "simt" and cout % 32 == 0:
-            srcs = [(w, a * 4 + b * 2 + c, (0, 0, 0, cout * 8, 8)) for a in (0, 1) for b in (0, 1) for c in (0, 1)]
-            return self._pack(srcs, (1, 1, 1), (1, 1, 1), (0, 0, 0), cin, cout, deconv.bias, bn)
-        phases = {}
-        for a in (0, 1):
-            for b in (0, 1):
-                for c in (0, 1):
-                    src = (w, a * 4 + b * 2 + c, (0, 0, 0, cout * 8, 8))
-                    phases[(a, b, c)] = self._pack(src, (1, 1, 1), (1, 1, 1), (0, 0, 0), cin, cout, deconv.bias, bn)
-        return phases
+        return pack_deconv3d_k2s2(deconv, bn, mode=self.mode)
 
     def prepare(self):
         ver = self._param_version()

@@ -67,7 +67,7 @@ class _EngineOwner(nn.Module):
 
 
 class VolumetricTriangulationNet(_EngineOwner):
-    def __init__(self, config, device="cuda:0", backend=None, conv_mode=None, use_cuda_graph=True):
+    def __init__(self, config, device="cuda:0", backend=None, conv_mode=None, use_cuda_graph=True, v2v_backend="torch"):
         super().__init__()
         m = config.model
         self.num_joints = m.backbone.num_joints
@@ -96,6 +96,13 @@ class VolumetricTriangulationNet(_EngineOwner):
 
         self.backend = backend or os.environ.get("LT_B200_BACKEND", "native")
         self.conv_mode = conv_mode or os.environ.get("LT_B200_CONV", "tc")
+        # v2v_backend="native" (backend="hybrid" only): every Conv3d / ConvTranspose3d of volume_net runs forward, data gradient and
+        # weight gradient on the native tensor-core kernels (autograd_ops.v2v_conv); BatchNorm, ReLU, pooling and adds stay on torch
+        if v2v_backend not in ("torch", "native"):
+            raise ValueError("unknown v2v_backend {!r}".format(v2v_backend))
+        if v2v_backend == "native" and (self.backend != "hybrid" or self.conv_mode != "tc"):
+            raise ValueError("v2v_backend='native' needs backend='hybrid' and conv_mode='tc' (got %r, %r)" % (self.backend, self.conv_mode))
+        self.v2v_backend = v2v_backend
         self.use_cuda_graph = use_cuda_graph
         self.clone_outputs = True
         self._engine = None
@@ -190,7 +197,7 @@ class VolumetricTriangulationNet(_EngineOwner):
                 raise RuntimeError("lt_b200 hybrid backend needs CUDA tensors (native custom ops); use backend='torch' on CPU")
             from . import autograd_ops as ops
         volumes = ops.unproject_heatmaps(features, proj_t, coord, self.volume_aggregation_method, vol_conf)
-        volumes = self.volume_net(volumes)
+        volumes = self.volume_net(volumes, ops.v2v_conv if self.v2v_backend == "native" else None)
         kp, volumes = ops.integrate_tensor_3d_with_coordinates(volumes * self.volume_multiplier, coord, self.volume_softmax)
         return kp, features, volumes, vol_conf, cuboids, coord, cen_t
 

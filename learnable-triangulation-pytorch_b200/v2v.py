@@ -6,10 +6,19 @@ front_layers.{0..3}, encoder_decoder.{encoder_res*,decoder_res*,decoder_upsample
 back_layers.{0..2}, output_layer.
 
 Parameters live here; inference runs through the native planner in engine.py.
-The torch forward below is the autograd / CPU plumbing path (backend="torch").
+The torch forward below is the autograd / CPU plumbing path (backend="torch").  Every forward takes an optional `conv`: a function
+(module, x) -> y that replaces the calls of the Conv3d / ConvTranspose3d modules (v2v_backend="native": autograd_ops.v2v_conv);
+BatchNorm, ReLU, pooling and the adds stay torch modules either way.
 """
 import torch.nn.functional as F
 from torch import nn
+
+
+def _seq(seq, x, conv):
+    """nn.Sequential.forward, with the convolutions through `conv` when one is given."""
+    for m in seq:
+        x = conv(m, x) if conv is not None and isinstance(m, (nn.Conv3d, nn.ConvTranspose3d)) else m(x)
+    return x
 
 
 class Basic3DBlock(nn.Module):
@@ -19,8 +28,8 @@ class Basic3DBlock(nn.Module):
         super().__init__()
         self.block = nn.Sequential(nn.Conv3d(cin, cout, k, 1, (k - 1) // 2), nn.BatchNorm3d(cout), nn.ReLU(True))
 
-    def forward(self, x):
-        return self.block(x)
+    def forward(self, x, conv=None):
+        return _seq(self.block, x, conv)
 
 
 class Res3DBlock(nn.Module):
@@ -34,8 +43,8 @@ class Res3DBlock(nn.Module):
         self.skip_con = nn.Sequential() if cin == cout else nn.Sequential(
             nn.Conv3d(cin, cout, 1, 1, 0), nn.BatchNorm3d(cout))
 
-    def forward(self, x):
-        return F.relu(self.res_branch(x) + self.skip_con(x), True)
+    def forward(self, x, conv=None):
+        return F.relu(_seq(self.res_branch, x, conv) + _seq(self.skip_con, x, conv), True)
 
 
 class Pool3DBlock(nn.Module):
@@ -55,8 +64,8 @@ class Upsample3DBlock(nn.Module):
         assert kernel_size == 2 and stride == 2
         self.block = nn.Sequential(nn.ConvTranspose3d(cin, cout, 2, 2, 0, 0), nn.BatchNorm3d(cout), nn.ReLU(True))
 
-    def forward(self, x):
-        return self.block(x)
+    def forward(self, x, conv=None):
+        return _seq(self.block, x, conv)
 
 
 # (level, encoder channels in->out); decoder mirrors it. reference v2v.py:73-101
@@ -77,14 +86,14 @@ class EncoderDecorder(nn.Module):  # (sic) the reference's class name
         for lvl, cin, _ in _ENC:
             setattr(self, "skip_res%d" % lvl, Res3DBlock(cin, cin))
 
-    def forward(self, x):
+    def forward(self, x, conv=None):
         skips = {}
         for lvl, _, _ in _ENC:
-            skips[lvl] = getattr(self, "skip_res%d" % lvl)(x)
-            x = getattr(self, "encoder_res%d" % lvl)(getattr(self, "encoder_pool%d" % lvl)(x))
-        x = self.mid_res(x)
+            skips[lvl] = getattr(self, "skip_res%d" % lvl)(x, conv)
+            x = getattr(self, "encoder_res%d" % lvl)(getattr(self, "encoder_pool%d" % lvl)(x), conv)
+        x = self.mid_res(x, conv)
         for lvl, _, _ in _DEC:
-            x = getattr(self, "decoder_upsample%d" % lvl)(getattr(self, "decoder_res%d" % lvl)(x)) + skips[lvl]
+            x = getattr(self, "decoder_upsample%d" % lvl)(getattr(self, "decoder_res%d" % lvl)(x, conv), conv) + skips[lvl]
         return x
 
 
@@ -102,5 +111,10 @@ class V2VModel(nn.Module):
                 nn.init.xavier_normal_(m.weight)
                 nn.init.constant_(m.bias, 0)
 
-    def forward(self, x):
-        return self.output_layer(self.back_layers(self.encoder_decoder(self.front_layers(x))))
+    def forward(self, x, conv=None):
+        for blk in self.front_layers:
+            x = blk(x, conv)
+        x = self.encoder_decoder(x, conv)
+        for blk in self.back_layers:
+            x = blk(x, conv)
+        return self.output_layer(x) if conv is None else conv(self.output_layer, x)
