@@ -210,7 +210,9 @@ typedef struct lt_conv_desc {
                                 Cout/G channels, block g = (a*ogh + b)*ogw + c being written (and its residual read) at the output
                                 offset (ood + a, ooh + b, oow + c) with channel index 0..Cout/G-1 (FC == Cout/G).  A k2 s2
                                 transposed conv (v2v.py:54-66) is ONE 1x1x1 GEMM this way: N = 8 x Cout, osd=osh=osw=2, ogd=ogh=ogw=2;
-                                scale/shift carry Cout entries (the per-channel values repeated G times).  LT_CONV_TC / TC1 only */
+                                scale/shift carry Cout entries (the per-channel values repeated G times).  A stride-2 data gradient
+                                writes all input phases this way (fp32 or split-fp16 output); group g stores only the positions of
+                                its phase inside the FD x FH x FW tensor.  LT_CONV_TC / TC1 only */
   int reserved0;             /* set to 0 (keeps the pointer below 8-byte aligned without implicit padding) */
   void* workspace;           /* optional device scratch for split-K (LT_CONV_TC / TC1 layers whose tiles fill the SMs
                                 unevenly: the K loop is spread over more CTAs and summed in a fixed order, see

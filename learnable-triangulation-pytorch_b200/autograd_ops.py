@@ -202,9 +202,9 @@ def integrate_tensor_3d_with_coordinates(volumes, coord_volumes, softmax=True):
     return IntegrateTensor3dFn.apply(volumes, coord_volumes, softmax)
 
 
-# ---- V2V convolutions for training (v2v_backend="native"): forward and data gradient on the forward conv kernels, weight gradient on
-# csrc/conv_wgrad.cu.  Activations are float32 channels_last_3d tensors, so the kernels read and write them in place of a transpose
-# and torch's BatchNorm / ReLU / pooling / adds run on them unchanged.
+# ---- Convolutions for training (v2v_backend="native", backbone_backend="native"): forward and data gradient on the forward conv
+# kernels, weight gradient on csrc/conv_wgrad.cu.  Activations are float32 channels_last(_3d) tensors, so the kernels read and write
+# them in place of a transpose and torch's BatchNorm / ReLU / pooling / adds run on them unchanged.  A 2-D map is a 3-D one with D = 1.
 
 class _Filter:
     """The nn.Conv attributes engine.pack_conv reads, for a filter that is not (or not only) a module's own."""
@@ -230,11 +230,25 @@ def _round_up(v, m):
     return (v + m - 1) // m * m
 
 
+def _as3(t, fill):
+    """A 2-D conv attribute (h, w) as its 3-D form (fill, h, w); 3-tuples pass unchanged."""
+    t = tuple(t)
+    return (fill,) * (3 - len(t)) + t
+
+
 def _cl(x):
-    """(N, C, D, H, W) -> contiguous float32 (N, D, H, W, C) (a view for channels_last_3d input)."""
+    """(N, C, [D,] H, W) -> contiguous float32 (N, D, H, W, C), D = 1 for 2-D maps (a view for channels_last(_3d) input)."""
     if not x.is_cuda:
-        raise RuntimeError("lt_b200 native V2V convolutions need CUDA tensors (got %s)" % x.device)
+        raise RuntimeError("lt_b200 native training convolutions need CUDA tensors (got %s)" % x.device)
+    if x.dim() == 4:
+        return x.float().contiguous(memory_format=torch.channels_last).permute(0, 2, 3, 1).unsqueeze(1)
     return x.float().contiguous(memory_format=torch.channels_last_3d).permute(0, 2, 3, 4, 1)
+
+
+def _from_cl(out, c, nd):
+    """(N, D, H, W, C') channels-last -> the (N, c, [D,] H, W) view of its first c channels (nd = 2 drops D = 1)."""
+    out = out[..., :c]
+    return out[:, 0].permute(0, 3, 1, 2) if nd == 2 else out.permute(0, 4, 1, 2, 3)
 
 
 def _to_s32(x_cl, cp, absmax_bits=None, inv_scale=None):
@@ -244,18 +258,26 @@ def _to_s32(x_cl, cp, absmax_bits=None, inv_scale=None):
     return out
 
 
-def conv_desc(N, in_dims, cin_p, cout_p, k, stride, pad, out_dims, out_c, out_fmt, out_scale=(1, 1, 1), out_full=None, groups=(1, 1, 1)):
+def conv_desc(N, in_dims, cin_p, cout_p, k, stride, pad, out_dims, out_c, out_fmt, out_scale=(1, 1, 1), out_full=None, groups=(1, 1, 1),
+              out_off=(0, 0, 0)):
     """lt_conv_desc of a split-fp16-input launch without ReLU or residual; out_full: the output tensor's grid (default out_dims)."""
     fd, fh, fw = out_full or out_dims
     return capi.ConvDesc(N=N, ID=in_dims[0], IH=in_dims[1], IW=in_dims[2], Cin=cin_p, OD=out_dims[0], OH=out_dims[1], OW=out_dims[2],
                          Cout=cout_p, KD=k[0], KH=k[1], KW=k[2], sd=stride[0], sh=stride[1], sw=stride[2], pd=pad[0], ph=pad[1], pw=pad[2],
-                         FD=fd, FH=fh, FW=fw, FC=out_c, osd=out_scale[0], osh=out_scale[1], osw=out_scale[2], relu=0, residual=capi.RES_NONE,
+                         FD=fd, FH=fh, FW=fw, FC=out_c, osd=out_scale[0], osh=out_scale[1], osw=out_scale[2],
+                         ood=out_off[0], ooh=out_off[1], oow=out_off[2], relu=0, residual=capi.RES_NONE,
                          in_format=capi.FMT_S32, out_format=out_fmt, ogd=groups[0], ogh=groups[1], ogw=groups[2])
 
 
-def conv3d_wgrad_desc(N, dims, cin, cout, k, padding):
-    """The forward launch of a stride-1 Conv3d as lt_conv_wgrad_fwd reads it: split-fp16 input and output gradient, 32-channel padded."""
-    return conv_desc(N, dims, _round_up(cin, 32), _round_up(cout, 32), k, (1, 1, 1), padding, dims, _round_up(cout, 32), capi.FMT_S32)
+def conv_out_dims(dims, k, stride, padding):
+    return tuple((n + 2 * p - kk) // s + 1 for n, kk, s, p in zip(dims, k, stride, padding))
+
+
+def conv3d_wgrad_desc(N, dims, cin, cout, k, padding, stride=(1, 1, 1)):
+    """The forward launch of a convolution (3-D form: a 2-D one has D = 1) as lt_conv_wgrad_fwd reads it: split-fp16 input and
+    output gradient, 32-channel padded."""
+    return conv_desc(N, dims, _round_up(cin, 32), _round_up(cout, 32), k, stride, padding, conv_out_dims(dims, k, stride, padding),
+                     _round_up(cout, 32), capi.FMT_S32)
 
 
 def conv_transpose3d_desc(N, dims, cin, cout):
@@ -266,12 +288,47 @@ def conv_transpose3d_desc(N, dims, cin, cout):
 
 
 def conv3d_dgrad_filter(weight_shape, padding):
-    """Data gradient of a stride-1 'same' Conv3d (Cout, Cin, kd, kh, kw) as a forward conv of dY: lt_conv_gather_weights_fwd source
-    (base, (s_td, s_th, s_tw, s_ci, s_co)) of the filter flipped in space with Cin and Cout swapped -- element (td, th, tw, ci' = co,
-    co' = ci) = w[co][ci][kd-1-td][kh-1-th][kw-1-tw] -- and the conv's (k, stride, pad, cin', cout')."""
-    cout, cin, kd, kh, kw = weight_shape
+    """Data gradient of a stride-1 'same' convolution (Cout, Cin, [kd,] kh, kw) as a forward conv of dY: lt_conv_gather_weights_fwd
+    source (base, (s_td, s_th, s_tw, s_ci, s_co)) of the filter flipped in space with Cin and Cout swapped -- element (td, th, tw,
+    ci' = co, co' = ci) = w[co][ci][kd-1-td][kh-1-th][kw-1-tw] -- and the conv's (k, stride, pad, cin', cout') in 3-D form.  With
+    1x1 filters it is the transposed filter of any stride."""
+    cout, cin = weight_shape[:2]
+    kd, kh, kw = _as3(weight_shape[2:], 1)
     T = kd * kh * kw
-    return (T - 1, (-kh * kw, -kw, -1, cin * T, T)), (kd, kh, kw), (1, 1, 1), tuple(padding), cout, cin
+    return (T - 1, (-kh * kw, -kw, -1, cin * T, T)), (kd, kh, kw), (1, 1, 1), _as3(padding, 0), cout, cin
+
+
+def conv_s2_dgrad_filter(weight_shape, stride):
+    """Data gradient of a 3-tap stride-2 pad-1 convolution (Cout, Cin, [kd,] kh, kw) as ONE grouped forward conv of dY.
+
+    Along a stride-2 axis, input phase a of dX reads dY positions {m, m+1} only: a = 0 takes tap 1 at m, a = 1 takes tap 2 at m
+    and tap 0 at m+1.  So all phases together are a 2-tap stride-1 pad-0 conv of dY (reads past the end arrive as TMA zero fill)
+    with one Cin-wide column block per phase, block g = (a ogh + b) ogw + c written to input phase (a, b, c) at output scale 2.
+    Tap u of phase a reads kernel index 1 + 2u (a = 0) or 2 - 2u (a = 1) of the filter zero-padded to 4 along every stride-2 axis:
+    index 3 is the zero of the tap phase 0 does not use.  Returns ([lt_conv_gather_weights_fwd (base, strides) per block, into the
+    padded filter], k, pad, groups, cin', cout') in 3-D form."""
+    cout, cin = weight_shape[:2]
+    k3, s3 = _as3(weight_shape[2:], 1), _as3(stride, 1)
+    kp = tuple(4 if s == 2 else kk for kk, s in zip(k3, s3))          # the padded filter's extents
+    tap_stride = (kp[1] * kp[2], kp[2], 1)
+    T = kp[0] * kp[1] * kp[2]
+    phases = [((1, 2), (2, -2)) if s == 2 else ((0, 0),) for s in s3]  # per axis and phase: (first kernel index, step per tap)
+    srcs = []
+    for pa in phases[0]:
+        for pb in phases[1]:
+            for pc in phases[2]:
+                base = pa[0] * tap_stride[0] + pb[0] * tap_stride[1] + pc[0] * tap_stride[2]
+                srcs.append((base, (pa[1] * tap_stride[0], pb[1] * tap_stride[1], pc[1] * tap_stride[2], cin * T, T)))
+    k = tuple(2 if s == 2 else 1 for s in s3)
+    return srcs, k, (0, 0, 0), tuple(2 if s == 2 else 1 for s in s3), cout, cin
+
+
+def pad_s2_filter(weight, stride):
+    """The filter zero-padded to 4 taps along every stride-2 axis (conv_s2_dgrad_filter's source)."""
+    pads = []
+    for s in reversed(_as3(stride, 1)[3 - (weight.dim() - 2):]):
+        pads += [0, 1 if s == 2 else 0]
+    return torch.nn.functional.pad(weight, pads)
 
 
 def conv_transpose3d_dgrad_filter(weight_shape):
@@ -281,14 +338,23 @@ def conv_transpose3d_dgrad_filter(weight_shape):
     return (0, (4, 2, 1, 8, cout * 8)), (2, 2, 2), (2, 2, 2), (0, 0, 0), cout, cin
 
 
-def _launch(x_s, cin_p, pk, out_dims, out_c, scale, shift, out_fmt=capi.FMT_F32, out_scale=(1, 1, 1), out_full=None, groups=(1, 1, 1)):
-    """One lt_conv_nd_fwd of packed filter `pk` over split-fp16 x_s; the full-resolution 3^3 / 7^3 layers take LT_CONV_TC_FOLD as in
-    the inference engine."""
+def conv_transpose2d_k4s2_dgrad_filter(weight_shape):
+    """Data gradient of ConvTranspose2d(k=4, s=2, p=1) (Cin, Cout, 4, 4): dX[i] = sum_{ky, co} dY[2 i - 1 + ky][co] w[ci][co][ky], a
+    4x4 stride-2 pad-1 conv of dY with element (th, tw, ci' = co, co' = ci) = w[ci][co][th][tw] (no flip); 3-D form."""
+    cin, cout = weight_shape[:2]
+    return (0, (0, 4, 1, 16, cout * 16)), (1, 4, 4), (1, 2, 2), (0, 1, 1), cout, cin
+
+
+def _launch(x_s, cin_p, pk, out_dims, out_c, scale, shift, out_fmt=capi.FMT_F32, out_scale=(1, 1, 1), out_full=None, groups=(1, 1, 1),
+            out_off=(0, 0, 0), out=None):
+    """One lt_conv_nd_fwd of packed filter `pk` over split-fp16 x_s into `out` (allocated when None); the full-resolution 3^3 / 7^3
+    layers take LT_CONV_TC_FOLD as in the inference engine."""
     N, D, H, W = x_s.shape[:4]
     fd, fh, fw = out_full or out_dims
     c_store = out_c if out_fmt == capi.FMT_F32 else 2 * out_c
-    out = torch.empty((N, fd, fh, fw, c_store), dtype=torch.float32 if out_fmt == capi.FMT_F32 else torch.float16, device=x_s.device)
-    d = conv_desc(N, (D, H, W), cin_p, pk.cout_p, pk.k, pk.stride, pk.pad, out_dims, out_c, out_fmt, out_scale, out_full, groups)
+    if out is None:
+        out = torch.empty((N, fd, fh, fw, c_store), dtype=torch.float32 if out_fmt == capi.FMT_F32 else torch.float16, device=x_s.device)
+    d = conv_desc(N, (D, H, W), cin_p, pk.cout_p, pk.k, pk.stride, pk.pad, out_dims, out_c, out_fmt, out_scale, out_full, groups, out_off)
     ws = _workspace(x_s.device, 0)
     d.workspace, d.workspace_bytes = ws.data_ptr(), ws.numel()
     impl, weight = capi.CONV_TC, pk.w
@@ -316,51 +382,101 @@ def _wgrad(desc, x_s, g_s, amax, cin, cout, taps, groups=1):
     return gw
 
 
-class Conv3dFn(torch.autograd.Function):
-    """nn.Conv3d with stride 1 and "same" padding (every Conv3d of v2v.py) on the tensor-core kernels, fp32-grade in all three passes.
-    forward: lt_conv_nd_fwd (scale 1 / S, shift = bias); data gradient: the same kernels over the output gradient with the filter
-    flipped in space and Cin / Cout swapped (re-gathered by lt_conv_gather_weights_fwd with negated tap strides); weight gradient:
-    lt_conv_wgrad_fwd; bias gradient: torch's sum of the output gradient."""
+def conv_kind(k, stride, padding):
+    """The supported geometry of a convolution in 3-D form: "same" (stride 1, odd kernel, padding k // 2), "s2k1" (1x1, stride 2 on
+    the strided axes) or "s2k3" (3 taps, stride 2, padding 1 on the strided axes; 1x1 on the others); ValueError otherwise."""
+    if all(s == 1 for s in stride):
+        if all(kk % 2 == 1 and p == kk // 2 for kk, p in zip(k, padding)):
+            return "same"
+    elif all(s in (1, 2) for s in stride):
+        strided = {(kk, p) for kk, s, p in zip(k, stride, padding) if s == 2}
+        plain_ok = all(kk == 1 and p == 0 for kk, s, p in zip(k, stride, padding) if s == 1)
+        if plain_ok and strided == {(1, 0)}:
+            return "s2k1"
+        if plain_ok and strided == {(3, 1)}:
+            return "s2k3"
+    raise ValueError("native conv: stride-1 'same' convolutions (odd kernel, padding k // 2), 1x1 stride 2 and 3-tap stride-2 "
+                     "pad-1 convolutions only, got k=%s stride=%s padding=%s" % (tuple(k), tuple(stride), tuple(padding)))
+
+
+def conv_s2_dgrad(g_s, weight, stride, in_dims, inv, out=None):
+    """dX (N, D, H, W, Cin) float32 of a 3-tap stride-2 pad-1 conv from the split-fp16 scaled output gradient g_s (1 / scale on the
+    device in `inv`): ONE grouped launch (conv_s2_dgrad_filter) writing every input phase over its own extent; into `out` if given."""
+    from .engine import pack_filter
+    cout, cin = weight.shape[:2]
+    srcs, k, pad, groups, ci, co = conv_s2_dgrad_filter(weight.shape, stride)
+    wp = pad_s2_filter(weight.detach().float(), stride).contiguous()
+    pk = pack_filter([(wp, base, strides) for base, strides in srcs], k, (1, 1, 1), pad, ci, co, None, None, out_fmt=capi.FMT_F32)
+    out, _ = _launch(g_s, _round_up(cout, 32), pk, tuple(g_s.shape[1:4]), cin, pk.scale * inv, pk.shift, out_scale=groups,
+                     out_full=in_dims, groups=groups, out=out)
+    return out
+
+
+class ConvNdFn(torch.autograd.Function):
+    """nn.Conv2d / nn.Conv3d on the tensor-core kernels, fp32-grade in all three passes, for the geometries of conv_kind (every conv
+    of v2v.py and of the backbone but its stem).  forward: lt_conv_nd_fwd (scale 1 / S, shift = bias).  Data gradient, as forward
+    convs of the output gradient: stride 1 -- the filter flipped in space with Cin / Cout swapped (re-gathered by
+    lt_conv_gather_weights_fwd with negated tap strides); 1x1 stride 2 -- the transposed filter into the even phase of dX (the
+    other phases are zero); 3-tap stride 2 -- one grouped launch writing every input phase (conv_s2_dgrad_filter).  Weight
+    gradient: lt_conv_wgrad_fwd on the forward's descriptor; bias gradient: torch's sum of the output gradient.  The float32 input
+    is saved (the tensor torch keeps anyway) and split to fp16 pairs again in the backward."""
 
     @staticmethod
-    def forward(ctx, x, weight, bias, padding):
+    def forward(ctx, x, weight, bias, stride, padding):
         from .engine import pack_conv
-        cout, cin, kd, kh, kw = weight.shape
-        if tuple(padding) != (kd // 2, kh // 2, kw // 2) or not (kd % 2 and kh % 2 and kw % 2):
-            raise ValueError("native Conv3d: stride 1 'same' convolutions only (odd kernel, padding k // 2), got k=%s padding=%s"
-                             % ((kd, kh, kw), tuple(padding)))
+        nd = weight.dim() - 2
+        cout, cin = weight.shape[:2]
+        k, st, pad = _as3(weight.shape[2:], 1), _as3(stride, 1), _as3(padding, 0)
+        kind = conv_kind(k, st, pad)
+        if kind == "s2k3" and cin % 32:
+            raise ValueError("native conv: 3-tap stride-2 convolutions need Cin % 32 == 0 (grouped data gradient), got %d" % cin)
         x_cl = _cl(x)
+        in_dims = tuple(x_cl.shape[1:4])
+        if kind == "s2k3" and any(n < 2 for n, s in zip(in_dims, st) if s == 2):
+            raise ValueError("native conv: 3-tap stride-2 convolutions need map sides of at least 2, got %s" % (in_dims,))
         cin_p = _round_up(cin, 32)
         x_s = _to_s32(x_cl, cin_p)
-        pk = pack_conv(_Filter(weight.detach(), None if bias is None else bias.detach(), (1, 1, 1), padding), None, cin_pad=cin_p,
+        pk = pack_conv(_Filter(weight.detach(), None if bias is None else bias.detach(), stride, padding), None, cin_pad=cin_p,
                        out_fmt=capi.FMT_F32)
-        out, _ = _launch(x_s, cin_p, pk, x_cl.shape[1:4], _round_up(cout, 4), pk.scale, pk.shift)
-        ctx.save_for_backward(x_s, weight)
-        ctx.padding = tuple(padding)
-        return out[..., :cout].permute(0, 4, 1, 2, 3)
+        out, _ = _launch(x_s, cin_p, pk, conv_out_dims(in_dims, k, st, pad), _round_up(cout, 4), pk.scale, pk.shift)
+        ctx.save_for_backward(x, weight)
+        ctx.geom = (k, st, pad, kind, in_dims)
+        return _from_cl(out, cout, nd)
 
     @staticmethod
     def backward(ctx, grad_out):
         from .engine import pack_filter
-        x_s, weight = ctx.saved_tensors
-        cout, cin, kd, kh, kw = weight.shape
-        T = kd * kh * kw
+        x, weight = ctx.saved_tensors
+        k, st, pad, kind, in_dims = ctx.geom
+        nd = weight.dim() - 2
+        cout, cin = weight.shape[:2]
+        T = k[0] * k[1] * k[2]
         cout_p = _round_up(cout, 32)
         g_s, g, amax, inv = _grad_s32(grad_out, cout_p)
-        N, D, H, W = g.shape[:4]
+        N, OD, OH, OW = g.shape[:4]
         gx = gw = gb = None
         if ctx.needs_input_grad[0]:
             w = weight.detach().float().contiguous()
-            (base, strides), k, stride, pad, ci, co = conv3d_dgrad_filter(weight.shape, ctx.padding)
-            pk = pack_filter((w, base, strides), k, stride, pad, ci, co, None, None, out_fmt=capi.FMT_F32)
-            out, _ = _launch(g_s, cout_p, pk, (D, H, W), _round_up(cin, 4), pk.scale * inv, pk.shift)
-            gx = out[..., :cin].permute(0, 4, 1, 2, 3)
+            if kind == "s2k3":
+                out = conv_s2_dgrad(g_s, w, st, in_dims, inv)
+            else:
+                (base, strides), kk, _, pd, ci, co = conv3d_dgrad_filter(weight.shape, pad)
+                pk = pack_filter((w, base, strides), kk, (1, 1, 1), pd, ci, co, None, None, out_fmt=capi.FMT_F32)
+                if kind == "same":
+                    out, _ = _launch(g_s, cout_p, pk, in_dims, _round_up(cin, 4), pk.scale * inv, pk.shift)
+                else:   # s2k1: dX is zero off the even phase
+                    out = torch.zeros((N,) + in_dims + (_round_up(cin, 4),), dtype=torch.float32, device=g.device)
+                    _launch(g_s, cout_p, pk, (OD, OH, OW), _round_up(cin, 4), pk.scale * inv, pk.shift, out_scale=st, out_full=in_dims,
+                            out=out)
+            gx = _from_cl(out, cin, nd)
         if ctx.needs_input_grad[1]:
-            d = conv3d_wgrad_desc(N, (D, H, W), cin, cout, (kd, kh, kw), ctx.padding)
-            gw = _wgrad(d, x_s, g_s, amax, cin, cout, T).reshape(kd, kh, kw, cin, cout).permute(4, 3, 0, 1, 2).contiguous()
+            x_s = _to_s32(_cl(x), _round_up(cin, 32))
+            d = conv3d_wgrad_desc(N, in_dims, cin, cout, k, pad, st)
+            gw = _wgrad(d, x_s, g_s, amax, cin, cout, T).reshape(T, cin, cout).permute(2, 1, 0).reshape(weight.shape).contiguous()
         if ctx.needs_input_grad[2]:
             gb = g.sum(dim=(0, 1, 2, 3))
-        return gx, gw, gb, None
+        return gx, gw, gb, None, None
+
 
 
 class ConvTranspose3dFn(torch.autograd.Function):
@@ -384,16 +500,16 @@ class ConvTranspose3dFn(torch.autograd.Function):
                          out_full=(2 * D, 2 * H, 2 * W), groups=(2, 2, 2))
         out = torch.empty((N, 2 * D, 2 * H, 2 * W, cout), dtype=torch.float32, device=x.device)
         capi.s32_to_f32(y_s, out, out[..., 0].numel(), cout)
-        ctx.save_for_backward(x_s, weight)
+        ctx.save_for_backward(x, weight)
         return out.permute(0, 4, 1, 2, 3)
 
     @staticmethod
     def backward(ctx, grad_out):
         from .engine import pack_filter
-        x_s, weight = ctx.saved_tensors
+        x, weight = ctx.saved_tensors
         cin, cout = weight.shape[:2]
         g_s, g, amax, inv = _grad_s32(grad_out, cout)
-        N, D, H, W = x_s.shape[:4]
+        N, D, H, W = x.shape[0], x.shape[2], x.shape[3], x.shape[4]
         gx = gw = gb = None
         if ctx.needs_input_grad[0]:
             w = weight.detach().float().contiguous()
@@ -402,6 +518,7 @@ class ConvTranspose3dFn(torch.autograd.Function):
             out, _ = _launch(g_s, cout, pk, (D, H, W), cin, pk.scale * inv, pk.shift)
             gx = out.permute(0, 4, 1, 2, 3)
         if ctx.needs_input_grad[1]:
+            x_s = _to_s32(_cl(x), cin)
             gw = _wgrad(conv_transpose3d_desc(N, (D, H, W), cin, cout), x_s, g_s, amax, cin, cout, 1, groups=8)       # [1][ci][g cout + co], g = a 4 + b 2 + c
             gw = gw.reshape(cin, 8, cout).permute(0, 2, 1).reshape(cin, cout, 2, 2, 2).contiguous()
         if ctx.needs_input_grad[2]:
@@ -409,14 +526,162 @@ class ConvTranspose3dFn(torch.autograd.Function):
         return gx, gw, gb
 
 
+def conv_transpose2d_k4s2_desc(N, dims, cin, cout, py, px):
+    """Phase (py, px) of ConvTranspose2d(k=4, s=2, p=1) as the forward launches it (the engine's 2x2 stride-1 conv into the
+    (py, px) sub-lattice of the 2H x 2W output), 3-D form with split-fp16 output gradient: lt_conv_wgrad_fwd's descriptor."""
+    from .engine import deconv2d_k4s2_phase
+    _, H, W = dims
+    cin_p, cout_p = _round_up(cin, 32), _round_up(cout, 32)
+    _, pad = deconv2d_k4s2_phase(py, px, cout)
+    return conv_desc(N, dims, cin_p, cout_p, (1, 2, 2), (1, 1, 1), pad, dims, cout_p, capi.FMT_S32, out_scale=(1, 2, 2),
+                     out_full=(1, 2 * H, 2 * W), out_off=(0, py, px))
+
+
+def conv_transpose2d_k4s2_wgrad_scatter(gw, py, px):
+    """Weight gradient [4 taps (i, j)][cin][cout] of phase (py, px) -> its (cin, cout, 2, 2) share of dW at kernel rows / columns
+    1 - py + 2 (1 - i) and 1 - px + 2 (1 - j) (tap i reads ky = 3 - py - 2i): assign to dW[:, :, 1 - py::2, 1 - px::2]."""
+    cin, cout = gw.shape[1:]
+    return gw.reshape(2, 2, cin, cout).flip(0, 1).permute(2, 3, 0, 1)
+
+
+class ConvTranspose2dK4Fn(torch.autograd.Function):
+    """nn.ConvTranspose2d(k=4, s=2, p=1) (the backbone's deconv_layers) on the tensor-core kernels: the forward is the inference
+    engine's four 2x2 stride-1 phase launches into one float32 output; the data gradient is a 4x4 stride-2 pad-1 conv of the output
+    gradient with the filter unflipped (Cin' = Cout, Cout' = Cin); the weight gradient is one lt_conv_wgrad_fwd per phase, each of the
+    16 taps belonging to exactly one phase."""
+
+    @staticmethod
+    def forward(ctx, x, weight, bias):
+        from .engine import pack_deconv2d_k4s2
+        cin, cout = weight.shape[:2]
+        x_cl = _cl(x)
+        N, _, H, W = x_cl.shape[:4]
+        cin_p, c_store = _round_up(cin, 32), _round_up(cout, 4)
+        x_s = _to_s32(x_cl, cin_p)
+        phases = pack_deconv2d_k4s2(_Filter(weight.detach(), None if bias is None else bias.detach(), (2, 2), (1, 1)), None,
+                                    out_fmt=capi.FMT_F32)
+        out = torch.empty((N, 1, 2 * H, 2 * W, c_store), dtype=torch.float32, device=x.device)
+        for (py, px), pk in phases.items():
+            _launch(x_s, cin_p, pk, (1, H, W), c_store, pk.scale, pk.shift, out_scale=(1, 2, 2), out_full=(1, 2 * H, 2 * W),
+                    out_off=(0, py, px), out=out)
+        ctx.save_for_backward(x, weight)
+        return _from_cl(out, cout, 2)
+
+    @staticmethod
+    def backward(ctx, grad_out):
+        from .engine import pack_filter
+        x, weight = ctx.saved_tensors
+        cin, cout = weight.shape[:2]
+        N, _, H, W = x.shape
+        cout_p = _round_up(cout, 32)
+        g_s, g, amax, inv = _grad_s32(grad_out, cout_p)
+        gx = gw = gb = None
+        if ctx.needs_input_grad[0]:
+            w = weight.detach().float().contiguous()
+            (base, strides), k, stride, pad, ci, co = conv_transpose2d_k4s2_dgrad_filter(weight.shape)
+            pk = pack_filter((w, base, strides), k, stride, pad, ci, co, None, None, out_fmt=capi.FMT_F32)
+            out, _ = _launch(g_s, cout_p, pk, (1, H, W), _round_up(cin, 4), pk.scale * inv, pk.shift)
+            gx = _from_cl(out, cin, 2)
+        if ctx.needs_input_grad[1]:
+            x_s = _to_s32(_cl(x), _round_up(cin, 32))
+            gw = torch.empty((cin, cout, 4, 4), dtype=torch.float32, device=g.device)
+            for py in (0, 1):
+                for px in (0, 1):
+                    gp = _wgrad(conv_transpose2d_k4s2_desc(N, (1, H, W), cin, cout, py, px), x_s, g_s, amax, cin, cout, 4)
+                    gw[:, :, 1 - py::2, 1 - px::2] = conv_transpose2d_k4s2_wgrad_scatter(gp, py, px)
+        if ctx.needs_input_grad[2]:
+            gb = g.sum(dim=(0, 1, 2, 3))
+        return gx, gw, gb
+
+
+def stem_wgrad_desc(N, H, W, cout):
+    """The stem's 4x4 stride-1 conv (front pad 2) over the (N, H/2, W/2, 32) space-to-depth input, 3-D form, as lt_conv_wgrad_fwd
+    reads it."""
+    dims = (1, H // 2, W // 2)
+    return conv_desc(N, dims, 32, _round_up(cout, 32), (1, 4, 4), (1, 1, 1), (0, 2, 2), dims, _round_up(cout, 32), capi.FMT_S32)
+
+
+def stem_wgrad_index(device):
+    """For every element (c, ky, kx) of a (3, 7, 7) stem filter, its row (tap (a, b), s2d channel) in the [16][12] rows of the
+    s2d conv's weight gradient: ky = 2a + r - 1, kx = 2b + s - 1, channel (r 2 + s) 3 + c (engine.stem_s2d_filter).  Every element
+    has exactly one such row; the 45 rows whose ky or kx falls outside [0, 7) are dropped."""
+    c = torch.arange(3, device=device).view(3, 1, 1)
+    ky = torch.arange(7, device=device).view(1, 7, 1)
+    kx = torch.arange(7, device=device).view(1, 1, 7)
+    a, r = (ky + 1) // 2, (ky + 1) % 2
+    b, s = (kx + 1) // 2, (kx + 1) % 2
+    return ((a * 4 + b) * 12 + (r * 2 + s) * 3 + c).reshape(-1)
+
+
+class StemConvFn(torch.autograd.Function):
+    """The backbone's 7x7 stride-2 pad-3 stem on 3-channel images, as the tensor-core inference runs it: lt_stem_s2d_fwd packs the
+    images into the 2x2 space-to-depth split-fp16 input, then a 4x4 stride-1 conv (engine.pack_stem_s2d).  Weight gradient:
+    lt_conv_wgrad_fwd of that 4x4 conv (12 real input channels), mapped back to (Cout, 3, 7, 7).  No image gradient."""
+
+    @staticmethod
+    def forward(ctx, images, weight, bias):
+        from .engine import pack_stem_s2d
+        if not images.is_cuda:
+            raise RuntimeError("lt_b200 native training convolutions need CUDA tensors (got %s)" % images.device)
+        N, C, H, W = images.shape
+        cout = weight.shape[0]
+        img = images.detach().float().contiguous()
+        x_s = torch.empty((N, 1, H // 2, W // 2, 64), dtype=torch.float16, device=images.device)
+        capi.stem_s2d(img, x_s, N, C, H, W)
+        pk = pack_stem_s2d(_Filter(weight.detach(), None if bias is None else bias.detach(), (2, 2), (3, 3)), None, out_fmt=capi.FMT_F32)
+        out, _ = _launch(x_s, 32, pk, (1, H // 2, W // 2), _round_up(cout, 4), pk.scale, pk.shift)
+        ctx.save_for_backward(img, weight)
+        return _from_cl(out, cout, 2)
+
+    @staticmethod
+    def backward(ctx, grad_out):
+        img, weight = ctx.saved_tensors
+        N, C, H, W = img.shape
+        cout = weight.shape[0]
+        g_s, g, amax, inv = _grad_s32(grad_out, _round_up(cout, 32))
+        gw = gb = None
+        if ctx.needs_input_grad[1]:
+            x_s = torch.empty((N, 1, H // 2, W // 2, 64), dtype=torch.float16, device=img.device)
+            capi.stem_s2d(img, x_s, N, C, H, W)
+            gs = _wgrad(stem_wgrad_desc(N, H, W, cout), x_s, g_s, amax, 12, cout, 16)           # [tap a 4 + b][s2d channel][cout]
+            gw = gs.reshape(16 * 12, cout)[stem_wgrad_index(img.device)].t().reshape(cout, 3, 7, 7).contiguous()
+        if ctx.needs_input_grad[2]:
+            gb = g.sum(dim=(0, 1, 2, 3))
+        return None, gw, gb
+
+
 def conv3d(x, weight, bias=None, padding=(0, 0, 0)):
     """F.conv3d(x, weight, bias, 1, padding) for stride-1 'same' filters on the native training kernels."""
-    return Conv3dFn.apply(x, weight, bias, tuple(padding))
+    return ConvNdFn.apply(x, weight, bias, (1, 1, 1), tuple(padding))
+
+
+def conv2d(x, weight, bias=None, stride=(1, 1), padding=(0, 0)):
+    """F.conv2d(x, weight, bias, stride, padding) for the geometries of conv_kind on the native training kernels."""
+    return ConvNdFn.apply(x, weight, bias, tuple(stride), tuple(padding))
 
 
 def conv_transpose3d(x, weight, bias=None):
     """F.conv_transpose3d(x, weight, bias, stride=2) for 2^3 filters on the native training kernels."""
     return ConvTranspose3dFn.apply(x, weight, bias)
+
+
+def conv_transpose2d_k4s2(x, weight, bias=None):
+    """F.conv_transpose2d(x, weight, bias, stride=2, padding=1) for 4x4 filters on the native training kernels."""
+    if tuple(weight.shape[2:]) != (4, 4):
+        raise ValueError("native ConvTranspose2d: 4x4 filters only, got %s" % (tuple(weight.shape),))
+    return ConvTranspose2dK4Fn.apply(x, weight, bias)
+
+
+def stem_conv(images, weight, bias=None):
+    """F.conv2d(images, weight, bias, 2, 3) for a (Cout, 3, 7, 7) stem filter on the native training kernels (no image gradient)."""
+    if tuple(weight.shape[1:]) != (3, 7, 7) or images.dim() != 4 or images.shape[1] != 3:
+        raise ValueError("native stem: 3-channel images and (Cout, 3, 7, 7) filters only, got %s and %s"
+                         % (tuple(images.shape), tuple(weight.shape)))
+    if images.shape[2] % 2 or images.shape[3] % 2:
+        raise ValueError("native stem: even image sides only (space-to-depth input), got %dx%d" % tuple(images.shape[2:]))
+    if images.requires_grad and torch.is_grad_enabled():
+        raise ValueError("native stem: image gradients are not computed; the images must not require grad")
+    return StemConvFn.apply(images, weight, bias)
 
 
 def v2v_conv(module, x):
@@ -428,3 +693,25 @@ def v2v_conv(module, x):
     if tuple(module.stride) != (1, 1, 1) or module.groups != 1 or tuple(module.dilation) != (1, 1, 1):
         raise ValueError("native Conv3d: stride 1, no groups, no dilation only")
     return conv3d(x, module.weight, module.bias, module.padding)
+
+
+def backbone_conv(module, x):
+    """A Conv2d / ConvTranspose2d module of the 2-D backbone (pose_resnet.py), its confidence heads or `process_features` applied
+    through the native functions (the module's own parameters): the 7x7 stride-2 stem on 3-channel images, stride-1 'same',
+    1x1 stride-2 and 3x3 stride-2 pad-1 convs, and k4 s2 p1 transposed convs.  ValueError for anything else."""
+    if isinstance(module, torch.nn.ConvTranspose2d):
+        if (tuple(module.kernel_size) != (4, 4) or tuple(module.stride) != (2, 2) or tuple(module.padding) != (1, 1)
+                or tuple(module.output_padding) != (0, 0) or module.groups != 1 or tuple(module.dilation) != (1, 1)
+                or module.padding_mode != "zeros"):
+            raise ValueError("native ConvTranspose2d: kernel 4, stride 2, padding 1, no output padding, groups or dilation only")
+        return conv_transpose2d_k4s2(x, module.weight, module.bias)
+    if not isinstance(module, torch.nn.Conv2d) or module.groups != 1 or tuple(module.dilation) != (1, 1):
+        raise ValueError("native Conv2d: no groups, no dilation only")
+    if isinstance(module.padding, str):
+        raise ValueError("native Conv2d: numeric padding only, got %r" % (module.padding,))
+    if module.padding_mode != "zeros":
+        raise ValueError("native Conv2d: zero padding only, got padding_mode=%r" % (module.padding_mode,))
+    if tuple(module.kernel_size) == (7, 7) and tuple(module.stride) == (2, 2) and tuple(module.padding) == (3, 3):
+        return stem_conv(x, module.weight, module.bias)
+    conv_kind(_as3(module.kernel_size, 1), _as3(module.stride, 1), _as3(module.padding, 0))
+    return conv2d(x, module.weight, module.bias, module.stride, module.padding)

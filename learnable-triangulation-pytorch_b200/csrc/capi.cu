@@ -101,8 +101,11 @@ extern "C" int lt_conv_nd_fwd(const lt_conv_desc* d, const void* in, const void*
   LT_REQUIRE(d->KD > 0 && d->KH > 0 && d->KW > 0 && d->sd > 0 && d->sh > 0 && d->sw > 0, "conv_nd: bad filter/stride");
   LT_REQUIRE(d->osd > 0 && d->osh > 0 && d->osw > 0, "conv_nd: bad output scale");
   const int gd = d->ogd > 1 ? d->ogd : 1, gh = d->ogh > 1 ? d->ogh : 1, gw = d->ogw > 1 ? d->ogw : 1;
-  LT_REQUIRE((d->OD - 1) * d->osd + d->ood + gd - 1 < d->FD && (d->OH - 1) * d->osh + d->ooh + gh - 1 < d->FH &&
-                 (d->OW - 1) * d->osw + d->oow + gw - 1 < d->FW && d->ood >= 0 && d->ooh >= 0 && d->oow >= 0,
+  // the output grid of group 0 lies inside the tensor and every group has a first position in it; a later group (an odd stride
+  // phase of an odd-sized tensor) stores only the positions inside (conv_tc's per-group output maps)
+  LT_REQUIRE((d->OD - 1) * d->osd + d->ood < d->FD && (d->OH - 1) * d->osh + d->ooh < d->FH && (d->OW - 1) * d->osw + d->oow < d->FW &&
+                 d->ood + gd - 1 < d->FD && d->ooh + gh - 1 < d->FH && d->oow + gw - 1 < d->FW && d->ood >= 0 && d->ooh >= 0 &&
+                 d->oow >= 0,
              "conv_nd: output mapping exceeds the output tensor");
   LT_REQUIRE(gd * gh * gw == 1 || impl == LT_CONV_TC || impl == LT_CONV_TC1,
              "conv_nd: grouped output (ogd/ogh/ogw) is only implemented by the tensor-core kernels");

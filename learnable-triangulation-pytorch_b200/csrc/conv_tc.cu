@@ -520,18 +520,31 @@ static void tc_plan(long m_tiles, int n_tiles, int nt, int chunks, int terms, in
   *grid_out = (int)(units < sm ? units : sm);
 }
 
+// Positions of one output axis that group phase `ph` of a launch writes: those of its sub-lattice off + ph + o os (o < n) that
+// lie inside the tensor's extent F, at most the launch's n.  A stride-2 data gradient of an odd-sized input has one position fewer
+// in its odd phase than in its even one; every other launch writes exactly n.
+static int group_extent(int n, int F, int off, int ph, int os) {
+  const int e = (F - off - ph + os - 1) / os;
+  return e < n ? e : n;
+}
+
 // Tensor maps of the staged epilogue.  Output position (ow, oh, od, nb) of group g is row ((nb FD + od osd + ood) FH + oh osh + ooh)
-// FW + ow osw + oow of the channels-last tensor plus the group's phase offset, so every output is a plain map over the launch's
-// OW x OH x OD x N grid: base at the (phase) origin, position strides scaled by osw / osh / osd.  Rows are FC x 4 bytes in both
-// formats (the C ABI requires FC % 4 == 0, so they are 16-byte multiples).
+// FW + ow osw + oow of the channels-last tensor plus the group's phase offset, so every output is a plain map over the group's
+// share of the launch's OW x OH x OD x N grid (group_extent): base at the (phase) origin, position strides scaled by osw / osh / osd,
+// so the TMA store clips what falls outside the tensor.  Rows are FC x 4 bytes in both formats (the C ABI requires FC % 4 == 0,
+// so they are 16-byte multiples).
 static int make_epi_maps(const TcParams& p, TcEpiMaps* m) {
   const int f32 = p.out_format == LT_FMT_F32;
   const uint64_t rowb = (uint64_t)p.FC * 4;
-  const uint64_t dims[5] = {(uint64_t)(f32 ? p.FC : 2 * p.FC), (uint64_t)p.OW, (uint64_t)p.OH, (uint64_t)p.OD, (uint64_t)p.N};
   const uint64_t str[4] = {rowb * p.osw, rowb * p.FW * p.osh, rowb * p.FW * p.FH * p.osd, rowb * p.FW * p.FH * p.FD};
   const uint32_t bx[5] = {f32 ? 32u : 64u, (uint32_t)p.bw, (uint32_t)p.bh, (uint32_t)p.bd, (uint32_t)p.bn};
   for (int g = 0; g < p.n_maps; ++g) {
-    const long pix0 = ((long)(p.ood + g / (p.gh * p.gw)) * p.FH + p.ooh + (g / p.gw) % p.gh) * p.FW + p.oow + g % p.gw;
+    const int ga = g / (p.gh * p.gw), gb = (g / p.gw) % p.gh, gc = g % p.gw;
+    const int ew = group_extent(p.OW, p.FW, p.oow, gc, p.osw), eh = group_extent(p.OH, p.FH, p.ooh, gb, p.osh),
+              ed = group_extent(p.OD, p.FD, p.ood, ga, p.osd);
+    LT_REQUIRE(ew > 0 && eh > 0 && ed > 0, "conv_tc: output group %d lies outside the %dx%dx%d output tensor", g, p.FD, p.FH, p.FW);
+    const uint64_t dims[5] = {(uint64_t)(f32 ? p.FC : 2 * p.FC), (uint64_t)ew, (uint64_t)eh, (uint64_t)ed, (uint64_t)p.N};
+    const long pix0 = ((long)(p.ood + ga) * p.FH + p.ooh + gb) * p.FW + p.oow + gc;
     int rc = make_map(&m->out[g], static_cast<const uint8_t*>(p.out) + pix0 * rowb, 5, dims, str, bx, nullptr, 1, f32);
     if (rc) return rc;
     if (p.residual == LT_RES_NONE) continue;
@@ -619,12 +632,12 @@ int make_in_map(CUtensorMap* tmA, const lt_conv_desc* d, int bw, int bh, int bd,
   return make_map(tmA, in, 5, dims, str, bx, es, 1);
 }
 
-// grouped output (k2 s2 transposed conv as one GEMM): every channel of the GEMM belongs to exactly one group, and a group fills the
-// output's channels exactly
+// grouped output (k2 s2 transposed conv, stride-2 data gradient: one GEMM, one output phase per channel block): every channel of the
+// GEMM belongs to exactly one group, and a group fills the output's channels exactly.  Split-fp16 or float32: the staged epilogue
+// stores whole 32-channel slabs of either format.
 static bool groups_ok(const lt_conv_desc* d, int CoutP) {
   const int G = out_groups(d);
-  return d->Cout % G == 0 && (d->Cout / G) % 32 == 0 && d->Cout / G == d->FC && CoutP == d->Cout && G <= kMaxOutMaps &&
-         d->out_format == LT_FMT_S32;
+  return d->Cout % G == 0 && (d->Cout / G) % 32 == 0 && d->Cout / G == d->FC && CoutP == d->Cout && G <= kMaxOutMaps;
 }
 
 // LT_CONV_TC (terms = 3) and LT_CONV_TC1 (terms = 1): weights packed as [tap][Cin/32][CoutP rows][32 hi | 32 lo] fp16,
@@ -643,7 +656,7 @@ int conv_tc_fwd_terms(const lt_conv_desc* d, const void* in, const void* weight,
   TcParams p;
   fill_params(d, p, CB, CoutP, Nt, terms, scale, shift, residual, out);
   if (p.n_maps > 1)
-    LT_REQUIRE(groups_ok(d, CoutP), "conv_tc: grouped output needs split-fp16 output, Cout / groups == FC, a multiple of 32");
+    LT_REQUIRE(groups_ok(d, CoutP), "conv_tc: grouped output needs Cout / groups == FC, a multiple of 32");
   CUtensorMap tmA, tmB;
   int rc = make_in_map(&tmA, d, p.bw, p.bh, p.bd, p.bn, in);
   if (rc) return rc;

@@ -174,6 +174,58 @@ def pack_deconv3d_k2s2(deconv, bn, mode="tc"):
     return phases
 
 
+def stem_s2d_filter(weight):
+    """7x7 stride-2 pad-3 stem filter (Cout, 3, 7, 7) -> canonical [4][4][32][Cout] filter of the equivalent 4x4 stride-1 conv
+    (front pad 2) over the 2x2 space-to-depth input (lt_stem_s2d_fwd).
+
+    Input row 2*oy - 3 + ky = 2*(oy + a) + r with a = tap offset in {-2..1}, r = row parity: ky = 2a + r + 3, and likewise kx;
+    s2d channel (r*2 + s)*3 + c.  Taps with ky or kx outside [0, 7) and channels 12..31 are zero.  The re-indexing is not affine
+    in the s2d channel, so it is a gather on the filter's device (no host round trip)."""
+    cout = weight.shape[0]
+    dev = weight.device
+    a = torch.arange(4, device=dev).view(4, 1, 1)
+    b = torch.arange(4, device=dev).view(1, 4, 1)
+    ch = torch.arange(32, device=dev).view(1, 1, 32)
+    rs, c = ch // 3, ch % 3
+    ky, kx = 2 * a + rs // 2 - 1, 2 * b + rs % 2 - 1
+    valid = (ch < 12) & (ky >= 0) & (ky < 7) & (kx >= 0) & (kx < 7)
+    idx = torch.where(valid, (c * 7 + ky.clamp(0, 6)) * 7 + kx.clamp(0, 6), 0)          # (4, 4, 32) into w[co] flattened
+    w = weight.detach().float().reshape(cout, 3 * 49)
+    wt = w[:, idx.reshape(-1)].reshape(cout, 4, 4, 32).permute(1, 2, 3, 0)
+    return torch.where(valid.unsqueeze(-1), wt, torch.zeros((), dtype=torch.float32, device=dev)).contiguous()
+
+
+def pack_stem_s2d(conv, bn, mode="tc", **kw):
+    """The stem conv as the tensor-core modes run it: stem_s2d_filter packed as a 4x4 stride-1 conv over 32 s2d channels."""
+    assert tuple(conv.weight.shape[1:]) == (3, 7, 7) and tuple(conv.stride) == (2, 2) and tuple(conv.padding) == (3, 3)
+    cout = conv.weight.shape[0]
+    wt = stem_s2d_filter(conv.weight)
+    pk = pack_filter((wt, 0, (0, 4 * 32 * cout, 32 * cout, cout, 1)), (1, 4, 4), (1, 1, 1), (0, 2, 2), 32, cout, conv.bias, bn, mode=mode,
+                     **kw)
+    pk.kmacs = 49 * 3 * cout
+    return pk
+
+
+def deconv2d_k4s2_phase(py, px, cout):
+    """Phase (py, px) of ConvTranspose2d(k=4, s=2, p=1) (Cin, Cout, 4, 4) as a 2x2 stride-1 conv: (lt_conv_gather_weights_fwd source
+    (base, strides), padding).  out[2m+py] takes ky in {3,1} (input rows m-1, m) for py=0 and {2,0} (rows m, m+1) for py=1: tap i
+    reads ky = 3 - py - 2i."""
+    return ((3 - py) * 4 + (3 - px), (0, -8, -2, cout * 16, 16)), (0, 1 - py, 1 - px)
+
+
+def pack_deconv2d_k4s2(deconv, bn, mode="tc", **kw):
+    """ConvTranspose2d(k=4, s=2, p=1) as four 2x2 stride-1 convs, one per output parity: {(py, px): ConvPack}."""
+    w = _f32(deconv.weight)  # (Cin, Cout, 4, 4)
+    assert tuple(deconv.kernel_size) == (4, 4) and tuple(deconv.stride) == (2, 2) and tuple(deconv.padding) == (1, 1)
+    cin, cout = w.shape[:2]
+    phases = {}
+    for py in (0, 1):
+        for px in (0, 1):
+            (base, strides), pad = deconv2d_k4s2_phase(py, px, cout)
+            phases[(py, px)] = pack_filter((w, base, strides), (1, 2, 2), (1, 1, 1), pad, cin, cout, deconv.bias, bn, mode=mode, **kw)
+    return phases
+
+
 class NativeEngine:
     def __init__(self, model, mode="tc", use_graph=True):
         assert mode in ("simt", "tc", "tc1")
@@ -211,43 +263,10 @@ class NativeEngine:
         return pack_conv(conv, bn, mode=self.mode, cin_pad=cin_pad, **kw)
 
     def _pack_stem_s2d(self, conv, bn):
-        """7x7 stride-2 pad-3 conv == 4x4 stride-1 conv (front pad 2) over the 2x2 space-to-depth input.
-
-        Input row 2*oy - 3 + ky = 2*(oy + a) + r with a = tap offset in {-2..1}, r = row parity:
-        ky = 2a + r + 3 (taps with ky outside [0, 7) get zero weights).  Channel order (r*2 + s)*3 + c.
-        The re-indexing is not affine in the s2d channel, so this one (64 x 3 x 7 x 7) filter is rearranged on the host.
-        """
-        w = conv.weight.detach().float().cpu()          # (64, 3, 7, 7)
-        assert tuple(w.shape[1:]) == (3, 7, 7) and tuple(conv.stride) == (2, 2) and tuple(conv.padding) == (3, 3)
-        cout = w.shape[0]
-        wt = torch.zeros((4, 4, 32, cout), dtype=torch.float32)
-        for ai, a in enumerate(range(-2, 2)):
-            for bi, b in enumerate(range(-2, 2)):
-                for r in (0, 1):
-                    for s in (0, 1):
-                        ky, kx = 2 * a + r + 3, 2 * b + s + 3
-                        if 0 <= ky < 7 and 0 <= kx < 7:
-                            c0 = (r * 2 + s) * 3
-                            wt[ai, bi, c0:c0 + 3] = w[:, :, ky, kx].t()
-        wt = wt.to(conv.weight.device)                  # one H2D copy; canonical [tap][ci][co] already
-        pk = self._pack((wt, 0, (0, 4 * 32 * cout, 32 * cout, cout, 1)), (1, 4, 4), (1, 1, 1), (0, 2, 2), 32, cout, conv.bias, bn)
-        pk.kmacs = 49 * 3 * cout
-        return pk
+        return pack_stem_s2d(conv, bn, mode=self.mode)
 
     def _pack_deconv2d_k4s2(self, deconv, bn):
-        """ConvTranspose2d(k=4, s=2, p=1) as four 2x2 stride-1 convs, one per output parity.
-
-        out[2m+py] takes ky in {3,1} (input rows m-1, m) for py=0 and {2,0} (rows m, m+1) for py=1: tap i reads ky = 3 - py - 2i.
-        """
-        w = _f32(deconv.weight)  # (Cin, Cout, 4, 4)
-        assert tuple(deconv.kernel_size) == (4, 4) and tuple(deconv.stride) == (2, 2) and tuple(deconv.padding) == (1, 1)
-        cin, cout = w.shape[:2]
-        phases = {}
-        for py in (0, 1):
-            for px in (0, 1):
-                src = (w, (3 - py) * 4 + (3 - px), (0, -8, -2, cout * 16, 16))
-                phases[(py, px)] = self._pack(src, (1, 2, 2), (1, 1, 1), (0, 1 - py, 1 - px), cin, cout, deconv.bias, bn)
-        return phases
+        return pack_deconv2d_k4s2(deconv, bn, mode=self.mode)
 
     def _pack_deconv3d_k2s2(self, deconv, bn):
         return pack_deconv3d_k2s2(deconv, bn, mode=self.mode)

@@ -10,7 +10,10 @@ optional {alg,vol}_confidences heads), so reference checkpoints load unchanged.
 These modules only *hold parameters* and provide an autograd-capable torch
 forward (backend="torch": training / CPU plumbing).  The product inference
 path walks this tree once (see engine.py) and runs hand-written sm_90a
-kernels instead.
+kernels instead.  Every forward takes an optional `conv`: a function
+(module, x) -> y that replaces the calls of the Conv2d / ConvTranspose2d
+modules (backbone_backend="native": autograd_ops.backbone_conv); BatchNorm,
+ReLU, max-pool, the adds and the heads' Linear layers stay torch modules.
 """
 import torch
 from torch import nn
@@ -29,6 +32,18 @@ RESNET_SPEC = {
 
 def _bn(c):
     return nn.BatchNorm2d(c, momentum=BN_MOMENTUM)
+
+
+def _conv(conv, m, x):
+    """m(x) for a convolution module, through `conv` when one is given."""
+    return m(x) if conv is None else conv(m, x)
+
+
+def _seq(seq, x, conv):
+    """nn.Sequential.forward, with the convolutions through `conv` when one is given."""
+    for m in seq:
+        x = conv(m, x) if conv is not None and isinstance(m, (nn.Conv2d, nn.ConvTranspose2d)) else m(x)
+    return x
 
 
 class ResidualUnit(nn.Module):
@@ -68,12 +83,12 @@ class ResidualUnit(nn.Module):
             out.append((self.conv3, self.bn3))
         return out
 
-    def forward(self, x):
-        shortcut = x if self.downsample is None else self.downsample(x)
+    def forward(self, x, conv=None):
+        shortcut = x if self.downsample is None else _seq(self.downsample, x, conv)
         st = self.stages()
         y = x
-        for i, (conv, bn) in enumerate(st):
-            y = bn(conv(y))
+        for i, (c, bn) in enumerate(st):
+            y = bn(_conv(conv, c, y))
             if i + 1 < len(st):
                 y = self.relu(y)
         return self.relu(y + shortcut)
@@ -94,8 +109,8 @@ class ConfidenceHead(nn.Module):
             nn.Linear(256, n_classes), nn.Sigmoid(),
         )
 
-    def forward(self, x):
-        x = self.features(x)
+    def forward(self, x, conv=None):
+        x = _seq(self.features, x, conv)
         return self.head(x.flatten(2).mean(dim=-1))
 
 
@@ -137,17 +152,20 @@ class PoseResNet(nn.Module):
         self.deconv_layers = nn.Sequential(*up)
         self.final_layer = nn.Conv2d(inplanes, num_joints, 1, 1, 0)
 
-    def trunk(self, x):
-        x = self.maxpool(self.relu(self.bn1(self.conv1(x))))
-        return self.layer4(self.layer3(self.layer2(self.layer1(x))))
+    def trunk(self, x, conv=None):
+        x = self.maxpool(self.relu(self.bn1(_conv(conv, self.conv1, x))))
+        for i in range(1, 5):
+            for unit in getattr(self, "layer%d" % i):
+                x = unit(x, conv)
+        return x
 
-    def forward(self, x):
+    def forward(self, x, conv=None):
         """-> (heatmaps, features, alg_confidences, vol_confidences), reference :293-318."""
-        x = self.trunk(x)
-        alg = self.alg_confidences(x) if hasattr(self, "alg_confidences") else None
-        vol = self.vol_confidences(x) if hasattr(self, "vol_confidences") else None
-        features = self.deconv_layers(x)
-        return self.final_layer(features), features, alg, vol
+        x = self.trunk(x, conv)
+        alg = self.alg_confidences(x, conv) if hasattr(self, "alg_confidences") else None
+        vol = self.vol_confidences(x, conv) if hasattr(self, "vol_confidences") else None
+        features = _seq(self.deconv_layers, x, conv)
+        return _conv(conv, self.final_layer, features), features, alg, vol
 
 
 def get_pose_net(config, device="cuda:0"):

@@ -46,6 +46,25 @@ def _base_points(batch, batch_size, kind, use_gt_pelvis):
     return pts
 
 
+def _check_backbone_backend(backbone_backend, backend, conv_mode):
+    """backbone_backend="native" (backend="hybrid" only): every Conv2d / ConvTranspose2d of the backbone, its confidence heads and
+    `process_features` runs forward, data gradient and weight gradient on the native tensor-core kernels (autograd_ops.backbone_conv);
+    BatchNorm, ReLU, max-pool, the adds and the heads' Linear layers stay on torch."""
+    if backbone_backend not in ("torch", "native"):
+        raise ValueError("unknown backbone_backend {!r}".format(backbone_backend))
+    if backbone_backend == "native" and (backend != "hybrid" or conv_mode != "tc"):
+        raise ValueError("backbone_backend='native' needs backend='hybrid' and conv_mode='tc' (got %r, %r)" % (backend, conv_mode))
+    return backbone_backend
+
+
+def _backbone_conv(model):
+    """The `conv` hook of the backbone's forward: None (torch modules) or autograd_ops.backbone_conv."""
+    if model.backbone_backend != "native":
+        return None
+    from .autograd_ops import backbone_conv
+    return backbone_conv
+
+
 class _EngineOwner(nn.Module):
     """Keeps the native engine's packed filters / CUDA graphs in step with the module's tensors: `.to()/.cuda()/.float()`
     (`_apply`) and `load_state_dict` invalidate them explicitly (tensor versions alone miss `p.data` updates)."""
@@ -67,7 +86,8 @@ class _EngineOwner(nn.Module):
 
 
 class VolumetricTriangulationNet(_EngineOwner):
-    def __init__(self, config, device="cuda:0", backend=None, conv_mode=None, use_cuda_graph=True, v2v_backend="torch"):
+    def __init__(self, config, device="cuda:0", backend=None, conv_mode=None, use_cuda_graph=True, v2v_backend="torch",
+                 backbone_backend="torch"):
         super().__init__()
         m = config.model
         self.num_joints = m.backbone.num_joints
@@ -103,6 +123,7 @@ class VolumetricTriangulationNet(_EngineOwner):
         if v2v_backend == "native" and (self.backend != "hybrid" or self.conv_mode != "tc"):
             raise ValueError("v2v_backend='native' needs backend='hybrid' and conv_mode='tc' (got %r, %r)" % (self.backend, self.conv_mode))
         self.v2v_backend = v2v_backend
+        self.backbone_backend = _check_backbone_backend(backbone_backend, self.backend, self.conv_mode)
         self.use_cuda_graph = use_cuda_graph
         self.clone_outputs = True
         self._engine = None
@@ -169,7 +190,8 @@ class VolumetricTriangulationNet(_EngineOwner):
         dev = images.device
         B, V = images.shape[:2]
         flat = images.reshape(-1, *images.shape[2:])
-        heatmaps, features, _, vol_conf = self.backbone(flat)
+        conv = _backbone_conv(self)
+        heatmaps, features, _, vol_conf = self.backbone(flat, conv)
         if vol_conf is not None:
             vol_conf = vol_conf.view(B, V, *vol_conf.shape[1:])
             if self.volume_aggregation_method == "conf_norm":
@@ -189,7 +211,7 @@ class VolumetricTriangulationNet(_EngineOwner):
         coord = torch.einsum("bij,bxyzj->bxyzi", rot_t, coord) + cen_t.view(B, 1, 1, 1, 3)
         if self.transfer_cmu_to_human36m:
             coord = coord.permute(0, 1, 3, 2, 4).flip(2)
-        features = self.process_features(features)
+        features = self.process_features(features) if conv is None else conv(self.process_features[0], features)
         features = features.view(B, V, *features.shape[1:])
         ops = torch_ops
         if self.backend == "hybrid":
@@ -209,7 +231,7 @@ class AlgebraicTriangulationNet(_EngineOwner):
     kernels (engine.algebraic_forward); "torch": autograd torch ops; "hybrid": torch backbone, native 2-D soft-argmax and DLT
     with their backward kernels (trains, any mode)."""
 
-    def __init__(self, config, device="cuda:0", backend=None, conv_mode=None):
+    def __init__(self, config, device="cuda:0", backend=None, conv_mode=None, backbone_backend="torch"):
         super().__init__()
         self.use_confidences = config.model.use_confidences
         config.model.backbone.alg_confidences = False
@@ -221,6 +243,7 @@ class AlgebraicTriangulationNet(_EngineOwner):
         self.heatmap_multiplier = config.model.heatmap_multiplier
         self.backend = backend or os.environ.get("LT_B200_BACKEND", "native")
         self.conv_mode = conv_mode or os.environ.get("LT_B200_CONV", "tc")
+        self.backbone_backend = _check_backbone_backend(backbone_backend, self.backend, self.conv_mode)
         self._engine = None
 
     def engine(self):
@@ -248,7 +271,7 @@ class AlgebraicTriangulationNet(_EngineOwner):
     def _forward_torch(self, images, proj_matricies, ops_backend="torch"):
         """The reference forward on torch autograd; ops_backend="hybrid" runs its 2-D soft-argmax and DLT on the native kernels."""
         B, V = images.shape[:2]
-        heatmaps, _, alg_conf, _ = self.backbone(images.reshape(-1, *images.shape[2:]))
+        heatmaps, _, alg_conf, _ = self.backbone(images.reshape(-1, *images.shape[2:]), _backbone_conv(self))
         if not self.use_confidences:
             alg_conf = torch.ones(B * V, heatmaps.shape[1], dtype=torch.float, device=images.device)
         kp2d, heatmaps = op.integrate_tensor_2d(heatmaps * self.heatmap_multiplier, self.heatmap_softmax, backend=ops_backend)
