@@ -357,6 +357,31 @@ int lt_volumetric_ce_bwd(const float* grad_loss, const int* index, const float* 
                          int B, int J, long nvox, void* stream);
 
 /* ------------------------------------------------------------------------------------------
+ * Batch-statistics BatchNorm for training, fused with the ReLU after it and the residual add of a residual unit.  Replaces
+ * nn.BatchNorm2d / nn.BatchNorm3d in train and eval mode with the nn.ReLU and the `+ shortcut` that follow them (pose_resnet.py:25-137
+ * residual units, stem and deconv stack; v2v.py:7-66 Basic3DBlock, Res3DBlock, Upsample3DBlock).
+ *   x, residual, y, grad_* maps: float32 channels-last [M][C], M = N*D*H*W, C % 4 == 0, 16-byte aligned; residual may be NULL
+ *   per-channel vectors [C]: gamma, beta, running_mean, running_var, save_mean, save_invstd
+ * Forward: y = act(gamma * (x - mean) * invstd + beta (+ residual)), act = ReLU when relu != 0.  training != 0: mean and the biased
+ * variance of the batch (M >= 2), save_invstd = 1 / sqrt(var + eps), and the running statistics updated in place as nn.BatchNorm does
+ * (running = (1 - momentum) * running + momentum * batch value, the variance unbiased by M / (M - 1)); training == 0: the running
+ * statistics are used and left alone (save_mean / save_invstd still receive the values used).
+ * Backward (the same relu / training; y is read only with relu, for the mask y > 0): g' = grad_y [y > 0];
+ *   grad_beta = sum g', grad_gamma = sum g' * xhat, xhat = (x - save_mean) * save_invstd;
+ *   grad_x = gamma * save_invstd * (g' - sum g' / M - xhat * sum g' xhat / M) (training) or gamma * save_invstd * g' (eval);
+ *   grad_residual = g' (NULL: not written); grad_gamma / grad_beta may be NULL.
+ * Per-channel sums are accumulated in float64 and merged in a fixed order (no atomics): bitwise repeatable, no host synchronisation.
+ * workspace: lt_batch_norm_workspace_bytes(M, C) bytes, for either direction.
+ * ---------------------------------------------------------------------------------------- */
+size_t lt_batch_norm_workspace_bytes(long M, int C);
+int lt_batch_norm_fwd(const float* x, const float* residual, const float* gamma, const float* beta, float* running_mean, float* running_var,
+                      float* save_mean, float* save_invstd, float* y, long M, int C, float eps, float momentum, int training, int relu,
+                      void* workspace, size_t workspace_bytes, void* stream);
+int lt_batch_norm_bwd(const float* x, const float* y, const float* grad_y, const float* gamma, const float* save_mean, const float* save_invstd,
+                      float* grad_x, float* grad_residual, float* grad_gamma, float* grad_beta, long M, int C, int training, int relu,
+                      void* workspace, size_t workspace_bytes, void* stream);
+
+/* ------------------------------------------------------------------------------------------
  * Layout / format helpers.
  * ---------------------------------------------------------------------------------------- */
 /* images [N][C][H][W] float32 -> [N][H][W][Cp] float32, channels >= C zero filled */

@@ -715,3 +715,76 @@ def backbone_conv(module, x):
         return stem_conv(x, module.weight, module.bias)
     conv_kind(_as3(module.kernel_size, 1), _as3(module.stride, 1), _as3(module.padding, 0))
     return conv2d(x, module.weight, module.bias, module.stride, module.padding)
+
+
+# ---- BatchNorm for training (norm_backend="native"): batch statistics, the ReLU after the BatchNorm and the residual add of a residual
+# unit on csrc/norm.cu, over the float32 channels-last maps the native convolutions produce.
+
+class BatchNormActFn(torch.autograd.Function):
+    """act(BatchNorm(x) (+ residual)) with act = ReLU or identity, for (N, C, [D,] H, W) float32 maps with C % 4 == 0: lt_batch_norm_fwd
+    and lt_batch_norm_bwd.  Train mode normalises with the batch statistics and updates the running buffers in place; eval mode uses
+    the running buffers.  x, the output (with ReLU, for its mask) and the per-channel mean / invstd are saved: the output is the tensor
+    the next convolution keeps anyway, so nothing extra is stored.  The output is channels_last(_3d), so the next native conv reads it
+    as a view."""
+
+    @staticmethod
+    def forward(ctx, x, weight, bias, residual, running_mean, running_var, eps, momentum, training, relu):
+        nd = x.dim() - 2
+        C = x.shape[1]
+        x_cl = _cl(x)
+        M = x_cl.numel() // C
+        r_cl = None if residual is None else _cl(residual)
+        y_cl = torch.empty_like(x_cl)
+        mean = torch.empty(C, dtype=torch.float32, device=x.device)
+        invstd = torch.empty_like(mean)
+        ws = _workspace(x.device, capi.batch_norm_workspace_bytes(M, C))
+        capi.batch_norm(x_cl, r_cl, weight.detach().float().contiguous(), bias.detach().float().contiguous(), running_mean, running_var,
+                        mean, invstd, y_cl, M, C, eps, momentum, training, relu, ws)
+        y = _from_cl(y_cl, C, nd)
+        ctx.save_for_backward(x, y if relu else None, mean, invstd, weight)
+        ctx.cfg = (M, C, nd, bool(training), bool(relu))
+        return y
+
+    @staticmethod
+    def backward(ctx, grad_out):
+        x, y, mean, invstd, weight = ctx.saved_tensors
+        M, C, nd, training, relu = ctx.cfg
+        x_cl = _cl(x)
+        g_cl = _cl(grad_out)
+        gx = torch.empty_like(x_cl)
+        gr = torch.empty_like(x_cl) if ctx.needs_input_grad[3] else None
+        gw = torch.empty(C, dtype=torch.float32, device=x.device)
+        gb = torch.empty_like(gw)
+        ws = _workspace(x.device, capi.batch_norm_workspace_bytes(M, C))
+        capi.batch_norm_bwd(x_cl, _cl(y) if relu else None, g_cl, weight.detach().float().contiguous(), mean, invstd, gx, gr, gw, gb, M, C,
+                            training, relu, ws)
+        return (_from_cl(gx, C, nd), gw, gb, None if gr is None else _from_cl(gr, C, nd), None, None, None, None, None, None)
+
+
+def batch_norm(module, x, relu=False, residual=None):
+    """`norm` hook of pose_resnet.PoseResNet / v2v.V2VModel: relu(module(x) + residual) (ReLU and residual optional) for an
+    nn.BatchNorm2d / BatchNorm3d on the native kernels, reading eps, momentum, training, the affine parameters and the running buffers
+    from the module; num_batches_tracked is incremented on the device in train mode, as nn.BatchNorm does.  ValueError for what the
+    kernels do not implement: momentum=None (cumulative average), affine=False, track_running_stats=False, C % 4 != 0, fewer than 2
+    values per channel in train mode; RuntimeError for CPU tensors."""
+    if module.momentum is None:
+        raise ValueError("native BatchNorm: momentum=None (cumulative moving average) is not supported")
+    if not module.affine:
+        raise ValueError("native BatchNorm: affine=False is not supported")
+    if not module.track_running_stats:
+        raise ValueError("native BatchNorm: track_running_stats=False is not supported")
+    C = module.num_features
+    if C % 4:
+        raise ValueError("native BatchNorm: the channel count must be a multiple of 4, got %d" % C)
+    if x.dim() not in (4, 5) or x.shape[1] != C:
+        raise ValueError("native BatchNorm: expected a (N, %d, [D,] H, W) map, got %s" % (C, tuple(x.shape)))
+    if residual is not None and tuple(residual.shape) != tuple(x.shape):
+        raise ValueError("native BatchNorm: residual %s differs from the input %s" % (tuple(residual.shape), tuple(x.shape)))
+    if module.training and x.numel() // C < 2:
+        raise ValueError("native BatchNorm: expected more than 1 value per channel when training, got input size %s" % (tuple(x.shape),))
+    if not x.is_cuda or (residual is not None and not residual.is_cuda):
+        raise RuntimeError("lt_b200 native BatchNorm needs CUDA tensors (got %s)" % x.device)
+    if module.training:
+        module.num_batches_tracked.add_(1)
+    return BatchNormActFn.apply(x, module.weight, module.bias, residual, module.running_mean, module.running_var, module.eps,
+                                module.momentum, module.training, relu)

@@ -12,7 +12,7 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 LIB = os.path.join(HERE, "liblt_b200.so")
 STAMP = os.path.join(HERE, ".liblt_b200.stamp")
-SOURCES = ["capi.cu", "unproject.cu", "softargmax.cu", "conv_simt.cu", "conv_tc.cu", "conv_fold.cu", "conv_tail.cu", "misc.cu", "algebraic.cu", "backward.cu", "loss.cu", "conv_wgrad.cu"]
+SOURCES = ["capi.cu", "unproject.cu", "softargmax.cu", "conv_simt.cu", "conv_tc.cu", "conv_fold.cu", "conv_tail.cu", "misc.cu", "algebraic.cu", "backward.cu", "loss.cu", "conv_wgrad.cu", "norm.cu"]
 ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]
 NVCC_FLAGS = ARCH + ["-O3", "-lineinfo", "-std=c++17",
                      "--expt-relaxed-constexpr", "-Xcompiler", "-fPIC", "-Xptxas", "-v"]

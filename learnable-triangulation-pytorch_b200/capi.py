@@ -100,6 +100,9 @@ SIGNATURES = {
     "lt_volumetric_ce_fwd": (c_int, [c_void_p] * 8 + [c_size_t, c_int, c_int, c_long, c_void_p]),
     "lt_volumetric_ce_bwd": (c_int, [c_void_p] * 5 + [c_int, c_int, c_long, c_void_p]),
     "lt_test_volumetric_ce_host": (c_int, [c_void_p] * 9 + [c_int, c_int, c_long]),
+    "lt_batch_norm_workspace_bytes": (c_size_t, [c_long, c_int]),
+    "lt_batch_norm_fwd": (c_int, [c_void_p] * 9 + [c_long, c_int, c_float, c_float, c_int, c_int, c_void_p, c_size_t, c_void_p]),
+    "lt_batch_norm_bwd": (c_int, [c_void_p] * 10 + [c_long, c_int, c_int, c_int, c_void_p, c_size_t, c_void_p]),
     "lt_nchw_to_nhwc_f32": (c_int, [c_void_p, c_void_p] + [c_int] * 5 + [c_void_p]),
     "lt_images_hwc_to_nchw_fwd": (c_int, [c_void_p, c_int, c_void_p, c_void_p] + [c_int] * 4 + [c_void_p]),
     "lt_stem_s2d_fwd": (c_int, [c_void_p, c_void_p] + [c_int] * 4 + [c_void_p]),
@@ -371,6 +374,28 @@ def volumetric_ce_bwd(grad_loss, index, picked, validity, grad_probs):
     B, J, nvox = grad_probs.shape
     _check(lib().lt_volumetric_ce_bwd(_ptr(grad_loss), _ptr(index), _ptr(picked), _ptr(validity), _ptr(grad_probs), B, J, nvox, _stream()),
            "lt_volumetric_ce_bwd")
+
+
+def batch_norm_workspace_bytes(M, C):
+    return lib().lt_batch_norm_workspace_bytes(M, C)
+
+
+def batch_norm(x, residual, gamma, beta, running_mean, running_var, save_mean, save_invstd, y, M, C, eps, momentum, training, relu,
+               workspace):
+    """x, residual (or None), y: float32 channels-last [M][C]; per-channel vectors [C]; the running statistics are updated in place
+    in training mode."""
+    _check(lib().lt_batch_norm_fwd(_ptr(x), _ptr(residual), _ptr(gamma), _ptr(beta), _ptr(running_mean), _ptr(running_var),
+                                   _ptr(save_mean), _ptr(save_invstd), _ptr(y), M, C, float(eps), float(momentum), int(training),
+                                   int(relu), _ptr(workspace), workspace.numel() * workspace.element_size(), _stream()),
+           "lt_batch_norm_fwd")
+
+
+def batch_norm_bwd(x, y, grad_y, gamma, save_mean, save_invstd, grad_x, grad_residual, grad_gamma, grad_beta, M, C, training, relu,
+                   workspace):
+    """grad_x, grad_residual (or None), grad_gamma and grad_beta are written; y (the forward's output) is read with relu only."""
+    _check(lib().lt_batch_norm_bwd(_ptr(x), _ptr(y), _ptr(grad_y), _ptr(gamma), _ptr(save_mean), _ptr(save_invstd), _ptr(grad_x),
+                                   _ptr(grad_residual), _ptr(grad_gamma), _ptr(grad_beta), M, C, int(training), int(relu),
+                                   _ptr(workspace), workspace.numel() * workspace.element_size(), _stream()), "lt_batch_norm_bwd")
 
 
 def _host_ptr(t):

@@ -12,8 +12,12 @@ forward (backend="torch": training / CPU plumbing).  The product inference
 path walks this tree once (see engine.py) and runs hand-written sm_90a
 kernels instead.  Every forward takes an optional `conv`: a function
 (module, x) -> y that replaces the calls of the Conv2d / ConvTranspose2d
-modules (backbone_backend="native": autograd_ops.backbone_conv); BatchNorm,
-ReLU, max-pool, the adds and the heads' Linear layers stay torch modules.
+modules (backbone_backend="native": autograd_ops.backbone_conv), and an
+optional `norm`: a function (module, x, relu=False, residual=None) ->
+act(module(x) + residual) that replaces each BatchNorm2d together with the
+ReLU right after it and, at the end of a residual unit, the shortcut add
+(norm_backend="native": autograd_ops.batch_norm).  Without `norm`, BatchNorm
+and ReLU stay torch modules; max-pool and the heads' Linear layers always do.
 """
 import torch
 from torch import nn
@@ -39,10 +43,24 @@ def _conv(conv, m, x):
     return m(x) if conv is None else conv(m, x)
 
 
-def _seq(seq, x, conv):
-    """nn.Sequential.forward, with the convolutions through `conv` when one is given."""
-    for m in seq:
+def _seq(seq, x, conv, norm=None):
+    """nn.Sequential.forward, with the convolutions through `conv` when one is given, and each BatchNorm2d, fused with an nn.ReLU
+    directly after it, through `norm` when one is given."""
+    if norm is None:
+        for m in seq:
+            x = conv(m, x) if conv is not None and isinstance(m, (nn.Conv2d, nn.ConvTranspose2d)) else m(x)
+        return x
+    mods = list(seq)
+    i = 0
+    while i < len(mods):
+        m = mods[i]
+        if isinstance(m, nn.BatchNorm2d):
+            relu = i + 1 < len(mods) and isinstance(mods[i + 1], nn.ReLU)
+            x = norm(m, x, relu=relu)
+            i += 2 if relu else 1
+            continue
         x = conv(m, x) if conv is not None and isinstance(m, (nn.Conv2d, nn.ConvTranspose2d)) else m(x)
+        i += 1
     return x
 
 
@@ -83,10 +101,14 @@ class ResidualUnit(nn.Module):
             out.append((self.conv3, self.bn3))
         return out
 
-    def forward(self, x, conv=None):
-        shortcut = x if self.downsample is None else _seq(self.downsample, x, conv)
+    def forward(self, x, conv=None, norm=None):
+        shortcut = x if self.downsample is None else _seq(self.downsample, x, conv, norm)
         st = self.stages()
         y = x
+        if norm is not None:
+            for i, (c, bn) in enumerate(st):
+                y = norm(bn, _conv(conv, c, y), relu=True, residual=shortcut if i + 1 == len(st) else None)
+            return y
         for i, (c, bn) in enumerate(st):
             y = bn(_conv(conv, c, y))
             if i + 1 < len(st):
@@ -109,8 +131,8 @@ class ConfidenceHead(nn.Module):
             nn.Linear(256, n_classes), nn.Sigmoid(),
         )
 
-    def forward(self, x, conv=None):
-        x = _seq(self.features, x, conv)
+    def forward(self, x, conv=None, norm=None):
+        x = _seq(self.features, x, conv, norm)
         return self.head(x.flatten(2).mean(dim=-1))
 
 
@@ -152,19 +174,22 @@ class PoseResNet(nn.Module):
         self.deconv_layers = nn.Sequential(*up)
         self.final_layer = nn.Conv2d(inplanes, num_joints, 1, 1, 0)
 
-    def trunk(self, x, conv=None):
-        x = self.maxpool(self.relu(self.bn1(_conv(conv, self.conv1, x))))
+    def trunk(self, x, conv=None, norm=None):
+        if norm is None:
+            x = self.maxpool(self.relu(self.bn1(_conv(conv, self.conv1, x))))
+        else:
+            x = self.maxpool(norm(self.bn1, _conv(conv, self.conv1, x), relu=True))
         for i in range(1, 5):
             for unit in getattr(self, "layer%d" % i):
-                x = unit(x, conv)
+                x = unit(x, conv, norm)
         return x
 
-    def forward(self, x, conv=None):
+    def forward(self, x, conv=None, norm=None):
         """-> (heatmaps, features, alg_confidences, vol_confidences), reference :293-318."""
-        x = self.trunk(x, conv)
-        alg = self.alg_confidences(x, conv) if hasattr(self, "alg_confidences") else None
-        vol = self.vol_confidences(x, conv) if hasattr(self, "vol_confidences") else None
-        features = _seq(self.deconv_layers, x, conv)
+        x = self.trunk(x, conv, norm)
+        alg = self.alg_confidences(x, conv, norm) if hasattr(self, "alg_confidences") else None
+        vol = self.vol_confidences(x, conv, norm) if hasattr(self, "vol_confidences") else None
+        features = _seq(self.deconv_layers, x, conv, norm)
         return _conv(conv, self.final_layer, features), features, alg, vol
 
 

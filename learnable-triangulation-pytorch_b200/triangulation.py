@@ -65,6 +65,29 @@ def _backbone_conv(model):
     return backbone_conv
 
 
+def _check_norm_backend(norm_backend, backend, backbone_backend, v2v_backend=None):
+    """norm_backend="native": every BatchNorm2d / BatchNorm3d of the backbone, its confidence heads and the V2V net, fused with the
+    ReLU after it and the residual add of a residual unit, trains on the native kernels (autograd_ops.batch_norm).  The kernels read
+    the channels-last maps the native convolutions produce, so it needs backend="hybrid" and the model's native conv backends
+    (backbone_backend="native", and v2v_backend="native" for the volumetric model: v2v_backend None stands for a model without one)."""
+    if norm_backend not in ("torch", "native"):
+        raise ValueError("unknown norm_backend {!r}".format(norm_backend))
+    if norm_backend == "native":
+        need = "backend='hybrid' and backbone_backend='native'" + ("" if v2v_backend is None else " and v2v_backend='native'")
+        if backend != "hybrid" or backbone_backend != "native" or v2v_backend not in (None, "native"):
+            raise ValueError("norm_backend='native' needs %s (got backend=%r, backbone_backend=%r%s)"
+                             % (need, backend, backbone_backend, "" if v2v_backend is None else ", v2v_backend=%r" % v2v_backend))
+    return norm_backend
+
+
+def _norm(model):
+    """The `norm` hook of the backbone's and the V2V net's forward: None (torch modules) or autograd_ops.batch_norm."""
+    if model.norm_backend != "native":
+        return None
+    from .autograd_ops import batch_norm
+    return batch_norm
+
+
 class _EngineOwner(nn.Module):
     """Keeps the native engine's packed filters / CUDA graphs in step with the module's tensors: `.to()/.cuda()/.float()`
     (`_apply`) and `load_state_dict` invalidate them explicitly (tensor versions alone miss `p.data` updates)."""
@@ -87,7 +110,7 @@ class _EngineOwner(nn.Module):
 
 class VolumetricTriangulationNet(_EngineOwner):
     def __init__(self, config, device="cuda:0", backend=None, conv_mode=None, use_cuda_graph=True, v2v_backend="torch",
-                 backbone_backend="torch"):
+                 backbone_backend="torch", norm_backend="torch"):
         super().__init__()
         m = config.model
         self.num_joints = m.backbone.num_joints
@@ -124,6 +147,7 @@ class VolumetricTriangulationNet(_EngineOwner):
             raise ValueError("v2v_backend='native' needs backend='hybrid' and conv_mode='tc' (got %r, %r)" % (self.backend, self.conv_mode))
         self.v2v_backend = v2v_backend
         self.backbone_backend = _check_backbone_backend(backbone_backend, self.backend, self.conv_mode)
+        self.norm_backend = _check_norm_backend(norm_backend, self.backend, self.backbone_backend, self.v2v_backend)
         self.use_cuda_graph = use_cuda_graph
         self.clone_outputs = True
         self._engine = None
@@ -191,7 +215,8 @@ class VolumetricTriangulationNet(_EngineOwner):
         B, V = images.shape[:2]
         flat = images.reshape(-1, *images.shape[2:])
         conv = _backbone_conv(self)
-        heatmaps, features, _, vol_conf = self.backbone(flat, conv)
+        norm = _norm(self)
+        heatmaps, features, _, vol_conf = self.backbone(flat, conv, norm)
         if vol_conf is not None:
             vol_conf = vol_conf.view(B, V, *vol_conf.shape[1:])
             if self.volume_aggregation_method == "conf_norm":
@@ -219,7 +244,7 @@ class VolumetricTriangulationNet(_EngineOwner):
                 raise RuntimeError("lt_b200 hybrid backend needs CUDA tensors (native custom ops); use backend='torch' on CPU")
             from . import autograd_ops as ops
         volumes = ops.unproject_heatmaps(features, proj_t, coord, self.volume_aggregation_method, vol_conf)
-        volumes = self.volume_net(volumes, ops.v2v_conv if self.v2v_backend == "native" else None)
+        volumes = self.volume_net(volumes, ops.v2v_conv if self.v2v_backend == "native" else None, norm)
         kp, volumes = ops.integrate_tensor_3d_with_coordinates(volumes * self.volume_multiplier, coord, self.volume_softmax)
         return kp, features, volumes, vol_conf, cuboids, coord, cen_t
 
@@ -231,7 +256,7 @@ class AlgebraicTriangulationNet(_EngineOwner):
     kernels (engine.algebraic_forward); "torch": autograd torch ops; "hybrid": torch backbone, native 2-D soft-argmax and DLT
     with their backward kernels (trains, any mode)."""
 
-    def __init__(self, config, device="cuda:0", backend=None, conv_mode=None, backbone_backend="torch"):
+    def __init__(self, config, device="cuda:0", backend=None, conv_mode=None, backbone_backend="torch", norm_backend="torch"):
         super().__init__()
         self.use_confidences = config.model.use_confidences
         config.model.backbone.alg_confidences = False
@@ -244,6 +269,7 @@ class AlgebraicTriangulationNet(_EngineOwner):
         self.backend = backend or os.environ.get("LT_B200_BACKEND", "native")
         self.conv_mode = conv_mode or os.environ.get("LT_B200_CONV", "tc")
         self.backbone_backend = _check_backbone_backend(backbone_backend, self.backend, self.conv_mode)
+        self.norm_backend = _check_norm_backend(norm_backend, self.backend, self.backbone_backend)
         self._engine = None
 
     def engine(self):
@@ -271,7 +297,7 @@ class AlgebraicTriangulationNet(_EngineOwner):
     def _forward_torch(self, images, proj_matricies, ops_backend="torch"):
         """The reference forward on torch autograd; ops_backend="hybrid" runs its 2-D soft-argmax and DLT on the native kernels."""
         B, V = images.shape[:2]
-        heatmaps, _, alg_conf, _ = self.backbone(images.reshape(-1, *images.shape[2:]), _backbone_conv(self))
+        heatmaps, _, alg_conf, _ = self.backbone(images.reshape(-1, *images.shape[2:]), _backbone_conv(self), _norm(self))
         if not self.use_confidences:
             alg_conf = torch.ones(B * V, heatmaps.shape[1], dtype=torch.float, device=images.device)
         kp2d, heatmaps = op.integrate_tensor_2d(heatmaps * self.heatmap_multiplier, self.heatmap_softmax, backend=ops_backend)

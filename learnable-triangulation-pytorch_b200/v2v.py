@@ -7,17 +7,33 @@ back_layers.{0..2}, output_layer.
 
 Parameters live here; inference runs through the native planner in engine.py.
 The torch forward below is the autograd / CPU plumbing path (backend="torch").  Every forward takes an optional `conv`: a function
-(module, x) -> y that replaces the calls of the Conv3d / ConvTranspose3d modules (v2v_backend="native": autograd_ops.v2v_conv);
-BatchNorm, ReLU, pooling and the adds stay torch modules either way.
+(module, x) -> y that replaces the calls of the Conv3d / ConvTranspose3d modules (v2v_backend="native": autograd_ops.v2v_conv),
+and an optional `norm`: a function (module, x, relu=False, residual=None) -> act(module(x) + residual) that replaces each BatchNorm3d
+together with the ReLU right after it and, in a Res3DBlock, the residual add (norm_backend="native": autograd_ops.batch_norm).
+Without `norm`, BatchNorm and ReLU stay torch modules; pooling and the decoder's `upsample + skip` adds always do.
 """
 import torch.nn.functional as F
 from torch import nn
 
 
-def _seq(seq, x, conv):
-    """nn.Sequential.forward, with the convolutions through `conv` when one is given."""
-    for m in seq:
+def _seq(seq, x, conv, norm=None):
+    """nn.Sequential.forward, with the convolutions through `conv` when one is given, and each BatchNorm3d, fused with an nn.ReLU
+    directly after it, through `norm` when one is given."""
+    if norm is None:
+        for m in seq:
+            x = conv(m, x) if conv is not None and isinstance(m, (nn.Conv3d, nn.ConvTranspose3d)) else m(x)
+        return x
+    mods = list(seq)
+    i = 0
+    while i < len(mods):
+        m = mods[i]
+        if isinstance(m, nn.BatchNorm3d):
+            relu = i + 1 < len(mods) and isinstance(mods[i + 1], nn.ReLU)
+            x = norm(m, x, relu=relu)
+            i += 2 if relu else 1
+            continue
         x = conv(m, x) if conv is not None and isinstance(m, (nn.Conv3d, nn.ConvTranspose3d)) else m(x)
+        i += 1
     return x
 
 
@@ -28,8 +44,8 @@ class Basic3DBlock(nn.Module):
         super().__init__()
         self.block = nn.Sequential(nn.Conv3d(cin, cout, k, 1, (k - 1) // 2), nn.BatchNorm3d(cout), nn.ReLU(True))
 
-    def forward(self, x, conv=None):
-        return _seq(self.block, x, conv)
+    def forward(self, x, conv=None, norm=None):
+        return _seq(self.block, x, conv, norm)
 
 
 class Res3DBlock(nn.Module):
@@ -43,8 +59,13 @@ class Res3DBlock(nn.Module):
         self.skip_con = nn.Sequential() if cin == cout else nn.Sequential(
             nn.Conv3d(cin, cout, 1, 1, 0), nn.BatchNorm3d(cout))
 
-    def forward(self, x, conv=None):
-        return F.relu(_seq(self.res_branch, x, conv) + _seq(self.skip_con, x, conv), True)
+    def forward(self, x, conv=None, norm=None):
+        if norm is None:
+            return F.relu(_seq(self.res_branch, x, conv) + _seq(self.skip_con, x, conv), True)
+        rb = self.res_branch
+        y = norm(rb[1], rb[0](x) if conv is None else conv(rb[0], x), relu=True)
+        z = rb[3](y) if conv is None else conv(rb[3], y)
+        return norm(rb[4], z, relu=True, residual=_seq(self.skip_con, x, conv, norm))
 
 
 class Pool3DBlock(nn.Module):
@@ -64,8 +85,8 @@ class Upsample3DBlock(nn.Module):
         assert kernel_size == 2 and stride == 2
         self.block = nn.Sequential(nn.ConvTranspose3d(cin, cout, 2, 2, 0, 0), nn.BatchNorm3d(cout), nn.ReLU(True))
 
-    def forward(self, x, conv=None):
-        return _seq(self.block, x, conv)
+    def forward(self, x, conv=None, norm=None):
+        return _seq(self.block, x, conv, norm)
 
 
 # (level, encoder channels in->out); decoder mirrors it. reference v2v.py:73-101
@@ -86,14 +107,14 @@ class EncoderDecorder(nn.Module):  # (sic) the reference's class name
         for lvl, cin, _ in _ENC:
             setattr(self, "skip_res%d" % lvl, Res3DBlock(cin, cin))
 
-    def forward(self, x, conv=None):
+    def forward(self, x, conv=None, norm=None):
         skips = {}
         for lvl, _, _ in _ENC:
-            skips[lvl] = getattr(self, "skip_res%d" % lvl)(x, conv)
-            x = getattr(self, "encoder_res%d" % lvl)(getattr(self, "encoder_pool%d" % lvl)(x), conv)
-        x = self.mid_res(x, conv)
+            skips[lvl] = getattr(self, "skip_res%d" % lvl)(x, conv, norm)
+            x = getattr(self, "encoder_res%d" % lvl)(getattr(self, "encoder_pool%d" % lvl)(x), conv, norm)
+        x = self.mid_res(x, conv, norm)
         for lvl, _, _ in _DEC:
-            x = getattr(self, "decoder_upsample%d" % lvl)(getattr(self, "decoder_res%d" % lvl)(x, conv), conv) + skips[lvl]
+            x = getattr(self, "decoder_upsample%d" % lvl)(getattr(self, "decoder_res%d" % lvl)(x, conv, norm), conv, norm) + skips[lvl]
         return x
 
 
@@ -111,10 +132,10 @@ class V2VModel(nn.Module):
                 nn.init.xavier_normal_(m.weight)
                 nn.init.constant_(m.bias, 0)
 
-    def forward(self, x, conv=None):
+    def forward(self, x, conv=None, norm=None):
         for blk in self.front_layers:
-            x = blk(x, conv)
-        x = self.encoder_decoder(x, conv)
+            x = blk(x, conv, norm)
+        x = self.encoder_decoder(x, conv, norm)
         for blk in self.back_layers:
-            x = blk(x, conv)
+            x = blk(x, conv, norm)
         return self.output_layer(x) if conv is None else conv(self.output_layer, x)
