@@ -10,17 +10,20 @@ optional {alg,vol}_confidences heads), so reference checkpoints load unchanged.
 These modules only *hold parameters* and provide an autograd-capable torch
 forward (backend="torch": training / CPU plumbing).  The product inference
 path walks this tree once (see engine.py) and runs hand-written sm_90a
-kernels instead.  Every forward takes an optional `conv`: a function
-(module, x) -> y that replaces the calls of the Conv2d / ConvTranspose2d
-modules (backbone_backend="native": autograd_ops.backbone_conv), and an
-optional `norm`: a function (module, x, relu=False, residual=None) ->
-act(module(x) + residual) that replaces each BatchNorm2d together with the
-ReLU right after it and, at the end of a residual unit, the shortcut add
-(norm_backend="native": autograd_ops.batch_norm).  Without `norm`, BatchNorm
-and ReLU stay torch modules; max-pool and the heads' Linear layers always do.
+kernels instead.  Every forward takes the `conv` and `norm` hooks of
+layers.py: `conv` applies each Conv2d / ConvTranspose2d (backbone_backend=
+"native": autograd_ops.backbone_conv), `norm` each BatchNorm2d together with
+the ReLU right after it and, at the end of a residual unit, the shortcut add
+(norm_backend="native": autograd_ops.batch_norm).  None, the default, stands
+for the torch formulas in layers.py.  Max-pool and the heads' Linear layers
+are always torch modules.  A ReLU module right after a BatchNorm is applied by
+`norm`, not called as a module, so a forward hook registered on it does not
+fire.
 """
 import torch
 from torch import nn
+
+from .layers import defaults, run
 
 BN_MOMENTUM = 0.1
 
@@ -36,32 +39,6 @@ RESNET_SPEC = {
 
 def _bn(c):
     return nn.BatchNorm2d(c, momentum=BN_MOMENTUM)
-
-
-def _conv(conv, m, x):
-    """m(x) for a convolution module, through `conv` when one is given."""
-    return m(x) if conv is None else conv(m, x)
-
-
-def _seq(seq, x, conv, norm=None):
-    """nn.Sequential.forward, with the convolutions through `conv` when one is given, and each BatchNorm2d, fused with an nn.ReLU
-    directly after it, through `norm` when one is given."""
-    if norm is None:
-        for m in seq:
-            x = conv(m, x) if conv is not None and isinstance(m, (nn.Conv2d, nn.ConvTranspose2d)) else m(x)
-        return x
-    mods = list(seq)
-    i = 0
-    while i < len(mods):
-        m = mods[i]
-        if isinstance(m, nn.BatchNorm2d):
-            relu = i + 1 < len(mods) and isinstance(mods[i + 1], nn.ReLU)
-            x = norm(m, x, relu=relu)
-            i += 2 if relu else 1
-            continue
-        x = conv(m, x) if conv is not None and isinstance(m, (nn.Conv2d, nn.ConvTranspose2d)) else m(x)
-        i += 1
-    return x
 
 
 class ResidualUnit(nn.Module):
@@ -91,7 +68,7 @@ class ResidualUnit(nn.Module):
             self.bn2 = _bn(planes)
             self.conv3 = nn.Conv2d(planes, planes * 4, 1, bias=False)
             self.bn3 = _bn(planes * 4)
-        self.relu = nn.ReLU(inplace=True)
+        self.relu = nn.ReLU(inplace=True)        # in the reference's module tree; `norm` applies the ReLU
         self.downsample = downsample
 
     def stages(self):
@@ -102,18 +79,13 @@ class ResidualUnit(nn.Module):
         return out
 
     def forward(self, x, conv=None, norm=None):
-        shortcut = x if self.downsample is None else _seq(self.downsample, x, conv, norm)
+        conv, norm = defaults(conv, norm)
+        shortcut = x if self.downsample is None else run(self.downsample, x, conv, norm)
         st = self.stages()
         y = x
-        if norm is not None:
-            for i, (c, bn) in enumerate(st):
-                y = norm(bn, _conv(conv, c, y), relu=True, residual=shortcut if i + 1 == len(st) else None)
-            return y
         for i, (c, bn) in enumerate(st):
-            y = bn(_conv(conv, c, y))
-            if i + 1 < len(st):
-                y = self.relu(y)
-        return self.relu(y + shortcut)
+            y = norm(bn, conv(c, y), relu=True, residual=shortcut if i + 1 == len(st) else None)
+        return y
 
 
 class ConfidenceHead(nn.Module):
@@ -132,7 +104,7 @@ class ConfidenceHead(nn.Module):
         )
 
     def forward(self, x, conv=None, norm=None):
-        x = _seq(self.features, x, conv, norm)
+        x = run(self.features, x, conv, norm)
         return self.head(x.flatten(2).mean(dim=-1))
 
 
@@ -146,7 +118,7 @@ class PoseResNet(nn.Module):
 
         self.conv1 = nn.Conv2d(num_input_channels, 64, 7, 2, 3, bias=False)
         self.bn1 = _bn(64)
-        self.relu = nn.ReLU(inplace=True)
+        self.relu = nn.ReLU(inplace=True)        # in the reference's module tree; `norm` applies the ReLU
         self.maxpool = nn.MaxPool2d(3, 2, 1)
 
         inplanes = 64
@@ -175,10 +147,8 @@ class PoseResNet(nn.Module):
         self.final_layer = nn.Conv2d(inplanes, num_joints, 1, 1, 0)
 
     def trunk(self, x, conv=None, norm=None):
-        if norm is None:
-            x = self.maxpool(self.relu(self.bn1(_conv(conv, self.conv1, x))))
-        else:
-            x = self.maxpool(norm(self.bn1, _conv(conv, self.conv1, x), relu=True))
+        conv, norm = defaults(conv, norm)
+        x = self.maxpool(norm(self.bn1, conv(self.conv1, x), relu=True))
         for i in range(1, 5):
             for unit in getattr(self, "layer%d" % i):
                 x = unit(x, conv, norm)
@@ -186,11 +156,12 @@ class PoseResNet(nn.Module):
 
     def forward(self, x, conv=None, norm=None):
         """-> (heatmaps, features, alg_confidences, vol_confidences), reference :293-318."""
+        conv, norm = defaults(conv, norm)
         x = self.trunk(x, conv, norm)
         alg = self.alg_confidences(x, conv, norm) if hasattr(self, "alg_confidences") else None
         vol = self.vol_confidences(x, conv, norm) if hasattr(self, "vol_confidences") else None
-        features = _seq(self.deconv_layers, x, conv, norm)
-        return _conv(conv, self.final_layer, features), features, alg, vol
+        features = run(self.deconv_layers, x, conv, norm)
+        return conv(self.final_layer, features), features, alg, vol
 
 
 def get_pose_net(config, device="cuda:0"):

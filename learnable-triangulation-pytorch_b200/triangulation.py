@@ -16,7 +16,7 @@ import numpy as np
 import torch
 from torch import nn
 
-from . import multiview, op, pose_resnet, torch_ops, volumetric
+from . import autograd_ops, layers, multiview, op, pose_resnet, torch_ops, volumetric
 from .v2v import V2VModel
 
 
@@ -46,46 +46,37 @@ def _base_points(batch, batch_size, kind, use_gt_pelvis):
     return pts
 
 
-def _check_backbone_backend(backbone_backend, backend, conv_mode):
-    """backbone_backend="native" (backend="hybrid" only): every Conv2d / ConvTranspose2d of the backbone, its confidence heads and
-    `process_features` runs forward, data gradient and weight gradient on the native tensor-core kernels (autograd_ops.backbone_conv);
-    BatchNorm, ReLU, max-pool, the adds and the heads' Linear layers stay on torch."""
-    if backbone_backend not in ("torch", "native"):
-        raise ValueError("unknown backbone_backend {!r}".format(backbone_backend))
-    if backbone_backend == "native" and (backend != "hybrid" or conv_mode != "tc"):
-        raise ValueError("backbone_backend='native' needs backend='hybrid' and conv_mode='tc' (got %r, %r)" % (backend, conv_mode))
-    return backbone_backend
+_NO_V2V = object()      # the v2v_backend of a model without a V2V net (None stays an unknown v2v_backend)
 
 
-def _backbone_conv(model):
-    """The `conv` hook of the backbone's forward: None (torch modules) or autograd_ops.backbone_conv."""
-    if model.backbone_backend != "native":
-        return None
-    from .autograd_ops import backbone_conv
-    return backbone_conv
+def _check_backends(backend, conv_mode, backbone_backend, norm_backend, v2v_backend=_NO_V2V):
+    """ValueError unless the training switches are known values in a supported combination.
 
-
-def _check_norm_backend(norm_backend, backend, backbone_backend, v2v_backend=None):
-    """norm_backend="native": every BatchNorm2d / BatchNorm3d of the backbone, its confidence heads and the V2V net, fused with the
-    ReLU after it and the residual add of a residual unit, trains on the native kernels (autograd_ops.batch_norm).  The kernels read
-    the channels-last maps the native convolutions produce, so it needs backend="hybrid" and the model's native conv backends
-    (backbone_backend="native", and v2v_backend="native" for the volumetric model: v2v_backend None stands for a model without one)."""
+    v2v_backend="native" / backbone_backend="native": every Conv3d / ConvTranspose3d of volume_net / every Conv2d / ConvTranspose2d
+    of the backbone, its confidence heads and `process_features` runs forward, data gradient and weight gradient on the native
+    tensor-core kernels.  Both need backend="hybrid" and conv_mode="tc".
+    norm_backend="native": every BatchNorm2d / BatchNorm3d of the backbone, its confidence heads and the V2V net, fused with the ReLU
+    after it and the residual add of a residual unit, trains on the native kernels.  The kernels read the channels-last maps the
+    native convolutions produce, so it needs backend="hybrid" and every conv switch of the model "native"."""
+    convs = [("backbone_backend", backbone_backend)] + ([] if v2v_backend is _NO_V2V else [("v2v_backend", v2v_backend)])
+    for name, value in reversed(convs):     # the V2V switch first
+        if value not in ("torch", "native"):
+            raise ValueError("unknown {} {!r}".format(name, value))
+        if value == "native" and (backend != "hybrid" or conv_mode != "tc"):
+            raise ValueError("%s='native' needs backend='hybrid' and conv_mode='tc' (got %r, %r)" % (name, backend, conv_mode))
     if norm_backend not in ("torch", "native"):
         raise ValueError("unknown norm_backend {!r}".format(norm_backend))
-    if norm_backend == "native":
-        need = "backend='hybrid' and backbone_backend='native'" + ("" if v2v_backend is None else " and v2v_backend='native'")
-        if backend != "hybrid" or backbone_backend != "native" or v2v_backend not in (None, "native"):
-            raise ValueError("norm_backend='native' needs %s (got backend=%r, backbone_backend=%r%s)"
-                             % (need, backend, backbone_backend, "" if v2v_backend is None else ", v2v_backend=%r" % v2v_backend))
-    return norm_backend
+    if norm_backend == "native" and (backend != "hybrid" or any(value != "native" for _, value in convs)):
+        raise ValueError("norm_backend='native' needs backend='hybrid' and %s (got backend=%r, %s)"
+                         % (" and ".join("%s='native'" % name for name, _ in convs), backend, ", ".join("%s=%r" % c for c in convs)))
 
 
-def _norm(model):
-    """The `norm` hook of the backbone's and the V2V net's forward: None (torch modules) or autograd_ops.batch_norm."""
-    if model.norm_backend != "native":
-        return None
-    from .autograd_ops import batch_norm
-    return batch_norm
+def _hooks(backbone_backend, norm_backend, v2v_backend="torch"):
+    """(backbone conv, V2V conv, norm) hooks of checked switches: the torch formulas in layers.py for "torch", autograd_ops'
+    native training functions for "native"."""
+    return (autograd_ops.backbone_conv if backbone_backend == "native" else layers.torch_conv,
+            autograd_ops.v2v_conv if v2v_backend == "native" else layers.torch_conv,
+            autograd_ops.batch_norm if norm_backend == "native" else layers.torch_norm)
 
 
 class _EngineOwner(nn.Module):
@@ -139,15 +130,10 @@ class VolumetricTriangulationNet(_EngineOwner):
 
         self.backend = backend or os.environ.get("LT_B200_BACKEND", "native")
         self.conv_mode = conv_mode or os.environ.get("LT_B200_CONV", "tc")
-        # v2v_backend="native" (backend="hybrid" only): every Conv3d / ConvTranspose3d of volume_net runs forward, data gradient and
-        # weight gradient on the native tensor-core kernels (autograd_ops.v2v_conv); BatchNorm, ReLU, pooling and adds stay on torch
-        if v2v_backend not in ("torch", "native"):
-            raise ValueError("unknown v2v_backend {!r}".format(v2v_backend))
-        if v2v_backend == "native" and (self.backend != "hybrid" or self.conv_mode != "tc"):
-            raise ValueError("v2v_backend='native' needs backend='hybrid' and conv_mode='tc' (got %r, %r)" % (self.backend, self.conv_mode))
+        _check_backends(self.backend, self.conv_mode, backbone_backend, norm_backend, v2v_backend)
         self.v2v_backend = v2v_backend
-        self.backbone_backend = _check_backbone_backend(backbone_backend, self.backend, self.conv_mode)
-        self.norm_backend = _check_norm_backend(norm_backend, self.backend, self.backbone_backend, self.v2v_backend)
+        self.backbone_backend = backbone_backend
+        self.norm_backend = norm_backend
         self.use_cuda_graph = use_cuda_graph
         self.clone_outputs = True
         self._engine = None
@@ -214,8 +200,7 @@ class VolumetricTriangulationNet(_EngineOwner):
         dev = images.device
         B, V = images.shape[:2]
         flat = images.reshape(-1, *images.shape[2:])
-        conv = _backbone_conv(self)
-        norm = _norm(self)
+        conv, v2v_conv, norm = _hooks(self.backbone_backend, self.norm_backend, self.v2v_backend)
         heatmaps, features, _, vol_conf = self.backbone(flat, conv, norm)
         if vol_conf is not None:
             vol_conf = vol_conf.view(B, V, *vol_conf.shape[1:])
@@ -236,7 +221,7 @@ class VolumetricTriangulationNet(_EngineOwner):
         coord = torch.einsum("bij,bxyzj->bxyzi", rot_t, coord) + cen_t.view(B, 1, 1, 1, 3)
         if self.transfer_cmu_to_human36m:
             coord = coord.permute(0, 1, 3, 2, 4).flip(2)
-        features = self.process_features(features) if conv is None else conv(self.process_features[0], features)
+        features = layers.run(self.process_features, features, conv, norm)
         features = features.view(B, V, *features.shape[1:])
         ops = torch_ops
         if self.backend == "hybrid":
@@ -244,7 +229,7 @@ class VolumetricTriangulationNet(_EngineOwner):
                 raise RuntimeError("lt_b200 hybrid backend needs CUDA tensors (native custom ops); use backend='torch' on CPU")
             from . import autograd_ops as ops
         volumes = ops.unproject_heatmaps(features, proj_t, coord, self.volume_aggregation_method, vol_conf)
-        volumes = self.volume_net(volumes, ops.v2v_conv if self.v2v_backend == "native" else None, norm)
+        volumes = self.volume_net(volumes, v2v_conv, norm)
         kp, volumes = ops.integrate_tensor_3d_with_coordinates(volumes * self.volume_multiplier, coord, self.volume_softmax)
         return kp, features, volumes, vol_conf, cuboids, coord, cen_t
 
@@ -268,8 +253,9 @@ class AlgebraicTriangulationNet(_EngineOwner):
         self.heatmap_multiplier = config.model.heatmap_multiplier
         self.backend = backend or os.environ.get("LT_B200_BACKEND", "native")
         self.conv_mode = conv_mode or os.environ.get("LT_B200_CONV", "tc")
-        self.backbone_backend = _check_backbone_backend(backbone_backend, self.backend, self.conv_mode)
-        self.norm_backend = _check_norm_backend(norm_backend, self.backend, self.backbone_backend)
+        _check_backends(self.backend, self.conv_mode, backbone_backend, norm_backend)
+        self.backbone_backend = backbone_backend
+        self.norm_backend = norm_backend
         self._engine = None
 
     def engine(self):
@@ -297,7 +283,8 @@ class AlgebraicTriangulationNet(_EngineOwner):
     def _forward_torch(self, images, proj_matricies, ops_backend="torch"):
         """The reference forward on torch autograd; ops_backend="hybrid" runs its 2-D soft-argmax and DLT on the native kernels."""
         B, V = images.shape[:2]
-        heatmaps, _, alg_conf, _ = self.backbone(images.reshape(-1, *images.shape[2:]), _backbone_conv(self), _norm(self))
+        conv, _, norm = _hooks(self.backbone_backend, self.norm_backend)
+        heatmaps, _, alg_conf, _ = self.backbone(images.reshape(-1, *images.shape[2:]), conv, norm)
         if not self.use_confidences:
             alg_conf = torch.ones(B * V, heatmaps.shape[1], dtype=torch.float, device=images.device)
         kp2d, heatmaps = op.integrate_tensor_2d(heatmaps * self.heatmap_multiplier, self.heatmap_softmax, backend=ops_backend)

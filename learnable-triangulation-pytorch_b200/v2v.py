@@ -6,35 +6,16 @@ front_layers.{0..3}, encoder_decoder.{encoder_res*,decoder_res*,decoder_upsample
 back_layers.{0..2}, output_layer.
 
 Parameters live here; inference runs through the native planner in engine.py.
-The torch forward below is the autograd / CPU plumbing path (backend="torch").  Every forward takes an optional `conv`: a function
-(module, x) -> y that replaces the calls of the Conv3d / ConvTranspose3d modules (v2v_backend="native": autograd_ops.v2v_conv),
-and an optional `norm`: a function (module, x, relu=False, residual=None) -> act(module(x) + residual) that replaces each BatchNorm3d
+The torch forward below is the autograd / CPU plumbing path (backend="torch").  Every forward takes the `conv` and `norm` hooks of
+layers.py: `conv` applies each Conv3d / ConvTranspose3d (v2v_backend="native": autograd_ops.v2v_conv), `norm` each BatchNorm3d
 together with the ReLU right after it and, in a Res3DBlock, the residual add (norm_backend="native": autograd_ops.batch_norm).
-Without `norm`, BatchNorm and ReLU stay torch modules; pooling and the decoder's `upsample + skip` adds always do.
+None, the default, stands for the torch formulas in layers.py.  Pooling and the decoder's `upsample + skip` adds are always torch.
+A ReLU module right after a BatchNorm is applied by `norm`, not called as a module, so a forward hook registered on it does not fire.
 """
 import torch.nn.functional as F
 from torch import nn
 
-
-def _seq(seq, x, conv, norm=None):
-    """nn.Sequential.forward, with the convolutions through `conv` when one is given, and each BatchNorm3d, fused with an nn.ReLU
-    directly after it, through `norm` when one is given."""
-    if norm is None:
-        for m in seq:
-            x = conv(m, x) if conv is not None and isinstance(m, (nn.Conv3d, nn.ConvTranspose3d)) else m(x)
-        return x
-    mods = list(seq)
-    i = 0
-    while i < len(mods):
-        m = mods[i]
-        if isinstance(m, nn.BatchNorm3d):
-            relu = i + 1 < len(mods) and isinstance(mods[i + 1], nn.ReLU)
-            x = norm(m, x, relu=relu)
-            i += 2 if relu else 1
-            continue
-        x = conv(m, x) if conv is not None and isinstance(m, (nn.Conv3d, nn.ConvTranspose3d)) else m(x)
-        i += 1
-    return x
+from .layers import defaults, run
 
 
 class Basic3DBlock(nn.Module):
@@ -45,7 +26,7 @@ class Basic3DBlock(nn.Module):
         self.block = nn.Sequential(nn.Conv3d(cin, cout, k, 1, (k - 1) // 2), nn.BatchNorm3d(cout), nn.ReLU(True))
 
     def forward(self, x, conv=None, norm=None):
-        return _seq(self.block, x, conv, norm)
+        return run(self.block, x, conv, norm)
 
 
 class Res3DBlock(nn.Module):
@@ -60,12 +41,11 @@ class Res3DBlock(nn.Module):
             nn.Conv3d(cin, cout, 1, 1, 0), nn.BatchNorm3d(cout))
 
     def forward(self, x, conv=None, norm=None):
-        if norm is None:
-            return F.relu(_seq(self.res_branch, x, conv) + _seq(self.skip_con, x, conv), True)
+        conv, norm = defaults(conv, norm)
         rb = self.res_branch
-        y = norm(rb[1], rb[0](x) if conv is None else conv(rb[0], x), relu=True)
-        z = rb[3](y) if conv is None else conv(rb[3], y)
-        return norm(rb[4], z, relu=True, residual=_seq(self.skip_con, x, conv, norm))
+        y = norm(rb[1], conv(rb[0], x), relu=True)
+        z = conv(rb[3], y)
+        return norm(rb[4], z, relu=True, residual=run(self.skip_con, x, conv, norm))
 
 
 class Pool3DBlock(nn.Module):
@@ -86,7 +66,7 @@ class Upsample3DBlock(nn.Module):
         self.block = nn.Sequential(nn.ConvTranspose3d(cin, cout, 2, 2, 0, 0), nn.BatchNorm3d(cout), nn.ReLU(True))
 
     def forward(self, x, conv=None, norm=None):
-        return _seq(self.block, x, conv, norm)
+        return run(self.block, x, conv, norm)
 
 
 # (level, encoder channels in->out); decoder mirrors it. reference v2v.py:73-101
@@ -133,9 +113,10 @@ class V2VModel(nn.Module):
                 nn.init.constant_(m.bias, 0)
 
     def forward(self, x, conv=None, norm=None):
+        conv, norm = defaults(conv, norm)
         for blk in self.front_layers:
             x = blk(x, conv, norm)
         x = self.encoder_decoder(x, conv, norm)
         for blk in self.back_layers:
             x = blk(x, conv, norm)
-        return self.output_layer(x) if conv is None else conv(self.output_layer, x)
+        return conv(self.output_layer, x)

@@ -1,4 +1,4 @@
-"""GPU tests of the native V2V training convolutions (autograd_ops.Conv3dFn / ConvTranspose3dFn: forward and data gradient on the
+"""GPU tests of the native V2V training convolutions (autograd_ops.ConvNdFn / ConvTranspose3dFn: forward and data gradient on the
 forward conv kernels, weight gradient on csrc/conv_wgrad.cu) against torch autograd in float64 on the device, and of a training
 step of the volumetric model with v2v_backend="native" against the cuDNN V2V."""
 import numpy as np

@@ -1,7 +1,7 @@
 """CPU checks of the native training BatchNorm (norm_backend="native": autograd_ops.batch_norm over csrc/norm.cu), no GPU needed: the
 option's rules, the `norm` hook of the backbone and the V2V net (every BatchNorm routed once with the right ReLU / residual flags, and
-a hook computing the torch formula reproduces the hook-free forward), the module attributes the hook rejects, and the argument checks
-of the C entry points.  The kernels themselves are covered by tests/test_gpu_norm_train.py."""
+a hook computing the torch formula reproduces the hook-free forward and its gradients), the module attributes the hook rejects, and
+the argument checks of the C entry points.  The kernels themselves are covered by tests/test_gpu_norm_train.py."""
 import copy
 
 import pytest
@@ -51,6 +51,14 @@ def _check_routing(net, record, flags):
         assert (relu, res) == flags(names[id(m)]), names[id(m)]
 
 
+def _check_grads(net, hooked, ref, got):
+    """The parameter gradients of sum(out.square().sum()) agree bit for bit between the two forwards."""
+    sum(o.square().sum() for o in ref).backward()
+    sum(o.square().sum() for o in got).backward()
+    for (n, p), (_, q) in zip(net.named_parameters(), hooked.named_parameters()):
+        assert p.grad is not None and torch.equal(p.grad, q.grad), n
+
+
 @pytest.mark.parametrize("layers,style", [(18, "simple"), (50, "simple"), (50, "caffe")])
 @pytest.mark.parametrize("train", [False, True])
 def test_norm_hook_routes_every_backbone_batchnorm(layers, style, train):
@@ -66,7 +74,7 @@ def test_norm_hook_routes_every_backbone_batchnorm(layers, style, train):
     hooked = copy.deepcopy(net)
     x = torch.randn(2, 3, 128, 128)
     record = []
-    with torch.no_grad():
+    with torch.set_grad_enabled(train):
         ref = net(x)
         got = hooked(x, None, _torch_norm(record))
     for a, b in zip(ref, got):
@@ -75,6 +83,8 @@ def test_norm_hook_routes_every_backbone_batchnorm(layers, style, train):
     for (n, a), (_, b) in zip(net.named_buffers(), hooked.named_buffers()):
         if not n.endswith("num_batches_tracked"):       # the recording hook leaves the counter to the real one
             assert torch.equal(a, b), n
+    if train:
+        _check_grads(net, hooked, ref, got)
 
 
 @pytest.mark.parametrize("train", [False, True])
@@ -84,11 +94,13 @@ def test_norm_hook_routes_every_v2v_batchnorm(train):
     hooked = copy.deepcopy(net)
     x = torch.randn(2, 4, 32, 32, 32)         # two samples: the 1^3 map of level 5 has one value per channel each
     record = []
-    with torch.no_grad():
+    with torch.set_grad_enabled(train):
         ref = net(x)
         got = hooked(x, None, _torch_norm(record))
     assert torch.equal(ref, got)
     _check_routing(hooked, record, _v2v_flags)
+    if train:
+        _check_grads(net, hooked, [ref], [got])
 
 
 def test_norm_hook_with_conv_hook_keeps_gradients():

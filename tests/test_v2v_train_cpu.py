@@ -1,4 +1,4 @@
-"""CPU checks of the native V2V training convolutions (autograd_ops.Conv3dFn / ConvTranspose3dFn), no GPU needed:
+"""CPU checks of the native V2V training convolutions (autograd_ops.ConvNdFn / ConvTranspose3dFn), no GPU needed:
 the filter re-gather that turns each data gradient into a forward convolution, and the weight-gradient kernel's index mapping
 (lt_test_conv_wgrad_host), both against torch autograd in float64."""
 import pytest

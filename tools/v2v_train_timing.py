@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""Time the V2V network's training passes with the native convolutions (v2v_backend="native": autograd_ops.Conv3dFn /
+"""Time the V2V network's training passes with the native convolutions (v2v_backend="native": autograd_ops.ConvNdFn /
 ConvTranspose3dFn) against cuDNN.
 
     python tools/v2v_train_timing.py [--iters N] [--steps N] [--rounds N] [--no-step] [--json OUT]
