@@ -120,7 +120,9 @@ int lt_unproject_aggregate_fwd(const float* features, const float* proj, const f
  *   LT_AGG_SOFTMAX: partial[B][2][nvox][C] = (sum_v s*exp(s), sum_v exp(s))   (unshifted)
  *   LT_AGG_SUM/CONF: partial[B][1][nvox][C] = sum_v s (*conf);  LT_AGG_MAX: max_v s
  * which one all-reduce (sum / max) over ranks completes; lt_unproject_finalize_fwd then divides
- * (softmax) and converts to out_format. */
+ * (softmax) and converts to out_format.
+ * Known limit of the unshifted softmax partials: exp(s) overflows above s ~ 88, and the result is 0/0 when every view's
+ * sample is below ~ -87 (fast kernel: __expf flushes to zero) or ~ -104 (generic kernel). */
 int lt_unproject_partial_fwd(const float* features, const float* proj, const float* coord, const float* conf,
                              float* partial, int B, int V_local, int C, int h, int w, long nvox,
                              int agg, void* stream);
