@@ -181,8 +181,9 @@ int lt_softargmax3d_fwd(const float* logits, long batch_stride, long voxel_strid
                         const float* coord, float* volumes_out, float* keypoints_out,
                         void* workspace, size_t workspace_bytes,
                         int B, int J, long nvox, float multiplier, int softmax, void* stream);
-/* Second half of lt_softargmax3d_fwd for compact channels-last logits (chan_stride 1, 20 <= voxel_stride <= 32) whose statistics were
- * produced by lt_v2v_tail_stats_fwd: merge of the G partials per (sample, joint) -> keypoints_out, then volumes_out (may be NULL). */
+/* Second half of lt_softargmax3d_fwd for compact channels-last logits (chan_stride 1, voxel_stride % 4 == 0, 20 <= voxel_stride <= 32,
+ * J <= voxel_stride, nvox % 8 == 0, nvox >= 16384; the layout lt_softargmax3d_fwd streams) whose statistics were produced by
+ * lt_v2v_tail_stats_fwd: merge of the G partials per (sample, joint) -> keypoints_out, then volumes_out (may be NULL). */
 int lt_softargmax3d_finish_fwd(const float* logits, long batch_stride, long voxel_stride, const float* coord, float* volumes_out,
                                float* keypoints_out, void* workspace, size_t workspace_bytes, int B, int J, long nvox, int G,
                                float multiplier, int softmax, void* stream);
@@ -278,7 +279,9 @@ int lt_v2v_tail_fwd(const void* x, const void* w1, const void* w2, const void* w
                     const float* scale2, const float* shift2, const float* scale3, const float* bias3, float* logits, long rows, int FC,
                     void* stream);
 /* The same kernel with the STATISTICS PASS of the volumetric soft-argmax (op.py:84-96: integrate_tensor_3d_with_coordinates) fused into
- * the epilogue that produces the logits (v2v.py:168-169 -> op.py:88-89): x [B * nvox][64], nvox % 128 == 0, FC <= 20, coord
+ * the epilogue that produces the logits (v2v.py:168-169 -> op.py:88-89): x [B * nvox][64], nvox % 128 == 0, nvox >= 16384, FC == 20
+ * (J 17..20; the statistics tile holds at most 20 floats per voxel, and lt_softargmax3d_finish_fwd streams no narrower rows, so any
+ * other width is refused rather than producing partials nothing can merge; J <= 16 takes lt_v2v_tail_fwd + lt_softargmax3d_fwd), coord
  * [B][nvox][3].  `workspace` (lt_softargmax3d_workspace_bytes(B, J, nvox)) receives the per-CTA online-softmax partials
  * [B][*n_partials][J][5]; lt_softargmax3d_finish_fwd with G = *n_partials (a host value known at launch time, safe under stream
  * capture) merges them into the key points and writes the normalised volumes.  softmax: 1 = softmax, 0 = ReLU (volume_softmax:false). */

@@ -318,7 +318,8 @@ extern "C" int lt_v2v_tail_fwd(const void* x, const void* w1, const void* w2, co
 }
 
 // Same kernel with the statistics pass of the volumetric soft-argmax (op.py:84-96) fused into the epilogue that produces the logits:
-// rows = B x nvox (nvox % 128 == 0, FC <= 20), coord [B][nvox][3]; `workspace` (lt_softargmax3d_workspace_bytes) receives the
+// rows = B x nvox (nvox % 128 == 0, nvox >= 16384, FC == 20: the statistics tile holds at most 20 floats per voxel and the finish
+// streams no narrower rows, stream_layout_ok), coord [B][nvox][3]; `workspace` (lt_softargmax3d_workspace_bytes) receives the
 // online-softmax partials [B][*n_partials][J][5]; lt_softargmax3d_finish_fwd(..., G = *n_partials, ...) then merges them into the key
 // points and writes the normalised volumes.  softmax: 1 = softmax, 0 = ReLU ("volume_softmax: false").
 extern "C" int lt_v2v_tail_stats_fwd(const void* x, const void* w1, const void* w2, const void* w3, const float* scale1, const float* shift1,
@@ -329,6 +330,9 @@ extern "C" int lt_v2v_tail_stats_fwd(const void* x, const void* w1, const void* 
              "v2v_tail_stats: null pointer");
   LT_REQUIRE(B > 0 && nvox > 0 && nvox % 128 == 0 && (long)B * nvox < (1L << 31), "v2v_tail_stats: bad sizes (B=%d nvox=%ld)", B, nvox);
   LT_REQUIRE(FC % 4 == 0 && FC >= 4 && FC <= kTailStatMaxFC && J > 0 && J <= FC, "v2v_tail_stats: need J <= FC <= %d, FC %% 4 == 0", kTailStatMaxFC);
+  // only partials that lt_softargmax3d_finish_fwd can merge: with FC <= 20 that is FC == 20 (J 17..20) and nvox >= 16384
+  LT_REQUIRE(stream_layout_ok(FC, J, nvox), "v2v_tail_stats: logits of width FC=%d (J=%d, nvox=%ld) are not covered by the streaming finish",
+             FC, J, nvox);
   LT_REQUIRE(softmax == 0 || softmax == 1, "v2v_tail_stats: mode must be 0 (ReLU) or 1 (softmax)");
   LT_REQUIRE(workspace_bytes >= lt_softargmax3d_workspace_bytes(B, J, nvox), "v2v_tail_stats: workspace too small");
   TailParams p;

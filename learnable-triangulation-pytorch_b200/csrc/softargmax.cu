@@ -190,7 +190,6 @@ constexpr int kStreamScratchBytes = 20480;             // CTA merge scratch [256
 constexpr int kStreamSmemBytes = kStreamStages * kStreamStageBytes + kStreamScratchBytes + 128 + 128;
 constexpr int kMaxStreamCtas = 640;
 constexpr int kMaxPartials = 1024;      // partial slots per sample the workspace is sized for (fused tail: 3 CTAs per SM)
-constexpr long kStreamMinVoxels = 16384;
 
 struct StreamParams {
   const float* logits;    // [B][nvox][vs]
@@ -396,13 +395,12 @@ __global__ void __launch_bounds__(kStreamThreads, 2) stream_normalize_kernel(con
       const int j = jg * 4 + ji;
       const bool jok = j < p.J;
       const float2 ms = jok ? __ldg(reinterpret_cast<const float2*>(p.stats + ((long)b * p.J + j) * 2)) : make_float2(0.f, 0.f);
-      const float nb = -ms.x * kLog2e;
       float* dst = p.volumes + ((long)b * p.J + (jok ? j : 0)) * p.nvox + v0;
       for (int rg = warp; rg < rgroups; rg += kStreamConsumers / 32) {
         const int r = rg * 8 + rr;
         if (jok && r < rows) {
           const float v = tile[r * p.vs + j] * p.mult;          // same rounding as the statistics pass
-          const float o = SM ? ex2f(fmaf(v, kLog2e, nb)) * ms.y : fmaxf(v, 0.0f);
+          const float o = SM ? ex2f((v - ms.x) * kLog2e) * ms.y : fmaxf(v, 0.0f);   // l - max first, as in st_push4
           __stcs(dst + r, o);
         }
       }
@@ -414,8 +412,7 @@ __global__ void __launch_bounds__(kStreamThreads, 2) stream_normalize_kernel(con
 
 static bool stream_shape_ok(const float* logits, long batch_stride, long voxel_stride, const float* coord, const float* volumes_out, int J,
                             long nvox) {
-  return J <= 32 && voxel_stride >= J && voxel_stride % 4 == 0 && voxel_stride >= 20 && voxel_stride <= 32 && nvox % 8 == 0 && batch_stride % 4 == 0 &&
-         nvox >= kStreamMinVoxels && ((uintptr_t)logits & 15) == 0 && ((uintptr_t)coord & 15) == 0 &&
+  return stream_layout_ok(voxel_stride, J, nvox) && batch_stride % 4 == 0 && ((uintptr_t)logits & 15) == 0 && ((uintptr_t)coord & 15) == 0 &&
          (!volumes_out || ((uintptr_t)volumes_out & 31) == 0);
 }
 

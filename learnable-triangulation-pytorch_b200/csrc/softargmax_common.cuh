@@ -64,16 +64,18 @@ __device__ __forceinline__ float ex2f(float x) {
   return r;
 }
 
-// fold four (logit, coordinate) pairs into one online-softmax state: one rescale + four exponentials
+// fold four (logit, coordinate) pairs into one online-softmax state: one rescale + four exponentials.  The exponents are formed as
+// (l - m) * log2(e), not as fma(l, log2(e), -m * log2(e)): the rounding of m * log2(e) grows with |m| and differs between running
+// maxima, which put up to ~2e-8 x |m| of relative error into the weights (4e-5 of scale at |m| = 1024); l - m is exact for the logits
+// that matter (Sterbenz), so the weights are as accurate at any offset as at m = 0.
 template <bool SM>
 __device__ __forceinline__ void st_push4(SoftState& s, const float (&l)[4], const float (&x)[4], const float (&y)[4], const float (&z)[4]) {
   if (SM) {
     const float mn = fmaxf(fmaxf(fmaxf(l[0], l[1]), fmaxf(l[2], l[3])), s.m);
     if (mn == -INFINITY) return;                 // nothing but padding so far
-    const float nb = -mn * kLog2e;
-    const float r = ex2f(fmaf(s.m, kLog2e, nb)); // exp(m_old - m_new); 0 for the first batch (m_old = -inf)
-    const float e0 = ex2f(fmaf(l[0], kLog2e, nb)), e1 = ex2f(fmaf(l[1], kLog2e, nb));
-    const float e2 = ex2f(fmaf(l[2], kLog2e, nb)), e3 = ex2f(fmaf(l[3], kLog2e, nb));
+    const float r = ex2f((s.m - mn) * kLog2e);   // exp(m_old - m_new); 0 for the first batch (m_old = -inf)
+    const float e0 = ex2f((l[0] - mn) * kLog2e), e1 = ex2f((l[1] - mn) * kLog2e);
+    const float e2 = ex2f((l[2] - mn) * kLog2e), e3 = ex2f((l[3] - mn) * kLog2e);
     s.d = fmaf(s.d, r, (e0 + e1) + (e2 + e3));
     s.sx = fmaf(s.sx, r, fmaf(e0, x[0], fmaf(e1, x[1], fmaf(e2, x[2], e3 * x[3]))));
     s.sy = fmaf(s.sy, r, fmaf(e0, y[0], fmaf(e1, y[1], fmaf(e2, y[2], e3 * y[3]))));
@@ -88,6 +90,15 @@ __device__ __forceinline__ void st_push4(SoftState& s, const float (&l)[4], cons
   }
 }
 
+
+// Logits layout the streaming kernels read (softargmax.cu): channels-last rows of vs floats with vs % 4 == 0, 20 <= vs <= 32 and
+// J <= vs, nvox % 8 == 0 and at least kStreamMinVoxels voxels.  lt_softargmax3d_fwd streams such logits (given aligned pointers),
+// lt_softargmax3d_finish_fwd accepts only them, and lt_v2v_tail_stats_fwd produces partials only for them, so every set of fused
+// partials can be merged.  engine.NativeEngine.v2v mirrors this test (_stream_layout_ok) when it decides to fuse.
+constexpr long kStreamMinVoxels = 16384;
+__host__ __device__ inline bool stream_layout_ok(long vs, int J, long nvox) {
+  return vs % 4 == 0 && vs >= 20 && vs <= 32 && J <= vs && nvox % 8 == 0 && nvox >= kStreamMinVoxels;
+}
 
 // Workspace layout shared by lt_softargmax3d_fwd (streaming path), lt_v2v_tail_stats_fwd and lt_softargmax3d_finish_fwd:
 // partial [B][G][J][5] floats, then (16-byte aligned) stats [B][J][2] = (max, 1 / sum)

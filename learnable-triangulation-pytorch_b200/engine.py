@@ -27,6 +27,12 @@ def _round_up(v, m):
     return (v + m - 1) // m * m
 
 
+def _stream_layout_ok(vs, J, nvox):
+    """Logits of voxel stride vs that the streaming soft-argmax kernels read: stream_layout_ok in csrc/softargmax_common.cuh.  The fused
+    V2V tail's statistics are merged by those kernels, so the engine fuses only for such a layout."""
+    return vs % 4 == 0 and 20 <= vs <= 32 and J <= vs and nvox % 8 == 0 and nvox >= 16384
+
+
 class Act:
     """Channels-last activation: `data` is float32 [N,D,H,W,C] or bfloat16 [N,D,H,W,2C] (split-fp16)."""
     __slots__ = ("data", "N", "D", "H", "W", "C", "fmt", "stats")
@@ -536,7 +542,8 @@ class NativeEngine:
             logits = Act(x.N, x.D, x.H, x.W, out_c, FMT_F32, x.data.device)
             rows = x.pixels
             nvox = x.D * x.H * x.W
-            fuse = (softargmax_args is not None and nvox % 128 == 0 and nvox >= 16384 and out_c <= 20
+            # the statistics tile takes at most 20 floats per voxel and the streaming finish no fewer: J 17..20 (out_c 20)
+            fuse = (softargmax_args is not None and nvox % 128 == 0 and out_c <= 20 and _stream_layout_ok(out_c, softargmax_args[1], nvox)
                     and softargmax_args[3] in (0, 1, False, True))
             with self._timed("conv_tail", flops=2.0 * rows * (b1.kmacs + b2.kmacs + b3.kmacs), nbytes=rows * (128 + 4 * out_c + (12 if fuse else 0)),
                              desc="N%d %dx%dx%d 32->32->32->%d k111 fused%s" % (x.N, x.D, x.H, x.W, b3.cout, " + soft-argmax statistics" if fuse else "")):
