@@ -348,7 +348,7 @@ def conv_transpose2d_k4s2_dgrad_filter(weight_shape):
 def _launch(x_s, cin_p, pk, out_dims, out_c, scale, shift, out_fmt=capi.FMT_F32, out_scale=(1, 1, 1), out_full=None, groups=(1, 1, 1),
             out_off=(0, 0, 0), out=None):
     """One lt_conv_nd_fwd of packed filter `pk` over split-fp16 x_s into `out` (allocated when None); the full-resolution 3^3 / 7^3
-    layers take LT_CONV_TC_FOLD as in the inference engine."""
+    layers take LT_CONV_TC_FOLD as in the inference engine (engine.fold_width_ok)."""
     N, D, H, W = x_s.shape[:4]
     fd, fh, fw = out_full or out_dims
     c_store = out_c if out_fmt == capi.FMT_F32 else 2 * out_c
@@ -357,8 +357,9 @@ def _launch(x_s, cin_p, pk, out_dims, out_c, scale, shift, out_fmt=capi.FMT_F32,
     d = conv_desc(N, (D, H, W), cin_p, pk.cout_p, pk.k, pk.stride, pk.pad, out_dims, out_c, out_fmt, out_scale, out_full, groups, out_off)
     ws = _workspace(x_s.device, 0)
     d.workspace, d.workspace_bytes = ws.data_ptr(), ws.numel()
+    from .engine import fold_width_ok
     impl, weight = capi.CONV_TC, pk.w
-    if pk.w_fold is not None and W >= 16 and out_c == 32 and out_fmt == capi.FMT_F32:
+    if pk.w_fold is not None and fold_width_ok(pk.k[2], W) and out_c == 32 and out_fmt == capi.FMT_F32:
         impl, weight = capi.CONV_TC_FOLD, pk.w_fold
         d.Cout = pk.cout
     capi.conv_nd(d, x_s, weight, scale, shift, None, out, impl)

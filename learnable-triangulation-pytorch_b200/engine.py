@@ -83,6 +83,12 @@ class _Timed:
 _TC_IMPL = {"simt": CONV_SIMT, "tc": CONV_TC, "tc1": CONV_TC1}
 
 
+def fold_width_ok(k, width):
+    """Whether LT_CONV_TC_FOLD takes a layer packed for it at this W: 3^3 (conv_lines_kernel, whole W lines as the m64 rows)
+    for 16 <= W <= 64, 7^3 (conv_fold_kernel) for W >= 16.  Wider 3^3 layers run on conv_tc_kernel."""
+    return width >= 16 and (k == 7 or width <= 64)
+
+
 def pack_filter(src, k, stride, pad, cin, cout, bias, bn, mode="tc", cin_pad=None, force_simt=False, out_fmt=None):
     """src = (filter tensor, base, (s_td, s_th, s_tw, s_ci, s_co)): where element (td, th, tw, ci, co) of this (phase of a)
     convolution sits inside the module's own weight tensor.  Everything below is our own kernels: gather to the canonical
@@ -132,9 +138,10 @@ def pack_filter(src, k, stride, pad, cin, cout, bias, bn, mode="tc", cin_pad=Non
         pk.w, pk.cin, pk.cout_p, pk.impl, pk.in_fmt = wp, cin_p, cout_p, CONV_SIMT, FMT_F32
     pk.scale = torch.empty(cout_p, dtype=torch.float32, device=dev)
     pk.shift = torch.empty(cout_p, dtype=torch.float32, device=dev)
-    # tensor-core accumulation steps on the main fp32 accumulator (one hi*hi MMA per 16 input channels and tap, in conv_tc_kernel and in
-    # conv_fold_kernel alike): lt_fold_bn_fwd compensates the expected truncation shrinkage (include/lt_b200.h)
-    steps = taps * (cin_p // 16) if use_tc else 0
+    # tensor-core accumulation steps on the main fp32 accumulator (one hi*hi MMA per 16 input channels and tap, in conv_tc_kernel and
+    # conv_fold_kernel alike; conv_lines_kernel, the 3^3 layers packed for LT_CONV_TC_FOLD, accumulates each kw column over the 9
+    # (kd, kh) taps and sums the three in fp32): lt_fold_bn_fwd compensates the expected truncation shrinkage (include/lt_b200.h)
+    steps = (9 if pk.w_fold is not None and k[0] == 3 else taps) * (cin_p // 16) if use_tc else 0
     for g in range(G):     # the per-channel affine repeats for every column block
         sc, sh = pk.scale[g * cout:g * cout + blk_p], pk.shift[g * cout:g * cout + blk_p]
         if bn is not None:
@@ -384,7 +391,8 @@ class NativeEngine:
         ws = self._splitk_workspace(x.data.device)
         d.workspace, d.workspace_bytes = ws.data_ptr(), ws.numel()
         impl, weight = pk.impl, pk.w
-        if (pk.w_fold is not None and x.W >= 16 and out.C == 32 and out_scale == (1, 1, 1) and (od, oh, ow) == (x.D, x.H, x.W)):
+        if (pk.w_fold is not None and fold_width_ok(kw, x.W) and out.C == 32 and out_scale == (1, 1, 1)
+                and (od, oh, ow) == (x.D, x.H, x.W)):
             impl, weight = CONV_TC_FOLD, pk.w_fold
             d.Cout = pk.cout
         label = {CONV_TC_FOLD: "conv_fold", CONV_SIMT: "conv_ffma"}.get(impl, "conv_tc")
