@@ -256,9 +256,10 @@ int lt_conv_tc_pack_weights(const float* w_tap_ci_co, void* packed, int taps, in
  *   nn.ConvTranspose: (Cin, Cout, k...); stride phases of a transposed conv: a tap sub-lattice walked with negative strides).
  * lt_fold_bn_fwd: eval-mode BatchNorm (pose_resnet.py:30-31, v2v.py:12) + conv bias -> per-channel scale / shift [CP] (double
  *   arithmetic, rounded once); mean == NULL: no BatchNorm.  accum_steps: tensor-core MMA steps that accumulate into the main fp32
- *   accumulator of the kernel that will consume this scale (taps x Cin / 16; 0 for the exact-fp32 kernels).  The tensor core adds
- *   with truncation, which shrinks a sum by an expected 0.28 x steps x 2^-24 (rate measured on the tensor-memory MMA of the kernels' first target, not re-measured for wgmma);
- *   the scale is multiplied by 1 + that, which halves the rms accumulation error.
+ *   accumulator of the kernel that will consume this scale (taps x Cin / 16 for conv_tc_kernel, whose split-K reduce rescales to one
+ *   split's share, and conv_fold_kernel; 9 x Cin / 16 for conv_lines_kernel; 0 for the exact-fp32 kernels).  The tensor core adds
+ *   with truncation, which shrinks a sum by an expected 0.28 x steps x 2^-24 (wgmma on an H100 80GB HBM3 at 700 W: 0.25 - 0.33,
+ *   tests/test_gpu_conv.py); the scale is multiplied by 1 + that, which halves the rms accumulation error.
  * lt_absmax_fwd: float bit pattern of max|w| over n elements.  Passed (optionally, else NULL) to the two calls above it selects the
  *   power-of-two filter pre-scale S = 2^(9 - floor(log2 max|w|)) of the tensor-core path: the gathered filter is multiplied by S,
  *   the folded scale by 1 / S (exact), so that the unscaled low halves of the split-fp16 weights stay normal numbers. */

@@ -362,6 +362,8 @@ def _launch(x_s, cin_p, pk, out_dims, out_c, scale, shift, out_fmt=capi.FMT_F32,
     if pk.w_fold is not None and fold_width_ok(pk.k[2], W) and out_c == 32 and out_fmt == capi.FMT_F32:
         impl, weight = capi.CONV_TC_FOLD, pk.w_fold
         d.Cout = pk.cout
+        if pk.scale_fold is not pk.scale:    # `scale` derives from pk.scale (conv_tc_kernel's steps): the lines kernel's gain instead
+            scale = scale * (pk.scale_fold / pk.scale.masked_fill(pk.scale == 0, 1.0))
     capi.conv_nd(d, x_s, weight, scale, shift, None, out, impl)
     return out, d
 

@@ -90,6 +90,13 @@ __device__ __forceinline__ float4 load_s32x4(const sh_t* row, int c) {
 // ~22-bit operands); Kaiming-sized filters (|w| ~ 0.03) would otherwise keep only ~2^-20 relative precision, which a
 // 152-layer trunk amplifies to ~1.5e-4 at the features (measured).  1 / S is folded into the
 // epilogue scale (exact).  absmax_bits: the float bit pattern of max|w| (lt_absmax_fwd), or null for "no scaling".
+// The tensor core adds with truncation: a sum accumulated in `steps` k16 steps shrinks by an expected kAccumTruncRate x steps x 2^-24
+// of itself.  Measured for wgmma on an H100 80GB HBM3 at 700 W (tests/test_gpu_conv.py, test_accumulation_gain): 0.25 - 0.33 over
+// the 7^3, 3^3, 3x3, 1x1 and split-K layers.  lt_fold_bn_fwd multiplies the folded scale by 1 + that (accum_gain) for the steps of the
+// kernel that will consume it; splitk_reduce_kernel rescales its sum to the steps of one split.
+constexpr double kAccumTruncRate = 0.28;
+__host__ __device__ inline double accum_gain(double steps) { return 1.0 + kAccumTruncRate * steps * 5.9604644775390625e-08; }   // 2^-24
+
 __device__ __forceinline__ float weight_pow2_scale(const unsigned* absmax_bits) {
   if (!absmax_bits) return 1.0f;
   const unsigned b = *absmax_bits;

@@ -31,7 +31,8 @@
 // the same epilogue with zero accumulators (scale 0, shift 0 for the padding channels: written as zeros).
 //
 // Per 16-wide K slice hi*hi accumulates into D1 and hi*lo + lo*hi into D2, as in conv_tc_kernel: D1 takes 9 Cin / 16 (3^3: one
-// column per kw) or K^3 Cin / 16 (7^3) accumulation steps per output (the accum_steps of the folded scale, engine.pack_filter).
+// column per kw) or K^3 Cin / 16 (7^3) accumulation steps per output (the accum_steps of the folded scale: ConvPack.scale_fold,
+// engine.pack_filter).
 //
 // Persistent grids: one CTA per SM; the producer warp runs its rings across tile (piece) boundaries.  An A stage is released as
 // soon as the consumers' ldmatrix reads of it have completed; a weight slice once the MMAs reading it have.

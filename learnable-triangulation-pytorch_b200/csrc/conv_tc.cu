@@ -441,6 +441,7 @@ __global__ void __launch_bounds__(256) splitk_reduce_kernel(const TcParams p, lo
       const float4 v = *reinterpret_cast<const float4*>(p.ws + ((size_t)z * m_tiles * 128 + tr) * p.ws_ld + co);
       a.x += v.x; a.y += v.y; a.z += v.z; a.w += v.w;
     }
+    a.x *= p.ws_gain; a.y *= p.ws_gain; a.z *= p.ws_gain; a.w *= p.ws_gain;
     const float4 sc = __ldg(reinterpret_cast<const float4*>(p.scale + co));
     const float4 sh = __ldg(reinterpret_cast<const float4*>(p.shift + co));
     float4 o = make_float4(fmaf(a.x, sc.x, sh.x), fmaf(a.y, sc.y, sh.y), fmaf(a.z, sc.z, sh.z), fmaf(a.w, sc.w, sh.w));
@@ -565,6 +566,10 @@ static int launch_tc(const CUtensorMap& tmA, const CUtensorMap& tmB, TcParams& p
   tc_plan(m_tiles, n_tiles, p.Nt, p.KD * p.KH * p.KW * p.CB, p.terms, p.n_maps, ws ? opts().tc_splitk : 0, ws_bytes, sm_count(),
           &splits, &grid);
   p.splits = splits;
+  // The folded scale compensates the truncation of all 2 x chunks k16 steps (engine.pack_filter); each split's partial accumulator
+  // takes 1 / splits of them, so the reduce pass scales the sum back to that gain.
+  const double steps = 2.0 * p.KD * p.KH * p.KW * p.CB;
+  p.ws_gain = (float)(accum_gain(steps / splits) / accum_gain(steps));
   p.ws = reinterpret_cast<float*>(ws);
   p.ws_ld = n_tiles * p.Nt;
   p.n_tiles = n_tiles;
@@ -614,7 +619,7 @@ void fill_params(const lt_conv_desc* d, TcParams& p, int CB, int CoutP, int Nt, 
   p.osd = d->osd; p.osh = d->osh; p.osw = d->osw; p.ood = d->ood; p.ooh = d->ooh; p.oow = d->oow;
   p.relu = d->relu; p.residual = d->residual; p.out_format = d->out_format;
   p.scale = scale; p.shift = shift; p.res = residual; p.out = out;
-  p.splits = 1; p.ws = nullptr; p.ws_ld = 0; p.stages = 0; p.n_tiles = 1;
+  p.splits = 1; p.ws = nullptr; p.ws_ld = 0; p.ws_gain = 1.0f; p.stages = 0; p.n_tiles = 1;
   p.n_maps = out_groups(d);
   p.oc = p.n_maps > 1 ? d->Cout / p.n_maps : CoutP;
   p.gh = d->ogh > 1 ? d->ogh : 1; p.gw = d->ogw > 1 ? d->ogw : 1;
@@ -752,7 +757,7 @@ extern "C" int lt_tc_gemm_selftest(const void* a, const void* b, float* d, int M
   p.relu = 0; p.residual = LT_RES_NONE; p.out_format = LT_FMT_F32;
   p.scale = ones; p.shift = zeros; p.res = nullptr; p.out = d;
   p.n_maps = 1; p.oc = N; p.gh = p.gw = 1;
-  p.splits = 1; p.ws = nullptr; p.ws_ld = 0; p.n_tiles = 1;
+  p.splits = 1; p.ws = nullptr; p.ws_ld = 0; p.ws_gain = 1.0f; p.n_tiles = 1;
   CUtensorMap tmA, tmB;
   {
     const uint64_t dims[5] = {(uint64_t)K, (uint64_t)M, 1, 1, 1};

@@ -24,6 +24,7 @@ struct TcParams {
   // writes its raw fp32 accumulator tile to ws[z][m tile][128][ws_ld]; splitk_reduce_kernel sums and applies the epilogue
   int splits, ws_ld;
   float* ws;
+  float ws_gain;   // splitk_reduce_kernel: accum_gain(steps of one split) / accum_gain(steps of the whole K loop), see launch_tc
   int n_tiles;   // N tiles of Nt channels (conv_tc_kernel work units: n_tiles x M tiles x splits)
   // grouped output (lt_conv_desc.ogd/ogh/ogw): output channel block g of `oc` channels goes to output map g (its own phase offset)
   int oc, n_maps;

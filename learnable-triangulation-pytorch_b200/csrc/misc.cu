@@ -245,8 +245,8 @@ __global__ void __launch_bounds__(256) gather_weights_kernel(const float* __rest
 
 // y = acc * scale + shift with scale = gamma / sqrt(var + eps), shift = beta - mean * scale (+ conv_bias * scale); double arithmetic,
 // rounded once.  Any of gamma / beta / bias may be null; mean == null means "no BatchNorm" (scale 1, shift = bias).
-// accum_gain = 1 + 0.28 * steps * 2^-24: compensates the expected shrinkage of a sum accumulated by `steps` truncating tensor-core
-// additions (rate measured on the kernels' first target, not re-measured for wgmma); 1 for the exact-fp32 kernels.
+// accum_gain(steps) (common.cuh): compensates the expected shrinkage of a sum accumulated by `steps` truncating tensor-core additions;
+// 1 for the exact-fp32 kernels.
 __global__ void fold_bn_kernel(const float* gamma, const float* beta, const float* mean, const float* var, const float* bias, double eps,
                                int C, int CP, const unsigned* absmax_bits, double accum_gain, float* scale, float* shift) {
   const int c = blockIdx.x * blockDim.x + threadIdx.x;
@@ -315,8 +315,8 @@ extern "C" int lt_fold_bn_fwd(const float* gamma, const float* beta, const float
                               int C, int CP, const unsigned int* absmax_bits, int accum_steps, float* scale, float* shift, void* stream) {
   using namespace lt;
   LT_REQUIRE(scale && shift && C > 0 && CP >= C && (!mean || var) && accum_steps >= 0, "fold_bn: bad arguments");
-  const double accum_gain = 1.0 + 0.28 * (double)accum_steps * 5.9604644775390625e-08;   // 2^-24
-  fold_bn_kernel<<<ceil_div(CP, 128), 128, 0, (cudaStream_t)stream>>>(gamma, beta, mean, var, conv_bias, (double)eps, C, CP, absmax_bits, accum_gain, scale, shift);
+  fold_bn_kernel<<<ceil_div(CP, 128), 128, 0, (cudaStream_t)stream>>>(gamma, beta, mean, var, conv_bias, (double)eps, C, CP, absmax_bits,
+                                                                   accum_gain((double)accum_steps), scale, shift);
   LT_CHECK_LAUNCH("fold_bn_kernel");
   return LT_OK;
 }

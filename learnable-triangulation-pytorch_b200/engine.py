@@ -54,7 +54,8 @@ class Act:
 
 class ConvPack:
     """One (phase of a) convolution, ready to launch: packed filter + folded scale/shift + geometry."""
-    __slots__ = ("w", "scale", "shift", "taps", "k", "stride", "pad", "cin", "cout", "cout_p", "impl", "in_fmt", "kmacs", "w_fold", "groups")
+    __slots__ = ("w", "scale", "shift", "taps", "k", "stride", "pad", "cin", "cout", "cout_p", "impl", "in_fmt", "kmacs", "w_fold", "scale_fold",
+                 "groups")
 
 
 def _f32(t):
@@ -136,20 +137,30 @@ def pack_filter(src, k, stride, pad, cin, cout, bias, bn, mode="tc", cin_pad=Non
             pk.w_fold = wf
     else:
         pk.w, pk.cin, pk.cout_p, pk.impl, pk.in_fmt = wp, cin_p, cout_p, CONV_SIMT, FMT_F32
-    pk.scale = torch.empty(cout_p, dtype=torch.float32, device=dev)
-    pk.shift = torch.empty(cout_p, dtype=torch.float32, device=dev)
-    # tensor-core accumulation steps on the main fp32 accumulator (one hi*hi MMA per 16 input channels and tap, in conv_tc_kernel and
-    # conv_fold_kernel alike; conv_lines_kernel, the 3^3 layers packed for LT_CONV_TC_FOLD, accumulates each kw column over the 9
-    # (kd, kh) taps and sums the three in fp32): lt_fold_bn_fwd compensates the expected truncation shrinkage (include/lt_b200.h)
-    steps = (9 if pk.w_fold is not None and k[0] == 3 else taps) * (cin_p // 16) if use_tc else 0
+    # tensor-core accumulation steps on the main fp32 accumulator, which lt_fold_bn_fwd compensates for the expected truncation shrinkage
+    # (accum_gain, csrc/common.cuh): one hi*hi MMA per 16 input channels and tap in conv_tc_kernel (its split-K reduce rescales to the
+    # steps of one split) and conv_fold_kernel; conv_lines_kernel, the 3^3 layers packed for LT_CONV_TC_FOLD, accumulates each kw column
+    # over the 9 (kd, kh) taps and sums the three in fp32.  A fold-packed 3^3 layer keeps both scales: it runs on conv_tc_kernel at
+    # widths and output mappings the lines kernel does not take.
+    steps = taps * (cin_p // 16) if use_tc else 0
+    fold_steps = 9 * (cin_p // 16) if pk.w_fold is not None and k[0] == 3 else steps
+    pk.scale, pk.shift = _fold_scale(bn, bias, cout, blk_p, cout_p, G, amax, steps, dev)
+    pk.scale_fold = pk.scale if fold_steps == steps else _fold_scale(bn, bias, cout, blk_p, cout_p, G, amax, fold_steps, dev)[0]
+    return pk
+
+
+def _fold_scale(bn, bias, cout, blk_p, cout_p, G, amax, steps, dev):
+    """(scale, shift) [cout_p] of lt_fold_bn_fwd for a filter whose kernel accumulates `steps` tensor-core steps per output."""
+    scale = torch.empty(cout_p, dtype=torch.float32, device=dev)
+    shift = torch.empty(cout_p, dtype=torch.float32, device=dev)
     for g in range(G):     # the per-channel affine repeats for every column block
-        sc, sh = pk.scale[g * cout:g * cout + blk_p], pk.shift[g * cout:g * cout + blk_p]
+        sc, sh = scale[g * cout:g * cout + blk_p], shift[g * cout:g * cout + blk_p]
         if bn is not None:
             capi.fold_bn(_f32(bn.weight), _f32(bn.bias), _f32(bn.running_mean), _f32(bn.running_var), _f32(bias), bn.eps, cout, blk_p,
                          sc, sh, amax, accum_steps=steps)
         else:
             capi.fold_bn(None, None, None, None, _f32(bias), 0.0, cout, blk_p, sc, sh, amax, accum_steps=steps)
-    return pk
+    return scale, shift
 
 
 def pack_conv(conv, bn, mode="tc", cin_pad=None, **kw):
@@ -390,15 +401,15 @@ class NativeEngine:
             assert residual.fmt == out.fmt and residual.C == out.C
         ws = self._splitk_workspace(x.data.device)
         d.workspace, d.workspace_bytes = ws.data_ptr(), ws.numel()
-        impl, weight = pk.impl, pk.w
+        impl, weight, scale = pk.impl, pk.w, pk.scale
         if (pk.w_fold is not None and fold_width_ok(kw, x.W) and out.C == 32 and out_scale == (1, 1, 1)
                 and (od, oh, ow) == (x.D, x.H, x.W)):
-            impl, weight = CONV_TC_FOLD, pk.w_fold
+            impl, weight, scale = CONV_TC_FOLD, pk.w_fold, pk.scale_fold
             d.Cout = pk.cout
         label = {CONV_TC_FOLD: "conv_fold", CONV_SIMT: "conv_ffma"}.get(impl, "conv_tc")
         with self._timed(label, flops=2.0 * x.N * od * oh * ow * pk.kmacs,
                          desc="N%d %dx%dx%d Cin%d Cout%d k%d%d%d s%d" % (x.N, od, oh, ow, pk.cin, pk.cout, kd, kh, kw, sw)):
-            capi.conv_nd(d, x.data, weight, pk.scale, pk.shift, None if residual is None else residual.data, out.data, impl)
+            capi.conv_nd(d, x.data, weight, scale, pk.shift, None if residual is None else residual.data, out.data, impl)
         self.launches += 1
         return out
 
