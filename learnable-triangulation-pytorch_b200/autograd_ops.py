@@ -13,7 +13,8 @@ numpy camera data).
 """
 import torch
 
-from . import capi
+from . import capi, engine
+from .engine import _round_up
 
 
 class UnprojectHeatmapsFn(torch.autograd.Function):
@@ -83,13 +84,6 @@ class IntegrateTensor3dFn(torch.autograd.Function):
         return grad_logits, None, None
 
 
-def pixel_grid(B, h, w, device):
-    """(B, h*w, 3) float32 coordinates (x, y, 0) of the pixels of an h x w map: the 2-D soft-argmax runs on the 3-D kernels."""
-    ys, xs = torch.meshgrid(torch.arange(h, device=device, dtype=torch.float32), torch.arange(w, device=device, dtype=torch.float32),
-                            indexing="ij")
-    return torch.stack([xs, ys, torch.zeros_like(xs)], dim=-1).reshape(1, h * w, 3).expand(B, h * w, 3).contiguous()
-
-
 class IntegrateTensor2dFn(torch.autograd.Function):
     """op.integrate_tensor_2d (reference op.py:11-47): (B, J, h, w) -> (coordinates (B, J, 2) [x, y in pixels], heat-maps)."""
 
@@ -98,7 +92,7 @@ class IntegrateTensor2dFn(torch.autograd.Function):
         B, J, h, w = heatmaps.shape
         dev = heatmaps.device
         logits = heatmaps.detach().float().contiguous()
-        grid = pixel_grid(B, h, w, dev)
+        grid = engine.pixel_grid(B, h, w, dev)
         out = torch.empty_like(logits)
         kp = torch.empty((B, J, 3), dtype=torch.float32, device=dev)
         ws = torch.empty(capi.softargmax3d_workspace_bytes(B, J, h * w) // 4 + 1, dtype=torch.float32, device=dev)
@@ -218,16 +212,12 @@ _WORKSPACE = {}
 
 
 def _workspace(device, nbytes):
-    """Scratch shared by the split-K conv launches and the weight gradient of one device (launches on one stream are ordered)."""
+    """Scratch of the weight-gradient and BatchNorm launches of one device (launches on one stream are ordered); it grows on demand."""
     ws = _WORKSPACE.get(device)
     if ws is None or ws.numel() < nbytes:
         ws = torch.empty(max(nbytes, 32 << 20), dtype=torch.uint8, device=device)
         _WORKSPACE[device] = ws
     return ws
-
-
-def _round_up(v, m):
-    return (v + m - 1) // m * m
 
 
 def _as3(t, fill):
@@ -258,33 +248,18 @@ def _to_s32(x_cl, cp, absmax_bits=None, inv_scale=None):
     return out
 
 
-def conv_desc(N, in_dims, cin_p, cout_p, k, stride, pad, out_dims, out_c, out_fmt, out_scale=(1, 1, 1), out_full=None, groups=(1, 1, 1),
-              out_off=(0, 0, 0)):
-    """lt_conv_desc of a split-fp16-input launch without ReLU or residual; out_full: the output tensor's grid (default out_dims)."""
-    fd, fh, fw = out_full or out_dims
-    return capi.ConvDesc(N=N, ID=in_dims[0], IH=in_dims[1], IW=in_dims[2], Cin=cin_p, OD=out_dims[0], OH=out_dims[1], OW=out_dims[2],
-                         Cout=cout_p, KD=k[0], KH=k[1], KW=k[2], sd=stride[0], sh=stride[1], sw=stride[2], pd=pad[0], ph=pad[1], pw=pad[2],
-                         FD=fd, FH=fh, FW=fw, FC=out_c, osd=out_scale[0], osh=out_scale[1], osw=out_scale[2],
-                         ood=out_off[0], ooh=out_off[1], oow=out_off[2], relu=0, residual=capi.RES_NONE,
-                         in_format=capi.FMT_S32, out_format=out_fmt, ogd=groups[0], ogh=groups[1], ogw=groups[2])
-
-
-def conv_out_dims(dims, k, stride, padding):
-    return tuple((n + 2 * p - kk) // s + 1 for n, kk, s, p in zip(dims, k, stride, padding))
-
-
 def conv3d_wgrad_desc(N, dims, cin, cout, k, padding, stride=(1, 1, 1)):
     """The forward launch of a convolution (3-D form: a 2-D one has D = 1) as lt_conv_wgrad_fwd reads it: split-fp16 input and
     output gradient, 32-channel padded."""
-    return conv_desc(N, dims, _round_up(cin, 32), _round_up(cout, 32), k, stride, padding, conv_out_dims(dims, k, stride, padding),
-                     _round_up(cout, 32), capi.FMT_S32)
+    cin_p, cout_p, out_dims = _round_up(cin, 32), _round_up(cout, 32), engine.conv_out_dims(dims, k, stride, padding)
+    return engine.conv_desc(N, dims, cin_p, cout_p, k, stride, padding, out_dims, out_dims, cout_p, capi.FMT_S32, capi.FMT_S32)
 
 
 def conv_transpose3d_desc(N, dims, cin, cout):
     """ConvTranspose3d(k=2, s=2) as the engine's one grouped 1x1x1 GEMM: N = 8 cout, block g = a 4 + b 2 + c to output phase (a, b, c)."""
     D, H, W = dims
-    return conv_desc(N, dims, cin, 8 * cout, (1, 1, 1), (1, 1, 1), (0, 0, 0), dims, cout, capi.FMT_S32, out_scale=(2, 2, 2),
-                     out_full=(2 * D, 2 * H, 2 * W), groups=(2, 2, 2))
+    return engine.conv_desc(N, dims, cin, 8 * cout, (1, 1, 1), (1, 1, 1), (0, 0, 0), dims, (2 * D, 2 * H, 2 * W), cout, capi.FMT_S32,
+                            capi.FMT_S32, out_scale=(2, 2, 2), out_groups=(2, 2, 2))
 
 
 def conv3d_dgrad_filter(weight_shape, padding):
@@ -345,29 +320,6 @@ def conv_transpose2d_k4s2_dgrad_filter(weight_shape):
     return (0, (0, 4, 1, 16, cout * 16)), (1, 4, 4), (1, 2, 2), (0, 1, 1), cout, cin
 
 
-def _launch(x_s, cin_p, pk, out_dims, out_c, scale, shift, out_fmt=capi.FMT_F32, out_scale=(1, 1, 1), out_full=None, groups=(1, 1, 1),
-            out_off=(0, 0, 0), out=None):
-    """One lt_conv_nd_fwd of packed filter `pk` over split-fp16 x_s into `out` (allocated when None); the full-resolution 3^3 / 7^3
-    layers take LT_CONV_TC_FOLD as in the inference engine (engine.fold_width_ok)."""
-    N, D, H, W = x_s.shape[:4]
-    fd, fh, fw = out_full or out_dims
-    c_store = out_c if out_fmt == capi.FMT_F32 else 2 * out_c
-    if out is None:
-        out = torch.empty((N, fd, fh, fw, c_store), dtype=torch.float32 if out_fmt == capi.FMT_F32 else torch.float16, device=x_s.device)
-    d = conv_desc(N, (D, H, W), cin_p, pk.cout_p, pk.k, pk.stride, pk.pad, out_dims, out_c, out_fmt, out_scale, out_full, groups, out_off)
-    ws = _workspace(x_s.device, 0)
-    d.workspace, d.workspace_bytes = ws.data_ptr(), ws.numel()
-    from .engine import fold_width_ok
-    impl, weight = capi.CONV_TC, pk.w
-    if pk.w_fold is not None and fold_width_ok(pk.k[2], W) and out_c == 32 and out_fmt == capi.FMT_F32:
-        impl, weight = capi.CONV_TC_FOLD, pk.w_fold
-        d.Cout = pk.cout
-        if pk.scale_fold is not pk.scale:    # `scale` derives from pk.scale (conv_tc_kernel's steps): the lines kernel's gain instead
-            scale = scale * (pk.scale_fold / pk.scale.masked_fill(pk.scale == 0, 1.0))
-    capi.conv_nd(d, x_s, weight, scale, shift, None, out, impl)
-    return out, d
-
-
 def _grad_s32(grad_out, cp):
     """dL/dy -> (split-fp16 of S dL/dy, (N, D, H, W, C) float32 view, absmax bits, 1 / S on the device): S = 2^(9 - floor(log2 max|g|))."""
     g = _cl(grad_out)
@@ -405,14 +357,13 @@ def conv_kind(k, stride, padding):
 def conv_s2_dgrad(g_s, weight, stride, in_dims, inv, out=None):
     """dX (N, D, H, W, Cin) float32 of a 3-tap stride-2 pad-1 conv from the split-fp16 scaled output gradient g_s (1 / scale on the
     device in `inv`): ONE grouped launch (conv_s2_dgrad_filter) writing every input phase over its own extent; into `out` if given."""
-    from .engine import pack_filter
-    cout, cin = weight.shape[:2]
+    cin = weight.shape[1]
     srcs, k, pad, groups, ci, co = conv_s2_dgrad_filter(weight.shape, stride)
     wp = pad_s2_filter(weight.detach().float(), stride).contiguous()
-    pk = pack_filter([(wp, base, strides) for base, strides in srcs], k, (1, 1, 1), pad, ci, co, None, None, out_fmt=capi.FMT_F32)
-    out, _ = _launch(g_s, _round_up(cout, 32), pk, tuple(g_s.shape[1:4]), cin, pk.scale * inv, pk.shift, out_scale=groups,
-                     out_full=in_dims, groups=groups, out=out)
-    return out
+    pk = engine.pack_filter([(wp, base, strides) for base, strides in srcs], k, (1, 1, 1), pad, ci, co, None, None, out_fmt=capi.FMT_F32)
+    out = engine.Act(g_s.shape[0], *in_dims, cin, capi.FMT_F32, g_s.device) if out is None else engine.Act.view(out)
+    engine.launch_conv(engine.Act.view(g_s), pk, out, out_dims=g_s.shape[1:4], out_scale=groups, out_groups=groups, scale_mul=inv)
+    return out.data
 
 
 class ConvNdFn(torch.autograd.Function):
@@ -426,7 +377,6 @@ class ConvNdFn(torch.autograd.Function):
 
     @staticmethod
     def forward(ctx, x, weight, bias, stride, padding):
-        from .engine import pack_conv
         nd = weight.dim() - 2
         cout, cin = weight.shape[:2]
         k, st, pad = _as3(weight.shape[2:], 1), _as3(stride, 1), _as3(padding, 0)
@@ -439,16 +389,16 @@ class ConvNdFn(torch.autograd.Function):
             raise ValueError("native conv: 3-tap stride-2 convolutions need map sides of at least 2, got %s" % (in_dims,))
         cin_p = _round_up(cin, 32)
         x_s = _to_s32(x_cl, cin_p)
-        pk = pack_conv(_Filter(weight.detach(), None if bias is None else bias.detach(), stride, padding), None, cin_pad=cin_p,
-                       out_fmt=capi.FMT_F32)
-        out, _ = _launch(x_s, cin_p, pk, conv_out_dims(in_dims, k, st, pad), _round_up(cout, 4), pk.scale, pk.shift)
+        pk = engine.pack_conv(_Filter(weight.detach(), None if bias is None else bias.detach(), stride, padding), None, cin_pad=cin_p,
+                              out_fmt=capi.FMT_F32)
+        out = engine.Act(x.shape[0], *engine.conv_out_dims(in_dims, k, st, pad), _round_up(cout, 4), capi.FMT_F32, x.device)
+        engine.launch_conv(engine.Act.view(x_s), pk, out)
         ctx.save_for_backward(x, weight)
         ctx.geom = (k, st, pad, kind, in_dims)
-        return _from_cl(out, cout, nd)
+        return _from_cl(out.data, cout, nd)
 
     @staticmethod
     def backward(ctx, grad_out):
-        from .engine import pack_filter
         x, weight = ctx.saved_tensors
         k, st, pad, kind, in_dims = ctx.geom
         nd = weight.dim() - 2
@@ -456,7 +406,7 @@ class ConvNdFn(torch.autograd.Function):
         T = k[0] * k[1] * k[2]
         cout_p = _round_up(cout, 32)
         g_s, g, amax, inv = _grad_s32(grad_out, cout_p)
-        N, OD, OH, OW = g.shape[:4]
+        N = g.shape[0]
         gx = gw = gb = None
         if ctx.needs_input_grad[0]:
             w = weight.detach().float().contiguous()
@@ -464,13 +414,11 @@ class ConvNdFn(torch.autograd.Function):
                 out = conv_s2_dgrad(g_s, w, st, in_dims, inv)
             else:
                 (base, strides), kk, _, pd, ci, co = conv3d_dgrad_filter(weight.shape, pad)
-                pk = pack_filter((w, base, strides), kk, (1, 1, 1), pd, ci, co, None, None, out_fmt=capi.FMT_F32)
-                if kind == "same":
-                    out, _ = _launch(g_s, cout_p, pk, in_dims, _round_up(cin, 4), pk.scale * inv, pk.shift)
-                else:   # s2k1: dX is zero off the even phase
-                    out = torch.zeros((N,) + in_dims + (_round_up(cin, 4),), dtype=torch.float32, device=g.device)
-                    _launch(g_s, cout_p, pk, (OD, OH, OW), _round_up(cin, 4), pk.scale * inv, pk.shift, out_scale=st, out_full=in_dims,
-                            out=out)
+                pk = engine.pack_filter((w, base, strides), kk, (1, 1, 1), pd, ci, co, None, None, out_fmt=capi.FMT_F32)
+                # s2k1: dX is zero off the even phase
+                out = engine.Act(N, *in_dims, _round_up(cin, 4), capi.FMT_F32, g.device, zero=kind == "s2k1")
+                engine.launch_conv(engine.Act.view(g_s), pk, out, out_scale=st, scale_mul=inv)
+                out = out.data
             gx = _from_cl(out, cin, nd)
         if ctx.needs_input_grad[1]:
             x_s = _to_s32(_cl(x), _round_up(cin, 32))
@@ -490,7 +438,6 @@ class ConvTranspose3dFn(torch.autograd.Function):
 
     @staticmethod
     def forward(ctx, x, weight, bias):
-        from .engine import pack_deconv3d_k2s2
         cin, cout = weight.shape[:2]
         if tuple(weight.shape[2:]) != (2, 2, 2) or cout % 32 or cin % 32:
             raise ValueError("native ConvTranspose3d: kernel 2, stride 2 and channel counts that are multiples of 32 only, got %s"
@@ -498,17 +445,15 @@ class ConvTranspose3dFn(torch.autograd.Function):
         x_cl = _cl(x)
         N, D, H, W = x_cl.shape[:4]
         x_s = _to_s32(x_cl, cin)
-        pk = pack_deconv3d_k2s2(_Filter(weight.detach(), None if bias is None else bias.detach(), (2, 2, 2), (0, 0, 0)), None)
-        y_s, _ = _launch(x_s, cin, pk, (D, H, W), cout, pk.scale, pk.shift, out_fmt=capi.FMT_S32, out_scale=(2, 2, 2),
-                         out_full=(2 * D, 2 * H, 2 * W), groups=(2, 2, 2))
+        pk = engine.pack_deconv3d_k2s2(_Filter(weight.detach(), None if bias is None else bias.detach(), (2, 2, 2), (0, 0, 0)), None)
+        y = engine.deconv3d_k2s2(engine.Act.view(x_s), pk, capi.FMT_S32, relu=False)
         out = torch.empty((N, 2 * D, 2 * H, 2 * W, cout), dtype=torch.float32, device=x.device)
-        capi.s32_to_f32(y_s, out, out[..., 0].numel(), cout)
+        capi.s32_to_f32(y.data, out, y.pixels, cout)
         ctx.save_for_backward(x, weight)
         return out.permute(0, 4, 1, 2, 3)
 
     @staticmethod
     def backward(ctx, grad_out):
-        from .engine import pack_filter
         x, weight = ctx.saved_tensors
         cin, cout = weight.shape[:2]
         g_s, g, amax, inv = _grad_s32(grad_out, cout)
@@ -517,9 +462,10 @@ class ConvTranspose3dFn(torch.autograd.Function):
         if ctx.needs_input_grad[0]:
             w = weight.detach().float().contiguous()
             (base, strides), k, stride, pad, ci, co = conv_transpose3d_dgrad_filter(weight.shape)
-            pk = pack_filter((w, base, strides), k, stride, pad, ci, co, None, None, out_fmt=capi.FMT_F32)
-            out, _ = _launch(g_s, cout, pk, (D, H, W), cin, pk.scale * inv, pk.shift)
-            gx = out.permute(0, 4, 1, 2, 3)
+            pk = engine.pack_filter((w, base, strides), k, stride, pad, ci, co, None, None, out_fmt=capi.FMT_F32)
+            out = engine.Act(N, D, H, W, cin, capi.FMT_F32, g.device)
+            engine.launch_conv(engine.Act.view(g_s), pk, out, scale_mul=inv)
+            gx = out.data.permute(0, 4, 1, 2, 3)
         if ctx.needs_input_grad[1]:
             x_s = _to_s32(_cl(x), cin)
             gw = _wgrad(conv_transpose3d_desc(N, (D, H, W), cin, cout), x_s, g_s, amax, cin, cout, 1, groups=8)       # [1][ci][g cout + co], g = a 4 + b 2 + c
@@ -532,12 +478,11 @@ class ConvTranspose3dFn(torch.autograd.Function):
 def conv_transpose2d_k4s2_desc(N, dims, cin, cout, py, px):
     """Phase (py, px) of ConvTranspose2d(k=4, s=2, p=1) as the forward launches it (the engine's 2x2 stride-1 conv into the
     (py, px) sub-lattice of the 2H x 2W output), 3-D form with split-fp16 output gradient: lt_conv_wgrad_fwd's descriptor."""
-    from .engine import deconv2d_k4s2_phase
     _, H, W = dims
     cin_p, cout_p = _round_up(cin, 32), _round_up(cout, 32)
-    _, pad = deconv2d_k4s2_phase(py, px, cout)
-    return conv_desc(N, dims, cin_p, cout_p, (1, 2, 2), (1, 1, 1), pad, dims, cout_p, capi.FMT_S32, out_scale=(1, 2, 2),
-                     out_full=(1, 2 * H, 2 * W), out_off=(0, py, px))
+    _, pad = engine.deconv2d_k4s2_phase(py, px, cout)
+    return engine.conv_desc(N, dims, cin_p, cout_p, (1, 2, 2), (1, 1, 1), pad, dims, (1, 2 * H, 2 * W), cout_p, capi.FMT_S32, capi.FMT_S32,
+                            out_scale=(1, 2, 2), out_off=(0, py, px))
 
 
 def conv_transpose2d_k4s2_wgrad_scatter(gw, py, px):
@@ -555,24 +500,16 @@ class ConvTranspose2dK4Fn(torch.autograd.Function):
 
     @staticmethod
     def forward(ctx, x, weight, bias):
-        from .engine import pack_deconv2d_k4s2
         cin, cout = weight.shape[:2]
-        x_cl = _cl(x)
-        N, _, H, W = x_cl.shape[:4]
-        cin_p, c_store = _round_up(cin, 32), _round_up(cout, 4)
-        x_s = _to_s32(x_cl, cin_p)
-        phases = pack_deconv2d_k4s2(_Filter(weight.detach(), None if bias is None else bias.detach(), (2, 2), (1, 1)), None,
-                                    out_fmt=capi.FMT_F32)
-        out = torch.empty((N, 1, 2 * H, 2 * W, c_store), dtype=torch.float32, device=x.device)
-        for (py, px), pk in phases.items():
-            _launch(x_s, cin_p, pk, (1, H, W), c_store, pk.scale, pk.shift, out_scale=(1, 2, 2), out_full=(1, 2 * H, 2 * W),
-                    out_off=(0, py, px), out=out)
+        x_s = _to_s32(_cl(x), _round_up(cin, 32))
+        phases = engine.pack_deconv2d_k4s2(_Filter(weight.detach(), None if bias is None else bias.detach(), (2, 2), (1, 1)), None,
+                                           out_fmt=capi.FMT_F32)
+        out = engine.deconv2d_k4s2(engine.Act.view(x_s), phases, capi.FMT_F32, relu=False)
         ctx.save_for_backward(x, weight)
-        return _from_cl(out, cout, 2)
+        return _from_cl(out.data, cout, 2)
 
     @staticmethod
     def backward(ctx, grad_out):
-        from .engine import pack_filter
         x, weight = ctx.saved_tensors
         cin, cout = weight.shape[:2]
         N, _, H, W = x.shape
@@ -582,9 +519,10 @@ class ConvTranspose2dK4Fn(torch.autograd.Function):
         if ctx.needs_input_grad[0]:
             w = weight.detach().float().contiguous()
             (base, strides), k, stride, pad, ci, co = conv_transpose2d_k4s2_dgrad_filter(weight.shape)
-            pk = pack_filter((w, base, strides), k, stride, pad, ci, co, None, None, out_fmt=capi.FMT_F32)
-            out, _ = _launch(g_s, cout_p, pk, (1, H, W), _round_up(cin, 4), pk.scale * inv, pk.shift)
-            gx = _from_cl(out, cin, 2)
+            pk = engine.pack_filter((w, base, strides), k, stride, pad, ci, co, None, None, out_fmt=capi.FMT_F32)
+            out = engine.Act(N, 1, H, W, _round_up(cin, 4), capi.FMT_F32, g.device)
+            engine.launch_conv(engine.Act.view(g_s), pk, out, scale_mul=inv)
+            gx = _from_cl(out.data, cin, 2)
         if ctx.needs_input_grad[1]:
             x_s = _to_s32(_cl(x), _round_up(cin, 32))
             gw = torch.empty((cin, cout, 4, 4), dtype=torch.float32, device=g.device)
@@ -601,7 +539,8 @@ def stem_wgrad_desc(N, H, W, cout):
     """The stem's 4x4 stride-1 conv (front pad 2) over the (N, H/2, W/2, 32) space-to-depth input, 3-D form, as lt_conv_wgrad_fwd
     reads it."""
     dims = (1, H // 2, W // 2)
-    return conv_desc(N, dims, 32, _round_up(cout, 32), (1, 4, 4), (1, 1, 1), (0, 2, 2), dims, _round_up(cout, 32), capi.FMT_S32)
+    return engine.conv_desc(N, dims, 32, _round_up(cout, 32), (1, 4, 4), (1, 1, 1), (0, 2, 2), dims, dims, _round_up(cout, 32), capi.FMT_S32,
+                            capi.FMT_S32)
 
 
 def stem_wgrad_index(device):
@@ -623,7 +562,6 @@ class StemConvFn(torch.autograd.Function):
 
     @staticmethod
     def forward(ctx, images, weight, bias):
-        from .engine import pack_stem_s2d
         if not images.is_cuda:
             raise RuntimeError("lt_b200 native training convolutions need CUDA tensors (got %s)" % images.device)
         N, C, H, W = images.shape
@@ -631,10 +569,12 @@ class StemConvFn(torch.autograd.Function):
         img = images.detach().float().contiguous()
         x_s = torch.empty((N, 1, H // 2, W // 2, 64), dtype=torch.float16, device=images.device)
         capi.stem_s2d(img, x_s, N, C, H, W)
-        pk = pack_stem_s2d(_Filter(weight.detach(), None if bias is None else bias.detach(), (2, 2), (3, 3)), None, out_fmt=capi.FMT_F32)
-        out, _ = _launch(x_s, 32, pk, (1, H // 2, W // 2), _round_up(cout, 4), pk.scale, pk.shift)
+        pk = engine.pack_stem_s2d(_Filter(weight.detach(), None if bias is None else bias.detach(), (2, 2), (3, 3)), None,
+                                  out_fmt=capi.FMT_F32)
+        out = engine.Act(N, 1, H // 2, W // 2, _round_up(cout, 4), capi.FMT_F32, images.device)
+        engine.launch_conv(engine.Act.view(x_s), pk, out, out_dims=(1, H // 2, W // 2))
         ctx.save_for_backward(img, weight)
-        return _from_cl(out, cout, 2)
+        return _from_cl(out.data, cout, 2)
 
     @staticmethod
     def backward(ctx, grad_out):

@@ -14,7 +14,6 @@ In the tensor-core modes every conv runs on the tensor cores: the 3-channel 7x7 
 4x4 stride-1 conv over the 2x2 space-to-depth image, the stride-2 convs through TMA traversal strides.
 """
 import math
-import os
 
 import torch
 from torch import nn
@@ -47,6 +46,16 @@ class Act:
             assert C % 32 == 0
             self.data = alloc((N, D, H, W, 2 * C), dtype=torch.float16, device=device)
 
+    @classmethod
+    def view(cls, data):
+        """An existing channels-last tensor as an Act, without copying: float32 [N,D,H,W,C] or float16 [N,D,H,W,2C] (split-fp16)."""
+        a = cls.__new__(cls)
+        a.N, a.D, a.H, a.W, c = data.shape
+        a.fmt = FMT_F32 if data.dtype == torch.float32 else FMT_S32
+        a.C = c if a.fmt == FMT_F32 else c // 2
+        a.data, a.stats = data, None
+        return a
+
     @property
     def pixels(self):
         return self.N * self.D * self.H * self.W
@@ -73,6 +82,7 @@ class _Timed:
         if self.tl is not None:
             self.e0, self.e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
             self.e0.record()
+        return self
 
     def __exit__(self, *exc):
         if self.tl is not None:
@@ -250,7 +260,91 @@ def pack_deconv2d_k4s2(deconv, bn, mode="tc", **kw):
     return phases
 
 
+def conv_out_dims(dims, k, stride, pad):
+    return tuple((n + 2 * p - kk) // s + 1 for n, kk, s, p in zip(dims, k, stride, pad))
+
+
+def conv_desc(N, in_dims, cin, cout, k, stride, pad, out_dims, out_full, out_c, in_fmt, out_fmt, out_scale=(1, 1, 1), out_off=(0, 0, 0),
+              out_groups=(1, 1, 1), relu=False, res_mode=RES_NONE):
+    """lt_conv_desc of one launch over an (N, in_dims, cin) input: out_dims is the grid the launch computes, out_full and out_c the
+    output tensor's (D, H, W) and channel count.  No workspace: launch_conv attaches the split-K scratch."""
+    return capi.ConvDesc(N=N, ID=in_dims[0], IH=in_dims[1], IW=in_dims[2], Cin=cin, OD=out_dims[0], OH=out_dims[1], OW=out_dims[2],
+                         Cout=cout, KD=k[0], KH=k[1], KW=k[2], sd=stride[0], sh=stride[1], sw=stride[2], pd=pad[0], ph=pad[1], pw=pad[2],
+                         FD=out_full[0], FH=out_full[1], FW=out_full[2], FC=out_c, osd=out_scale[0], osh=out_scale[1], osw=out_scale[2],
+                         ood=out_off[0], ooh=out_off[1], oow=out_off[2], relu=int(relu), residual=res_mode, in_format=in_fmt,
+                         out_format=out_fmt, ogd=out_groups[0], ogh=out_groups[1], ogw=out_groups[2])
+
+
+SPLITK_WS_BYTES = 32 << 20
+_SPLITK_WS = {}
+
+
+def splitk_workspace(device):
+    """The split-K scratch of every lt_conv_nd_fwd launch on `device` (inference and training): one fixed buffer, so a layer's split
+    count, and with it the rounding of its result, depends on its shape only.  Launches on one stream are ordered; the engine's eager
+    warm-up forward allocates it before any CUDA-graph capture."""
+    ws = _SPLITK_WS.get(device)
+    if ws is None:
+        ws = _SPLITK_WS[device] = torch.empty(SPLITK_WS_BYTES, dtype=torch.uint8, device=device)
+    return ws
+
+
+def launch_conv(x, pk, out, relu=False, residual=None, res_mode=RES_NONE, out_dims=None, out_scale=(1, 1, 1), out_off=(0, 0, 0),
+                out_groups=(1, 1, 1), scale_mul=None, workspace=None):
+    """One lt_conv_nd_fwd of packed filter `pk` over Act x into Act out (and residual) -> the impl launched.  out_dims: the grid the
+    launch computes (default: the conv's own output), written at out_scale / out_off / out_groups of `out`.  A fold-packed layer runs on
+    LT_CONV_TC_FOLD, with the fold filter, its real Cout and scale_fold, when the kernel takes its width and `out` is its own 32-channel
+    grid.  scale_mul: device tensor the scale is multiplied by (1 / S of a scaled output gradient).  workspace: split-K scratch
+    (default splitk_workspace; an empty tensor forces single-pass launches)."""
+    assert x.fmt == pk.in_fmt and x.C == pk.cin, (x.fmt, pk.in_fmt, x.C, pk.cin)
+    if residual is not None:
+        assert residual.fmt == out.fmt and residual.C == out.C
+    in_dims = (x.D, x.H, x.W)
+    out_dims = conv_out_dims(in_dims, pk.k, pk.stride, pk.pad) if out_dims is None else tuple(out_dims)
+    d = conv_desc(x.N, in_dims, x.C, pk.cout_p, pk.k, pk.stride, pk.pad, out_dims, (out.D, out.H, out.W), out.C, x.fmt, out.fmt,
+                  out_scale, out_off, out_groups, relu, res_mode)
+    ws = splitk_workspace(x.data.device) if workspace is None else workspace
+    d.workspace, d.workspace_bytes = ws.data_ptr(), ws.numel()
+    impl, weight, scale = pk.impl, pk.w, pk.scale
+    if (pk.w_fold is not None and fold_width_ok(pk.k[2], x.W) and out.C == 32 and tuple(out_scale) == (1, 1, 1)
+            and out_dims == in_dims):
+        impl, weight, scale = CONV_TC_FOLD, pk.w_fold, pk.scale_fold
+        d.Cout = pk.cout
+    if scale_mul is not None:
+        scale = scale * scale_mul
+    capi.conv_nd(d, x.data, weight, scale, pk.shift, None if residual is None else residual.data, out.data, impl)
+    return impl
+
+
+def deconv2d_k4s2(x, phases, out_fmt, relu, conv=launch_conv):
+    """ConvTranspose2d(k=4, s=2, p=1) of x from its phase packs (pack_deconv2d_k4s2): each phase a 2x2 stride-1 conv into its (py, px)
+    sub-lattice of one (N, 1, 2H, 2W) output.  conv: the launch, with launch_conv's arguments."""
+    c = next(iter(phases.values())).cout
+    out = Act(x.N, 1, 2 * x.H, 2 * x.W, _round_up(c, 4 if out_fmt == FMT_F32 else 32), out_fmt, x.data.device)
+    for (py, px), pk in phases.items():
+        conv(x, pk, out=out, relu=relu, out_scale=(1, 2, 2), out_off=(0, py, px), out_dims=(1, x.H, x.W))
+    return out
+
+
+def deconv3d_k2s2(x, pk, out_fmt, relu, residual=None, conv=launch_conv):
+    """ConvTranspose3d(k=2, s=2) of x as the one grouped 1x1x1 GEMM of pack_deconv3d_k2s2 (N = 8 Cout, column block g = a 4 + b 2 + c
+    written to output phase (a, b, c) of one (N, 2D, 2H, 2W) output); `residual` is added after the ReLU."""
+    out = Act(x.N, 2 * x.D, 2 * x.H, 2 * x.W, pk.cout // 8, out_fmt, x.data.device)
+    conv(x, pk, out=out, relu=relu, residual=residual, res_mode=RES_NONE if residual is None else RES_AFTER_RELU, out_scale=(2, 2, 2),
+         out_dims=(x.D, x.H, x.W), out_groups=(2, 2, 2))
+    return out
+
+
+def pixel_grid(B, h, w, device):
+    """(B, h*w, 3) float32 coordinates (x, y, 0) of the pixels of an h x w map: the 2-D soft-argmax runs on the 3-D kernels."""
+    ys, xs = torch.meshgrid(torch.arange(h, device=device, dtype=torch.float32), torch.arange(w, device=device, dtype=torch.float32),
+                            indexing="ij")
+    return torch.stack([xs, ys, torch.zeros_like(xs)], dim=-1).reshape(1, h * w, 3).expand(B, h * w, 3).contiguous()
+
+
 class NativeEngine:
+    _splitk_ws = None              # split-K scratch of the convs: None = splitk_workspace; an empty tensor forces single-pass launches
+
     def __init__(self, model, mode="tc", use_graph=True):
         assert mode in ("simt", "tc", "tc1")
         self.model = model
@@ -370,57 +464,25 @@ class NativeEngine:
 
     def _conv(self, x, pk, relu, residual=None, res_mode=RES_NONE, out=None, out_scale=(1, 1, 1), out_off=(0, 0, 0),
               out_dims=None, out_fmt=None, out_c=None, out_groups=(1, 1, 1)):
-        """Launch one conv. `out` (with out_scale/out_off) lets transposed-conv phases share an output tensor.
+        """Launch one conv (launch_conv). `out` (with out_scale/out_off) lets transposed-conv phases share an output tensor.
 
         out_c: channel stride of a float32 output narrower than the padded N tile (the TMA store clips the padding)."""
         if pk.impl == CONV_SIMT:
             x = self._as_f32(x)
-        assert x.fmt == pk.in_fmt and x.C == pk.cin, (x.fmt, pk.in_fmt, x.C, pk.cin)
-        kd, kh, kw = pk.k
-        sd, sh, sw = pk.stride
-        pd, ph, pw = pk.pad
-        if out_dims is None:
-            od = (x.D + 2 * pd - kd) // sd + 1
-            oh = (x.H + 2 * ph - kh) // sh + 1
-            ow = (x.W + 2 * pw - kw) // sw + 1
-        else:
-            od, oh, ow = out_dims
+        od, oh, ow = conv_out_dims((x.D, x.H, x.W), pk.k, pk.stride, pk.pad) if out_dims is None else out_dims
         if out is None:
             fmt = self.act_fmt if out_fmt is None else out_fmt
             c = _round_up(pk.cout, 32) if fmt == FMT_S32 else pk.cout_p
             if out_c is not None and fmt == FMT_F32 and pk.cout <= out_c <= pk.cout_p:
                 c = out_c
             out = Act(x.N, od, oh, ow, c, fmt, x.data.device)
-        d = capi.ConvDesc(N=x.N, ID=x.D, IH=x.H, IW=x.W, Cin=x.C, OD=od, OH=oh, OW=ow, Cout=pk.cout_p,
-                          KD=kd, KH=kh, KW=kw, sd=sd, sh=sh, sw=sw, pd=pd, ph=ph, pw=pw,
-                          FD=out.D, FH=out.H, FW=out.W, FC=out.C,
-                          osd=out_scale[0], osh=out_scale[1], osw=out_scale[2], ood=out_off[0], ooh=out_off[1], oow=out_off[2],
-                          relu=int(relu), residual=res_mode, in_format=x.fmt, out_format=out.fmt,
-                          ogd=out_groups[0], ogh=out_groups[1], ogw=out_groups[2])
-        if residual is not None:
-            assert residual.fmt == out.fmt and residual.C == out.C
-        ws = self._splitk_workspace(x.data.device)
-        d.workspace, d.workspace_bytes = ws.data_ptr(), ws.numel()
-        impl, weight, scale = pk.impl, pk.w, pk.scale
-        if (pk.w_fold is not None and fold_width_ok(kw, x.W) and out.C == 32 and out_scale == (1, 1, 1)
-                and (od, oh, ow) == (x.D, x.H, x.W)):
-            impl, weight, scale = CONV_TC_FOLD, pk.w_fold, pk.scale_fold
-            d.Cout = pk.cout
-        label = {CONV_TC_FOLD: "conv_fold", CONV_SIMT: "conv_ffma"}.get(impl, "conv_tc")
-        with self._timed(label, flops=2.0 * x.N * od * oh * ow * pk.kmacs,
-                         desc="N%d %dx%dx%d Cin%d Cout%d k%d%d%d s%d" % (x.N, od, oh, ow, pk.cin, pk.cout, kd, kh, kw, sw)):
-            capi.conv_nd(d, x.data, weight, scale, pk.shift, None if residual is None else residual.data, out.data, impl)
+        kd, kh, kw = pk.k
+        with self._timed("conv_tc", flops=2.0 * x.N * od * oh * ow * pk.kmacs,
+                         desc="N%d %dx%dx%d Cin%d Cout%d k%d%d%d s%d" % (x.N, od, oh, ow, pk.cin, pk.cout, kd, kh, kw, pk.stride[2])) as t:
+            impl = launch_conv(x, pk, out, relu, residual, res_mode, (od, oh, ow), out_scale, out_off, out_groups, workspace=self._splitk_ws)
+            t.label = {CONV_TC_FOLD: "conv_fold", CONV_SIMT: "conv_ffma"}.get(impl, "conv_tc")
         self.launches += 1
         return out
-
-    def _splitk_workspace(self, device):
-        """Scratch for the split-K path of lt_conv_nd_fwd (deep V2V levels: 1-32 M tiles); one buffer shared by all layers
-        (launches on one stream are ordered).  Allocated before any CUDA-graph capture by the eager warm-up forward."""
-        ws = getattr(self, "_splitk_ws", None)
-        if ws is None or ws.device != device:
-            ws = torch.empty(int(os.environ.get("LT_SPLITK_WS_MB", "32")) << 20, dtype=torch.uint8, device=device)
-            self._splitk_ws = ws
-        return ws
 
     def _timed(self, label, flops=0.0, nbytes=0.0, desc=""):
         return _Timed(self.timeline, label, flops, nbytes, desc)
@@ -435,17 +497,11 @@ class NativeEngine:
         return y
 
     def _deconv2d(self, x, phases):
-        c = next(iter(phases.values())).cout
-        out = Act(x.N, 1, 2 * x.H, 2 * x.W, c, self.act_fmt, x.data.device)
-        for (py, px), pk in phases.items():
-            self._conv(x, pk, relu=True, out=out, out_scale=(1, 2, 2), out_off=(0, py, px), out_dims=(1, x.H, x.W))
-        return out
+        return deconv2d_k4s2(x, phases, self.act_fmt, relu=True, conv=self._conv)
 
     def _deconv3d(self, x, phases, skip):
         if isinstance(phases, ConvPack):      # merged: one GEMM, eight output groups
-            out = Act(x.N, 2 * x.D, 2 * x.H, 2 * x.W, phases.cout // 8, self.act_fmt, x.data.device)
-            return self._conv(x, phases, relu=True, residual=skip, res_mode=RES_AFTER_RELU, out=out, out_scale=(2, 2, 2),
-                              out_dims=(x.D, x.H, x.W), out_groups=(2, 2, 2))
+            return deconv3d_k2s2(x, phases, self.act_fmt, relu=True, residual=skip, conv=self._conv)
         c = next(iter(phases.values())).cout
         out = Act(x.N, 2 * x.D, 2 * x.H, 2 * x.W, c, self.act_fmt, x.data.device)
         for (a, b, cc), pk in phases.items():
@@ -818,9 +874,7 @@ class NativeEngine:
         # 2-D soft-argmax (op.py:11-47) = the 3-D kernels with pixel-index coordinates (x, y, 0)
         key = ("grid2d", h, w, B * V)
         if getattr(self, "_grid_key", None) != key:
-            ys, xs = torch.meshgrid(torch.arange(h, device=dev, dtype=torch.float32), torch.arange(w, device=dev, dtype=torch.float32), indexing="ij")
-            g = torch.stack([xs, ys, torch.zeros_like(xs)], dim=-1).reshape(1, h * w, 3)
-            self._grid2d, self._grid_key = g.expand(B * V, h * w, 3).contiguous(), key
+            self._grid2d, self._grid_key = pixel_grid(B * V, h, w, dev), key
         heat = torch.empty((B * V, J, h, w), dtype=torch.float32, device=dev)
         kp = torch.empty((B * V, J, 3), dtype=torch.float32, device=dev)
         ws = torch.empty(capi.softargmax3d_workspace_bytes(B * V, J, h * w) // 4 + 1, dtype=torch.float32, device=dev)

@@ -11,7 +11,7 @@ import os
 
 import torch
 
-from . import autograd_ops, capi, torch_ops
+from . import autograd_ops, capi, engine, torch_ops
 
 _AGGS = ("sum", "max", "softmax", "conf", "conf_norm")
 
@@ -85,7 +85,7 @@ def integrate_tensor_2d(heatmaps, softmax=True, backend=None):
         return autograd_ops.integrate_tensor_2d(heatmaps, softmax)
     B, J, h, w = heatmaps.shape
     dev = heatmaps.device
-    grid = autograd_ops.pixel_grid(B, h, w, dev)
+    grid = engine.pixel_grid(B, h, w, dev)
     logits = heatmaps.float().contiguous()
     out = torch.empty_like(logits)
     kp = torch.empty((B, J, 3), dtype=torch.float32, device=dev)

@@ -22,7 +22,7 @@ import torch.nn.functional as F
 from lt_b200 import capi, engine as eng_mod
 
 SMS = 132
-WS_BYTES = 32 << 20            # NativeEngine._splitk_workspace default
+WS_BYTES = 32 << 20            # engine.SPLITK_WS_BYTES: the split-K scratch of every conv launch
 RES_NONE, RES_BEFORE, RES_AFTER = capi.RES_NONE, capi.RES_BEFORE_RELU, capi.RES_AFTER_RELU
 F32, S32 = capi.FMT_F32, capi.FMT_S32
 ACCUM_RATE = 0.28              # lt_fold_bn_fwd: scale x (1 + ACCUM_RATE x steps x 2^-24)

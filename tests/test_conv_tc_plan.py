@@ -4,7 +4,7 @@ import pytest
 from lt_b200 import capi
 
 SMS = 132
-WS = 32 << 20           # engine default split-K workspace (LT_SPLITK_WS_MB)
+WS = 32 << 20           # engine.SPLITK_WS_BYTES: the split-K scratch of every conv launch
 
 # (N, out D, H, W, Cin, Cout, kernel, stride, splits expected at 132 SMs)
 CONFIG2 = [

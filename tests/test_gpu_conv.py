@@ -151,7 +151,7 @@ Part = namedtuple("Part", "impl L cin desc_cout folded_steps phase ws")
 
 
 def case_launches(c):
-    """The lt_conv_nd_fwd launches of a case, host-only: as the engine would issue them (engine._conv, _deconv2d, _deconv3d)."""
+    """The lt_conv_nd_fwd launches of a case, host-only: as the engine would issue them (engine.launch_conv, deconv2d_k4s2, deconv3d_k2s2)."""
     tc = c.mode != "simt"
     impl0 = {"tc": TC, "tc1": TC1, "simt": SIMT}[c.mode]
     ws = WS_BYTES if c.ws else 0
