@@ -300,6 +300,18 @@ int lt_v2v_tail_stats_fwd(const void* x, const void* w1, const void* w2, const v
  * which is divided out exactly.  wgmma with four-term products (fp32-grade).  Deterministic: the K split over positions writes
  * fp32 partial tiles into `workspace` (lt_conv_wgrad_workspace_bytes(desc) bytes) that a second pass sums in a fixed order. */
 size_t lt_conv_wgrad_workspace_bytes(const lt_conv_desc* desc);
+/* Work decomposition of one lt_conv_wgrad_fwd launch on a GPU with `sm_count` SMs, computed on the host without touching the
+ * device.  The grid is taps x desc->Cin / 32 x ngroups x splits CTAs of nwg consumer warpgroups, one per 32-channel output block
+ * (conv_wgrad_kernel<1 / 2 / 4>; the last group may have fewer active ones); each CTA runs its share of the m_tiles M tiles of 128
+ * output positions (split z takes tiles [z m_tiles / splits, (z + 1) m_tiles / splits)) through a TMA ring of `stages` tiles. */
+typedef struct lt_conv_wgrad_launch_plan {
+  int nwg;                   /* warpgroups per CTA: 1, 2 or 4 */
+  int ngroups;               /* CTAs along the output channels: ceil(Cout / 32 / nwg) */
+  int m_tiles;               /* M tiles of 128 output positions (the K of the GEMM) */
+  int splits;                /* K split count, 1 = none */
+  int stages;                /* TMA ring depth in M tiles */
+} lt_conv_wgrad_launch_plan;
+int lt_conv_wgrad_plan(const lt_conv_desc* desc, int sm_count, lt_conv_wgrad_launch_plan* plan);
 int lt_conv_wgrad_fwd(const lt_conv_desc* desc, const void* in, const void* grad_out, const unsigned int* grad_absmax_bits, int Cin,
                       int Cout, float* grad_w, void* workspace, size_t workspace_bytes, void* stream);
 

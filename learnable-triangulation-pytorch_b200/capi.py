@@ -41,6 +41,11 @@ class ConvTcPlan(ctypes.Structure):
     _fields_ = [(n, c_int) for n in ("nt", "m_tiles", "n_tiles", "chunks", "splits", "grid")]
 
 
+class ConvWgradPlan(ctypes.Structure):
+    """Mirror of `struct lt_conv_wgrad_launch_plan` (include/lt_b200.h)."""
+    _fields_ = [(n, c_int) for n in ("nwg", "ngroups", "m_tiles", "splits", "stages")]
+
+
 class Options(ctypes.Structure):
     """Mirror of `struct lt_options` (include/lt_b200.h): kernel-selection switches, all defaulting to the measured-best path."""
     _fields_ = [(n, c_int) for n in ("tc_persist", "tc_splitk", "tc_bres", "tc_direct_epilogue", "fold_fast_issue", "fold_debug",
@@ -85,6 +90,7 @@ SIGNATURES = {
     "lt_softargmax3d_finish_fwd": (c_int, [c_void_p, c_long, c_long, c_void_p, c_void_p, c_void_p, c_void_p, c_size_t, c_int, c_int, c_long, c_int,
                                            c_float, c_int, c_void_p]),
     "lt_conv_wgrad_workspace_bytes": (c_size_t, [ctypes.POINTER(ConvDesc)]),
+    "lt_conv_wgrad_plan": (c_int, [ctypes.POINTER(ConvDesc), c_int, ctypes.POINTER(ConvWgradPlan)]),
     "lt_conv_wgrad_fwd": (c_int, [ctypes.POINTER(ConvDesc)] + [c_void_p] * 3 + [c_int, c_int, c_void_p, c_void_p, c_size_t, c_void_p]),
     "lt_test_conv_wgrad_host": (c_int, [ctypes.POINTER(ConvDesc), c_void_p, c_void_p, c_int, c_int, c_void_p]),
     "lt_f32_to_s32_scaled": (c_int, [c_void_p, c_void_p, c_long, c_int, c_int, c_void_p, c_void_p, c_void_p]),
@@ -462,6 +468,13 @@ def f32_to_s32_scaled(inp, out, pixels, C, CP, absmax_bits=None, inv_scale=None)
 
 def conv_wgrad_workspace_bytes(desc):
     return lib().lt_conv_wgrad_workspace_bytes(ctypes.byref(desc))
+
+
+def conv_wgrad_plan(desc, sm_count):
+    """Host-only work decomposition of an lt_conv_wgrad_fwd launch (lt_conv_wgrad_plan): dict of nwg, ngroups, m_tiles, splits, stages."""
+    plan = ConvWgradPlan()
+    _check(lib().lt_conv_wgrad_plan(ctypes.byref(desc), sm_count, ctypes.byref(plan)), "lt_conv_wgrad_plan")
+    return {name: getattr(plan, name) for name, _ in ConvWgradPlan._fields_}
 
 
 def conv_wgrad(desc, inp, grad_out, grad_absmax_bits, cin, cout, grad_w, workspace):

@@ -48,13 +48,16 @@ static inline int ceil_div(long a, long b) { return (int)((a + b - 1) / b); }
 // one).  Price: for |x| < ~0.125 the low part is an fp16 subnormal, i.e. the representation error is
 // max(2^-22 |x|, 2^-25) absolute -- 3e-8, far below the 1e-3 contract for BatchNorm-scaled activations and Kaiming-scaled
 // weights (CPU emulation on the calibrated test model: per-layer relative error 1.9e-7..9.0e-7;
-// checked on the GPU by tests/test_gpu_tc.py / test_gpu_forward.py).  |x| is saturated at the fp16 maximum (65504).
+// checked on the GPU by tests/test_gpu_tc.py / test_gpu_forward.py).  Finite |x| is saturated at the fp16 maximum (65504).
+// Non-finite values stay non-finite, so a diverging training run shows NaN instead of running on finite garbage: NaN gives NaN
+// halves, +-Inf gives hi = +-Inf and lo = NaN (Inf - Inf); the in-kernel split_s32x2 (cvt.rn.satfinite) keeps NaN as NaN
+// (tests/test_conv_bwd_cpu.py pins the rule, tests/test_gpu_conv_bwd.py checks it end to end).
 typedef __half sh_t;
 constexpr float kLoScale = 1.0f;   // kept as named constants: the two-accumulator kernels (conv_tc.cu, conv_tc_fold.cu) form D1 + kLoInv * D2
 constexpr float kLoInv = 1.0f;
 
 __device__ __forceinline__ void split_s32(float x, sh_t& hi, sh_t& lo) {
-  x = fminf(fmaxf(x, -65504.0f), 65504.0f);
+  if (fabsf(x) <= 3.402823466e+38f) x = fminf(fmaxf(x, -65504.0f), 65504.0f);   // finite only: fmaxf would turn NaN into -65504
   hi = __float2half_rn(x);
   lo = __float2half_rn((x - __half2float(hi)) * kLoScale);
 }
@@ -97,12 +100,16 @@ __device__ __forceinline__ float4 load_s32x4(const sh_t* row, int c) {
 constexpr double kAccumTruncRate = 0.28;
 __host__ __device__ inline double accum_gain(double steps) { return 1.0 + kAccumTruncRate * steps * 5.9604644775390625e-08; }   // 2^-24
 
+// The same scale serves the output gradients of training (lt_f32_to_s32_scaled): there max|v| may lie anywhere in float32's range,
+// so the exponent 9 - e is clamped to [-126, 126], where S and 1 / S are exact normal floats (an all-zero tensor gets S = 1).
+// Filters never come near the clamp.
 __device__ __forceinline__ float weight_pow2_scale(const unsigned* absmax_bits) {
   if (!absmax_bits) return 1.0f;
   const unsigned b = *absmax_bits;
-  const int e = (int)(b >> 23) - 127;     // floor(log2(max)) for normal floats
-  if (b == 0u || e < -100 || e > 100) return 1.0f;
-  return exp2f((float)(9 - e));
+  if (b == 0u) return 1.0f;
+  const int e = (int)(b >> 23) - 127;     // floor(log2(max)) for normal floats (-127 for subnormals)
+  const int s = min(max(9 - e, -126), 126);
+  return __int_as_float((s + 127) << 23);
 }
 
 __device__ __forceinline__ float warp_sum(float v) {

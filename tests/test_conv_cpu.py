@@ -30,10 +30,13 @@ ACCUM_RATE = 0.28              # lt_fold_bn_fwd: scale x (1 + ACCUM_RATE x steps
 
 # ------------------------------------------------------------------------------------------ split-fp16 and packed layouts
 def split_np(x):
-    """float32 -> (hi, lo) float16 as split_s32 (common.cuh): clamp to +-65504, hi = fp16_rn(x), lo = fp16_rn(x - hi)."""
-    x = np.clip(np.asarray(x, dtype=np.float32), np.float32(-65504.0), np.float32(65504.0))
-    hi = x.astype(np.float16)
-    lo = (x - hi.astype(np.float32)).astype(np.float16)
+    """float32 -> (hi, lo) float16 as split_s32 (common.cuh): clamp finite values to +-65504, hi = fp16_rn(x), lo = fp16_rn(x - hi).
+    NaN stays NaN in both halves, +-Inf gives hi = +-Inf and lo = NaN."""
+    x = np.asarray(x, dtype=np.float32)
+    x = np.where(np.isfinite(x), np.clip(x, np.float32(-65504.0), np.float32(65504.0)), x)
+    with np.errstate(invalid="ignore"):
+        hi = x.astype(np.float16)
+        lo = (x - hi.astype(np.float32)).astype(np.float16)
     return hi, lo
 
 
