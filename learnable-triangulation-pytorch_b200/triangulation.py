@@ -17,6 +17,7 @@ import torch
 from torch import nn
 
 from . import autograd_ops, layers, multiview, op, pose_resnet, torch_ops, volumetric
+from .train_graph import TrainGraphs
 from .v2v import V2VModel
 
 
@@ -79,14 +80,39 @@ def _hooks(backbone_backend, norm_backend, v2v_backend="torch"):
             autograd_ops.batch_norm if norm_backend == "native" else layers.torch_norm)
 
 
+def _upload(device, *arrays):
+    """float32 tensors on `device` of host arrays (float64 cast last): on CUDA through one page-locked buffer and one asynchronous
+    copy, so the host part of a forward does not wait for the device."""
+    flat = [torch.from_numpy(np.ascontiguousarray(a)).float().reshape(-1) for a in arrays]
+    host = torch.cat(flat)
+    if device.type == "cuda":
+        host = host.pin_memory().to(device, non_blocking=True)
+    return tuple(t.view(a.shape) for t, a in zip(host.split([f.numel() for f in flat]), arrays))
+
+
+def _check_train_graph(train_graph, backend):
+    if train_graph and backend != "hybrid":
+        raise ValueError("train_graph=True needs backend='hybrid' (got %r)" % (backend,))
+
+
 class _EngineOwner(nn.Module):
-    """Keeps the native engine's packed filters / CUDA graphs in step with the module's tensors: `.to()/.cuda()/.float()`
-    (`_apply`) and `load_state_dict` invalidate them explicitly (tensor versions alone miss `p.data` updates)."""
+    """Keeps the native engine's packed filters / CUDA graphs and the training graphs (train_graph.TrainGraphs) in step with the
+    module's tensors: `.to()/.cuda()/.float()` (`_apply`) and `load_state_dict` invalidate them explicitly (tensor versions alone
+    miss `p.data` updates)."""
 
     def _invalidate_engine(self):
         eng = self.__dict__.get("_engine")
         if eng is not None:
             eng.invalidate()
+        graphs = self.__dict__.get("_train_graphs")
+        if graphs is not None:
+            graphs.invalidate()
+
+    def _run_device(self, fn, inputs):
+        """fn(*inputs): the device part of the forward, replayed from CUDA graphs with train_graph=True in a training forward."""
+        if self._train_graphs is not None and self.training and torch.is_grad_enabled():
+            return self._train_graphs.run(self, fn, inputs, self.clone_outputs)
+        return fn(*inputs)
 
     def _apply(self, fn, *args, **kwargs):
         out = super()._apply(fn, *args, **kwargs)
@@ -101,7 +127,7 @@ class _EngineOwner(nn.Module):
 
 class VolumetricTriangulationNet(_EngineOwner):
     def __init__(self, config, device="cuda:0", backend=None, conv_mode=None, use_cuda_graph=True, v2v_backend="torch",
-                 backbone_backend="torch", norm_backend="torch"):
+                 backbone_backend="torch", norm_backend="torch", train_graph=False):
         super().__init__()
         m = config.model
         self.num_joints = m.backbone.num_joints
@@ -131,12 +157,14 @@ class VolumetricTriangulationNet(_EngineOwner):
         self.backend = backend or os.environ.get("LT_B200_BACKEND", "native")
         self.conv_mode = conv_mode or os.environ.get("LT_B200_CONV", "tc")
         _check_backends(self.backend, self.conv_mode, backbone_backend, norm_backend, v2v_backend)
+        _check_train_graph(train_graph, self.backend)
         self.v2v_backend = v2v_backend
         self.backbone_backend = backbone_backend
         self.norm_backend = norm_backend
         self.use_cuda_graph = use_cuda_graph
         self.clone_outputs = True
         self._engine = None
+        self._train_graphs = TrainGraphs() if train_graph else None
 
     # ---------------------------------------------------------------- host-side geometry
     def _host_geometry(self, batch, batch_size, image_shape, heatmap_shape):
@@ -197,25 +225,37 @@ class VolumetricTriangulationNet(_EngineOwner):
         return kp, features, volumes, vol_conf, cuboids, coord, base_points
 
     def _forward_torch(self, images, batch):
+        """backend "torch" / "hybrid": the host part (geometry with the heat-map size of backbone_map_size, its upload), then
+        _device_forward, from CUDA graphs with train_graph=True."""
+        if self.backend == "hybrid" and not images.is_cuda:
+            raise RuntimeError("lt_b200 hybrid backend needs CUDA tensors (native custom ops); use backend='torch' on CPU")
+        B = images.shape[0]
+        H, W = images.shape[3:]
+        hm_shape = (backbone_map_size(H), backbone_map_size(W))
+        proj, base, position, step, rots, cuboids = self._host_geometry(batch, B, (H, W), hm_shape)
+        geometry = _upload(images.device, proj, position, base, step, rots)
+        kp, features, volumes, vol_conf, coord = self._run_device(self._device_forward, (images,) + geometry)
+        return kp, features, volumes, vol_conf, cuboids, coord, geometry[2]
+
+    def _device_forward(self, images, proj_t, pos_t, cen_t, step_t, rot_t):
+        """Everything the torch / hybrid forward runs on the device: (images, projections (B, V, 3, 4), cuboid position (B, 3), base
+        point (B, 3), voxel step (3,), rotations (B, 3, 3)) -> (kp, features, volumes, vol_conf, coord)."""
         dev = images.device
         B, V = images.shape[:2]
         flat = images.reshape(-1, *images.shape[2:])
         conv, v2v_conv, norm = _hooks(self.backbone_backend, self.norm_backend, self.v2v_backend)
         heatmaps, features, _, vol_conf = self.backbone(flat, conv, norm)
+        hm_shape = (backbone_map_size(images.shape[3]), backbone_map_size(images.shape[4]))
+        if tuple(heatmaps.shape[2:]) != hm_shape:
+            raise RuntimeError("heat-map size %s differs from the size %s used for the projection matrices"
+                               % (tuple(heatmaps.shape[2:]), hm_shape))
         if vol_conf is not None:
             vol_conf = vol_conf.view(B, V, *vol_conf.shape[1:])
             if self.volume_aggregation_method == "conf_norm":
                 vol_conf = vol_conf / vol_conf.sum(dim=1, keepdim=True)
-        image_shape, hm_shape = tuple(images.shape[3:]), tuple(heatmaps.shape[2:])
-        proj, base, position, step, rots, cuboids = self._host_geometry(batch, B, image_shape, hm_shape)
-        proj_t = torch.from_numpy(proj).to(dev)
         n = self.volume_size
         idx = torch.arange(n, device=dev, dtype=torch.float)
         grid = torch.stack(torch.meshgrid(idx, idx, idx, indexing="ij"), dim=-1)              # (n, n, n, 3)
-        pos_t = torch.from_numpy(position).float().to(dev)
-        cen_t = torch.from_numpy(base).float().to(dev)
-        step_t = torch.from_numpy(step).float().to(dev)
-        rot_t = torch.from_numpy(rots).float().to(dev)
         coord = pos_t.view(B, 1, 1, 1, 3) + step_t * grid.unsqueeze(0)
         coord = coord - cen_t.view(B, 1, 1, 1, 3)
         coord = torch.einsum("bij,bxyzj->bxyzi", rot_t, coord) + cen_t.view(B, 1, 1, 1, 3)
@@ -223,15 +263,11 @@ class VolumetricTriangulationNet(_EngineOwner):
             coord = coord.permute(0, 1, 3, 2, 4).flip(2)
         features = layers.run(self.process_features, features, conv, norm)
         features = features.view(B, V, *features.shape[1:])
-        ops = torch_ops
-        if self.backend == "hybrid":
-            if not images.is_cuda:
-                raise RuntimeError("lt_b200 hybrid backend needs CUDA tensors (native custom ops); use backend='torch' on CPU")
-            from . import autograd_ops as ops
+        ops = autograd_ops if self.backend == "hybrid" else torch_ops
         volumes = ops.unproject_heatmaps(features, proj_t, coord, self.volume_aggregation_method, vol_conf)
         volumes = self.volume_net(volumes, v2v_conv, norm)
         kp, volumes = ops.integrate_tensor_3d_with_coordinates(volumes * self.volume_multiplier, coord, self.volume_softmax)
-        return kp, features, volumes, vol_conf, cuboids, coord, cen_t
+        return kp, features, volumes, vol_conf, coord
 
 
 class AlgebraicTriangulationNet(_EngineOwner):
@@ -241,7 +277,8 @@ class AlgebraicTriangulationNet(_EngineOwner):
     kernels (engine.algebraic_forward); "torch": autograd torch ops; "hybrid": torch backbone, native 2-D soft-argmax and DLT
     with their backward kernels (trains, any mode)."""
 
-    def __init__(self, config, device="cuda:0", backend=None, conv_mode=None, backbone_backend="torch", norm_backend="torch"):
+    def __init__(self, config, device="cuda:0", backend=None, conv_mode=None, backbone_backend="torch", norm_backend="torch",
+                 train_graph=False):
         super().__init__()
         self.use_confidences = config.model.use_confidences
         config.model.backbone.alg_confidences = False
@@ -254,9 +291,12 @@ class AlgebraicTriangulationNet(_EngineOwner):
         self.backend = backend or os.environ.get("LT_B200_BACKEND", "native")
         self.conv_mode = conv_mode or os.environ.get("LT_B200_CONV", "tc")
         _check_backends(self.backend, self.conv_mode, backbone_backend, norm_backend)
+        _check_train_graph(train_graph, self.backend)
         self.backbone_backend = backbone_backend
         self.norm_backend = norm_backend
+        self.clone_outputs = True
         self._engine = None
+        self._train_graphs = TrainGraphs() if train_graph else None
 
     def engine(self):
         if self._engine is None:
@@ -271,7 +311,7 @@ class AlgebraicTriangulationNet(_EngineOwner):
             # torch/cuDNN backbone with the native 2-D soft-argmax and DLT (forward + backward kernels) in the autograd graph
             if not images.is_cuda:
                 raise RuntimeError("lt_b200 hybrid backend needs CUDA tensors (native custom ops); use backend='torch' on CPU")
-            return self._forward_torch(images, proj_matricies, ops_backend="hybrid")
+            return self._run_device(self._forward_torch, (images, proj_matricies))
         if not images.is_cuda:
             raise RuntimeError("lt_b200 native backend needs CUDA tensors; construct the model with backend='torch' for CPU/autograd")
         if self.training or torch.is_grad_enabled():
@@ -280,8 +320,10 @@ class AlgebraicTriangulationNet(_EngineOwner):
             return self.engine().algebraic_forward(images.float().contiguous(), proj_matricies.float().contiguous(),
                                                    self.heatmap_multiplier, self.use_confidences, self.heatmap_softmax)
 
-    def _forward_torch(self, images, proj_matricies, ops_backend="torch"):
-        """The reference forward on torch autograd; ops_backend="hybrid" runs its 2-D soft-argmax and DLT on the native kernels."""
+    def _forward_torch(self, images, proj_matricies):
+        """The reference forward on torch autograd, (images, proj_matricies) -> (kp3d, kp2d, heatmaps, alg_conf): everything runs on
+        the device.  backend="hybrid" runs its 2-D soft-argmax and DLT on the native kernels."""
+        ops_backend = "hybrid" if self.backend == "hybrid" else "torch"
         B, V = images.shape[:2]
         conv, _, norm = _hooks(self.backbone_backend, self.norm_backend)
         heatmaps, _, alg_conf, _ = self.backbone(images.reshape(-1, *images.shape[2:]), conv, norm)
@@ -294,6 +336,9 @@ class AlgebraicTriangulationNet(_EngineOwner):
         alg_conf = alg_conf / alg_conf.sum(dim=1, keepdim=True) + 1e-5
         h, w = heatmaps.shape[3:]
         H, W = images.shape[3:]
-        kp2d = kp2d * torch.tensor([W / w, H / h], device=images.device, dtype=kp2d.dtype)
+        # the (W / w, H / h) scale is filled on the device: a host-to-device copy would synchronise and cannot be captured
+        scale = torch.full((2,), W / w, device=images.device, dtype=kp2d.dtype)
+        scale[1].fill_(H / h)
+        kp2d = kp2d * scale
         kp3d = multiview.triangulate_batch_of_points(proj_matricies, kp2d, confidences_batch=alg_conf, backend=ops_backend)
         return kp3d, kp2d, heatmaps, alg_conf
