@@ -346,8 +346,9 @@ int lt_triangulate_dlt_fwd(const float* proj, const float* keypoints_2d, const f
  * be NULL; confidences NULL means all ones).  Both are WRITTEN, not accumulated into (unlike lt_unproject_aggregate_bwd).
  * Projection matrices get no gradient (they come from numpy camera data in the reference too).  One thread per (sample, joint)
  * redoes the forward's float64 eigen-solve (same code, same order of operations) and applies the first-order eigenvector
- * perturbation.  Where the smallest eigenvalue of A^T A is tied with another (gap <= 1e-12 of the largest eigenvalue) the
- * derivative does not exist; the tied term is dropped, so the gradient stays finite (torch's SVD backward is not finite there). */
+ * perturbation.  Where the smallest eigenvalue of A^T A is tied with another (gap <= 1e-12 of the larger of the two, or below
+ * 1e-30 of the largest eigenvalue) the derivative does not exist; the tied term is dropped, so the gradient stays finite (torch's
+ * SVD backward is not finite there). */
 int lt_triangulate_dlt_bwd(const float* proj, const float* keypoints_2d, const float* confidences, const float* grad_out,
                            float* grad_keypoints_2d, float* grad_confidences, int B, int V, int J, void* stream);
 
@@ -433,8 +434,8 @@ int lt_tc_gemm_selftest(const void* a_fp16, const void* b_fp16, float* d, int M,
                         int variant, void* stream);
 
 /* ------------------------------------------------------------------------------------------
- * Test hooks (NOT part of the product path): the per-item code of the backward kernels executed on the CPU with HOST
- * pointers, so that the `-m "not gpu"` suite can check the gradient arithmetic against torch autograd without a GPU.
+ * Test hooks (NOT part of the product path): the per-item code of the backward kernels (and of the DLT forward) executed on
+ * the CPU with HOST pointers, so that the `-m "not gpu"` suite can check the arithmetic against references without a GPU.
  * Same arguments as the device entry points minus scratch / stream (softmax: modes 0, 1 and 2 as in lt_softargmax3d_bwd).
  * ---------------------------------------------------------------------------------------- */
 int lt_test_unproject_aggregate_bwd_host(const float* features, const float* proj, const float* coord, const float* conf,
@@ -442,6 +443,8 @@ int lt_test_unproject_aggregate_bwd_host(const float* features, const float* pro
                                          long nvox, int agg);
 int lt_test_softargmax3d_bwd_host(const float* probs, const float* coord, const float* grad_keypoints, const float* grad_volumes,
                                   float* grad_logits, int B, int J, long nvox, float multiplier, int softmax);
+int lt_test_triangulate_dlt_fwd_host(const float* proj, const float* keypoints_2d, const float* confidences, float* out, int B,
+                                     int V, int J);
 int lt_test_triangulate_dlt_bwd_host(const float* proj, const float* keypoints_2d, const float* confidences, const float* grad_out,
                                      float* grad_keypoints_2d, float* grad_confidences, int B, int V, int J);
 /* lt_volumetric_ce_fwd (+ lt_volumetric_ce_bwd when grad_probs is not NULL, grad_loss then a HOST pointer) on host pointers, with

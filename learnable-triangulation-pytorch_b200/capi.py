@@ -101,6 +101,7 @@ SIGNATURES = {
     "lt_view_normalize_fwd": (c_int, [c_void_p, c_int, c_int, c_int, c_float, c_void_p]),
     "lt_triangulate_dlt_fwd": (c_int, [c_void_p] * 4 + [c_int] * 3 + [c_void_p]),
     "lt_triangulate_dlt_bwd": (c_int, [c_void_p] * 6 + [c_int] * 3 + [c_void_p]),
+    "lt_test_triangulate_dlt_fwd_host": (c_int, [c_void_p] * 4 + [c_int] * 3),
     "lt_test_triangulate_dlt_bwd_host": (c_int, [c_void_p] * 6 + [c_int] * 3),
     "lt_volumetric_ce_workspace_bytes": (c_size_t, [c_int, c_int, c_long]),
     "lt_volumetric_ce_fwd": (c_int, [c_void_p] * 8 + [c_size_t, c_int, c_int, c_long, c_void_p]),
@@ -423,6 +424,13 @@ def volumetric_ce_host(probs, coord, keypoints_gt, validity, grad_loss=None, gra
                                             _host_ptr(loss), index.data_ptr(), _host_ptr(picked), _host_ptr(g), _host_ptr(grad_probs),
                                             B, J, nvox), "lt_test_volumetric_ce_host")
     return float(loss[0]), index, picked
+
+
+def triangulate_dlt_host(proj, kp2d, conf, out):
+    """lt_test_triangulate_dlt_fwd_host: the forward kernel's per-item code run on CPU tensors (test hook, no GPU needed)."""
+    B, V, J = kp2d.shape[:3]
+    _check(lib().lt_test_triangulate_dlt_fwd_host(_host_ptr(proj), _host_ptr(kp2d), _host_ptr(conf), _host_ptr(out), B, V, J),
+           "lt_test_triangulate_dlt_fwd_host")
 
 
 def triangulate_dlt_bwd_host(proj, kp2d, conf, grad_out, grad_kp2d, grad_conf):

@@ -66,13 +66,23 @@ __global__ void view_normalize_kernel(float* __restrict__ conf, int B, int V, in
 // Jacobi eigen-solve run in float64 (forming A^T A squares the condition number, fp32 would not do); the reference's
 // `-vh[:, 3]` sign cancels in the dehomogenisation.
 
+// (p2 * x - p0) * cf with one float32 rounding per operation, as the reference rounds it: on the device __fmul_rn / __fsub_rn
+// keep nvcc from contracting the subtraction into an FFMA; the host compiler is not asked for FMA, so the plain operators match.
+__host__ __device__ __forceinline__ float dlt_entry(float p2, float x, float p0, float cf) {
+#ifdef __CUDA_ARCH__
+  return __fmul_rn(__fsub_rn(__fmul_rn(p2, x), p0), cf);
+#else
+  return (p2 * x - p0) * cf;
+#endif
+}
+
 // the two DLT rows of view v, as the forward rounds them: formed in float32 like the reference (multiview.py:159-161), then
-// widened.  cf = 1 gives the unweighted rows x*P[2] - P[0], y*P[2] - P[1].
+// widened; bit-identical on the device and the host.  cf = 1 gives the unweighted rows x*P[2] - P[0], y*P[2] - P[1].
 __host__ __device__ __forceinline__ void dlt_rows(const float* P, float x, float y, float cf, double r0[4], double r1[4]) {
 #pragma unroll
   for (int c = 0; c < 4; ++c) {
-    r0[c] = (double)((P[8 + c] * x - P[c]) * cf);
-    r1[c] = (double)((P[8 + c] * y - P[4 + c]) * cf);
+    r0[c] = (double)dlt_entry(P[8 + c], x, P[c], cf);
+    r1[c] = (double)dlt_entry(P[8 + c], y, P[4 + c], cf);
   }
 }
 
@@ -145,29 +155,43 @@ __host__ __device__ __forceinline__ void dlt_column(const double E[4][4], int m,
   }
 }
 
+// Forward of the weighted DLT for item (b, j): out[b][j] = u[0:3] / u[3].  A point at infinity (u[3] = 0) gives the IEEE
+// quotients (inf or nan), as the reference's division does.
+__host__ __device__ __forceinline__ void dlt_fwd_item(const float* __restrict__ proj, const float* __restrict__ kp2d,
+                                                      const float* __restrict__ conf, float* __restrict__ out, int b, int j, int V,
+                                                      int J) {
+  double M[4][4], E[4][4], u[4];
+  dlt_column(E, dlt_eigen(proj, kp2d, conf, b, j, V, J, M, E), u);
+  const double w = u[3];
+  const long bj = (long)b * J + j;
+  out[bj * 3 + 0] = (float)(u[0] / w);
+  out[bj * 3 + 1] = (float)(u[1] / w);
+  out[bj * 3 + 2] = (float)(u[2] / w);
+}
+
 __global__ void __launch_bounds__(128) triangulate_dlt_kernel(const float* __restrict__ proj, const float* __restrict__ kp2d,
                                                               const float* __restrict__ conf, float* __restrict__ out, int B, int V, int J) {
   const int idx = blockIdx.x * blockDim.x + threadIdx.x;
   if (idx >= B * J) return;
-  const int b = idx / J, j = idx % J;
-  double M[4][4], E[4][4], u[4];
-  dlt_column(E, dlt_eigen(proj, kp2d, conf, b, j, V, J, M, E), u);
-  const double w = u[3];
-  out[(long)idx * 3 + 0] = (float)(u[0] / w);
-  out[(long)idx * 3 + 1] = (float)(u[1] / w);
-  out[(long)idx * 3 + 2] = (float)(u[2] / w);
+  dlt_fwd_item(proj, kp2d, conf, out, idx / J, idx % J, V, J);
 }
 
-// Eigenvalue gaps at or below this fraction of the largest eigenvalue count as ties (see dlt_bwd_item).
+// Tie rule of dlt_bwd_item: a gap |lambda_0 - lambda_k| at or below kDltTieTol of the larger of the two eigenvalues, or below
+// kDltGapFloor of the largest one, counts as a tie.  The relative test, not one against the largest eigenvalue, is what keeps
+// graded systems: the fourth column of A is ~1e3x the others, so with confidences of (1, 1e-4, 1e-4, 1e-4) the two smallest
+// eigenvalues are ~1e-17 and ~1e-14 of the largest, yet the float64 Jacobi solve resolves them and their gap carries the main
+// term of the gradient.  The floor only bounds 1 / gap; confidence ratios down to 1e-6 give gaps of ~1e-18 of the largest
+// eigenvalue and are kept.
 constexpr double kDltTieTol = 1e-12;
+constexpr double kDltGapFloor = 1e-30;
 
 // Backward of the weighted DLT for item (b, j).  With (lambda_k, e_k) the eigenpairs of M = A^T A, u = e_0 the smallest:
 //   X = u[0:3] / u[3]  ->  g_u = [g_X / u[3], -(g_X . u[0:3]) / u[3]^2]
 //   w = sum_{k != 0} (g_u . e_k) / (lambda_0 - lambda_k) e_k          (first-order perturbation of the eigenvector)
 //   G_A = A (w u^T + u w^T): row r of A gets (a_r . w) u + (a_r . u) w
 //   d x = c (G_A[r0] . P[2]),  d y = c (G_A[r1] . P[2]),  d c = G_A[r0] . (x P[2] - P[0]) + G_A[r1] . (y P[2] - P[1]).
-// Independent of the sign of u.  A term whose gap |lambda_0 - lambda_k| is at most kDltTieTol * max |lambda| is dropped: on an
-// exact tie the derivative does not exist (torch's SVD backward returns non-finite values there); dropping keeps it finite.
+// Independent of the sign of u.  A term whose gap is a tie by the rule above (kDltTieTol) is dropped: on an exact tie the
+// derivative does not exist (torch's SVD backward returns non-finite values there); dropping keeps it finite.
 // grad_kp / grad_conf are WRITTEN (every (v, j) of the item), grad_conf may be null.
 __host__ __device__ __forceinline__ void dlt_bwd_item(const float* __restrict__ proj, const float* __restrict__ kp2d,
                                                       const float* __restrict__ conf, const float* __restrict__ grad_out,
@@ -190,7 +214,7 @@ __host__ __device__ __forceinline__ void dlt_bwd_item(const float* __restrict__ 
 #pragma unroll
   for (int k = 0; k < 4; ++k) {
     const double gap = lam0 - M[k][k];
-    if (k == m || !(fabs(gap) > kDltTieTol * lmax)) continue;
+    if (k == m || !(fabs(gap) > kDltTieTol * fmax(fabs(lam0), fabs(M[k][k])) + kDltGapFloor * lmax)) continue;
     const double s = (gu[0] * E[0][k] + gu[1] * E[1][k] + gu[2] * E[2][k] + gu[3] * E[3][k]) / gap;
 #pragma unroll
     for (int r = 0; r < 4; ++r) w[r] += s * E[r][k];
@@ -278,7 +302,15 @@ extern "C" int lt_triangulate_dlt_bwd(const float* proj, const float* keypoints_
   return LT_OK;
 }
 
-// test hook: the backward's per-item code on the CPU (host pointers), for the `-m "not gpu"` gradient tests
+// test hooks: the forward's and the backward's per-item code on the CPU (host pointers), for the `-m "not gpu"` tests
+extern "C" int lt_test_triangulate_dlt_fwd_host(const float* proj, const float* keypoints_2d, const float* confidences, float* out,
+                                                int B, int V, int J) {
+  LT_REQUIRE(proj && keypoints_2d && out && B > 0 && V > 0 && J > 0, "test_triangulate_dlt_fwd_host: bad arguments");
+  for (int b = 0; b < B; ++b)
+    for (int j = 0; j < J; ++j) dlt_fwd_item(proj, keypoints_2d, confidences, out, b, j, V, J);
+  return LT_OK;
+}
+
 extern "C" int lt_test_triangulate_dlt_bwd_host(const float* proj, const float* keypoints_2d, const float* confidences,
                                                 const float* grad_out, float* grad_keypoints_2d, float* grad_confidences, int B, int V,
                                                 int J) {
