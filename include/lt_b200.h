@@ -151,10 +151,22 @@ int lt_feature_scatter_fwd(const float* feats, float* const* peer_buffers, int n
 /* Backward of lt_unproject_aggregate_fwd for the training loop (train.py:236 total_loss.backward(); the reference gets it
  * from autograd through F.grid_sample and the aggregation ops of op.py:131-162).  grad_out [B][nvox][C] float32;
  * grad_features [B][V][h][w][C] and grad_conf [B][V][C] (LT_AGG_CONF, may be NULL) are ACCUMULATED into (zero them first).
- * Projection matrices and coordinate volumes carry no gradient (they do not in the reference either).  C % 4 == 0. */
+ * Projection matrices and coordinate volumes get no gradient here: lt_unproject_aggregate_bwd_geom adds them.  C % 4 == 0. */
 int lt_unproject_aggregate_bwd(const float* features, const float* proj, const float* coord, const float* conf,
                                const float* grad_out, float* grad_features, float* grad_conf, int B, int V, int C, int h, int w,
                                long nvox, int agg, void* stream);
+/* lt_unproject_aggregate_bwd plus the gradients the reference's torch graph gives the geometry (the matmul, the division by depth
+ * and F.grid_sample with respect to the grid, op.py:113-147): grad_proj [B][V][12] and grad_coord [B][nvox][3], either may be NULL;
+ * both are WRITTEN, not accumulated into.  grad_features / grad_conf are accumulated into by the same per-item code as
+ * lt_unproject_aggregate_bwd.  The sample derivative is torch's grid_sampler_2d_backward convention (weight derivatives of the taps
+ * inside the map, the same floor cell); a voxel that fails the depth test or has no tap inside the map contributes exactly 0.
+ * Deterministic: no float atomics in the geometry sums (dP accumulates in float64 in a fixed order).  No host synchronisation.
+ * C / 4 must be a power of two <= 32.  workspace: lt_unproject_aggregate_bwd_geom_workspace_bytes(B, V, nvox) bytes. */
+size_t lt_unproject_aggregate_bwd_geom_workspace_bytes(int B, int V, long nvox);
+int lt_unproject_aggregate_bwd_geom(const float* features, const float* proj, const float* coord, const float* conf,
+                                    const float* grad_out, float* grad_features, float* grad_conf, float* grad_proj, float* grad_coord,
+                                    void* workspace, size_t workspace_bytes, int B, int V, int C, int h, int w, long nvox, int agg,
+                                    void* stream);
 
 /* ------------------------------------------------------------------------------------------
  * Volumetric soft-argmax.  Replaces op.integrate_tensor_3d_with_coordinates (op.py:84-96).
@@ -176,6 +188,10 @@ int lt_unproject_aggregate_bwd(const float* features, const float* proj, const f
  * scratch: >= B*J floats in mode 1, >= 2*B*J floats in mode 2, unused in mode 0. */
 int lt_softargmax3d_bwd(const float* probs, const float* coord, const float* grad_keypoints, const float* grad_volumes,
                         float* grad_logits, float* scratch, int B, int J, long nvox, float multiplier, int softmax, void* stream);
+/* Coordinate gradient of the soft-argmax (modes 0 and 1, where kp = sum_i probs_i x_i): grad_coord[b][i] = sum_j probs[b][j][i]
+ * grad_keypoints[b][j], joints summed in order, WRITTEN.  Mode 2 (the 2-D op, whose pixel grid is no input) is rejected. */
+int lt_softargmax3d_coord_bwd(const float* probs, const float* grad_keypoints, float* grad_coord, int B, int J, long nvox, int softmax,
+                              void* stream);
 size_t lt_softargmax3d_workspace_bytes(int B, int J, long nvox);
 int lt_softargmax3d_fwd(const float* logits, long batch_stride, long voxel_stride, long chan_stride,
                         const float* coord, float* volumes_out, float* keypoints_out,
@@ -344,13 +360,20 @@ int lt_triangulate_dlt_fwd(const float* proj, const float* keypoints_2d, const f
 /* Backward of lt_triangulate_dlt_fwd for the training loop: what autograd derives through the reference's per-(sample, joint)
  * torch.svd (multiview.py:141-183).  grad_out [B][J][3] -> grad_keypoints_2d [B][V][J][2] and grad_confidences [B][V][J] (may
  * be NULL; confidences NULL means all ones).  Both are WRITTEN, not accumulated into (unlike lt_unproject_aggregate_bwd).
- * Projection matrices get no gradient (they come from numpy camera data in the reference too).  One thread per (sample, joint)
+ * Projection matrices get no gradient here: lt_triangulate_dlt_proj_bwd gives it.  One thread per (sample, joint)
  * redoes the forward's float64 eigen-solve (same code, same order of operations) and applies the first-order eigenvector
  * perturbation.  Where the smallest eigenvalue of A^T A is tied with another (gap <= 1e-12 of the larger of the two, or below
  * 1e-30 of the largest eigenvalue) the derivative does not exist; the tied term is dropped, so the gradient stays finite (torch's
  * SVD backward is not finite there). */
 int lt_triangulate_dlt_bwd(const float* proj, const float* keypoints_2d, const float* confidences, const float* grad_out,
                            float* grad_keypoints_2d, float* grad_confidences, int B, int V, int J, void* stream);
+/* Projection-matrix gradient of lt_triangulate_dlt_fwd (the reference's torch.svd backward through A = c (x P[2] - P[0]),
+ * c (y P[2] - P[1]), multiview.py:159-163): grad_proj [B][V][3][4], WRITTEN.  The same eigen-solve, perturbation and tie rule as
+ * lt_triangulate_dlt_bwd; per-(sample, joint) float64 partials in `workspace` (lt_triangulate_dlt_proj_bwd_workspace_bytes(B, V, J)
+ * bytes), then summed over the joints in a fixed order: deterministic. */
+size_t lt_triangulate_dlt_proj_bwd_workspace_bytes(int B, int V, int J);
+int lt_triangulate_dlt_proj_bwd(const float* proj, const float* keypoints_2d, const float* confidences, const float* grad_out,
+                                float* grad_proj, void* workspace, size_t workspace_bytes, int B, int V, int J, void* stream);
 
 /* ------------------------------------------------------------------------------------------
  * Volumetric cross-entropy loss of the volumetric training recipe.  Replaces VolumetricCELoss (mvn/models/loss.py:52-80, called
@@ -447,6 +470,12 @@ int lt_test_triangulate_dlt_fwd_host(const float* proj, const float* keypoints_2
                                      int V, int J);
 int lt_test_triangulate_dlt_bwd_host(const float* proj, const float* keypoints_2d, const float* confidences, const float* grad_out,
                                      float* grad_keypoints_2d, float* grad_confidences, int B, int V, int J);
+int lt_test_unproject_aggregate_bwd_geom_host(const float* features, const float* proj, const float* coord, const float* conf,
+                                              const float* grad_out, float* grad_features, float* grad_conf, float* grad_proj,
+                                              float* grad_coord, int B, int V, int C, int h, int w, long nvox, int agg);
+int lt_test_softargmax3d_coord_bwd_host(const float* probs, const float* grad_keypoints, float* grad_coord, int B, int J, long nvox);
+int lt_test_triangulate_dlt_proj_bwd_host(const float* proj, const float* keypoints_2d, const float* confidences, const float* grad_out,
+                                          float* grad_proj, int B, int V, int J);
 /* lt_volumetric_ce_fwd (+ lt_volumetric_ce_bwd when grad_probs is not NULL, grad_loss then a HOST pointer) on host pointers, with
  * the kernels' distance, argmin key, term and gradient code: loss.py:52-80. */
 int lt_test_volumetric_ce_host(const float* probs, const float* coord, const float* keypoints_gt, const float* validity, float* loss,

@@ -8,8 +8,9 @@ autograd.  Volumetric model: the unprojection + aggregation and the 3-D soft-arg
 Python loops over (sample, view) pairs with ~10 passes over a (V, C, N^3) staging tensor.  Algebraic model: the 2-D
 soft-argmax (op.py:11-47, both branches) and the confidence-weighted DLT, which the reference runs as one torch.svd per
 (sample, joint) (multiview.py:171-183).  Gradients: feature maps / heat-maps, `conf` and algebraic confidences, V2V logits,
-2-D key points; projection matrices and coordinate volumes carry none (they do not in the reference either: they come from
-numpy camera data).
+2-D key points, and -- when they require grad, as at op level where a caller may refine cameras or learn a cuboid -- projection
+matrices (unprojection, DLT) and coordinate volumes (unprojection, 3-D soft-argmax).  The models' geometry comes from numpy and
+requires no grad, so their training steps launch no geometry kernel.
 """
 import torch
 
@@ -36,6 +37,7 @@ class UnprojectHeatmapsFn(torch.autograd.Function):
         ctx.save_for_backward(feats_cl, proj, coord, conf if conf is not None else torch.empty(0, device=heatmaps.device))
         ctx.agg, ctx.vol_shape, ctx.has_conf = agg, vol_shape, conf is not None
         ctx.conf_shape = None if vol_confidences is None else tuple(vol_confidences.shape)
+        ctx.geom_shapes = (tuple(proj_matricies.shape), tuple(coord_volumes.shape))
         return out_cl.permute(0, 2, 1).reshape(B, C, *vol_shape).contiguous()
 
     @staticmethod
@@ -48,9 +50,21 @@ class UnprojectHeatmapsFn(torch.autograd.Function):
         grad_feats = torch.zeros_like(feats_cl)
         need_conf = ctx.has_conf and ctx.needs_input_grad[3]
         grad_conf = torch.zeros((B, V, C), dtype=torch.float32, device=feats_cl.device) if need_conf else None
-        capi.unproject_aggregate_bwd(feats_cl, proj, coord, conf, g_cl, grad_feats, grad_conf, ctx.agg)
+        need_proj, need_coord = ctx.needs_input_grad[1], ctx.needs_input_grad[2]
+        grad_proj = grad_coord = None
+        if need_proj or need_coord:
+            dev = feats_cl.device
+            grad_proj = torch.empty((B, V, 12), dtype=torch.float32, device=dev) if need_proj else None
+            grad_coord = torch.empty((B, nvox, 3), dtype=torch.float32, device=dev) if need_coord else None
+            ws = torch.empty(capi.unproject_aggregate_bwd_geom_workspace_bytes(B, V, nvox), dtype=torch.uint8, device=dev)
+            capi.unproject_aggregate_bwd_geom(feats_cl, proj, coord, conf, g_cl, grad_feats, grad_conf, grad_proj, grad_coord, ctx.agg, ws)
+            proj_shape, coord_shape = ctx.geom_shapes
+            grad_proj = grad_proj.reshape(proj_shape) if need_proj else None
+            grad_coord = grad_coord.reshape(coord_shape) if need_coord else None
+        else:
+            capi.unproject_aggregate_bwd(feats_cl, proj, coord, conf, g_cl, grad_feats, grad_conf, ctx.agg)
         grad_heat = grad_feats.permute(0, 1, 4, 2, 3)                                       # (B, V, C, h, w) view
-        return grad_heat, None, None, (grad_conf.reshape(ctx.conf_shape) if need_conf else None), None
+        return grad_heat, grad_proj, grad_coord, (grad_conf.reshape(ctx.conf_shape) if need_conf else None), None
 
 
 class IntegrateTensor3dFn(torch.autograd.Function):
@@ -68,6 +82,7 @@ class IntegrateTensor3dFn(torch.autograd.Function):
         capi.softargmax3d(logits, J * nvox, 1, nvox, coord, out, keypoints, ws, B, J, nvox, 1.0, softmax)
         ctx.save_for_backward(out, coord)
         ctx.softmax = bool(softmax)
+        ctx.coord_shape = tuple(coord_volumes.shape)
         return keypoints, out
 
     @staticmethod
@@ -81,7 +96,12 @@ class IntegrateTensor3dFn(torch.autograd.Function):
         grad_logits = torch.empty_like(probs)
         scratch = torch.empty(B * J, dtype=torch.float32, device=dev)
         capi.softargmax3d_bwd(probs, coord, g_kp, g_vol, grad_logits, scratch, B, J, nvox, 1.0, ctx.softmax)
-        return grad_logits, None, None
+        grad_coord = None
+        if ctx.needs_input_grad[1]:
+            grad_coord = torch.empty((B, nvox, 3), dtype=torch.float32, device=dev)
+            capi.softargmax3d_coord_bwd(probs.reshape(B, J, nvox), g_kp, grad_coord, B, J, nvox, ctx.softmax)
+            grad_coord = grad_coord.reshape(ctx.coord_shape)
+        return grad_logits, grad_coord, None
 
 
 class IntegrateTensor2dFn(torch.autograd.Function):
@@ -119,7 +139,7 @@ class IntegrateTensor2dFn(torch.autograd.Function):
 
 class TriangulateDltFn(torch.autograd.Function):
     """multiview.triangulate_batch_of_points (reference multiview.py:141-183): (B, V, 3, 4), (B, V, J, 2), (B, V, J) or None
-    -> (B, J, 3).  Gradients reach the key points and the confidences, not the projection matrices."""
+    -> (B, J, 3).  Gradients reach the key points, the confidences and the projection matrices."""
 
     @staticmethod
     def forward(ctx, proj_matricies, points, confidences):
@@ -138,10 +158,18 @@ class TriangulateDltFn(torch.autograd.Function):
         proj, kp, conf = ctx.saved_tensors
         conf = conf if ctx.has_conf else None
         need_conf = ctx.has_conf and ctx.needs_input_grad[2]
-        grad_kp = torch.empty_like(kp)
-        grad_conf = torch.empty_like(conf) if need_conf else None
-        capi.triangulate_dlt_bwd(proj, kp, conf, grad_out.float().contiguous(), grad_kp, grad_conf)
-        return None, (grad_kp if ctx.needs_input_grad[1] else None), grad_conf
+        g = grad_out.float().contiguous()
+        grad_kp = grad_conf = grad_proj = None
+        if ctx.needs_input_grad[1] or need_conf:
+            grad_kp = torch.empty_like(kp)
+            grad_conf = torch.empty_like(conf) if need_conf else None
+            capi.triangulate_dlt_bwd(proj, kp, conf, g, grad_kp, grad_conf)
+        if ctx.needs_input_grad[0]:
+            B, V, J = kp.shape[:3]
+            grad_proj = torch.empty_like(proj)
+            ws = torch.empty(capi.triangulate_dlt_proj_bwd_workspace_bytes(B, V, J), dtype=torch.uint8, device=proj.device)
+            capi.triangulate_dlt_proj_bwd(proj, kp, conf, g, grad_proj, ws)
+        return grad_proj, (grad_kp if ctx.needs_input_grad[1] else None), grad_conf
 
 
 class VolumetricCEFn(torch.autograd.Function):

@@ -72,6 +72,11 @@ SIGNATURES = {
     "lt_feature_scatter_fwd": (c_int, [c_void_p, ctypes.POINTER(c_void_p), c_int, c_int, c_int, c_int, c_int, c_long, c_void_p]),
     "lt_unproject_aggregate_bwd": (c_int, [c_void_p] * 7 + [c_int] * 5 + [c_long, c_int, c_void_p]),
     "lt_softargmax3d_bwd": (c_int, [c_void_p] * 6 + [c_int, c_int, c_long, c_float, c_int, c_void_p]),
+    "lt_unproject_aggregate_bwd_geom_workspace_bytes": (c_size_t, [c_int, c_int, c_long]),
+    "lt_unproject_aggregate_bwd_geom": (c_int, [c_void_p] * 10 + [c_size_t] + [c_int] * 5 + [c_long, c_int, c_void_p]),
+    "lt_softargmax3d_coord_bwd": (c_int, [c_void_p] * 3 + [c_int, c_int, c_long, c_int, c_void_p]),
+    "lt_test_unproject_aggregate_bwd_geom_host": (c_int, [c_void_p] * 9 + [c_int] * 5 + [c_long, c_int]),
+    "lt_test_softargmax3d_coord_bwd_host": (c_int, [c_void_p] * 3 + [c_int, c_int, c_long]),
     "lt_test_unproject_aggregate_bwd_host": (c_int, [c_void_p] * 7 + [c_int] * 5 + [c_long, c_int]),
     "lt_test_softargmax3d_bwd_host": (c_int, [c_void_p] * 5 + [c_int, c_int, c_long, c_float, c_int]),
     "lt_softargmax3d_workspace_bytes": (c_size_t, [c_int, c_int, c_long]),
@@ -103,6 +108,9 @@ SIGNATURES = {
     "lt_triangulate_dlt_bwd": (c_int, [c_void_p] * 6 + [c_int] * 3 + [c_void_p]),
     "lt_test_triangulate_dlt_fwd_host": (c_int, [c_void_p] * 4 + [c_int] * 3),
     "lt_test_triangulate_dlt_bwd_host": (c_int, [c_void_p] * 6 + [c_int] * 3),
+    "lt_triangulate_dlt_proj_bwd_workspace_bytes": (c_size_t, [c_int] * 3),
+    "lt_triangulate_dlt_proj_bwd": (c_int, [c_void_p] * 6 + [c_size_t] + [c_int] * 3 + [c_void_p]),
+    "lt_test_triangulate_dlt_proj_bwd_host": (c_int, [c_void_p] * 5 + [c_int] * 3),
     "lt_volumetric_ce_workspace_bytes": (c_size_t, [c_int, c_int, c_long]),
     "lt_volumetric_ce_fwd": (c_int, [c_void_p] * 8 + [c_size_t, c_int, c_int, c_long, c_void_p]),
     "lt_volumetric_ce_bwd": (c_int, [c_void_p] * 5 + [c_int, c_int, c_long, c_void_p]),
@@ -267,6 +275,28 @@ def softargmax3d_bwd(probs, coord, grad_keypoints, grad_volumes, grad_logits, sc
                                      B, J, nvox, float(multiplier), int(softmax), _stream()), "lt_softargmax3d_bwd")
 
 
+def unproject_aggregate_bwd_geom(features_cl, proj, coord, conf, grad_out_cl, grad_features_cl, grad_conf, grad_proj, grad_coord, agg,
+                                 workspace):
+    """lt_unproject_aggregate_bwd_geom: grad_features_cl / grad_conf accumulated into, grad_proj (B, V, 12) and grad_coord (B, nvox, 3)
+    (either None) written; workspace: unproject_aggregate_bwd_geom_workspace_bytes(B, V, nvox) bytes."""
+    B, V, h, w, C = features_cl.shape
+    nvox = coord.shape[1]
+    _check(lib().lt_unproject_aggregate_bwd_geom(_ptr(features_cl), _ptr(proj), _ptr(coord), _ptr(conf), _ptr(grad_out_cl),
+                                                 _ptr(grad_features_cl), _ptr(grad_conf), _ptr(grad_proj), _ptr(grad_coord), _ptr(workspace),
+                                                 workspace.numel() * workspace.element_size(), B, V, C, h, w, nvox, agg, _stream()),
+           "lt_unproject_aggregate_bwd_geom")
+
+
+def unproject_aggregate_bwd_geom_workspace_bytes(B, V, nvox):
+    return lib().lt_unproject_aggregate_bwd_geom_workspace_bytes(B, V, nvox)
+
+
+def softargmax3d_coord_bwd(probs, grad_keypoints, grad_coord, B, J, nvox, softmax):
+    """grad_coord (B, nvox, 3) = sum_j probs (B, J, nvox) x grad_keypoints (B, J, 3), written; modes 0 and 1 only."""
+    _check(lib().lt_softargmax3d_coord_bwd(_ptr(probs), _ptr(grad_keypoints), _ptr(grad_coord), B, J, nvox, int(softmax), _stream()),
+           "lt_softargmax3d_coord_bwd")
+
+
 def softargmax3d_workspace_bytes(B, J, nvox):
     return lib().lt_softargmax3d_workspace_bytes(B, J, nvox)
 
@@ -363,6 +393,17 @@ def triangulate_dlt_bwd(proj, kp2d, conf, grad_out, grad_kp2d, grad_conf):
                                         _stream()), "lt_triangulate_dlt_bwd")
 
 
+def triangulate_dlt_proj_bwd(proj, kp2d, conf, grad_out, grad_proj, workspace):
+    """grad_proj (B, V, 3, 4) is written; workspace: triangulate_dlt_proj_bwd_workspace_bytes(B, V, J) bytes."""
+    B, V, J = kp2d.shape[:3]
+    _check(lib().lt_triangulate_dlt_proj_bwd(_ptr(proj), _ptr(kp2d), _ptr(conf), _ptr(grad_out), _ptr(grad_proj), _ptr(workspace),
+                                             workspace.numel() * workspace.element_size(), B, V, J, _stream()), "lt_triangulate_dlt_proj_bwd")
+
+
+def triangulate_dlt_proj_bwd_workspace_bytes(B, V, J):
+    return lib().lt_triangulate_dlt_proj_bwd_workspace_bytes(B, V, J)
+
+
 def volumetric_ce_workspace_bytes(B, J, nvox):
     return lib().lt_volumetric_ce_workspace_bytes(B, J, nvox)
 
@@ -445,6 +486,31 @@ def softargmax3d_bwd_host(probs, coord, grad_keypoints, grad_volumes, grad_logit
     _check(lib().lt_test_softargmax3d_bwd_host(_host_ptr(probs), _host_ptr(coord), _host_ptr(grad_keypoints), _host_ptr(grad_volumes),
                                                _host_ptr(grad_logits), B, J, nvox, float(multiplier), int(mode)),
            "lt_test_softargmax3d_bwd_host")
+
+
+def unproject_aggregate_bwd_geom_host(features, proj, coord, conf, grad_out, grad_features, grad_conf, grad_proj, grad_coord, agg):
+    """lt_test_unproject_aggregate_bwd_geom_host: the geometry variant's per-item code and the q / dP / dX arithmetic run on CPU tensors
+    (test hook, no GPU needed).  Shapes as unproject_aggregate_bwd_geom."""
+    B, V, h, w, C = features.shape
+    nvox = coord.shape[1]
+    _check(lib().lt_test_unproject_aggregate_bwd_geom_host(_host_ptr(features), _host_ptr(proj), _host_ptr(coord), _host_ptr(conf),
+                                                           _host_ptr(grad_out), _host_ptr(grad_features), _host_ptr(grad_conf),
+                                                           _host_ptr(grad_proj), _host_ptr(grad_coord), B, V, C, h, w, nvox, agg),
+           "lt_test_unproject_aggregate_bwd_geom_host")
+
+
+def softargmax3d_coord_bwd_host(probs, grad_keypoints, grad_coord):
+    """lt_test_softargmax3d_coord_bwd_host: the coordinate gradient's per-item code on CPU tensors (test hook)."""
+    B, J, nvox = probs.shape
+    _check(lib().lt_test_softargmax3d_coord_bwd_host(_host_ptr(probs), _host_ptr(grad_keypoints), _host_ptr(grad_coord), B, J, nvox),
+           "lt_test_softargmax3d_coord_bwd_host")
+
+
+def triangulate_dlt_proj_bwd_host(proj, kp2d, conf, grad_out, grad_proj):
+    """lt_test_triangulate_dlt_proj_bwd_host: the projection gradient's per-item and merge code on CPU tensors (test hook)."""
+    B, V, J = kp2d.shape[:3]
+    _check(lib().lt_test_triangulate_dlt_proj_bwd_host(_host_ptr(proj), _host_ptr(kp2d), _host_ptr(conf), _host_ptr(grad_out),
+                                                       _host_ptr(grad_proj), B, V, J), "lt_test_triangulate_dlt_proj_bwd_host")
 
 
 def nchw_to_nhwc(inp, out, N, C, H, W, Cp):

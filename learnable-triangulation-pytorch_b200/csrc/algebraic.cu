@@ -1,9 +1,11 @@
 // Small kernels of the algebraic-triangulation path and the confidence heads (SURVEY section 8f rows 2 and 4):
 //   - global-average-pool + 3-layer MLP + sigmoid tail of GlobalAveragePoolingHead (pose_resnet.py:163-174)
 //   - normalisation of per-view confidences (triangulation.py:173-174, :268-269)
-//   - confidence-weighted DLT triangulation (multiview.py:141-183) and its backward, one thread per (sample, joint)
+//   - confidence-weighted DLT triangulation (multiview.py:141-183) and its backward, one thread per (sample, joint); the
+//     projection-matrix gradient as per-(sample, joint) partials summed over the joints in a fixed order
 #include "common.cuh"
 #include <math.h>
+#include <stdlib.h>
 
 namespace lt {
 
@@ -189,15 +191,16 @@ constexpr double kDltGapFloor = 1e-30;
 //   X = u[0:3] / u[3]  ->  g_u = [g_X / u[3], -(g_X . u[0:3]) / u[3]^2]
 //   w = sum_{k != 0} (g_u . e_k) / (lambda_0 - lambda_k) e_k          (first-order perturbation of the eigenvector)
 //   G_A = A (w u^T + u w^T): row r of A gets (a_r . w) u + (a_r . u) w
-//   d x = c (G_A[r0] . P[2]),  d y = c (G_A[r1] . P[2]),  d c = G_A[r0] . (x P[2] - P[0]) + G_A[r1] . (y P[2] - P[1]).
+//   d x = c (G_A[r0] . P[2]),  d y = c (G_A[r1] . P[2]),  d c = G_A[r0] . (x P[2] - P[0]) + G_A[r1] . (y P[2] - P[1]),
+//   d P[0] = -c G_A[r0],  d P[1] = -c G_A[r1],  d P[2] = c (x G_A[r0] + y G_A[r1])   (the float32 rounding of the rows as identity).
 // Independent of the sign of u.  A term whose gap is a tie by the rule above (kDltTieTol) is dropped: on an exact tie the
 // derivative does not exist (torch's SVD backward returns non-finite values there); dropping keeps it finite.
-// grad_kp / grad_conf are WRITTEN (every (v, j) of the item), grad_conf may be null.
-__host__ __device__ __forceinline__ void dlt_bwd_item(const float* __restrict__ proj, const float* __restrict__ kp2d,
-                                                      const float* __restrict__ conf, const float* __restrict__ grad_out,
-                                                      float* __restrict__ grad_kp, float* __restrict__ grad_conf, int b, int j,
-                                                      int V, int J) {
-  double M[4][4], E[4][4], u[4];
+// dlt_perturbation gives u and w of item (b, j); dlt_row_grads the rows G_A[r0], G_A[r1] of view v.  Both item functions below
+// use them, so the key-point, confidence and projection gradients follow one derivation.
+__host__ __device__ __forceinline__ void dlt_perturbation(const float* __restrict__ proj, const float* __restrict__ kp2d,
+                                                          const float* __restrict__ conf, const float* __restrict__ grad_out, int b, int j,
+                                                          int V, int J, double u[4], double w[4]) {
+  double M[4][4], E[4][4];
   const int m = dlt_eigen(proj, kp2d, conf, b, j, V, J, M, E);
   dlt_column(E, m, u);
   double lam0 = M[0][0], lmax = fabs(M[0][0]);
@@ -210,7 +213,8 @@ __host__ __device__ __forceinline__ void dlt_bwd_item(const float* __restrict__ 
   const double gx = grad_out[bj * 3], gy = grad_out[bj * 3 + 1], gz = grad_out[bj * 3 + 2];
   const double iw = 1.0 / u[3];
   const double gu[4] = {gx * iw, gy * iw, gz * iw, -(gx * u[0] + gy * u[1] + gz * u[2]) * iw * iw};
-  double w[4] = {0.0, 0.0, 0.0, 0.0};
+#pragma unroll
+  for (int r = 0; r < 4; ++r) w[r] = 0.0;
 #pragma unroll
   for (int k = 0; k < 4; ++k) {
     const double gap = lam0 - M[k][k];
@@ -219,30 +223,49 @@ __host__ __device__ __forceinline__ void dlt_bwd_item(const float* __restrict__ 
 #pragma unroll
     for (int r = 0; r < 4; ++r) w[r] += s * E[r][k];
   }
+}
+
+// G_A rows g0 (from x) and g1 (from y) of view P with key point (x, y) and confidence cf
+__host__ __device__ __forceinline__ void dlt_row_grads(const float* P, float x, float y, float cf, const double u[4], const double w[4],
+                                                       double g0[4], double g1[4]) {
+  double a0[4], a1[4];
+  dlt_rows(P, x, y, cf, a0, a1);
+  double aw0 = 0.0, au0 = 0.0, aw1 = 0.0, au1 = 0.0;
+#pragma unroll
+  for (int c = 0; c < 4; ++c) {
+    aw0 += a0[c] * w[c]; au0 += a0[c] * u[c];
+    aw1 += a1[c] * w[c]; au1 += a1[c] * u[c];
+  }
+#pragma unroll
+  for (int c = 0; c < 4; ++c) {
+    g0[c] = aw0 * u[c] + au0 * w[c];
+    g1[c] = aw1 * u[c] + au1 * w[c];
+  }
+}
+
+// grad_kp / grad_conf are WRITTEN (every (v, j) of the item), grad_conf may be null.
+__host__ __device__ __forceinline__ void dlt_bwd_item(const float* __restrict__ proj, const float* __restrict__ kp2d,
+                                                      const float* __restrict__ conf, const float* __restrict__ grad_out,
+                                                      float* __restrict__ grad_kp, float* __restrict__ grad_conf, int b, int j,
+                                                      int V, int J) {
+  double u[4], w[4];
+  dlt_perturbation(proj, kp2d, conf, grad_out, b, j, V, J, u, w);
   for (int v = 0; v < V; ++v) {
     const float* P = proj + ((long)b * V + v) * 12;
     const long vj = ((long)b * V + v) * J + j;
     const float x = kp2d[vj * 2], y = kp2d[vj * 2 + 1];
     const float cf = conf ? conf[vj] : 1.0f;
-    double a0[4], a1[4];
-    dlt_rows(P, x, y, cf, a0, a1);
-    double aw0 = 0.0, au0 = 0.0, aw1 = 0.0, au1 = 0.0;
-#pragma unroll
-    for (int c = 0; c < 4; ++c) {
-      aw0 += a0[c] * w[c]; au0 += a0[c] * u[c];
-      aw1 += a1[c] * w[c]; au1 += a1[c] * u[c];
-    }
     double g0[4], g1[4], dx = 0.0, dy = 0.0;
+    dlt_row_grads(P, x, y, cf, u, w, g0, g1);
 #pragma unroll
     for (int c = 0; c < 4; ++c) {
-      g0[c] = aw0 * u[c] + au0 * w[c];
-      g1[c] = aw1 * u[c] + au1 * w[c];
       dx += g0[c] * (double)P[8 + c];
       dy += g1[c] * (double)P[8 + c];
     }
     grad_kp[vj * 2] = (float)(cf * dx);
     grad_kp[vj * 2 + 1] = (float)(cf * dy);
     if (grad_conf) {
+      double a0[4], a1[4];
       dlt_rows(P, x, y, 1.0f, a0, a1);
       double dc = 0.0;
 #pragma unroll
@@ -252,6 +275,37 @@ __host__ __device__ __forceinline__ void dlt_bwd_item(const float* __restrict__ 
   }
 }
 
+// d P of item (b, j), float64, WRITTEN to partial[((b J + j) V + v) 12 + e] for every view
+__host__ __device__ __forceinline__ void dlt_proj_bwd_item(const float* __restrict__ proj, const float* __restrict__ kp2d,
+                                                           const float* __restrict__ conf, const float* __restrict__ grad_out,
+                                                           double* __restrict__ partial, int b, int j, int V, int J) {
+  double u[4], w[4];
+  dlt_perturbation(proj, kp2d, conf, grad_out, b, j, V, J, u, w);
+  for (int v = 0; v < V; ++v) {
+    const float* P = proj + ((long)b * V + v) * 12;
+    const long vj = ((long)b * V + v) * J + j;
+    const double x = kp2d[vj * 2], y = kp2d[vj * 2 + 1];
+    const float cf = conf ? conf[vj] : 1.0f;
+    double g0[4], g1[4];
+    dlt_row_grads(P, (float)x, (float)y, cf, u, w, g0, g1);
+    double* d = partial + (((long)b * J + j) * V + v) * 12;
+#pragma unroll
+    for (int c = 0; c < 4; ++c) {
+      d[c] = -(double)cf * g0[c];
+      d[4 + c] = -(double)cf * g1[c];
+      d[8 + c] = (double)cf * (x * g0[c] + y * g1[c]);
+    }
+  }
+}
+
+// d P[b][v][e] = sum_j partial (joints in order)
+__host__ __device__ __forceinline__ void dlt_proj_merge_item(const double* __restrict__ partial, float* __restrict__ grad_proj, int V, int J,
+                                                             int b, int v, int e) {
+  double s = 0.0;
+  for (int j = 0; j < J; ++j) s += partial[(((long)b * J + j) * V + v) * 12 + e];
+  grad_proj[((long)b * V + v) * 12 + e] = (float)s;
+}
+
 __global__ void __launch_bounds__(128) triangulate_dlt_bwd_kernel(const float* __restrict__ proj, const float* __restrict__ kp2d,
                                                                   const float* __restrict__ conf, const float* __restrict__ grad_out,
                                                                   float* __restrict__ grad_kp, float* __restrict__ grad_conf, int B,
@@ -259,6 +313,21 @@ __global__ void __launch_bounds__(128) triangulate_dlt_bwd_kernel(const float* _
   const int idx = blockIdx.x * blockDim.x + threadIdx.x;
   if (idx >= B * J) return;
   dlt_bwd_item(proj, kp2d, conf, grad_out, grad_kp, grad_conf, idx / J, idx % J, V, J);
+}
+
+__global__ void __launch_bounds__(128) triangulate_dlt_proj_bwd_kernel(const float* __restrict__ proj, const float* __restrict__ kp2d,
+                                                                       const float* __restrict__ conf, const float* __restrict__ grad_out,
+                                                                       double* __restrict__ partial, int B, int V, int J) {
+  const int idx = blockIdx.x * blockDim.x + threadIdx.x;
+  if (idx >= B * J) return;
+  dlt_proj_bwd_item(proj, kp2d, conf, grad_out, partial, idx / J, idx % J, V, J);
+}
+
+__global__ void __launch_bounds__(128) triangulate_dlt_proj_merge_kernel(const double* __restrict__ partial, float* __restrict__ grad_proj,
+                                                                         int B, int V, int J) {
+  const int idx = blockIdx.x * blockDim.x + threadIdx.x;
+  if (idx >= B * V * 12) return;
+  dlt_proj_merge_item(partial, grad_proj, V, J, idx / (V * 12), (idx / 12) % V, idx % 12);
 }
 
 }  // namespace lt
@@ -302,6 +371,24 @@ extern "C" int lt_triangulate_dlt_bwd(const float* proj, const float* keypoints_
   return LT_OK;
 }
 
+extern "C" size_t lt_triangulate_dlt_proj_bwd_workspace_bytes(int B, int V, int J) {
+  return (B > 0 && V > 0 && J > 0) ? (size_t)B * J * V * 12 * sizeof(double) : 0;
+}
+
+extern "C" int lt_triangulate_dlt_proj_bwd(const float* proj, const float* keypoints_2d, const float* confidences, const float* grad_out,
+                                           float* grad_proj, void* workspace, size_t workspace_bytes, int B, int V, int J, void* stream) {
+  LT_REQUIRE(proj && keypoints_2d && grad_out && grad_proj && workspace && B > 0 && V > 0 && J > 0, "triangulate_dlt_proj_bwd: bad arguments");
+  LT_REQUIRE(workspace_bytes >= lt_triangulate_dlt_proj_bwd_workspace_bytes(B, V, J), "triangulate_dlt_proj_bwd: workspace of %zu bytes, %zu needed",
+             workspace_bytes, lt_triangulate_dlt_proj_bwd_workspace_bytes(B, V, J));
+  double* partial = static_cast<double*>(workspace);
+  cudaStream_t st = (cudaStream_t)stream;
+  triangulate_dlt_proj_bwd_kernel<<<ceil_div((long)B * J, 128), 128, 0, st>>>(proj, keypoints_2d, confidences, grad_out, partial, B, V, J);
+  LT_CHECK_LAUNCH("triangulate_dlt_proj_bwd_kernel");
+  triangulate_dlt_proj_merge_kernel<<<ceil_div((long)B * V * 12, 128), 128, 0, st>>>(partial, grad_proj, B, V, J);
+  LT_CHECK_LAUNCH("triangulate_dlt_proj_merge_kernel");
+  return LT_OK;
+}
+
 // test hooks: the forward's and the backward's per-item code on the CPU (host pointers), for the `-m "not gpu"` tests
 extern "C" int lt_test_triangulate_dlt_fwd_host(const float* proj, const float* keypoints_2d, const float* confidences, float* out,
                                                 int B, int V, int J) {
@@ -318,5 +405,19 @@ extern "C" int lt_test_triangulate_dlt_bwd_host(const float* proj, const float* 
              "test_triangulate_dlt_bwd_host: bad arguments");
   for (int b = 0; b < B; ++b)
     for (int j = 0; j < J; ++j) dlt_bwd_item(proj, keypoints_2d, confidences, grad_out, grad_keypoints_2d, grad_confidences, b, j, V, J);
+  return LT_OK;
+}
+
+extern "C" int lt_test_triangulate_dlt_proj_bwd_host(const float* proj, const float* keypoints_2d, const float* confidences,
+                                                     const float* grad_out, float* grad_proj, int B, int V, int J) {
+  LT_REQUIRE(proj && keypoints_2d && grad_out && grad_proj && B > 0 && V > 0 && J > 0, "test_triangulate_dlt_proj_bwd_host: bad arguments");
+  double* partial = static_cast<double*>(malloc(lt_triangulate_dlt_proj_bwd_workspace_bytes(B, V, J)));
+  LT_REQUIRE(partial, "test_triangulate_dlt_proj_bwd_host: out of memory");
+  for (int b = 0; b < B; ++b)
+    for (int j = 0; j < J; ++j) dlt_proj_bwd_item(proj, keypoints_2d, confidences, grad_out, partial, b, j, V, J);
+  for (int b = 0; b < B; ++b)
+    for (int v = 0; v < V; ++v)
+      for (int e = 0; e < 12; ++e) dlt_proj_merge_item(partial, grad_proj, V, J, b, v, e);
+  free(partial);
   return LT_OK;
 }

@@ -3,8 +3,9 @@
 // `total_loss.backward()` (train.py:236) needs from op.unproject_heatmaps (op.py:99-166) and
 // op.integrate_tensor_3d_with_coordinates (op.py:84-96) when they run on the native kernels inside the torch training
 // graph (`backend="hybrid"`: torch convolutions, native custom ops).  Gradients flow to the feature maps (and to the
-// per-view confidences of the `conf` aggregation) and to the V2V logits; projection matrices and coordinate volumes carry
-// no gradient in the reference either (they are built from numpy inputs).
+// per-view confidences of the `conf` aggregation) and to the V2V logits.  The models build their geometry from numpy, but the
+// op-level drop-ins differentiate projection matrices and coordinate volumes like the reference's torch graph does, so the
+// geometry variant below (lt_unproject_aggregate_bwd_geom) and lt_softargmax3d_coord_bwd give those gradients too.
 //
 // Unprojection backward (HBM / atomics bound): one thread per (voxel, 4 channels) recomputes the four bilinear taps of every
 // view exactly as the forward does, re-aggregates, forms the per-view sample gradient
@@ -19,6 +20,7 @@
 // The DLT backward of the algebraic model is in algebraic.cu (it shares the forward's eigen-solve).
 #include "common.cuh"
 #include <math.h>
+#include <stdlib.h>
 
 // The per-item bodies are __host__ __device__: the kernels run them on the GPU, and lt_test_*_bwd_host (bottom of the file)
 // runs the SAME code on the CPU so that `-m "not gpu"` tests can check the gradient arithmetic against torch autograd
@@ -36,8 +38,18 @@ struct BwdTaps {
   float w[4];     // bilinear weight, 0 where the tap is outside the map or the depth test failed
 };
 
-// identical arithmetic to make_taps() in unproject.cu (op.py:116-135, multiview.py:89-110)
-__host__ __device__ __forceinline__ BwdTaps bwd_taps(const float* __restrict__ P, float X, float Y, float Z, int h, int w) {
+// What the geometry gradient needs of one (voxel, view) beyond the taps: the tap validity (a tap with weight 0 can still carry
+// a derivative), d w_k / d ix and d w_k / d iy of the taps inside the map (torch's grid_sampler_2d_backward convention: the same
+// floor cell, also at integer positions and at border taps), the projected position and the depth.
+struct GeomTaps {
+  float dx[4], dy[4];   // 0 where the tap is outside the map or the depth test failed
+  float x, y, pz;       // pz after the 0 -> 1 replacement
+  bool live;            // depth test passed and at least one tap is inside the map
+};
+
+// identical arithmetic to make_taps() in unproject.cu (op.py:116-135, multiview.py:89-110); kGeom also fills *gt
+template <bool kGeom>
+__host__ __device__ __forceinline__ BwdTaps bwd_taps_impl(const float* __restrict__ P, float X, float Y, float Z, int h, int w, GeomTaps* gt) {
   BwdTaps t;
   float px = fmaf(Z, P[2], fmaf(Y, P[1], X * P[0])) + P[3];
   float py = fmaf(Z, P[6], fmaf(Y, P[5], X * P[4])) + P[7];
@@ -62,7 +74,20 @@ __host__ __device__ __forceinline__ BwdTaps bwd_taps(const float* __restrict__ P
   t.w[1] = (depth_ok && vx1 && vy0) ? (ix - x0) * (y1 - iy) : 0.0f;
   t.w[2] = (depth_ok && vx0 && vy1) ? (x1 - ix) * (iy - y0) : 0.0f;
   t.w[3] = (depth_ok && vx1 && vy1) ? (ix - x0) * (iy - y0) : 0.0f;
+  if (kGeom) {
+    const bool in[4] = {depth_ok && vx0 && vy0, depth_ok && vx1 && vy0, depth_ok && vx0 && vy1, depth_ok && vx1 && vy1};
+    const float ddx[4] = {-(y1 - iy), y1 - iy, -(iy - y0), iy - y0};
+    const float ddy[4] = {-(x1 - ix), -(ix - x0), x1 - ix, ix - x0};
+#pragma unroll
+    for (int k = 0; k < 4; ++k) { gt->dx[k] = in[k] ? ddx[k] : 0.0f; gt->dy[k] = in[k] ? ddy[k] : 0.0f; }
+    gt->x = x; gt->y = y; gt->pz = pz;
+    gt->live = in[0] || in[1] || in[2] || in[3];
+  }
   return t;
+}
+
+__host__ __device__ __forceinline__ BwdTaps bwd_taps(const float* __restrict__ P, float X, float Y, float Z, int h, int w) {
+  return bwd_taps_impl<false>(P, X, Y, Z, h, w, nullptr);
 }
 
 __host__ __device__ __forceinline__ float4 sample4(const float* __restrict__ fmap, int C, int c0, const BwdTaps& t) {
@@ -98,6 +123,32 @@ __host__ __device__ __forceinline__ void scatter4(float* __restrict__ gmap, int 
       red_add_v4(gmap + (long)t.o[k] * C + c0, make_float4(gs.x * t.w[k], gs.y * t.w[k], gs.z * t.w[k], gs.w * t.w[k]));
 }
 
+// (G_ix, G_iy) of one 4-channel quad: sum_c gs_c d s_c / d ix and d s_c / d iy over the taps inside the map
+__host__ __device__ __forceinline__ float2 geom_partial(const float* __restrict__ fmap, int C, int c0, const BwdTaps& t, const GeomTaps& gt,
+                                                        float4 gs) {
+  float gix = 0.0f, giy = 0.0f;
+#pragma unroll
+  for (int k = 0; k < 4; ++k)
+    if (gt.dx[k] != 0.0f || gt.dy[k] != 0.0f) {
+      const float4 q = LT_LD(reinterpret_cast<const float4*>(fmap + (long)t.o[k] * C + c0));
+      const float d = fmaf(gs.w, q.w, fmaf(gs.z, q.z, fmaf(gs.y, q.y, gs.x * q.x)));
+      gix = fmaf(gt.dx[k], d, gix);
+      giy = fmaf(gt.dy[k], d, giy);
+    }
+  return make_float2(gix, giy);
+}
+
+// q = dL/dp of p = P [X, 1] from the voxel's (G_ix, G_iy) summed over all channels: G_x = G_ix (w - 1) / h, G_y = G_iy (h - 1) / w
+// (ix = x / h (w - 1), iy = y / w (h - 1)), then through x = px / pz, y = py / pz.  Exactly 0 for a voxel that fails the depth test
+// or has no tap inside the map (pz may be 2^-60 there: no inf * 0).
+__host__ __device__ __forceinline__ void geom_q(const GeomTaps& gt, float gix, float giy, int h, int w, float q[3]) {
+  if (!gt.live) { q[0] = q[1] = q[2] = 0.0f; return; }
+  const float gx = gix * ((float)(w - 1) / (float)h), gy = giy * ((float)(h - 1) / (float)w);
+  q[0] = gx / gt.pz;
+  q[1] = gy / gt.pz;
+  q[2] = -fmaf(gx, gt.x, gy * gt.y) / gt.pz;
+}
+
 struct UnprojBwdParams {
   const float* features;   // [B][V][h][w][C]
   const float* proj;       // [B][V][12]
@@ -108,12 +159,40 @@ struct UnprojBwdParams {
   float* grad_conf;        // [B][V][C] or null, accumulated into
   int B, V, C, h, w, agg;
   long nvox;
+  float* geom_q;           // geometry variant: [B][V][nvox][3] q per (sample, view, voxel), written (the host hook accumulates
+                           // (G_ix, G_iy) into its first two slots instead and forms q afterwards)
 };
 
 constexpr int kBwdSmemViews = 64;
 
+// The quad's (G_ix, G_iy) of view v, summed over the C / 4 quads of the voxel.  GPU: those are C / 4 adjacent lanes of one warp
+// (C / 4 is a power of two <= 32, the grid stride a multiple of 32 and the item count a multiple of C / 4), summed by a fixed
+// butterfly; the voxel's first quad forms q and writes it.  Host: items run in order, so (G_ix, G_iy) accumulates in place.
+__host__ __device__ __forceinline__ void geom_emit(const UnprojBwdParams& p, int b, int v, long vox, int quad, const GeomTaps& gt, float2 G) {
+  float* dst = p.geom_q + (((long)b * p.V + v) * p.nvox + vox) * 3;
+#ifdef __CUDA_ARCH__
+  const int quads = p.C >> 2;
+  const unsigned lane = threadIdx.x & 31;
+  const unsigned mask = quads == 32 ? 0xffffffffu : (((1u << quads) - 1u) << (lane & ~(unsigned)(quads - 1)));
+  for (int o = 1; o < quads; o <<= 1) {
+    G.x += __shfl_xor_sync(mask, G.x, o);
+    G.y += __shfl_xor_sync(mask, G.y, o);
+  }
+  if (quad == 0) {
+    float q[3];
+    geom_q(gt, G.x, G.y, p.h, p.w, q);
+    dst[0] = q[0]; dst[1] = q[1]; dst[2] = q[2];
+  }
+#else
+  (void)gt; (void)quad;
+  dst[0] += G.x; dst[1] += G.y;
+#endif
+}
+
 // one (voxel, 4-channel quad) of sample b.  projs: the sample's first kBwdSmemViews projection matrices (shared memory on
-// the GPU) or null; gconf_acc: [V][C] accumulator of d conf (shared memory on the GPU, the output itself on the host) or null
+// the GPU) or null; gconf_acc: [V][C] accumulator of d conf (shared memory on the GPU, the output itself on the host) or null.
+// kGeom also hands every view's (G_ix, G_iy) to geom_emit, once per view on every path (the GPU lanes of a voxel meet there).
+template <bool kGeom>
 __host__ __device__ __forceinline__ void unproject_bwd_item(const UnprojBwdParams& p, int b, long it, const float* projs, float* gconf_acc) {
   const int quads = p.C >> 2;
   const long map_elems = (long)p.h * p.w * p.C;
@@ -130,7 +209,8 @@ __host__ __device__ __forceinline__ void unproject_bwd_item(const UnprojBwdParam
 
     if (p.agg == LT_AGG_SUM || p.agg == LT_AGG_CONF) {
       for (int v = 0; v < p.V; ++v) {
-        const BwdTaps t = bwd_taps(view_proj(v), X, Y, Z, p.h, p.w);
+        GeomTaps gt;
+        const BwdTaps t = bwd_taps_impl<kGeom>(view_proj(v), X, Y, Z, p.h, p.w, &gt);
         float4 gs = g;
         if (p.agg == LT_AGG_CONF) {
           const float4 cf = LT_LD(reinterpret_cast<const float4*>(p.conf + ((long)b * p.V + v) * p.C + c0));
@@ -142,6 +222,7 @@ __host__ __device__ __forceinline__ void unproject_bwd_item(const UnprojBwdParam
           gs = make_float4(g.x * cf.x, g.y * cf.y, g.z * cf.z, g.w * cf.w);
         }
         scatter4(gb + v * map_elems, p.C, c0, t, gs);
+        if (kGeom) geom_emit(p, b, v, vox, c0 >> 2, gt, geom_partial(fb + v * map_elems, p.C, c0, t, gt, gs));
       }
     } else if (p.agg == LT_AGG_MAX) {
       // torch.max(dim=0) routes the gradient to the first view that attains the maximum
@@ -156,8 +237,14 @@ __host__ __device__ __forceinline__ void unproject_bwd_item(const UnprojBwdParam
       }
       for (int v = 0; v < p.V; ++v) {
         const float4 gs = make_float4(v == ax ? g.x : 0.f, v == ay ? g.y : 0.f, v == az ? g.z : 0.f, v == aw ? g.w : 0.f);
-        if (gs.x != 0.f || gs.y != 0.f || gs.z != 0.f || gs.w != 0.f)
+        if (kGeom) {
+          GeomTaps gt;
+          const BwdTaps t = bwd_taps_impl<true>(view_proj(v), X, Y, Z, p.h, p.w, &gt);
+          if (gs.x != 0.f || gs.y != 0.f || gs.z != 0.f || gs.w != 0.f) scatter4(gb + v * map_elems, p.C, c0, t, gs);
+          geom_emit(p, b, v, vox, c0 >> 2, gt, geom_partial(fb + v * map_elems, p.C, c0, t, gt, gs));
+        } else if (gs.x != 0.f || gs.y != 0.f || gs.z != 0.f || gs.w != 0.f) {
           scatter4(gb + v * map_elems, p.C, c0, bwd_taps(view_proj(v), X, Y, Z, p.h, p.w), gs);
+        }
       }
     } else {
       // softmax over views: out = sum_v s_v p_v;  d out / d s_v = p_v (1 + s_v - out).  Three passes over the views
@@ -176,17 +263,21 @@ __host__ __device__ __forceinline__ void unproject_bwd_item(const UnprojBwdParam
       }
       const float4 out = make_float4(num.x / den.x, num.y / den.y, num.z / den.z, num.w / den.w);
       for (int v = 0; v < p.V; ++v) {
-        const BwdTaps t = bwd_taps(view_proj(v), X, Y, Z, p.h, p.w);
+        GeomTaps gt;
+        const BwdTaps t = bwd_taps_impl<kGeom>(view_proj(v), X, Y, Z, p.h, p.w, &gt);
         const float4 s = sample4(fb + v * map_elems, p.C, c0, t);
         const float4 gs = make_float4(g.x * (expf(s.x - m.x) / den.x) * (1.0f + s.x - out.x), g.y * (expf(s.y - m.y) / den.y) * (1.0f + s.y - out.y),
                                       g.z * (expf(s.z - m.z) / den.z) * (1.0f + s.z - out.z), g.w * (expf(s.w - m.w) / den.w) * (1.0f + s.w - out.w));
         scatter4(gb + v * map_elems, p.C, c0, t, gs);
+        if (kGeom) geom_emit(p, b, v, vox, c0 >> 2, gt, geom_partial(fb + v * map_elems, p.C, c0, t, gt, gs));
       }
     }
   }
 }
 
-__global__ void __launch_bounds__(256) unproject_bwd_kernel(const UnprojBwdParams p) {
+// the body of unproject_bwd_kernel (kGeom = false) and unproject_bwd_geom_kernel (true)
+template <bool kGeom>
+__device__ __forceinline__ void unproject_bwd_body(const UnprojBwdParams& p) {
   __shared__ float sP[kBwdSmemViews * 12];
   extern __shared__ float sConf[];          // [V][C] block-level accumulator of d conf (only with grad_conf)
   const int b = blockIdx.y;
@@ -197,11 +288,104 @@ __global__ void __launch_bounds__(256) unproject_bwd_kernel(const UnprojBwdParam
   __syncthreads();
   const long items = p.nvox * (p.C >> 2);
   for (long it = (long)blockIdx.x * blockDim.x + threadIdx.x; it < items; it += (long)gridDim.x * blockDim.x)
-    unproject_bwd_item(p, b, it, sP, want_gconf ? sConf : nullptr);
+    unproject_bwd_item<kGeom>(p, b, it, sP, want_gconf ? sConf : nullptr);
   if (want_gconf) {
     __syncthreads();
     for (int i = threadIdx.x; i < p.V * p.C; i += blockDim.x) atomicAdd(p.grad_conf + (long)b * p.V * p.C + i, sConf[i]);
   }
+}
+
+__global__ void __launch_bounds__(256) unproject_bwd_kernel(const UnprojBwdParams p) { unproject_bwd_body<false>(p); }
+__global__ void __launch_bounds__(256) unproject_bwd_geom_kernel(const UnprojBwdParams p) { unproject_bwd_body<true>(p); }
+
+// ---- second pass of the geometry gradient: deterministic sums of q (no float atomics) ----
+// dP_v[r][:] = sum_voxels q_r [X, Y, Z, 1]: fixed voxel chunks per CTA summed in float64 (fixed butterfly, warps in order), the
+// chunks merged in order.  dX = sum_v sum_r q_r P_v[r][0:3] per voxel, views in order.
+constexpr int kGeomChunk = 8192;        // voxels per dP partial
+constexpr int kGeomThreads = 256;
+
+__host__ __device__ __forceinline__ int geom_chunks(long nvox) { return (int)((nvox + kGeomChunk - 1) / kGeomChunk); }
+
+// the 12 float64 terms voxel `vox` adds to dP of (b, v)
+__host__ __device__ __forceinline__ void geom_dp_terms(const float* __restrict__ coord, const float* __restrict__ q, long nvox, int b,
+                                                       int bv, long vox, double t[12]) {
+  const float* cp = coord + ((long)b * nvox + vox) * 3;
+  const float* qp = q + ((long)bv * nvox + vox) * 3;
+  const double X4[4] = {(double)LT_LD(cp), (double)LT_LD(cp + 1), (double)LT_LD(cp + 2), 1.0};
+#pragma unroll
+  for (int r = 0; r < 3; ++r) {
+    const double qr = (double)LT_LD(qp + r);
+#pragma unroll
+    for (int c = 0; c < 4; ++c) t[r * 4 + c] = qr * X4[c];
+  }
+}
+
+__host__ __device__ __forceinline__ void geom_dx_item(const float* __restrict__ proj, const float* __restrict__ q, float* __restrict__ grad_coord,
+                                                      int V, long nvox, int b, long vox) {
+  float d[3] = {0.0f, 0.0f, 0.0f};
+  for (int v = 0; v < V; ++v) {
+    const float* P = proj + ((long)b * V + v) * 12;
+    const float* qp = q + (((long)b * V + v) * nvox + vox) * 3;
+#pragma unroll
+    for (int r = 0; r < 3; ++r) {
+      const float qr = LT_LD(qp + r);
+#pragma unroll
+      for (int k = 0; k < 3; ++k) d[k] = fmaf(qr, LT_LD(P + r * 4 + k), d[k]);
+    }
+  }
+  float* out = grad_coord + ((long)b * nvox + vox) * 3;
+  out[0] = d[0]; out[1] = d[1]; out[2] = d[2];
+}
+
+__device__ __forceinline__ double warp_sum_f64(double v) {
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
+  return v;
+}
+
+// grid (chunks, B * V): partial[(bv * chunks + chunk) * 12 + e]
+__global__ void __launch_bounds__(kGeomThreads) unproject_geom_dp_partial_kernel(const float* __restrict__ coord, const float* __restrict__ q,
+                                                                                 double* __restrict__ partial, int V, long nvox) {
+  const int bv = blockIdx.y, b = bv / V, chunk = blockIdx.x;
+  const long v0 = (long)chunk * kGeomChunk, v1 = min(nvox, v0 + kGeomChunk);
+  double acc[12];
+#pragma unroll
+  for (int e = 0; e < 12; ++e) acc[e] = 0.0;
+  for (long vox = v0 + threadIdx.x; vox < v1; vox += kGeomThreads) {
+    double t[12];
+    geom_dp_terms(coord, q, nvox, b, bv, vox, t);
+#pragma unroll
+    for (int e = 0; e < 12; ++e) acc[e] += t[e];
+  }
+  __shared__ double sh[kGeomThreads / 32][12];
+#pragma unroll
+  for (int e = 0; e < 12; ++e) {
+    const double s = warp_sum_f64(acc[e]);
+    if ((threadIdx.x & 31) == 0) sh[threadIdx.x >> 5][e] = s;
+  }
+  __syncthreads();
+  if (threadIdx.x < 12) {
+    double s = 0.0;
+    for (int k = 0; k < kGeomThreads / 32; ++k) s += sh[k][threadIdx.x];
+    partial[((long)bv * gridDim.x + chunk) * 12 + threadIdx.x] = s;
+  }
+}
+
+// one thread per (b, v, e): the chunks in order
+__global__ void unproject_geom_dp_merge_kernel(const double* __restrict__ partial, float* __restrict__ grad_proj, int BV, int chunks) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= BV * 12) return;
+  const int bv = i / 12, e = i % 12;
+  double s = 0.0;
+  for (int k = 0; k < chunks; ++k) s += partial[((long)bv * chunks + k) * 12 + e];
+  grad_proj[i] = (float)s;
+}
+
+__global__ void __launch_bounds__(256) unproject_geom_dx_kernel(const float* __restrict__ proj, const float* __restrict__ q,
+                                                                float* __restrict__ grad_coord, int B, int V, long nvox) {
+  const long i = (long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= (long)B * nvox) return;
+  geom_dx_item(proj, q, grad_coord, V, nvox, (int)(i / nvox), i % nvox);
 }
 
 // ---- soft-argmax backward, NCDHW: volumes / logits / grads are [B][J][nvox] ----
@@ -293,6 +477,28 @@ __global__ void __launch_bounds__(256) softargmax_bwd_apply_kernel(const SoftBwd
   }
 }
 
+// d coord[b][i] = sum_j probs[b][j][i] g_kp[b][j] (kp = sum_i p_i x_i in modes 0 and 1), joints in order
+__host__ __device__ __forceinline__ void softargmax_coord_bwd_item(const float* __restrict__ probs, const float* __restrict__ g_kp,
+                                                                   float* __restrict__ grad_coord, int J, long nvox, int b, long i) {
+  float d[3] = {0.0f, 0.0f, 0.0f};
+  for (int j = 0; j < J; ++j) {
+    const float pi = LT_LD(probs + ((long)b * J + j) * nvox + i);
+    const float* g = g_kp + ((long)b * J + j) * 3;
+    d[0] = fmaf(pi, LT_LD(g), d[0]);
+    d[1] = fmaf(pi, LT_LD(g + 1), d[1]);
+    d[2] = fmaf(pi, LT_LD(g + 2), d[2]);
+  }
+  float* out = grad_coord + ((long)b * nvox + i) * 3;
+  out[0] = d[0]; out[1] = d[1]; out[2] = d[2];
+}
+
+__global__ void __launch_bounds__(256) softargmax_coord_bwd_kernel(const float* __restrict__ probs, const float* __restrict__ g_kp,
+                                                                   float* __restrict__ grad_coord, int J, long nvox) {
+  const int b = blockIdx.y;
+  for (long i = (long)blockIdx.x * blockDim.x + threadIdx.x; i < nvox; i += (long)gridDim.x * blockDim.x)
+    softargmax_coord_bwd_item(probs, g_kp, grad_coord, J, nvox, b, i);
+}
+
 }  // namespace lt
 
 using namespace lt;
@@ -315,6 +521,66 @@ extern "C" int lt_unproject_aggregate_bwd(const float* features, const float* pr
   LT_REQUIRE(smem <= 40 * 1024, "unproject_bwd: V * C too large for the confidence-gradient accumulator");
   unproject_bwd_kernel<<<dim3((unsigned)blocks, (unsigned)B), 256, smem, (cudaStream_t)stream>>>(p);
   LT_CHECK_LAUNCH("unproject_bwd_kernel");
+  return LT_OK;
+}
+
+static size_t geom_q_bytes(int B, int V, long nvox) { return ((size_t)B * V * nvox * 3 * sizeof(float) + 255) & ~(size_t)255; }
+
+extern "C" size_t lt_unproject_aggregate_bwd_geom_workspace_bytes(int B, int V, long nvox) {
+  if (B <= 0 || V <= 0 || nvox <= 0) return 0;
+  return geom_q_bytes(B, V, nvox) + (size_t)B * V * geom_chunks(nvox) * 12 * sizeof(double);
+}
+
+extern "C" int lt_unproject_aggregate_bwd_geom(const float* features, const float* proj, const float* coord, const float* conf,
+                                               const float* grad_out, float* grad_features, float* grad_conf, float* grad_proj,
+                                               float* grad_coord, void* workspace, size_t workspace_bytes, int B, int V, int C, int h,
+                                               int w, long nvox, int agg, void* stream) {
+  LT_REQUIRE(features && proj && coord && grad_out && grad_features && workspace, "unproject_bwd_geom: null pointer");
+  LT_REQUIRE(B > 0 && V > 0 && C > 0 && h > 0 && w > 0 && nvox > 0, "unproject_bwd_geom: non-positive size");
+  LT_REQUIRE(C % 4 == 0 && C <= 128 && ((C / 4) & (C / 4 - 1)) == 0,
+             "unproject_bwd_geom: C / 4 must be a power of two <= 32 (the voxel's channel quads are summed within a warp), C=%d", C);
+  LT_REQUIRE(agg >= LT_AGG_SUM && agg <= LT_AGG_CONF, "unproject_bwd_geom: unknown aggregation %d", agg);
+  LT_REQUIRE(agg != LT_AGG_CONF || conf, "unproject_bwd_geom: LT_AGG_CONF needs confidences");
+  LT_REQUIRE(B <= 65535 && (long)B * V <= 65535, "unproject_bwd_geom: batch too large");
+  LT_REQUIRE(workspace_bytes >= lt_unproject_aggregate_bwd_geom_workspace_bytes(B, V, nvox),
+             "unproject_bwd_geom: workspace of %zu bytes, %zu needed", workspace_bytes, lt_unproject_aggregate_bwd_geom_workspace_bytes(B, V, nvox));
+  float* q = reinterpret_cast<float*>(workspace);
+  double* partial = reinterpret_cast<double*>(reinterpret_cast<char*>(workspace) + geom_q_bytes(B, V, nvox));
+  UnprojBwdParams p{features, proj, coord, conf, grad_out, grad_features, grad_conf, B, V, C, h, w, agg, nvox, q};
+  const long items = nvox * (C / 4);
+  long blocks = (items + 255) / 256;
+  const long cap = (long)sm_count() * 8;
+  if (blocks > cap) blocks = cap;
+  const size_t smem = (grad_conf && agg == LT_AGG_CONF) ? (size_t)V * C * sizeof(float) : 0;
+  LT_REQUIRE(smem <= 40 * 1024, "unproject_bwd_geom: V * C too large for the confidence-gradient accumulator");
+  cudaStream_t st = (cudaStream_t)stream;
+  unproject_bwd_geom_kernel<<<dim3((unsigned)blocks, (unsigned)B), 256, smem, st>>>(p);
+  LT_CHECK_LAUNCH("unproject_bwd_geom_kernel");
+  if (grad_proj) {
+    const int chunks = geom_chunks(nvox);
+    unproject_geom_dp_partial_kernel<<<dim3((unsigned)chunks, (unsigned)(B * V)), kGeomThreads, 0, st>>>(coord, q, partial, V, nvox);
+    LT_CHECK_LAUNCH("unproject_geom_dp_partial_kernel");
+    unproject_geom_dp_merge_kernel<<<ceil_div((long)B * V * 12, 128), 128, 0, st>>>(partial, grad_proj, B * V, chunks);
+    LT_CHECK_LAUNCH("unproject_geom_dp_merge_kernel");
+  }
+  if (grad_coord) {
+    unproject_geom_dx_kernel<<<ceil_div((long)B * nvox, 256), 256, 0, st>>>(proj, q, grad_coord, B, V, nvox);
+    LT_CHECK_LAUNCH("unproject_geom_dx_kernel");
+  }
+  return LT_OK;
+}
+
+extern "C" int lt_softargmax3d_coord_bwd(const float* probs, const float* grad_keypoints, float* grad_coord, int B, int J, long nvox,
+                                         int softmax, void* stream) {
+  LT_REQUIRE(probs && grad_keypoints && grad_coord, "softargmax3d_coord_bwd: null pointer");
+  LT_REQUIRE(B > 0 && J > 0 && nvox > 0 && B <= 65535, "softargmax3d_coord_bwd: bad sizes");
+  LT_REQUIRE(softmax == 0 || softmax == 1,
+             "softargmax3d_coord_bwd: mode must be 0 (ReLU) or 1 (softmax), got %d (mode 2, the 2-D op, has no coordinate input)", softmax);
+  long bx = (nvox + 255) / 256;
+  const long cap = (long)sm_count() * 8;
+  if (bx > cap) bx = cap;
+  softargmax_coord_bwd_kernel<<<dim3((unsigned)bx, (unsigned)B), 256, 0, (cudaStream_t)stream>>>(probs, grad_keypoints, grad_coord, J, nvox);
+  LT_CHECK_LAUNCH("softargmax_coord_bwd_kernel");
   return LT_OK;
 }
 
@@ -347,7 +613,52 @@ extern "C" int lt_test_unproject_aggregate_bwd_host(const float* features, const
   const long items = nvox * (C / 4);
   for (int b = 0; b < B; ++b)
     for (long it = 0; it < items; ++it)
-      unproject_bwd_item(p, b, it, nullptr, (grad_conf && agg == LT_AGG_CONF) ? grad_conf + (long)b * V * C : nullptr);
+      unproject_bwd_item<false>(p, b, it, nullptr, (grad_conf && agg == LT_AGG_CONF) ? grad_conf + (long)b * V * C : nullptr);
+  return LT_OK;
+}
+
+extern "C" int lt_test_unproject_aggregate_bwd_geom_host(const float* features, const float* proj, const float* coord, const float* conf,
+                                                         const float* grad_out, float* grad_features, float* grad_conf, float* grad_proj,
+                                                         float* grad_coord, int B, int V, int C, int h, int w, long nvox, int agg) {
+  LT_REQUIRE(features && proj && coord && grad_out && grad_features && C % 4 == 0 && B > 0 && V > 0 && nvox > 0,
+             "test_unproject_bwd_geom_host: bad arguments");
+  LT_REQUIRE(agg >= LT_AGG_SUM && agg <= LT_AGG_CONF && (agg != LT_AGG_CONF || conf), "test_unproject_bwd_geom_host: bad aggregation");
+  float* q = static_cast<float*>(calloc((size_t)B * V * nvox * 3, sizeof(float)));
+  LT_REQUIRE(q, "test_unproject_bwd_geom_host: out of memory");
+  UnprojBwdParams p{features, proj, coord, conf, grad_out, grad_features, grad_conf, B, V, C, h, w, agg, nvox, q};
+  const long items = nvox * (C / 4);
+  for (int b = 0; b < B; ++b)
+    for (long it = 0; it < items; ++it)
+      unproject_bwd_item<true>(p, b, it, nullptr, (grad_conf && agg == LT_AGG_CONF) ? grad_conf + (long)b * V * C : nullptr);
+  for (int b = 0; b < B; ++b)       // (G_ix, G_iy) -> q, as the voxel's first lane forms it on the GPU
+    for (int v = 0; v < V; ++v)
+      for (long vox = 0; vox < nvox; ++vox) {
+        const float* cp = coord + ((long)b * nvox + vox) * 3;
+        GeomTaps gt;
+        bwd_taps_impl<true>(proj + ((long)b * V + v) * 12, cp[0], cp[1], cp[2], h, w, &gt);
+        float* qp = q + (((long)b * V + v) * nvox + vox) * 3;
+        geom_q(gt, qp[0], qp[1], h, w, qp);
+      }
+  for (int bv = 0; grad_proj && bv < B * V; ++bv) {
+    double acc[12] = {0.0};
+    for (long vox = 0; vox < nvox; ++vox) {
+      double t[12];
+      geom_dp_terms(coord, q, nvox, bv / V, bv, vox, t);
+      for (int e = 0; e < 12; ++e) acc[e] += t[e];
+    }
+    for (int e = 0; e < 12; ++e) grad_proj[(long)bv * 12 + e] = (float)acc[e];
+  }
+  for (int b = 0; grad_coord && b < B; ++b)
+    for (long vox = 0; vox < nvox; ++vox) geom_dx_item(proj, q, grad_coord, V, nvox, b, vox);
+  free(q);
+  return LT_OK;
+}
+
+extern "C" int lt_test_softargmax3d_coord_bwd_host(const float* probs, const float* grad_keypoints, float* grad_coord, int B, int J,
+                                                   long nvox) {
+  LT_REQUIRE(probs && grad_keypoints && grad_coord && B > 0 && J > 0 && nvox > 0, "test_softargmax3d_coord_bwd_host: bad arguments");
+  for (int b = 0; b < B; ++b)
+    for (long i = 0; i < nvox; ++i) softargmax_coord_bwd_item(probs, grad_keypoints, grad_coord, J, nvox, b, i);
   return LT_OK;
 }
 
