@@ -405,10 +405,11 @@ int lt_volumetric_ce_bwd(const float* grad_loss, const int* index, const float* 
  *   x, residual, y, grad_* maps: float32 channels-last [M][C], M = N*D*H*W, C % 4 == 0, 16-byte aligned; residual may be NULL
  *   per-channel vectors [C]: gamma, beta, running_mean, running_var, save_mean, save_invstd
  * Forward: y = act(gamma * (x - mean) * invstd + beta (+ residual)), act = ReLU when relu != 0.  training != 0: mean and the biased
- * variance of the batch (M >= 2), save_invstd = 1 / sqrt(var + eps), and the running statistics updated in place as nn.BatchNorm does
+ * variance of the batch (M >= 2), save_invstd = 1 / sqrt(var + eps) (0 when var = eps = 0, as torch does), and the running statistics updated in place as nn.BatchNorm does
  * (running = (1 - momentum) * running + momentum * batch value, the variance unbiased by M / (M - 1)); training == 0: the running
  * statistics are used and left alone (save_mean / save_invstd still receive the values used).
- * Backward (the same relu / training; y is read only with relu, for the mask y > 0): g' = grad_y [y > 0];
+ * Backward (the same relu / training; y is read only with relu, for its mask): g' = grad_y [!(y <= 0)], torch's threshold_backward,
+ * so a NaN output passes its gradient; the forward's ReLU keeps NaN, as torch.relu does;
  *   grad_beta = sum g', grad_gamma = sum g' * xhat, xhat = (x - save_mean) * save_invstd;
  *   grad_x = gamma * save_invstd * (g' - sum g' / M - xhat * sum g' xhat / M) (training) or gamma * save_invstd * g' (eval);
  *   grad_residual = g' (NULL: not written); grad_gamma / grad_beta may be NULL.
@@ -416,6 +417,20 @@ int lt_volumetric_ce_bwd(const float* grad_loss, const int* index, const float* 
  * workspace: lt_batch_norm_workspace_bytes(M, C) bytes, for either direction.
  * ---------------------------------------------------------------------------------------- */
 size_t lt_batch_norm_workspace_bytes(long M, int C);
+/* Host-only launch plan of lt_batch_norm_fwd / _bwd for `sm_count` SMs (both launch from it with the device's count).  A CTA is tc x ry
+ * = up to 256 threads: tc threads over float4 columns of one channel block, ry rows at a time.  Reduce passes run cblocks x splits
+ * CTAs; split z takes rows [z rows_per_split, min((z + 1) rows_per_split, M)). */
+typedef struct lt_batch_norm_launch_plan {
+  int tc;                /* float4 columns per CTA: min(C / 4, 32) */
+  int ry;                /* rows per CTA step: 256 / tc */
+  int cblocks;           /* CTAs along the channels: ceil(C / 4 / tc) */
+  int want_splits;       /* row splits of one wave of 4 CTAs per SM: ceil(4 sm_count / cblocks) */
+  int max_splits;        /* row splits the workspace holds, independent of the device: min(ceil(M / (16 ry)), ceil(1024 / cblocks)) */
+  int splits;            /* row splits launched: ceil(M / rows_per_split) <= min(want_splits, max_splits) */
+  long rows_per_split;   /* ceil(M / min(want_splits, max_splits)) */
+  int row_blocks;        /* CTAs along M of an apply pass: about two waves, at most ceil(M / (4 ry)) */
+} lt_batch_norm_launch_plan;
+int lt_batch_norm_plan(long M, int C, int sm_count, lt_batch_norm_launch_plan* plan);
 int lt_batch_norm_fwd(const float* x, const float* residual, const float* gamma, const float* beta, float* running_mean, float* running_var,
                       float* save_mean, float* save_invstd, float* y, long M, int C, float eps, float momentum, int training, int relu,
                       void* workspace, size_t workspace_bytes, void* stream);

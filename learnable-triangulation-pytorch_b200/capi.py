@@ -46,6 +46,12 @@ class ConvWgradPlan(ctypes.Structure):
     _fields_ = [(n, c_int) for n in ("nwg", "ngroups", "m_tiles", "splits", "stages")]
 
 
+class BatchNormPlan(ctypes.Structure):
+    """Mirror of `struct lt_batch_norm_launch_plan` (include/lt_b200.h)."""
+    _fields_ = [(n, c_int) for n in ("tc", "ry", "cblocks", "want_splits", "max_splits", "splits")] + [("rows_per_split", c_long),
+                                                                                                        ("row_blocks", c_int)]
+
+
 class Options(ctypes.Structure):
     """Mirror of `struct lt_options` (include/lt_b200.h): kernel-selection switches, all defaulting to the measured-best path."""
     _fields_ = [(n, c_int) for n in ("tc_persist", "tc_splitk", "tc_bres", "tc_direct_epilogue", "fold_fast_issue", "fold_debug",
@@ -116,6 +122,7 @@ SIGNATURES = {
     "lt_volumetric_ce_bwd": (c_int, [c_void_p] * 5 + [c_int, c_int, c_long, c_void_p]),
     "lt_test_volumetric_ce_host": (c_int, [c_void_p] * 9 + [c_int, c_int, c_long]),
     "lt_batch_norm_workspace_bytes": (c_size_t, [c_long, c_int]),
+    "lt_batch_norm_plan": (c_int, [c_long, c_int, c_int, ctypes.POINTER(BatchNormPlan)]),
     "lt_batch_norm_fwd": (c_int, [c_void_p] * 9 + [c_long, c_int, c_float, c_float, c_int, c_int, c_void_p, c_size_t, c_void_p]),
     "lt_batch_norm_bwd": (c_int, [c_void_p] * 10 + [c_long, c_int, c_int, c_int, c_void_p, c_size_t, c_void_p]),
     "lt_nchw_to_nhwc_f32": (c_int, [c_void_p, c_void_p] + [c_int] * 5 + [c_void_p]),
@@ -426,6 +433,14 @@ def volumetric_ce_bwd(grad_loss, index, picked, validity, grad_probs):
 
 def batch_norm_workspace_bytes(M, C):
     return lib().lt_batch_norm_workspace_bytes(M, C)
+
+
+def batch_norm_plan(M, C, sm_count):
+    """Host-only launch plan of lt_batch_norm_fwd / _bwd (lt_batch_norm_plan): dict of tc, ry, cblocks, want_splits, max_splits, splits,
+    rows_per_split, row_blocks."""
+    plan = BatchNormPlan()
+    _check(lib().lt_batch_norm_plan(M, C, sm_count, ctypes.byref(plan)), "lt_batch_norm_plan")
+    return {name: getattr(plan, name) for name, _ in BatchNormPlan._fields_}
 
 
 def batch_norm(x, residual, gamma, beta, running_mean, running_var, save_mean, save_invstd, y, M, C, eps, momentum, training, relu,

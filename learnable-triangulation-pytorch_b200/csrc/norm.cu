@@ -5,15 +5,17 @@
 // (tc, ry) grid: tc threads over float4 columns of one channel block (tc = min(C/4, 32)), ry = kBnThreads / tc rows at a time.
 //   bn_reduce_kernel<0>     forward statistics: per (row split, channel) the sums of d = x - x[0][c] and d^2 (shifted sums: no
 //                           cancellation when |mean| >> std), accumulated in fp64 and summed over the CTA's rows in a fixed order;
-//   bn_finalize_fwd_kernel  per channel: the splits merged in a fixed order (8 lanes, then the lanes in order) -> mean, invstd = 1 / sqrt(var_biased + eps), the running
-//                           statistics (unbiased variance) and the apply coefficients; in eval mode the running statistics instead;
-//   bn_apply_fwd_kernel     y = act(a (x - mean) + beta [+ r]), a = gamma invstd.  (x - mean) is formed first, as torch does: the folded
-//                           form a x + (beta - a mean) loses ~log2(|mean| / std) bits of y;
-//   bn_reduce_kernel<1>     backward: per (row split, channel) the sums of g' and g' (x - mean), g' = g [y > 0] under ReLU, in fp64;
+//   bn_finalize_fwd_kernel  per channel: the splits merged in a fixed order (8 lanes, then the lanes in order) -> mean,
+//                           invstd = 1 / sqrt(var_biased + eps) (0 when both are 0, as in torch), the running statistics (unbiased
+//                           variance) and the apply coefficients; in eval mode the running statistics instead;
+//   bn_apply_fwd_kernel     y = act(a (x - mean) + beta [+ r]), a = gamma invstd, act(NaN) = NaN as in torch.relu.  (x - mean) is
+//                           formed first, as torch does: the folded form a x + (beta - a mean) loses ~log2(|mean| / std) bits of y;
+//   bn_reduce_kernel<1>     backward: per (row split, channel) the sums of g' and g' (x - mean), g' = g [!(y <= 0)] under ReLU
+//                           (torch's threshold_backward: a NaN output passes its gradient), in fp64;
 //   bn_finalize_bwd_kernel  dbeta = sum g', dgamma = invstd sum g' (x - mean) and the apply coefficients;
 //   bn_apply_bwd_kernel     dx = a (g' - sum g' / M - xhat sum g' xhat / M) (train) or a g' (eval); dr = g' when asked for.
-// No floating-point atomics and no host synchronisation: the split count depends on M, C and the SM count only, so results repeat
-// bit for bit on one device.
+// No floating-point atomics and no host synchronisation: the launch plan (bn_plan, lt_batch_norm_plan) depends on M, C and the SM
+// count only, so results repeat bit for bit on one device.
 #include "common.cuh"
 #include <math.h>
 
@@ -48,22 +50,27 @@ static inline int bn_max_splits(long M, int C) {
   return s < 1 ? 1 : (int)s;
 }
 
-// Row splits of a reduce pass: one wave of kBnCtasPerSm CTAs per SM, within bn_max_splits.
-static inline int bn_splits(long M, int C, int sms) {
+// The launch plan of both directions for `sms` SMs: reduce passes of one wave of kBnCtasPerSm CTAs per SM within bn_max_splits,
+// each split then taking ceil(M / splits) rows (which can leave fewer splits); apply passes of about two waves along M.
+static inline lt_batch_norm_launch_plan bn_plan(long M, int C, int sms) {
   const BnGeom g = bn_geom(C);
-  const int want = ceil_div((long)(sms > 0 ? sms : 132) * kBnCtasPerSm, g.cblocks);
-  const int mx = bn_max_splits(M, C);
-  return want < 1 ? 1 : (want > mx ? mx : want);
-}
-
-// CTAs along M of an apply pass: about two waves.
-static inline int bn_row_blocks(long M, int C, int sms) {
-  const BnGeom g = bn_geom(C);
+  if (sms <= 0) sms = 132;
+  lt_batch_norm_launch_plan p;
+  p.tc = g.tc;
+  p.ry = g.ry;
+  p.cblocks = g.cblocks;
+  p.want_splits = ceil_div((long)sms * kBnCtasPerSm, g.cblocks);
+  if (p.want_splits < 1) p.want_splits = 1;
+  p.max_splits = bn_max_splits(M, C);
+  const int s = p.want_splits < p.max_splits ? p.want_splits : p.max_splits;
+  p.rows_per_split = (M + s - 1) / s;
+  p.splits = (int)((M + p.rows_per_split - 1) / p.rows_per_split);
   const long by_rows = (M + (long)g.ry * kBnUnroll - 1) / ((long)g.ry * kBnUnroll);
-  long want = ((long)(sms > 0 ? sms : 132) * kBnCtasPerSm * 2 + g.cblocks - 1) / g.cblocks;   // two waves
-  if (want > by_rows) want = by_rows;
-  if (want > 65535) want = 65535;
-  return want < 1 ? 1 : (int)want;
+  long rb = ((long)sms * kBnCtasPerSm * 2 + g.cblocks - 1) / g.cblocks;   // two waves
+  if (rb > by_rows) rb = by_rows;
+  if (rb > 65535) rb = 65535;
+  p.row_blocks = rb < 1 ? 1 : (int)rb;
+  return p;
 }
 
 // workspace: fp64 partials [splits][2][C], then float coefficients [5][C]
@@ -114,7 +121,7 @@ __global__ void __launch_bounds__(kBnThreads) bn_reduce_kernel(const float* __re
             a0[k] += dx;
             a1[k] = fma(dx, dx, a1[k]);
           } else {
-            const double g = f4(yv[u], k) > 0.0f ? (double)f4(gv[u], k) : 0.0;
+            const double g = !(f4(yv[u], k) <= 0.0f) ? (double)f4(gv[u], k) : 0.0;
             a0[k] += g;
             a1[k] = fma(g, dx, a1[k]);
           }
@@ -178,7 +185,8 @@ __global__ void __launch_bounds__(32 * kBnLanes) bn_finalize_fwd_kernel(
     if (var < 0.0) var = 0.0;
     const double mean = (double)x[c] + dm;
     mean_f = (float)mean;
-    invstd_f = (float)(1.0 / sqrt(var + (double)eps));
+    // a constant channel with eps = 0 normalises with invstd 0, as torch's batch statistics do (y = beta, dx = dgamma = 0)
+    invstd_f = var == 0.0 && eps == 0.0f ? 0.0f : (float)(1.0 / sqrt(var + (double)eps));
     const float var_unbiased = (float)(var * ((double)M / (double)(M - 1)));
     running_mean[c] = momentum * mean_f + (1.0f - momentum) * running_mean[c];
     running_var[c] = momentum * var_unbiased + (1.0f - momentum) * running_var[c];
@@ -227,7 +235,7 @@ __global__ void __launch_bounds__(kBnThreads) bn_apply_fwd_kernel(const float* _
       for (int k = 0; k < 4; ++k) {
         o[k] = fmaf(a[k], f4(v[u], k) - mu[k], b[k]);
         if (RES) o[k] += f4(rv[u], k);
-        if (RELU) o[k] = fmaxf(o[k], 0.0f);
+        if (RELU) o[k] = o[k] < 0.0f ? 0.0f : o[k];    // NaN stays NaN, as torch.relu
       }
       st4(y + row * C + 4 * c4, make_float4(o[0], o[1], o[2], o[3]));
     }
@@ -253,11 +261,13 @@ __global__ void __launch_bounds__(32 * kBnLanes) bn_finalize_bwd_kernel(
   coef[4 * C + c] = training ? (float)(dg / (double)M) : 0.0f;
 }
 
-// grid (cblocks, row blocks), block (tc, ry): dx = a (g' - k1 - xhat k2), xhat = (x - mean) invstd; dr = g' (DRES)
+// grid (cblocks, row blocks), block (tc, ry): dx = a (g' - k1 - xhat k2), xhat = (x - mean) invstd (training) or a g' (eval);
+// dr = g' (DRES)
 template <bool RELU, bool DRES>
 __global__ void __launch_bounds__(kBnThreads) bn_apply_bwd_kernel(const float* __restrict__ x, const float* __restrict__ y,
                                                                   const float* __restrict__ gy, const float* __restrict__ coef,
-                                                                  float* __restrict__ gx, float* __restrict__ gr, long M, int C) {
+                                                                  float* __restrict__ gx, float* __restrict__ gr, long M, int C,
+                                                                  int training) {
   const int c4 = blockIdx.x * blockDim.x + threadIdx.x;
   if (c4 >= (C >> 2)) return;
   float mu[4], is[4], a[4], k1[4], k2[4];
@@ -286,14 +296,14 @@ __global__ void __launch_bounds__(kBnThreads) bn_apply_bwd_kernel(const float* _
     for (int u = 0; u < kBnUnroll; ++u) {
       const long row = rb + u * step;
       if (row >= M) break;
-      const float4 g = make_float4(yv[u].x > 0.0f ? gv[u].x : 0.0f, yv[u].y > 0.0f ? gv[u].y : 0.0f, yv[u].z > 0.0f ? gv[u].z : 0.0f,
-                                   yv[u].w > 0.0f ? gv[u].w : 0.0f);
+      const float4 g = make_float4(!(yv[u].x <= 0.0f) ? gv[u].x : 0.0f, !(yv[u].y <= 0.0f) ? gv[u].y : 0.0f,
+                                   !(yv[u].z <= 0.0f) ? gv[u].z : 0.0f, !(yv[u].w <= 0.0f) ? gv[u].w : 0.0f);
       if (DRES) st4(gr + row * C + 4 * c4, g);
       float o[4];
 #pragma unroll
       for (int k = 0; k < 4; ++k) {
         const float xhat = (f4(v[u], k) - mu[k]) * is[k];
-        o[k] = a[k] * (f4(g, k) - k1[k] - xhat * k2[k]);
+        o[k] = training ? a[k] * (f4(g, k) - k1[k] - xhat * k2[k]) : a[k] * f4(g, k);   // eval: no x term, so a non-finite x stays local
       }
       st4(gx + row * C + 4 * c4, make_float4(o[0], o[1], o[2], o[3]));
     }
@@ -318,6 +328,14 @@ extern "C" size_t lt_batch_norm_workspace_bytes(long M, int C) {
   return bn_partial_bytes(M, C) + (size_t)5 * C * sizeof(float);
 }
 
+extern "C" int lt_batch_norm_plan(long M, int C, int sm_count, lt_batch_norm_launch_plan* plan) {
+  LT_REQUIRE(plan && sm_count > 0, "batch_norm_plan: bad arguments");
+  const int rc = bn_check_sizes("batch_norm_plan", M, C, 0);
+  if (rc != LT_OK) return rc;
+  *plan = bn_plan(M, C, sm_count);
+  return LT_OK;
+}
+
 extern "C" int lt_batch_norm_fwd(const float* x, const float* residual, const float* gamma, const float* beta, float* running_mean,
                                  float* running_var, float* save_mean, float* save_invstd, float* y, long M, int C, float eps,
                                  float momentum, int training, int relu, void* workspace, size_t workspace_bytes, void* stream) {
@@ -329,23 +347,18 @@ extern "C" int lt_batch_norm_fwd(const float* x, const float* residual, const fl
   LT_REQUIRE(aligned16(x) && aligned16(residual) && aligned16(y) && aligned16(workspace), "batch_norm_fwd: maps must be 16-byte aligned");
   LT_REQUIRE(eps >= 0.0f, "batch_norm_fwd: eps must be >= 0");
   const cudaStream_t s = (cudaStream_t)stream;
-  const int sms = sm_count();
-  const BnGeom g = bn_geom(C);
+  const lt_batch_norm_launch_plan p = bn_plan(M, C, sm_count());
   double* part = reinterpret_cast<double*>(workspace);
   float* coef = reinterpret_cast<float*>(reinterpret_cast<char*>(workspace) + bn_partial_bytes(M, C));
-  const dim3 block(g.tc, g.ry);
-  int splits = 0;
+  const dim3 block(p.tc, p.ry);
   if (training) {
-    splits = bn_splits(M, C, sms);
-    const long rows_per_split = (M + splits - 1) / splits;
-    splits = (int)((M + rows_per_split - 1) / rows_per_split);
-    bn_reduce_kernel<0, false><<<dim3(g.cblocks, splits), block, 0, s>>>(x, nullptr, nullptr, nullptr, M, C, rows_per_split, part);
+    bn_reduce_kernel<0, false><<<dim3(p.cblocks, p.splits), block, 0, s>>>(x, nullptr, nullptr, nullptr, M, C, p.rows_per_split, part);
     LT_CHECK_LAUNCH("bn_reduce_kernel");
   }
-  bn_finalize_fwd_kernel<<<ceil_div(C, 32), dim3(32, kBnLanes), 0, s>>>(part, splits, x, gamma, beta, running_mean, running_var, save_mean, save_invstd,
-                                                           coef, M, C, eps, momentum, training);
+  bn_finalize_fwd_kernel<<<ceil_div(C, 32), dim3(32, kBnLanes), 0, s>>>(part, training ? p.splits : 0, x, gamma, beta, running_mean, running_var,
+                                                           save_mean, save_invstd, coef, M, C, eps, momentum, training);
   LT_CHECK_LAUNCH("bn_finalize_fwd_kernel");
-  const dim3 grid(g.cblocks, bn_row_blocks(M, C, sms));
+  const dim3 grid(p.cblocks, p.row_blocks);
   if (residual) {
     if (relu) bn_apply_fwd_kernel<true, true><<<grid, block, 0, s>>>(x, residual, coef, y, M, C);
     else bn_apply_fwd_kernel<true, false><<<grid, block, 0, s>>>(x, residual, coef, y, M, C);
@@ -368,27 +381,24 @@ extern "C" int lt_batch_norm_bwd(const float* x, const float* y, const float* gr
   LT_REQUIRE(aligned16(x) && aligned16(y) && aligned16(grad_y) && aligned16(grad_x) && aligned16(grad_residual) && aligned16(workspace),
              "batch_norm_bwd: maps must be 16-byte aligned");
   const cudaStream_t s = (cudaStream_t)stream;
-  const int sms = sm_count();
-  const BnGeom g = bn_geom(C);
+  const lt_batch_norm_launch_plan p = bn_plan(M, C, sm_count());
   double* part = reinterpret_cast<double*>(workspace);
   float* coef = reinterpret_cast<float*>(reinterpret_cast<char*>(workspace) + bn_partial_bytes(M, C));
-  const dim3 block(g.tc, g.ry);
-  int splits = bn_splits(M, C, sms);
-  const long rows_per_split = (M + splits - 1) / splits;
-  splits = (int)((M + rows_per_split - 1) / rows_per_split);
-  if (relu) bn_reduce_kernel<1, true><<<dim3(g.cblocks, splits), block, 0, s>>>(x, grad_y, y, save_mean, M, C, rows_per_split, part);
-  else bn_reduce_kernel<1, false><<<dim3(g.cblocks, splits), block, 0, s>>>(x, grad_y, nullptr, save_mean, M, C, rows_per_split, part);
+  const dim3 block(p.tc, p.ry);
+  const dim3 rgrid(p.cblocks, p.splits);
+  if (relu) bn_reduce_kernel<1, true><<<rgrid, block, 0, s>>>(x, grad_y, y, save_mean, M, C, p.rows_per_split, part);
+  else bn_reduce_kernel<1, false><<<rgrid, block, 0, s>>>(x, grad_y, nullptr, save_mean, M, C, p.rows_per_split, part);
   LT_CHECK_LAUNCH("bn_reduce_kernel");
-  bn_finalize_bwd_kernel<<<ceil_div(C, 32), dim3(32, kBnLanes), 0, s>>>(part, splits, gamma, save_mean, save_invstd, grad_gamma, grad_beta, coef, M, C,
-                                                           training);
+  bn_finalize_bwd_kernel<<<ceil_div(C, 32), dim3(32, kBnLanes), 0, s>>>(part, p.splits, gamma, save_mean, save_invstd, grad_gamma, grad_beta, coef,
+                                                           M, C, training);
   LT_CHECK_LAUNCH("bn_finalize_bwd_kernel");
-  const dim3 grid(g.cblocks, bn_row_blocks(M, C, sms));
+  const dim3 grid(p.cblocks, p.row_blocks);
   if (relu) {
-    if (grad_residual) bn_apply_bwd_kernel<true, true><<<grid, block, 0, s>>>(x, y, grad_y, coef, grad_x, grad_residual, M, C);
-    else bn_apply_bwd_kernel<true, false><<<grid, block, 0, s>>>(x, y, grad_y, coef, grad_x, nullptr, M, C);
+    if (grad_residual) bn_apply_bwd_kernel<true, true><<<grid, block, 0, s>>>(x, y, grad_y, coef, grad_x, grad_residual, M, C, training);
+    else bn_apply_bwd_kernel<true, false><<<grid, block, 0, s>>>(x, y, grad_y, coef, grad_x, nullptr, M, C, training);
   } else {
-    if (grad_residual) bn_apply_bwd_kernel<false, true><<<grid, block, 0, s>>>(x, nullptr, grad_y, coef, grad_x, grad_residual, M, C);
-    else bn_apply_bwd_kernel<false, false><<<grid, block, 0, s>>>(x, nullptr, grad_y, coef, grad_x, nullptr, M, C);
+    if (grad_residual) bn_apply_bwd_kernel<false, true><<<grid, block, 0, s>>>(x, nullptr, grad_y, coef, grad_x, grad_residual, M, C, training);
+    else bn_apply_bwd_kernel<false, false><<<grid, block, 0, s>>>(x, nullptr, grad_y, coef, grad_x, nullptr, M, C, training);
   }
   LT_CHECK_LAUNCH("bn_apply_bwd_kernel");
   return LT_OK;
