@@ -374,6 +374,23 @@ int lt_triangulate_dlt_bwd(const float* proj, const float* keypoints_2d, const f
 size_t lt_triangulate_dlt_proj_bwd_workspace_bytes(int B, int V, int J);
 int lt_triangulate_dlt_proj_bwd(const float* proj, const float* keypoints_2d, const float* confidences, const float* grad_out,
                                 float* grad_proj, void* workspace, size_t workspace_bytes, int B, int V, int J, void* stream);
+/* RANSAC triangulation baseline (RANSACTriangulationNet, triangulation.py:17-128).
+ * Heat-map arg-max: logits channels-last float32 [N][h][w][C] (C >= J, the final conv's padded output) -> heatmaps [N][J][h][w]
+ * (the raw logits) and keypoints_2d int64 [N][J][2] of torch.max's first maximal index (a NaN counts as the maximum):
+ * x = trunc(float32(idx % w) * scale_x), y = trunc(float32(idx / w) * scale_y) with scale = float32(image side / map side).
+ * One read and one write of the maps; per-slice bests in `workspace` (lt_heatmap_argmax_workspace_bytes(N, J, h, w) bytes),
+ * merged in a fixed order by a second small kernel. */
+size_t lt_heatmap_argmax_workspace_bytes(int N, int J, int h, int w);
+int lt_heatmap_argmax_fwd(const float* logits, int C, float* heatmaps, long long* keypoints_2d, void* workspace, size_t workspace_bytes,
+                          int N, int J, int h, int w, float scale_x, float scale_y, void* stream);
+/* RANSAC triangulation: proj [B][V][3][4] float32, keypoints_2d int64 [B][V][J][2], the drawn view pairs int32
+ * [B][J][n_iters][2] -> keypoints_3d [B][J][3] float32 and, if not NULL, inliers [B][J] uint64 (bit v = view v is an inlier).
+ * One thread per (sample, joint), float64 throughout: per pair the 2-view DLT (rows x P[2] - P[0], y P[2] - P[1] formed in
+ * float64) and the views with 0.5 |p - pi(X)| < eps; the first largest set wins; the DLT on it; with `direct`, the Huber
+ * (f_scale 1) reprojection cost minimised by iteratively reweighted Levenberg-Marquardt.  2 <= V <= 64; no atomics, no host
+ * synchronisation; the same result as lt_test_triangulate_ransac_host bit for bit. */
+int lt_triangulate_ransac_fwd(const float* proj, const long long* keypoints_2d, const int* pairs, int B, int V, int J, int n_iters,
+                              double eps, int direct, float* keypoints_3d, unsigned long long* inliers, void* stream);
 
 /* ------------------------------------------------------------------------------------------
  * Volumetric cross-entropy loss of the volumetric training recipe.  Replaces VolumetricCELoss (mvn/models/loss.py:52-80, called
@@ -499,6 +516,9 @@ int lt_test_volumetric_ce_host(const float* probs, const float* coord, const flo
  * host pointers, summed in double over plain float32 channels-last tensors: in [N][ID][IH][IW][desc->Cin], grad_out [N][FD][FH][FW][FC]
  * -> grad_w [taps][Cin][G * Cout]. */
 int lt_test_conv_wgrad_host(const lt_conv_desc* desc, const float* in, const float* grad_out, int Cin, int Cout, float* grad_w);
+/* lt_triangulate_ransac_fwd's per-item code on host pointers. */
+int lt_test_triangulate_ransac_host(const float* proj, const long long* keypoints_2d, const int* pairs, int B, int V, int J, int n_iters,
+                                    double eps, int direct, float* keypoints_3d, unsigned long long* inliers);
 
 #ifdef __cplusplus
 }

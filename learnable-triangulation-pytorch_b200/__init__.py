@@ -10,7 +10,7 @@ Python identifier; `lt_b200.py` at the repo root is the import shim).
 """
 from . import loss, multiview, op, pipeline, pose_resnet, v2v, volumetric  # noqa: F401
 from .multiview import Camera  # noqa: F401
-from .triangulation import AlgebraicTriangulationNet, VolumetricTriangulationNet  # noqa: F401
+from .triangulation import AlgebraicTriangulationNet, RANSACTriangulationNet, VolumetricTriangulationNet  # noqa: F401
 from .v2v import V2VModel  # noqa: F401
 
 __version__ = "0.1.0"
@@ -33,6 +33,7 @@ def install(mvn_package=None):
     ref_loss.VolumetricCELoss = loss.VolumetricCELoss
     tri.VolumetricTriangulationNet = VolumetricTriangulationNet
     tri.AlgebraicTriangulationNet = AlgebraicTriangulationNet
+    tri.RANSACTriangulationNet = RANSACTriangulationNet
     ref_op.integrate_tensor_2d = op.integrate_tensor_2d
     ref_op.unproject_heatmaps = op.unproject_heatmaps
     ref_op.integrate_tensor_3d_with_coordinates = op.integrate_tensor_3d_with_coordinates

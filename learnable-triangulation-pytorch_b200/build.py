@@ -12,7 +12,9 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 LIB = os.path.join(HERE, "liblt_b200.so")
 STAMP = os.path.join(HERE, ".liblt_b200.stamp")
-SOURCES = ["capi.cu", "unproject.cu", "softargmax.cu", "conv_simt.cu", "conv_tc.cu", "conv_fold.cu", "conv_tail.cu", "misc.cu", "algebraic.cu", "backward.cu", "loss.cu", "conv_wgrad.cu", "norm.cu"]
+SOURCES = ["capi.cu", "unproject.cu", "softargmax.cu", "conv_simt.cu", "conv_tc.cu", "conv_fold.cu", "conv_tail.cu", "misc.cu", "algebraic.cu", "backward.cu", "loss.cu", "conv_wgrad.cu", "norm.cu", "ransac.cu"]
+# per-source additions: ransac.cu contracts no multiply-add, so its host test hook runs the device code's exact operations
+SOURCE_FLAGS = {"ransac.cu": ["-fmad=false"]}
 ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]
 NVCC_FLAGS = ARCH + ["-O3", "-lineinfo", "-std=c++17",
                      "--expt-relaxed-constexpr", "-Xcompiler", "-fPIC", "-Xptxas", "-v"]
@@ -28,6 +30,7 @@ def _digest():
                 h.update(name.encode())
                 h.update(f.read())
     h.update(" ".join(NVCC_FLAGS).encode())
+    h.update(repr(sorted(SOURCE_FLAGS.items())).encode())
     return h.hexdigest()
 
 
@@ -48,7 +51,7 @@ def build(force=False, verbose=False):
     os.makedirs(os.path.join(HERE, "build"), exist_ok=True)
     for src in SOURCES:
         obj = os.path.join(HERE, "build", src.replace(".cu", ".o"))
-        cmd = [nvcc] + NVCC_FLAGS + ["-c", os.path.join(CSRC, src), "-o", obj]
+        cmd = [nvcc] + NVCC_FLAGS + SOURCE_FLAGS.get(src, []) + ["-c", os.path.join(CSRC, src), "-o", obj]
         procs.append((src, subprocess.Popen(cmd, stdout=subprocess.PIPE, stderr=subprocess.STDOUT, text=True)))
         objs.append(obj)
     log = []

@@ -19,7 +19,7 @@ AGG = {"sum": 0, "max": 1, "softmax": 2, "conf": 3, "conf_norm": 3}
 CONV_SIMT, CONV_TC, CONV_TC1, CONV_TC_FOLD = 0, 1, 2, 3
 RES_NONE, RES_BEFORE_RELU, RES_AFTER_RELU = 0, 1, 2
 
-c_int, c_long, c_float, c_void_p, c_size_t = ctypes.c_int, ctypes.c_long, ctypes.c_float, ctypes.c_void_p, ctypes.c_size_t
+c_int, c_long, c_float, c_double, c_void_p, c_size_t = ctypes.c_int, ctypes.c_long, ctypes.c_float, ctypes.c_double, ctypes.c_void_p, ctypes.c_size_t
 
 
 class ConvDesc(ctypes.Structure):
@@ -117,6 +117,10 @@ SIGNATURES = {
     "lt_triangulate_dlt_proj_bwd_workspace_bytes": (c_size_t, [c_int] * 3),
     "lt_triangulate_dlt_proj_bwd": (c_int, [c_void_p] * 6 + [c_size_t] + [c_int] * 3 + [c_void_p]),
     "lt_test_triangulate_dlt_proj_bwd_host": (c_int, [c_void_p] * 5 + [c_int] * 3),
+    "lt_heatmap_argmax_workspace_bytes": (c_size_t, [c_int] * 4),
+    "lt_heatmap_argmax_fwd": (c_int, [c_void_p, c_int, c_void_p, c_void_p, c_void_p, c_size_t] + [c_int] * 4 + [c_float, c_float, c_void_p]),
+    "lt_triangulate_ransac_fwd": (c_int, [c_void_p] * 3 + [c_int] * 4 + [c_double, c_int, c_void_p, c_void_p, c_void_p]),
+    "lt_test_triangulate_ransac_host": (c_int, [c_void_p] * 3 + [c_int] * 4 + [c_double, c_int, c_void_p, c_void_p]),
     "lt_volumetric_ce_workspace_bytes": (c_size_t, [c_int, c_int, c_long]),
     "lt_volumetric_ce_fwd": (c_int, [c_void_p] * 8 + [c_size_t, c_int, c_int, c_long, c_void_p]),
     "lt_volumetric_ce_bwd": (c_int, [c_void_p] * 5 + [c_int, c_int, c_long, c_void_p]),
@@ -411,6 +415,28 @@ def triangulate_dlt_proj_bwd_workspace_bytes(B, V, J):
     return lib().lt_triangulate_dlt_proj_bwd_workspace_bytes(B, V, J)
 
 
+def heatmap_argmax_workspace_bytes(N, J, h, w):
+    return lib().lt_heatmap_argmax_workspace_bytes(N, J, h, w)
+
+
+def heatmap_argmax(logits, C, heatmaps, keypoints_2d, workspace, N, J, h, w, scale_x, scale_y):
+    """logits channels-last float32 (N, h, w, C) -> heatmaps (N, J, h, w) float32 and keypoints_2d (N, J, 2) int64, both written;
+    scale_x / scale_y: image side over map side (rounded to float32 as the reference's float32 product rounds it)."""
+    assert keypoints_2d.dtype == torch.int64
+    _check(lib().lt_heatmap_argmax_fwd(_ptr(logits), C, _ptr(heatmaps), _ptr(keypoints_2d), _ptr(workspace),
+                                       workspace.numel() * workspace.element_size(), N, J, h, w, float(scale_x), float(scale_y),
+                                       _stream()), "lt_heatmap_argmax_fwd")
+
+
+def triangulate_ransac(proj, kp2d, pairs, n_iters, eps, direct, out, inliers=None):
+    """proj (B, V, 3, 4) float32, kp2d (B, V, J, 2) int64, pairs (B, J, n_iters, 2) int32 -> out (B, J, 3) float32 and inliers
+    (B, J) int64 bit masks (optional), written."""
+    B, V, J = kp2d.shape[:3]
+    assert kp2d.dtype == torch.int64 and pairs.dtype == torch.int32 and (inliers is None or inliers.dtype == torch.int64)
+    _check(lib().lt_triangulate_ransac_fwd(_ptr(proj), _ptr(kp2d), _ptr(pairs), B, V, J, int(n_iters), float(eps), int(bool(direct)),
+                                           _ptr(out), _ptr(inliers), _stream()), "lt_triangulate_ransac_fwd")
+
+
 def volumetric_ce_workspace_bytes(B, J, nvox):
     return lib().lt_volumetric_ce_workspace_bytes(B, J, nvox)
 
@@ -494,6 +520,17 @@ def triangulate_dlt_bwd_host(proj, kp2d, conf, grad_out, grad_kp2d, grad_conf):
     B, V, J = kp2d.shape[:3]
     _check(lib().lt_test_triangulate_dlt_bwd_host(_host_ptr(proj), _host_ptr(kp2d), _host_ptr(conf), _host_ptr(grad_out),
                                                   _host_ptr(grad_kp2d), _host_ptr(grad_conf), B, V, J), "lt_test_triangulate_dlt_bwd_host")
+
+
+def triangulate_ransac_host(proj, kp2d, pairs, n_iters, eps, direct, out, inliers=None):
+    """lt_test_triangulate_ransac_host: the RANSAC kernel's per-item code on CPU tensors (test hook, no GPU needed).  Dtypes as
+    triangulate_ransac."""
+    B, V, J = kp2d.shape[:3]
+    for t, dt in ((kp2d, torch.int64), (pairs, torch.int32)) + (() if inliers is None else ((inliers, torch.int64),)):
+        assert not t.is_cuda and t.is_contiguous() and t.dtype == dt, "test hooks need contiguous CPU tensors of the kernel's dtypes"
+    _check(lib().lt_test_triangulate_ransac_host(_host_ptr(proj), kp2d.data_ptr(), pairs.data_ptr(), B, V, J, int(n_iters), float(eps),
+                                                 int(bool(direct)), _host_ptr(out), None if inliers is None else inliers.data_ptr()),
+           "lt_test_triangulate_ransac_host")
 
 
 def softargmax3d_bwd_host(probs, coord, grad_keypoints, grad_volumes, grad_logits, B, J, nvox, multiplier, mode):

@@ -893,6 +893,34 @@ class NativeEngine:
         self.launches += 2
         return kp3d, kp2d, heat.view(B, V, J, h, w), conf
 
+    # ------------------------------------------------------------------ RANSAC baseline
+    def ransac_forward(self, images, proj, pairs, n_iters, eps, direct):
+        """RANSACTriangulationNet.forward (triangulation.py:27-70), device side.
+
+        images (B, V, 3, H, W), proj (B, V, 3, 4) float32 image-space projection matrices, pairs (B, J, n_iters, 2) int32 drawn views.
+        -> keypoints_3d (B, J, 3), keypoints_2d (B, V, J, 2) int64 in image pixels, heatmaps (B, V, J, h, w) raw, confidences
+           (B, V, J) zeros."""
+        self.prepare()
+        self.launches = 0
+        B, V = images.shape[:2]
+        H, W = images.shape[3:]
+        dev = images.device
+        J = self.model.backbone.num_joints
+        trunk = self.backbone_trunk(images.reshape(B * V, *images.shape[2:]))
+        logits = self._conv(self.backbone_upsample(trunk), self._packs["final"], relu=False, out_fmt=FMT_F32)   # (BV,1,h,w,C)
+        h, w = logits.H, logits.W
+        heat = torch.empty((B * V, J, h, w), dtype=torch.float32, device=dev)
+        kp2d = torch.empty((B, V, J, 2), dtype=torch.int64, device=dev)
+        ws = torch.empty(capi.heatmap_argmax_workspace_bytes(B * V, J, h, w) // 4, dtype=torch.float32, device=dev)
+        with self._timed("heatmap_argmax", nbytes=4.0 * B * V * h * w * (logits.C + J)):
+            capi.heatmap_argmax(logits.data, logits.C, heat, kp2d, ws, B * V, J, h, w, W / w, H / h)      # :44-52
+        kp3d = torch.empty((B, J, 3), dtype=torch.float32, device=dev)
+        with self._timed("triangulate_ransac"):
+            capi.triangulate_ransac(proj, kp2d, pairs, n_iters, eps, direct, kp3d)                       # :58-65
+        self.launches += 3
+        conf = torch.zeros((B, V, J), dtype=torch.float32, device=dev)                                     # :59, the "plug"
+        return kp3d, kp2d, heat.view(B, V, J, h, w), conf
+
     def forward(self, images, proj, position, center, step, rot):
         """All inputs are CUDA float32 tensors. Returns (keypoints, features, volumes, coord_volumes)."""
         self.prepare()

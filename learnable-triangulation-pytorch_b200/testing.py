@@ -205,3 +205,27 @@ def randomize_backbone_weights(model, seed=0, calib_size=128, calib_images=4, br
 
 
 BN_MOMENTUM = 0.1
+
+
+def make_ransac_config(num_layers=152, direct_optimization=True, num_joints=17):
+    """The `model:` section of experiments/human36m/eval/human36m_ransac.yaml with init_weights off."""
+    return AttrDict({
+        "image_shape": [384, 384],
+        "model": {"name": "ransac", "init_weights": False, "direct_optimization": direct_optimization,
+                  "backbone": {"name": "resnet%d" % num_layers, "style": "simple", "init_weights": False,
+                               "num_joints": num_joints, "num_layers": num_layers}},
+    })
+
+
+class _BackboneHolder(nn.Module):
+    def __init__(self, backbone):
+        super().__init__()
+        self.backbone = backbone
+        self.heatmap_multiplier = 1.0
+
+
+@torch.no_grad()
+def randomize_ransac_weights(model, seed=0, calib_size=64):
+    """randomize_backbone_weights for a model whose heat maps are used raw (RANSACTriangulationNet): heat-map spread ~3."""
+    randomize_backbone_weights(_BackboneHolder(model.backbone), seed=seed, calib_size=calib_size)
+    return model.eval()

@@ -11,6 +11,7 @@ sm_90a kernels through engine.NativeEngine.  backend="torch": autograd-capable t
 (training, CPU plumbing).  Nothing switches backend silently.
 """
 import os
+import random
 
 import numpy as np
 import torch
@@ -80,10 +81,10 @@ def _hooks(backbone_backend, norm_backend, v2v_backend="torch"):
             autograd_ops.batch_norm if norm_backend == "native" else layers.torch_norm)
 
 
-def _upload(device, *arrays):
-    """float32 tensors on `device` of host arrays (float64 cast last): on CUDA through one page-locked buffer and one asynchronous
-    copy, so the host part of a forward does not wait for the device."""
-    flat = [torch.from_numpy(np.ascontiguousarray(a)).float().reshape(-1) for a in arrays]
+def _upload(device, *arrays, dtype=torch.float32):
+    """`dtype` (float32 by default) tensors on `device` of host arrays (float64 cast last): on CUDA through one page-locked buffer
+    and one asynchronous copy, so the host part of a forward does not wait for the device."""
+    flat = [torch.from_numpy(np.ascontiguousarray(a)).to(dtype).reshape(-1) for a in arrays]
     host = torch.cat(flat)
     if device.type == "cuda":
         host = host.pin_memory().to(device, non_blocking=True)
@@ -342,3 +343,174 @@ class AlgebraicTriangulationNet(_EngineOwner):
         kp2d = kp2d * scale
         kp3d = multiview.triangulate_batch_of_points(proj_matricies, kp2d, confidences_batch=alg_conf, backend=ops_backend)
         return kp3d, kp2d, heatmaps, alg_conf
+
+
+def draw_view_pairs(batch_size, n_joints, n_views, n_iters):
+    """(B, J, n_iters, 2) int32 view pairs, drawn with Python's global `random` in the reference's order (sample outer, joint
+    inner, then the draws; triangulation.py:60-64, :84-85), each `sorted(random.sample(range(V), 2))`.  Python <= 3.10 sampled the
+    reference's set of small ints as this range (later versions refuse a set), so after `random.seed(s)` the pairs, and
+    `random.getstate()` afterwards, are the reference's."""
+    views = range(n_views)
+    pairs = np.empty((batch_size, n_joints, n_iters, 2), dtype=np.int32)
+    for b in range(batch_size):
+        for j in range(n_joints):
+            for i in range(n_iters):
+                pairs[b, j, i] = sorted(random.sample(views, 2))
+    return pairs
+
+
+def _dlt64(rows, mask):
+    """rows (N, V, 2, 4) float64 DLT rows, mask (N, V) bool -> (N, 3): the smallest eigenvector of A^T A over the masked views."""
+    A = (rows * mask[:, :, None, None]).reshape(rows.shape[0], -1, 4)
+    u = torch.linalg.eigh(A.transpose(1, 2) @ A)[1][..., 0]
+    return u[:, :3] / u[:, 3:]
+
+
+def _project64(P, X):
+    """pi(X) (N, V, 2) and the depth w (N, V, 1) of points X (N, 3) through P (N, V, 3, 4), float64 (multiview.py:89-110)."""
+    uvw = torch.einsum("nvij,nj->nvi", P, torch.cat([X, torch.ones_like(X[:, :1])], 1))
+    return uvw[..., :2] / uvw[..., 2:], uvw[..., 2:]
+
+
+def _error2(P, pts, X):
+    """(0.5 |p - pi(X)|)^2 per view, (N, V): the square of multiview.py:186-193's reprojection error."""
+    return 0.25 * ((pts - _project64(P, X)[0]) ** 2).sum(-1)
+
+
+def triangulate_ransac_batch(proj, keypoints_2d, pairs, reprojection_error_epsilon=15, direct_optimization=True, max_iters=1000):
+    """Batched float64 torch formulation of triangulate_ransac (triangulation.py:72-128) over every (sample, joint) at once, on any
+    device: proj (B, V, 3, 4), keypoints_2d (B, V, J, 2) int64, pairs (B, J, n_iters, 2) -> (keypoints_3d (B, J, 3) float64, inlier
+    mask (B, J, V) bool).  The same steps as the native kernel (csrc/ransac.cu): pair DLTs, strict inlier test, first largest set,
+    inlier DLT, and the Huber refinement by iteratively reweighted Levenberg-Marquardt."""
+    B, V, J = keypoints_2d.shape[:3]
+    N, n_iters = B * J, pairs.shape[2]
+    dev = keypoints_2d.device
+    P = proj.to(dev, torch.float64)[:, None].expand(B, J, V, 3, 4).reshape(N, V, 3, 4)
+    pts = keypoints_2d.to(torch.float64).permute(0, 2, 1, 3).reshape(N, V, 2)
+    rows = torch.stack([pts[..., 0:1] * P[:, :, 2] - P[:, :, 0], pts[..., 1:2] * P[:, :, 2] - P[:, :, 1]], dim=2)   # (N, V, 2, 4)
+    ar = torch.arange(N, device=dev)
+    pr = pairs.to(dev).reshape(N, n_iters, 2).long()
+    best = torch.zeros((N, V), dtype=torch.bool, device=dev)
+    best_n = torch.zeros(N, dtype=torch.long, device=dev)
+    for i in range(n_iters):
+        mask = torch.zeros((N, V), dtype=torch.bool, device=dev)
+        mask[ar, pr[:, i, 0]] = True
+        mask[ar, pr[:, i, 1]] = True
+        mask = mask | (_error2(P, pts, _dlt64(rows, mask)).sqrt() < reprojection_error_epsilon)
+        n = mask.sum(1)
+        better = n > best_n
+        best = torch.where(better[:, None], mask, best)
+        best_n = torch.where(better, n, best_n)
+    best = best | (best_n == 0)[:, None]               # the reference's "no inliers -> all views" (:100-101)
+    X = _dlt64(rows, best)
+    if direct_optimization:
+        X = _refine_huber(P, pts, best, X, max_iters)
+    return X.reshape(B, J, 3), best.reshape(B, J, V)
+
+
+def _refine_huber(P, pts, mask, X, max_iters):
+    """1/2 sum over the inliers of rho(f^2) (Huber, f_scale 1) minimised per item from X as ransac_refine (csrc/ransac.cu) does:
+    weights 1 / max(f, 1) on the residual components, the Gauss-Newton curvature of f above f = 1, Marquardt damping, steps kept
+    only where they lower the cost."""
+    w_in = mask.to(X.dtype)
+
+    def cost(X):
+        z = _error2(P, pts, X)
+        return 0.5 * (torch.where(z <= 1, z, 2 * z.sqrt() - 1) * w_in).sum(1)
+
+    c = cost(X)
+    active = torch.isfinite(c)
+    lam = torch.full_like(c, 1e-3)
+    for _ in range(max_iters):
+        if not bool(active.any()):
+            break
+        puv, w = _project64(P, X)
+        r = 0.5 * (puv - pts)                                                            # (N, V, 2)
+        f = r.norm(dim=-1)
+        outer = f > 1
+        wt = torch.where(outer, 1 / f, torch.ones_like(f)) * w_in
+        Jac = 0.5 * (P[:, :, :2, :3] - puv[..., None] * P[:, :, 2:3, :3]) / w[..., None]  # (N, V, 2, 3)
+        jtr = torch.einsum("nvai,nva->nvi", Jac, r)
+        jr = torch.where(outer[..., None], jtr / f[..., None], torch.zeros_like(jtr))      # radial direction of the Huber branch
+        H = torch.einsum("nv,nvai,nvaj->nij", wt, Jac, Jac) - torch.einsum("nv,nvi,nvj->nij", wt, jr, jr)
+        g = torch.einsum("nv,nvi->ni", wt, jtr)
+        A = H + torch.diag_embed(lam[:, None] * torch.diagonal(H, dim1=1, dim2=2))
+        d = -torch.linalg.solve_ex(A, g[..., None])[0][..., 0]
+        Xn = X + d
+        cn = cost(Xn)
+        acc = active & (cn < c)
+        X = torch.where(acc[:, None], Xn, X)
+        c = torch.where(acc, cn, c)
+        lam = torch.where(acc, (lam * 0.1).clamp(min=1e-12), lam * 10)
+        done = acc & (d.norm(dim=1) <= 1e-12 * X.norm(dim=1))
+        active = active & ~done & ~(~acc & (lam > 1e16))
+    return X
+
+
+class RANSACTriangulationNet(_EngineOwner):
+    """Drop-in for reference mvn/models/triangulation.py:17-128 (the "ransac" model of train.py): raw backbone heat maps -> arg-max
+    key points -> per-(sample, joint) RANSAC over view pairs, the inlier DLT and, with `config.model.direct_optimization`, the Huber
+    refinement of the reprojection error.  Same ctor keys, config side effects, `backbone` attribute, state_dict keys and 4-tuple.
+    The view pairs are drawn on the host with Python's `random` in the reference's order (draw_view_pairs).
+    backend="native": eval / no-grad on the kernels (engine.ransac_forward); "torch": the torch backbone and the batched float64
+    formulation triangulate_ransac_batch (CPU or GPU).  Neither trains through the RANSAC, as the reference does not."""
+
+    n_iters = 10                        # triangulate_ransac's defaults (:72)
+    reprojection_error_epsilon = 15
+
+    def __init__(self, config, device="cuda:0", backend=None, conv_mode=None):
+        super().__init__()
+        config.model.backbone.alg_confidences = False      # the reference mutates the caller's config here (:21-23); so do we
+        config.model.backbone.vol_confidences = False
+        self.backbone = pose_resnet.get_pose_net(config.model.backbone, device=device)
+        self.direct_optimization = config.model.direct_optimization
+        self.backend = backend or os.environ.get("LT_B200_BACKEND", "native")
+        if self.backend not in ("native", "torch"):
+            raise ValueError("unknown backend {!r} (RANSACTriangulationNet has 'native' and 'torch')".format(self.backend))
+        self.conv_mode = conv_mode or os.environ.get("LT_B200_CONV", "tc")
+        self._engine = None
+        self._train_graphs = None
+
+    def engine(self):
+        if self._engine is None:
+            from .engine import NativeEngine
+            self._engine = NativeEngine(self, mode=self.conv_mode, use_graph=False)
+        return self._engine
+
+    def forward(self, images, proj_matricies, batch):
+        B, V = images.shape[:2]
+        assert V >= 2                                       # triangulate_ransac (:74), before anything is drawn
+        if self.backend == "torch":
+            return self._forward_torch(images, proj_matricies)
+        if not images.is_cuda:
+            raise RuntimeError("lt_b200 native backend needs CUDA tensors; construct the model with backend='torch' for CPU/autograd")
+        if self.training or torch.is_grad_enabled():
+            raise RuntimeError("lt_b200 native backend is inference-only: use model.eval() under torch.no_grad(), or backend='torch'")
+        H, W = images.shape[3:]
+        if H % 2 or W % 2:
+            raise ValueError("lt_b200 native backend needs even image sides (space-to-depth stem), got %dx%d" % (H, W))
+        dev = images.device
+        pairs = draw_view_pairs(B, self.backbone.num_joints, V, self.n_iters)
+        with torch.cuda.device(dev):
+            pairs_t, = _upload(dev, pairs, dtype=torch.int32)
+            return self.engine().ransac_forward(images.float().contiguous(), proj_matricies.to(dev, torch.float32).contiguous(), pairs_t,
+                                                self.n_iters, self.reprojection_error_epsilon, self.direct_optimization)
+
+    def _forward_torch(self, images, proj_matricies):
+        """The reference forward with the batched torch RANSAC: -> (keypoints_3d, keypoints_2d int64, heatmaps, confidences)."""
+        B, V = images.shape[:2]
+        H, W = images.shape[3:]
+        dev = images.device
+        heatmaps, _, _, _ = self.backbone(images.reshape(-1, *images.shape[2:]), layers.torch_conv, layers.torch_norm)
+        J, h, w = heatmaps.shape[1:]
+        heatmaps = heatmaps.view(B, V, J, h, w)
+        _, idx = torch.max(heatmaps.view(B, V, J, -1), dim=-1)                  # :45-52
+        kp = torch.stack([idx % w, idx // w], dim=-1)
+        keypoints_2d = torch.zeros_like(kp)
+        keypoints_2d[..., 0] = kp[..., 0] * (W / w)
+        keypoints_2d[..., 1] = kp[..., 1] * (H / h)
+        pairs = torch.from_numpy(draw_view_pairs(B, J, V, self.n_iters))
+        kp3d, _ = triangulate_ransac_batch(proj_matricies, keypoints_2d.detach(), pairs, self.reprojection_error_epsilon,
+                                           self.direct_optimization)
+        confidences = torch.zeros((B, V, J), dtype=torch.float32, device=dev)   # :59, the "plug"
+        return kp3d.float(), keypoints_2d, heatmaps, confidences
