@@ -36,6 +36,10 @@ __global__ void __launch_bounds__(256) coord_volume_kernel(const float* __restri
 }
 
 // ---- max pooling, channels-last, 4 channels per thread ----------------------------------------------
+// torch's max_pool rule per lane, in window order: a value replaces the running maximum if it is greater or NaN, so a NaN in the
+// window gives NaN (fmaxf would drop it); taps in the padding are skipped, i.e. they count as -inf.
+__device__ __forceinline__ float pool_max(float m, float v) { return (v > m || isnan(v)) ? v : m; }
+
 struct PoolParams {
   const void* in; void* out; int format;
   int N, ID, IH, IW, C, kd, kh, kw, sd, sh, sw, pd, ph, pw, OD, OH, OW;
@@ -65,7 +69,7 @@ __global__ void __launch_bounds__(256) maxpool_kernel(const PoolParams p) {
           float4 v;
           if (p.format == LT_FMT_F32) v = __ldg(reinterpret_cast<const float4*>(reinterpret_cast<const float*>(p.in) + pix * p.C + c));
           else v = load_s32x4(reinterpret_cast<const sh_t*>(p.in) + pix * 2 * p.C, c);
-          m.x = fmaxf(m.x, v.x); m.y = fmaxf(m.y, v.y); m.z = fmaxf(m.z, v.z); m.w = fmaxf(m.w, v.w);
+          m.x = pool_max(m.x, v.x); m.y = pool_max(m.y, v.y); m.z = pool_max(m.z, v.z); m.w = pool_max(m.w, v.w);
         }
       }
     }
@@ -221,10 +225,15 @@ static inline unsigned grid_for(long total, int per_block = 256) {
 // (Cout, Cin, KD, KH, KW), transposed convs (Cin, Cout, ...) and their stride phases (a sub-lattice of taps walked with negative
 // strides) are all affine maps, so ONE kernel replaces the permute / slice / pad / contiguous chain.
 __global__ void __launch_bounds__(256) absmax_kernel(const float* __restrict__ w, long n, unsigned* __restrict__ out_bits) {
+  // max |w| over the finite elements only: each non-finite element is skipped on its own, so an Inf does not hide the finite
+  // values its warp read (fmaxf already drops NaN)
   float m = 0.0f;
-  for (long i = (long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (long)gridDim.x * blockDim.x) m = fmaxf(m, fabsf(w[i]));
+  for (long i = (long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (long)gridDim.x * blockDim.x) {
+    const float a = fabsf(w[i]);
+    if (a < INFINITY) m = fmaxf(m, a);
+  }
   m = warp_max(m);
-  if ((threadIdx.x & 31) == 0 && m > 0.0f && m < INFINITY) atomicMax(out_bits, __float_as_uint(m));   // non-negative floats order like their bits
+  if ((threadIdx.x & 31) == 0 && m > 0.0f) atomicMax(out_bits, __float_as_uint(m));   // non-negative floats order like their bits
 }
 
 __global__ void __launch_bounds__(256) gather_weights_kernel(const float* __restrict__ w, long base, long s_td, long s_th, long s_tw, long s_ci,
