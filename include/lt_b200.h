@@ -102,6 +102,25 @@ int lt_coord_volume_fwd(const float* position, const float* center, const float*
                         float* out, int B, int n, int transfer_cmu, void* stream);
 
 /* ------------------------------------------------------------------------------------------
+ * Cuboid placement from predicted key points (TwoStageTriangulationNet).  Replaces the host
+ * hand-off of the reference's two-stage protocol: the algebraic model's evaluation writes
+ * results.pkl, the volumetric run reloads it as batch['pred_keypoints_3d'] (pred_results_path)
+ * and places each cuboid around its pelvis on the host, triangulation.py:284-296.
+ *   keypoints_3d[B][J][3] : float32 key points (the algebraic model's output)
+ *   kind                  : LT_KIND_MPII (joint 6, J >= 7) or LT_KIND_COCO (mean of joints 11
+ *                           and 12, J >= 13)
+ *   center[B][3]          : the base point, float32; the coco mean is the float32 sum halved in
+ *                           float32, as numpy computes it on the float32 array
+ *   position[B][3]        : float32((double)center - cuboid_side / 2), formed in float64
+ * No FMA contraction: the values equal what the host path uploads for the same key points bit
+ * for bit.  It writes the buffers lt_coord_volume_fwd reads.  A few threads per batch, not a hot
+ * path: what it saves is the device-to-host copy and synchronisation between the two stages.
+ * ---------------------------------------------------------------------------------------- */
+enum lt_skeleton_kind { LT_KIND_MPII = 0, LT_KIND_COCO = 1 };
+int lt_cuboid_from_keypoints_fwd(const float* keypoints_3d, int B, int J, int kind, double cuboid_side, float* center,
+                                 float* position, void* stream);
+
+/* ------------------------------------------------------------------------------------------
  * Fused unprojection + view aggregation.  Replaces op.unproject_heatmaps (op.py:99-166):
  * per voxel, per view: project with proj (3x4), depth mask, bilinear sample of the feature map
  * (grid_sample align_corners=True, zero padding, incl. the reference's x/H, y/W normalisation

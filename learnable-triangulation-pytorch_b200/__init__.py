@@ -10,7 +10,8 @@ Python identifier; `lt_b200.py` at the repo root is the import shim).
 """
 from . import loss, multiview, op, pipeline, pose_resnet, v2v, volumetric  # noqa: F401
 from .multiview import Camera  # noqa: F401
-from .triangulation import AlgebraicTriangulationNet, RANSACTriangulationNet, VolumetricTriangulationNet  # noqa: F401
+from .triangulation import (AlgebraicTriangulationNet, RANSACTriangulationNet, TwoStageTriangulationNet,  # noqa: F401
+                            VolumetricTriangulationNet)
 from .v2v import V2VModel  # noqa: F401
 
 __version__ = "0.1.0"

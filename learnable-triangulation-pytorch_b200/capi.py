@@ -16,6 +16,7 @@ LIB_PATH = os.path.join(_HERE, "liblt_b200.so")
 
 FMT_F32, FMT_S32 = 0, 1
 AGG = {"sum": 0, "max": 1, "softmax": 2, "conf": 3, "conf_norm": 3}
+KIND = {"mpii": 0, "coco": 1}
 CONV_SIMT, CONV_TC, CONV_TC1, CONV_TC_FOLD = 0, 1, 2, 3
 RES_NONE, RES_BEFORE_RELU, RES_AFTER_RELU = 0, 1, 2
 
@@ -70,6 +71,7 @@ SIGNATURES = {
     "lt_last_error_string": (ctypes.c_char_p, []),
     "lt_device_info": (c_int, [ctypes.POINTER(c_int)] * 3),
     "lt_coord_volume_fwd": (c_int, [c_void_p] * 5 + [c_int, c_int, c_int, c_void_p]),
+    "lt_cuboid_from_keypoints_fwd": (c_int, [c_void_p, c_int, c_int, c_int, c_double, c_void_p, c_void_p, c_void_p]),
     "lt_unproject_aggregate_fwd": (c_int, [c_void_p] * 5 + [c_int] * 6 + [c_long, c_int, c_void_p]),
     "lt_unproject_partial_fwd": (c_int, [c_void_p] * 5 + [c_int] * 5 + [c_long, c_int, c_void_p]),
     "lt_unproject_finalize_fwd": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_long, c_int, c_void_p]),
@@ -223,6 +225,15 @@ def coord_volume(position, center, step, rot, out, transfer_cmu=False):
     B, n = out.shape[0], out.shape[1]
     _check(lib().lt_coord_volume_fwd(_ptr(position), _ptr(center), _ptr(step), _ptr(rot), _ptr(out), B, n,
                                      int(transfer_cmu), _stream()), "lt_coord_volume_fwd")
+
+
+def cuboid_from_keypoints(keypoints_3d, kind, cuboid_side, center, position):
+    """keypoints_3d (B, J, 3) float32 -> center and position (B, 3) float32, written: the base point of skeleton `kind` ("mpii" or
+    "coco") and base - cuboid_side / 2 formed in float64, as the host geometry computes them."""
+    B, J = keypoints_3d.shape[:2]
+    assert keypoints_3d.dtype == center.dtype == position.dtype == torch.float32
+    _check(lib().lt_cuboid_from_keypoints_fwd(_ptr(keypoints_3d), B, J, KIND[kind], float(cuboid_side), _ptr(center), _ptr(position),
+                                              _stream()), "lt_cuboid_from_keypoints_fwd")
 
 
 def unproject_aggregate(features_cl, proj, coord, conf, out, out_format, agg):

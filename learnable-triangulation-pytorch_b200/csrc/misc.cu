@@ -35,6 +35,23 @@ __global__ void __launch_bounds__(256) coord_volume_kernel(const float* __restri
   }
 }
 
+// ---- cuboid placement from predicted key points ------------------------------------------------------
+// One thread per (sample, axis): the values _base_points / _host_geometry compute on the host from the key points as float32
+// numpy rows.  The coco hip midpoint is the float32 sum halved in float32, as numpy's / 2 on a float32 array (x * 0.5 rounds to
+// the same float as x / 2); position = base - side / 2 is formed in float64 and rounded to float32 last.  Explicit _rn
+// intrinsics: nothing is contracted into an FMA.  Not a hot path: a few threads per batch between the algebraic and the
+// volumetric stage.
+__global__ void cuboid_from_keypoints_kernel(const float* __restrict__ keypoints, int B, int J, int kind, double side,
+                                             float* __restrict__ center, float* __restrict__ position) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= B * 3) return;
+  const int b = i / 3, c = i - b * 3;
+  const float* kp = keypoints + (long)b * J * 3;
+  const float base = kind == LT_KIND_COCO ? __fmul_rn(__fadd_rn(kp[11 * 3 + c], kp[12 * 3 + c]), 0.5f) : kp[6 * 3 + c];
+  center[i] = base;
+  position[i] = __double2float_rn(__dsub_rn((double)base, __ddiv_rn(side, 2.0)));
+}
+
 // ---- max pooling, channels-last, 4 channels per thread ----------------------------------------------
 // torch's max_pool rule per lane, in window order: a value replaces the running maximum if it is greater or NaN, so a NaN in the
 // window gives NaN (fmaxf would drop it); taps in the padding are skipped, i.e. they count as -inf.
@@ -357,6 +374,17 @@ extern "C" int lt_coord_volume_fwd(const float* position, const float* center, c
   LT_REQUIRE(B > 0 && n > 1, "coord_volume: bad size B=%d n=%d", B, n);
   coord_volume_kernel<<<grid_for((long)B * n * n * n), 256, 0, (cudaStream_t)stream>>>(position, center, step, rot, out, B, n, transfer_cmu);
   LT_CHECK_LAUNCH("coord_volume_kernel");
+  return LT_OK;
+}
+
+extern "C" int lt_cuboid_from_keypoints_fwd(const float* keypoints_3d, int B, int J, int kind, double cuboid_side, float* center,
+                                            float* position, void* stream) {
+  LT_REQUIRE(keypoints_3d && center && position, "cuboid_from_keypoints: null pointer");
+  LT_REQUIRE(kind == LT_KIND_MPII || kind == LT_KIND_COCO, "cuboid_from_keypoints: unknown skeleton kind %d", kind);
+  LT_REQUIRE(B > 0 && J > (kind == LT_KIND_COCO ? 12 : 6), "cuboid_from_keypoints: bad size B=%d J=%d for skeleton kind %d", B, J, kind);
+  cuboid_from_keypoints_kernel<<<ceil_div(B * 3, 128), 128, 0, (cudaStream_t)stream>>>(keypoints_3d, B, J, kind, cuboid_side, center,
+                                                                                      position);
+  LT_CHECK_LAUNCH("cuboid_from_keypoints_kernel");
   return LT_OK;
 }
 

@@ -356,6 +356,7 @@ class NativeEngine:
         self._packs_version = None
         self._epoch = 0
         self._graphs = {}
+        self._grids2d = {}         # (h, w, B*V, device) -> pixel_grid of the algebraic forward's 2-D soft-argmax
         self.launches = 0          # kernels launched by the last eager forward (our own kernels only)
         self.timeline = None       # set to [] to record (label, flops, bytes, start_evt, end_evt) per launch
         capi.lib()                 # fail loudly if the extension is missing
@@ -871,18 +872,22 @@ class NativeEngine:
         trunk = self.backbone_trunk(images.reshape(B * V, *images.shape[2:]))
         logits = self._conv(self.backbone_upsample(trunk), self._packs["final"], relu=False, out_fmt=FMT_F32)   # (BV,1,h,w,32)
         h, w = logits.H, logits.W
-        # 2-D soft-argmax (op.py:11-47) = the 3-D kernels with pixel-index coordinates (x, y, 0)
-        key = ("grid2d", h, w, B * V)
-        if getattr(self, "_grid_key", None) != key:
-            self._grid2d, self._grid_key = pixel_grid(B * V, h, w, dev), key
+        # 2-D soft-argmax (op.py:11-47) = the 3-D kernels with pixel-index coordinates (x, y, 0).  One grid per shape, kept: a grid
+        # made during a CUDA-graph capture is filled only by a replay, and a captured graph reads its grid at a fixed address
+        key = (h, w, B * V, dev)
+        grid = self._grids2d.get(key)
+        if grid is None:
+            grid = self._grids2d[key] = pixel_grid(B * V, h, w, dev)
         heat = torch.empty((B * V, J, h, w), dtype=torch.float32, device=dev)
         kp = torch.empty((B * V, J, 3), dtype=torch.float32, device=dev)
         ws = torch.empty(capi.softargmax3d_workspace_bytes(B * V, J, h * w) // 4 + 1, dtype=torch.float32, device=dev)
-        capi.softargmax3d(logits.data, h * w * logits.C, logits.C, 1, self._grid2d, heat, kp, ws, B * V, J, h * w, heatmap_multiplier,
+        capi.softargmax3d(logits.data, h * w * logits.C, logits.C, 1, grid, heat, kp, ws, B * V, J, h * w, heatmap_multiplier,
                           1 if heatmap_softmax else 2)    # op.py:25-41: ReLU heat-maps, centre of mass / mass
         self.launches += 3
-        kp2d = kp[:, :, :2].reshape(B, V, J, 2) * torch.tensor([W / w, H / h], device=dev, dtype=torch.float32)   # :181-184
-        kp2d = kp2d.contiguous()
+        # the (W / w, H / h) scale (:181-184) is filled on the device: a host-to-device copy cannot be captured
+        scale = torch.full((2,), W / w, device=dev, dtype=torch.float32)
+        scale[1].fill_(H / h)
+        kp2d = (kp[:, :, :2].reshape(B, V, J, 2) * scale).contiguous()
         if use_confidences:
             conf = self.confidence_head(trunk, "alg_confidences").view(B, V, J)
         else:

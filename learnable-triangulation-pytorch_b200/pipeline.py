@@ -164,7 +164,8 @@ def prepare_batch(batch, device, config=None, is_train=True, normalize_u8=False,
 class InferenceStream:
     """Pipelined serving loop over host batches.
 
-        stream = InferenceStream(model)                    # model: VolumetricTriangulationNet on a CUDA device, eval
+        stream = InferenceStream(model)                    # model: VolumetricTriangulationNet or TwoStageTriangulationNet
+                                                           # on a CUDA device, eval
         for keypoints in stream.run(batches):              # batches: iterable of collated batch dicts
             ...                                            # keypoints: (B, J, 3) float32 numpy array
 

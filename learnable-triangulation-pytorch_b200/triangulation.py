@@ -10,6 +10,7 @@ backend="native" (default; eval/no-grad on a CUDA device): host geometry is vect
 sm_90a kernels through engine.NativeEngine.  backend="torch": autograd-capable torch ops
 (training, CPU plumbing).  Nothing switches backend silently.
 """
+import collections.abc
 import os
 import random
 
@@ -17,7 +18,7 @@ import numpy as np
 import torch
 from torch import nn
 
-from . import autograd_ops, layers, multiview, op, pose_resnet, torch_ops, volumetric
+from . import autograd_ops, capi, layers, multiview, op, pose_resnet, torch_ops, volumetric
 from .train_graph import TrainGraphs
 from .v2v import V2VModel
 
@@ -46,6 +47,12 @@ def _base_points(batch, batch_size, kind, use_gt_pelvis):
         else:
             raise KeyError("unknown skeleton kind {!r}".format(kind))
     return pts
+
+
+def _place_cuboids(base, sides):
+    """Cuboid corner base - sides / 2 (B, 3) float64 and the per-sample volumetric.Cuboid3D (triangulation.py:298-303)."""
+    position = base - sides / 2
+    return position, [volumetric.Cuboid3D(position[b], sides) for b in range(base.shape[0])]
 
 
 _NO_V2V = object()      # the v2v_backend of a model without a V2V net (None stays an unknown v2v_backend)
@@ -169,18 +176,23 @@ class VolumetricTriangulationNet(_EngineOwner):
 
     # ---------------------------------------------------------------- host-side geometry
     def _host_geometry(self, batch, batch_size, image_shape, heatmap_shape):
-        proj = multiview.stack_projections(batch["cameras"], image_shape, heatmap_shape)      # (B, V, 3, 4) f32
         base = _base_points(batch, batch_size, self.kind, self.use_gt_pelvis)                 # (B, 3) f64
+        proj, sides, step, rots = self._pelvis_free_geometry(batch, batch_size, image_shape, heatmap_shape)
+        position, cuboids = _place_cuboids(base, sides)
+        return proj, base, position, step, rots, cuboids
+
+    def _pelvis_free_geometry(self, batch, batch_size, image_shape, heatmap_shape):
+        """The host geometry that does not depend on the pelvis: heat-map-space projections (B, V, 3, 4) float32, the cuboid sides
+        (3,) and voxel step (3,) float64, rotations (B, 3, 3) float64 (a random angle per sample in training)."""
+        proj = multiview.stack_projections(batch["cameras"], image_shape, heatmap_shape)
         sides = np.array([self.cuboid_side] * 3, dtype=np.float64)
-        position = base - sides / 2
-        cuboids = [volumetric.Cuboid3D(position[b], sides) for b in range(batch_size)]
         axis = [0, 1, 0] if self.kind == "coco" else [0, 0, 1]
         rots = np.empty((batch_size, 3, 3), dtype=np.float64)
         for b in range(batch_size):
             theta = np.random.uniform(0.0, 2 * np.pi) if self.training else 0.0   # triangulation.py:318-321
             rots[b] = volumetric.get_rotation_matrix(axis, theta)
         step = sides / (self.volume_size - 1)
-        return proj, base, position, step, rots, cuboids
+        return proj, sides, step, rots
 
     def engine(self):
         if self._engine is None:
@@ -514,3 +526,145 @@ class RANSACTriangulationNet(_EngineOwner):
                                            self.direct_optimization)
         confidences = torch.zeros((B, V, J), dtype=torch.float32, device=dev)   # :59, the "plug"
         return kp3d.float(), keypoints_2d, heatmaps, confidences
+
+
+class LazyCuboids(collections.abc.Sequence):
+    """The per-sample volumetric.Cuboid3D of a TwoStageTriangulationNet forward, built on first access.  That access copies the
+    device base points to the host, the forward's only synchronisation, paid only by a caller that reads the cuboids (e.g. for
+    visualisation).  The positions are base - side / 2 in float64 from those float32 base points, as _host_geometry forms them from
+    the same key points, so each Cuboid3D equals the two-pass protocol's."""
+
+    def __init__(self, base_points, cuboid_side):
+        self._base = base_points
+        self._side = cuboid_side
+        self._items = None
+
+    def _built(self):
+        if self._items is None:
+            base = self._base.cpu().numpy().astype(np.float64)
+            self._items = _place_cuboids(base, np.array([self._side] * 3, dtype=np.float64))[1]
+            self._base = None
+        return self._items
+
+    def __len__(self):
+        return self._base.shape[0] if self._items is None else len(self._items)
+
+    def __getitem__(self, i):
+        return self._built()[i]
+
+
+class TwoStageTriangulationNet(_EngineOwner):
+    """The volumetric model without ground truth: each sample's cuboid is placed at the pelvis of an algebraic model's key points,
+    on the device.  This is the reference's two-stage protocol (evaluate AlgebraicTriangulationNet, reload its results file as
+    batch['pred_keypoints_3d'] for a volumetric config with use_gt_pelvis: false) without the host round trip between the stages.
+
+    forward(images, proj_matricies, batch) returns the volumetric model's 7-tuple.  proj_matricies are the image-space matrices the
+    algebraic model takes; None derives them from batch['cameras'] as prepare_batch does.  The volumetric stage keeps its host geometry
+    from batch['cameras'].  The algebraic forward, the hand-off (lt_cuboid_from_keypoints_fwd) and the volumetric device forward replay
+    from one CUDA graph per input shape, re-captured when either model's packed weights go stale.  `base_points` is the device pelvis;
+    `cuboids` is a LazyCuboids.  Native backend, inference only."""
+
+    def __init__(self, algebraic, volumetric):
+        super().__init__()
+        if not isinstance(algebraic, AlgebraicTriangulationNet) or not isinstance(volumetric, VolumetricTriangulationNet):
+            raise ValueError("TwoStageTriangulationNet takes an AlgebraicTriangulationNet and a VolumetricTriangulationNet (got %s, %s)"
+                             % (type(algebraic).__name__, type(volumetric).__name__))
+        for name, m in (("algebraic", algebraic), ("volumetric", volumetric)):
+            if m.backend != "native":
+                raise ValueError("TwoStageTriangulationNet runs the native backend only; the %s model has backend=%r" % (name, m.backend))
+        devices = {str(t.device) for m in (algebraic, volumetric) for t in m.parameters()}
+        if len(devices) != 1:
+            raise ValueError("both models must live on one device (got %s)" % ", ".join(sorted(devices)))
+        if algebraic.backbone.num_joints != volumetric.num_joints:
+            raise ValueError("the models predict different joint counts (algebraic %d, volumetric %d)"
+                             % (algebraic.backbone.num_joints, volumetric.num_joints))
+        if volumetric.use_gt_pelvis:
+            raise ValueError("the volumetric model has use_gt_pelvis=True; the two-stage model places its cuboids at the algebraic "
+                             "model's pelvis, so it needs a model configured with use_gt_pelvis=False")
+        if volumetric.kind not in capi.KIND:
+            raise ValueError("unknown skeleton kind {!r} (mpii or coco)".format(volumetric.kind))
+        pelvis_joint = 12 if volumetric.kind == "coco" else 6
+        if volumetric.num_joints <= pelvis_joint:
+            raise ValueError("skeleton kind %r reads joint %d, but the models predict %d joints"
+                             % (volumetric.kind, pelvis_joint, volumetric.num_joints))
+        self.algebraic = algebraic
+        self.volumetric = volumetric
+        self.training = algebraic.training or volumetric.training      # the mode of the models it was given; .eval() sets all three
+        self.clone_outputs = True
+        self._graphs = {}
+
+    def _invalidate_engine(self):
+        self._graphs = {}
+        self.algebraic._invalidate_engine()
+        self.volumetric._invalidate_engine()
+
+    def forward(self, images, proj_matricies, batch):
+        if self.algebraic.training or self.volumetric.training or torch.is_grad_enabled():
+            raise RuntimeError("TwoStageTriangulationNet is inference-only: call model.eval() under torch.no_grad()")
+        if not images.is_cuda:
+            raise RuntimeError("TwoStageTriangulationNet runs the native backend: it needs CUDA tensors (got %s)" % images.device)
+        dev = images.device
+        if next(self.parameters()).device != dev:
+            raise RuntimeError("the images are on %s, the models on %s" % (dev, next(self.parameters()).device))
+        B = images.shape[0]
+        H, W = images.shape[3:]
+        if H % 2 or W % 2:
+            raise ValueError("lt_b200 native backend needs even image sides (space-to-depth stem), got %dx%d" % (H, W))
+        hm_shape = (backbone_map_size(H), backbone_map_size(W))
+        proj_hm, _, step, rots = self.volumetric._pelvis_free_geometry(batch, B, (H, W), hm_shape)
+        host = (proj_hm, step, rots.reshape(B, 9))
+        if proj_matricies is None:
+            host += (multiview.stack_projections(batch["cameras"]),)                # datasets/utils.py:61-63
+        with torch.cuda.device(dev):
+            up = _upload(dev, *host)
+            proj_img = up[3] if proj_matricies is None else proj_matricies.to(dev, torch.float32).contiguous()
+            outs = self._replay(images.float().contiguous(), proj_img, *up[:3])
+        if self.clone_outputs:
+            outs = tuple(o.clone() for o in outs)
+        center, kp, features, volumes, coord = outs[:5]
+        if tuple(features.shape[3:]) != hm_shape:
+            raise RuntimeError("feature map %s differs from the heat-map size %s used for the projection matrices"
+                               % (tuple(features.shape[3:]), hm_shape))
+        vol_conf = outs[5] if len(outs) > 5 else None
+        cuboids = LazyCuboids(center if self.clone_outputs else center.clone(), self.volumetric.cuboid_side)
+        return kp, features, volumes, vol_conf, cuboids, coord, center
+
+    def _replay(self, *inputs):
+        """_device_forward(*inputs) replayed from the graph of this input shape; captured on a miss or when either engine's packed
+        weights are stale.  -> the graph's static outputs."""
+        version = (self.algebraic.engine()._param_version(), self.volumetric.engine()._param_version())
+        key = (tuple(inputs[0].shape), inputs[0].device)
+        entry = self._graphs.get(key)
+        if entry is None or entry[0] != version:
+            self._graphs.pop(key, None)                  # free the stale graph's memory before capturing its successor
+            entry = self._graphs[key] = (version,) + self._capture(inputs)
+        _, graph, static_in, static_out = entry
+        for dst, src in zip(static_in, inputs):
+            dst.copy_(src, non_blocking=True)
+        graph.replay()
+        return static_out
+
+    def _capture(self, inputs):
+        self.algebraic.engine().prepare()
+        self.volumetric.engine().prepare()
+        static_in = [t.clone() for t in inputs]
+        side = torch.cuda.Stream(device=inputs[0].device)
+        side.wait_stream(torch.cuda.current_stream())
+        with torch.cuda.stream(side):
+            self._device_forward(*static_in)     # warm-up: module loads, function attributes, the soft-argmax grid
+        torch.cuda.current_stream().wait_stream(side)
+        torch.cuda.synchronize()
+        graph = torch.cuda.CUDAGraph()
+        with torch.cuda.graph(graph):
+            static_out = self._device_forward(*static_in)
+        return graph, static_in, static_out
+
+    def _device_forward(self, images, proj_img, proj_hm, step, rot):
+        """Both stages and the hand-off on the device: (images, image-space and heat-map-space projections, voxel step, rotations
+        (B, 9)) -> (base points, kp, features, volumes, coord[, vol_conf])."""
+        a, v = self.algebraic, self.volumetric
+        kp_alg = a.engine().algebraic_forward(images, proj_img, a.heatmap_multiplier, a.use_confidences, a.heatmap_softmax)[0]
+        center = torch.empty((images.shape[0], 3), dtype=torch.float32, device=images.device)
+        position = torch.empty_like(center)
+        capi.cuboid_from_keypoints(kp_alg, v.kind, v.cuboid_side, center, position)
+        return (center,) + tuple(v.engine()._device_forward(images, proj_hm, position, center, step, rot))
