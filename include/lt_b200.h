@@ -435,6 +435,27 @@ int lt_volumetric_ce_bwd(const float* grad_loss, const int* index, const float* 
                          int B, int J, long nvox, void* stream);
 
 /* ------------------------------------------------------------------------------------------
+ * Keypoint criteria of the training recipe.  Replace KeypointsMSELoss, KeypointsMSESmoothLoss, KeypointsMAELoss and
+ * KeypointsL2Loss (mvn/models/loss.py:7-49), whose divisor max(1, sum v) is read to the host with .item() (and MSESmooth's
+ * boolean-mask index synchronises once more).  pred, gt [n_points][dim] float32 (n_points = B * J), validity [n_points]:
+ *   LT_KP_MSE         sum (gt - pred)^2 v / (dim * max(1, sum v))
+ *   LT_KP_MSE_SMOOTH  the same with every d = (gt - pred)^2 v > threshold (strictly) replaced by d^0.1 * threshold^0.9
+ *   LT_KP_MAE         sum |gt - pred| v / (dim * max(1, sum v))
+ *   LT_KP_L2          sum over points of sqrt(sum_d (gt - pred)^2 v) / max(1, sum v)
+ * Every term is formed in float64 and multiplied by v whatever v is (a non-finite residual at v = 0 gives NaN, as in the
+ * reference); the terms and sum v are summed in float64 in a fixed order inside one CTA (bitwise-equal repeats).  loss: one float
+ * (the float64 quotient rounded); norm: one double, the divisor, kept on the device for the backward.  No host synchronisation. */
+enum lt_keypoints_loss_kind { LT_KP_MSE = 0, LT_KP_MSE_SMOOTH = 1, LT_KP_MAE = 2, LT_KP_L2 = 3 };
+int lt_keypoints_loss_fwd(const float* pred, const float* gt, const float* validity, float* loss, double* norm, int kind,
+                          double threshold, int n_points, int dim, void* stream);
+/* Backward: grad_loss (DEVICE pointer, one float) and norm (lt_keypoints_loss_fwd's) -> grad_pred [n_points][dim] WRITTEN in full:
+ * g / norm times the derivative autograd takes through the reference formula, in float64, rounded once.  MSE_SMOOTH's replaced
+ * branch has 0.1 d^-0.9 threshold^0.9 dd/dpred; L2's is -(g / (2 sqrt(s))) v 2 (gt - pred), NaN where s = 0, as in torch.  The
+ * ground truth and the validity get no gradient. */
+int lt_keypoints_loss_bwd(const float* grad_loss, const float* pred, const float* gt, const float* validity, const double* norm,
+                          float* grad_pred, int kind, double threshold, int n_points, int dim, void* stream);
+
+/* ------------------------------------------------------------------------------------------
  * Batch-statistics BatchNorm for training, fused with the ReLU after it and the residual add of a residual unit.  Replaces
  * nn.BatchNorm2d / nn.BatchNorm3d in train and eval mode with the nn.ReLU and the `+ shortcut` that follow them (pose_resnet.py:25-137
  * residual units, stem and deconv stack; v2v.py:7-66 Basic3DBlock, Res3DBlock, Upsample3DBlock).
@@ -531,6 +552,10 @@ int lt_test_triangulate_dlt_proj_bwd_host(const float* proj, const float* keypoi
  * the kernels' distance, argmin key, term and gradient code: loss.py:52-80. */
 int lt_test_volumetric_ce_host(const float* probs, const float* coord, const float* keypoints_gt, const float* validity, float* loss,
                                int* index, float* picked, const float* grad_loss, float* grad_probs, int B, int J, long nvox);
+/* lt_keypoints_loss_fwd (+ lt_keypoints_loss_bwd when grad_pred is not NULL, grad_loss then a HOST pointer) on host pointers, with
+ * the kernels' term, derivative and summation order: loss.py:7-49. */
+int lt_test_keypoints_loss_host(const float* pred, const float* gt, const float* validity, float* loss, double* norm,
+                                const float* grad_loss, float* grad_pred, int kind, double threshold, int n_points, int dim);
 /* lt_conv_wgrad_fwd's index mapping (which input row and which output-gradient row meet for a tap, M tile, row and output group) on
  * host pointers, summed in double over plain float32 channels-last tensors: in [N][ID][IH][IW][desc->Cin], grad_out [N][FD][FH][FW][FC]
  * -> grad_w [taps][Cin][G * Cout]. */

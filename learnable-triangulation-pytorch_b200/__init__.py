@@ -10,6 +10,7 @@ Python identifier; `lt_b200.py` at the repo root is the import shim).
 """
 from . import loss, multiview, op, pipeline, pose_resnet, v2v, volumetric  # noqa: F401
 from .multiview import Camera  # noqa: F401
+from .train_graph import TrainStep  # noqa: F401
 from .triangulation import (AlgebraicTriangulationNet, RANSACTriangulationNet, TwoStageTriangulationNet,  # noqa: F401
                             VolumetricTriangulationNet)
 from .v2v import V2VModel  # noqa: F401
@@ -18,11 +19,12 @@ __version__ = "0.1.0"
 
 
 def install(mvn_package=None):
-    """Swap the reference's models, their custom ops and the volumetric cross-entropy loss for the native ones.
+    """Swap the reference's models, their custom ops, the keypoint criteria and the volumetric cross-entropy loss for the native
+    ones.
 
     `mvn_package` is the already-imported reference package (`import mvn`); if None it is imported.
     After this, the reference `train.py` (which does `from mvn.models.triangulation import
-    VolumetricTriangulationNet` and `from mvn.models.loss import ... VolumetricCELoss` at import time) picks up the
+    VolumetricTriangulationNet` and `from mvn.models.loss import KeypointsMSELoss, ..., VolumetricCELoss` at import time) picks up the
     native implementation unchanged.
     """
     import importlib
@@ -31,7 +33,8 @@ def install(mvn_package=None):
     tri = importlib.import_module(mvn_package.__name__ + ".models.triangulation")
     ref_op = importlib.import_module(mvn_package.__name__ + ".utils.op")
     ref_loss = importlib.import_module(mvn_package.__name__ + ".models.loss")
-    ref_loss.VolumetricCELoss = loss.VolumetricCELoss
+    for name in ("KeypointsMSELoss", "KeypointsMSESmoothLoss", "KeypointsMAELoss", "KeypointsL2Loss", "VolumetricCELoss"):
+        setattr(ref_loss, name, getattr(loss, name))
     tri.VolumetricTriangulationNet = VolumetricTriangulationNet
     tri.AlgebraicTriangulationNet = AlgebraicTriangulationNet
     tri.RANSACTriangulationNet = RANSACTriangulationNet

@@ -207,6 +207,33 @@ def volumetric_ce_loss(probs, coord, keypoints_gt, validity):
     return VolumetricCEFn.apply(probs, coord, keypoints_gt, validity)
 
 
+class KeypointsLossFn(torch.autograd.Function):
+    """The keypoint criteria (reference loss.py:7-49) on csrc/loss.cu: pred, gt (n, dim), validity (n,), float32 CUDA -> 0-dim loss.
+    `kind` is a capi.KEYPOINTS_LOSS name.  Only pred gets a gradient; the ground truth and the validity are data."""
+
+    @staticmethod
+    def forward(ctx, pred, gt, validity, kind, threshold):
+        p = pred.detach().contiguous()
+        loss = torch.empty(1, dtype=torch.float32, device=p.device)
+        norm = torch.empty(1, dtype=torch.float64, device=p.device)
+        capi.keypoints_loss(p, gt, validity, loss, norm, kind, threshold)
+        ctx.save_for_backward(p, gt, validity, norm)
+        ctx.kind, ctx.threshold = kind, threshold
+        return loss.reshape(())
+
+    @staticmethod
+    def backward(ctx, grad_loss):
+        p, gt, validity, norm = ctx.saved_tensors
+        grad = torch.empty_like(p)
+        capi.keypoints_loss_bwd(grad_loss.float().reshape(1).contiguous(), p, gt, validity, norm, grad, ctx.kind, ctx.threshold)
+        return grad, None, None, None, None
+
+
+def keypoints_loss(pred, gt, validity, kind, threshold=400.0):
+    """-> 0-dim loss; pred, gt (n, dim) and validity (n,) as KeypointsLossFn (gt and validity contiguous)."""
+    return KeypointsLossFn.apply(pred, gt, validity, kind, threshold)
+
+
 def integrate_tensor_2d(heatmaps, softmax=True):
     return IntegrateTensor2dFn.apply(heatmaps, softmax)
 

@@ -127,6 +127,9 @@ SIGNATURES = {
     "lt_volumetric_ce_fwd": (c_int, [c_void_p] * 8 + [c_size_t, c_int, c_int, c_long, c_void_p]),
     "lt_volumetric_ce_bwd": (c_int, [c_void_p] * 5 + [c_int, c_int, c_long, c_void_p]),
     "lt_test_volumetric_ce_host": (c_int, [c_void_p] * 9 + [c_int, c_int, c_long]),
+    "lt_keypoints_loss_fwd": (c_int, [c_void_p] * 5 + [c_int, c_double, c_int, c_int, c_void_p]),
+    "lt_keypoints_loss_bwd": (c_int, [c_void_p] * 6 + [c_int, c_double, c_int, c_int, c_void_p]),
+    "lt_test_keypoints_loss_host": (c_int, [c_void_p] * 7 + [c_int, c_double, c_int, c_int]),
     "lt_batch_norm_workspace_bytes": (c_size_t, [c_long, c_int]),
     "lt_batch_norm_plan": (c_int, [c_long, c_int, c_int, ctypes.POINTER(BatchNormPlan)]),
     "lt_batch_norm_fwd": (c_int, [c_void_p] * 9 + [c_long, c_int, c_float, c_float, c_int, c_int, c_void_p, c_size_t, c_void_p]),
@@ -468,6 +471,23 @@ def volumetric_ce_bwd(grad_loss, index, picked, validity, grad_probs):
            "lt_volumetric_ce_bwd")
 
 
+KEYPOINTS_LOSS = {"mse": 0, "mse_smooth": 1, "mae": 2, "l2": 3}
+
+
+def keypoints_loss(pred, gt, validity, loss, norm, kind, threshold=400.0):
+    """pred, gt (n, dim), validity (n,) float32 -> loss (1,) float32 and norm (1,) float64 (the divisor), written."""
+    n, dim = pred.shape
+    _check(lib().lt_keypoints_loss_fwd(_ptr(pred), _ptr(gt), _ptr(validity), _ptr(loss), _ptr(norm), KEYPOINTS_LOSS[kind],
+                                       float(threshold), n, dim, _stream()), "lt_keypoints_loss_fwd")
+
+
+def keypoints_loss_bwd(grad_loss, pred, gt, validity, norm, grad_pred, kind, threshold=400.0):
+    """grad_loss: one float32 on the device; grad_pred (n, dim) is written in full."""
+    n, dim = pred.shape
+    _check(lib().lt_keypoints_loss_bwd(_ptr(grad_loss), _ptr(pred), _ptr(gt), _ptr(validity), _ptr(norm), _ptr(grad_pred),
+                                       KEYPOINTS_LOSS[kind], float(threshold), n, dim, _stream()), "lt_keypoints_loss_bwd")
+
+
 def batch_norm_workspace_bytes(M, C):
     return lib().lt_batch_norm_workspace_bytes(M, C)
 
@@ -517,6 +537,19 @@ def volumetric_ce_host(probs, coord, keypoints_gt, validity, grad_loss=None, gra
                                             _host_ptr(loss), index.data_ptr(), _host_ptr(picked), _host_ptr(g), _host_ptr(grad_probs),
                                             B, J, nvox), "lt_test_volumetric_ce_host")
     return float(loss[0]), index, picked
+
+
+def keypoints_loss_host(pred, gt, validity, kind, threshold=400.0, grad_loss=None, grad_pred=None):
+    """lt_test_keypoints_loss_host: the criteria kernels' term, derivative and summation order run on CPU tensors (test hook, no GPU
+    needed).  Returns (loss float, divisor float); grad_pred (n, dim), if given, is written."""
+    n, dim = pred.shape
+    loss = torch.empty(1, dtype=torch.float32)
+    norm = torch.empty(1, dtype=torch.float64)
+    g = None if grad_loss is None else torch.tensor([float(grad_loss)], dtype=torch.float32)
+    _check(lib().lt_test_keypoints_loss_host(_host_ptr(pred), _host_ptr(gt), _host_ptr(validity), _host_ptr(loss), norm.data_ptr(),
+                                             _host_ptr(g), _host_ptr(grad_pred), KEYPOINTS_LOSS[kind], float(threshold), n, dim),
+           "lt_test_keypoints_loss_host")
+    return float(loss[0]), float(norm[0])
 
 
 def triangulate_dlt_host(proj, kp2d, conf, out):

@@ -278,3 +278,170 @@ extern "C" int lt_test_volumetric_ce_host(const float* probs, const float* coord
   }
   return LT_OK;
 }
+
+// ---------------------------------------------------------------------------------------------------------------------------------
+// Keypoint criteria of the training recipe (KeypointsMSELoss, KeypointsMSESmoothLoss, KeypointsMAELoss, KeypointsL2Loss,
+// loss.py:7-49) and their backward.  pred, gt [n][dim], validity [n]; every term is formed in float64 from the float32 inputs and
+// multiplied by v whatever v is (a non-finite residual at v = 0 gives NaN, as in the reference).
+//   kp_loss_fwd_kernel  one CTA: thread t sums the terms (and v) of points t, t + kKpThreads, ... in float64, then a fixed tree
+//                       over the threads: the same sum on every call.  The divisor dim * max(1, sum v) (L2: max(1, sum v)) stays
+//                       on the device for the backward; the loss is the float64 quotient rounded to float32.
+//   kp_loss_bwd_kernel  one thread per element: g / divisor times the derivative autograd takes through the reference formula.
+// The term, the derivative and the summation order are shared with the host test hook.
+namespace lt {
+
+constexpr int kKpThreads = 256;
+enum { kKpMse = 0, kKpMseSmooth = 1, kKpMae = 2, kKpL2 = 3 };
+
+// one point's term: MSE sum_d (gt - pred)^2 v; MSE_SMOOTH the same with each d = (gt - pred)^2 v > t replaced by d^0.1 t^0.9
+// (t09 = t^0.9); MAE sum_d |gt - pred| v; L2 sqrt(sum_d (gt - pred)^2 v)
+__host__ __device__ __forceinline__ double kp_term(const float* pred, const float* gt, double v, int dim, int kind, double t,
+                                                   double t09) {
+  double acc = 0.0;
+  for (int k = 0; k < dim; ++k) {
+    const double r = (double)gt[k] - (double)pred[k];
+    if (kind == kKpMae) {
+      acc += fabs(r) * v;
+    } else {
+      double d = r * r * v;
+      if (kind == kKpMseSmooth && d > t) d = pow(d, 0.1) * t09;
+      acc += d;
+    }
+  }
+  return kind == kKpL2 ? sqrt(acc) : acc;
+}
+
+// d loss / d pred[k] times g, where g = grad_loss / divisor: autograd's chain through the reference formula (sub, pow 2 or abs,
+// mul by v; MSE_SMOOTH's pow 0.1 on the replaced branch; L2's sum over d and sqrt, whose backward g / (2 sqrt(s)) is inf at s = 0,
+// so a zero-length residual gives NaN as in torch)
+__host__ __device__ __forceinline__ double kp_grad(const float* pred, const float* gt, double v, int k, int dim, int kind, double t,
+                                                   double t09, double g) {
+  const double r = (double)gt[k] - (double)pred[k];
+  if (kind == kKpMae) return -(g * v * (double)((r > 0.0) - (r < 0.0)));      // torch's sgn: 0 at 0 and at NaN
+  double gd = g;
+  if (kind == kKpMseSmooth) {
+    const double d = r * r * v;
+    if (d > t) gd = g * t09 * (0.1 * pow(d, -0.9));
+  } else if (kind == kKpL2) {
+    double s = 0.0;
+    for (int q = 0; q < dim; ++q) {
+      const double rq = (double)gt[q] - (double)pred[q];
+      s += rq * rq * v;
+    }
+    gd = g / (2.0 * sqrt(s));
+  }
+  return -(gd * v * (2.0 * r));
+}
+
+__host__ __device__ __forceinline__ double kp_divisor(double sum_v, int dim, int kind) {
+  const double m = sum_v > 1.0 ? sum_v : 1.0;          // python's max(1, x): 1 for a NaN sum as well
+  return kind == kKpL2 ? m : (double)dim * m;
+}
+
+__global__ void __launch_bounds__(kKpThreads) kp_loss_fwd_kernel(const float* __restrict__ pred, const float* __restrict__ gt,
+                                                                 const float* __restrict__ validity, int n, int dim, int kind,
+                                                                 double t, double t09, float* __restrict__ loss,
+                                                                 double* __restrict__ norm) {
+  __shared__ double s_term[kKpThreads], s_v[kKpThreads];
+  double acc = 0.0, acc_v = 0.0;
+  for (int p = threadIdx.x; p < n; p += kKpThreads) {
+    const double v = validity[p];
+    acc += kp_term(pred + (long)p * dim, gt + (long)p * dim, v, dim, kind, t, t09);
+    acc_v += v;
+  }
+  s_term[threadIdx.x] = acc;
+  s_v[threadIdx.x] = acc_v;
+  __syncthreads();
+  for (int s = kKpThreads / 2; s > 0; s >>= 1) {
+    if (threadIdx.x < s) {
+      s_term[threadIdx.x] += s_term[threadIdx.x + s];
+      s_v[threadIdx.x] += s_v[threadIdx.x + s];
+    }
+    __syncthreads();
+  }
+  if (threadIdx.x == 0) {
+    const double d = kp_divisor(s_v[0], dim, kind);
+    *norm = d;
+    *loss = (float)(s_term[0] / d);
+  }
+}
+
+__global__ void __launch_bounds__(kKpThreads) kp_loss_bwd_kernel(const float* __restrict__ grad_loss, const float* __restrict__ pred,
+                                                                 const float* __restrict__ gt, const float* __restrict__ validity,
+                                                                 const double* __restrict__ norm, float* __restrict__ grad_pred,
+                                                                 int n, int dim, int kind, double t, double t09) {
+  const long i = (long)blockIdx.x * kKpThreads + threadIdx.x;
+  if (i >= (long)n * dim) return;
+  const long p = i / dim;
+  const double g = (double)*grad_loss / *norm;
+  grad_pred[i] = (float)kp_grad(pred + p * dim, gt + p * dim, validity[p], (int)(i - p * dim), dim, kind, t, t09, g);
+}
+
+}  // namespace lt
+
+static int kp_check(const float* pred, const float* gt, const float* validity, int kind, int n_points, int dim) {
+  LT_REQUIRE(pred && gt && validity, "keypoints_loss: null pointer");
+  LT_REQUIRE(n_points > 0 && dim > 0, "keypoints_loss: bad sizes");
+  LT_REQUIRE((long)n_points * dim < 0x7fffffffL, "keypoints_loss: n_points * dim must be < 2^31");
+  LT_REQUIRE(kind >= kKpMse && kind <= kKpL2, "keypoints_loss: unknown kind %d", kind);
+  return LT_OK;
+}
+
+extern "C" int lt_keypoints_loss_fwd(const float* pred, const float* gt, const float* validity, float* loss, double* norm, int kind,
+                                     double threshold, int n_points, int dim, void* stream) {
+  const int rc = kp_check(pred, gt, validity, kind, n_points, dim);
+  if (rc != LT_OK) return rc;
+  LT_REQUIRE(loss && norm, "keypoints_loss: null pointer");
+  kp_loss_fwd_kernel<<<1, kKpThreads, 0, (cudaStream_t)stream>>>(pred, gt, validity, n_points, dim, kind, threshold,
+                                                                 pow(threshold, 0.9), loss, norm);
+  LT_CHECK_LAUNCH("kp_loss_fwd_kernel");
+  return LT_OK;
+}
+
+extern "C" int lt_keypoints_loss_bwd(const float* grad_loss, const float* pred, const float* gt, const float* validity,
+                                     const double* norm, float* grad_pred, int kind, double threshold, int n_points, int dim,
+                                     void* stream) {
+  const int rc = kp_check(pred, gt, validity, kind, n_points, dim);
+  if (rc != LT_OK) return rc;
+  LT_REQUIRE(grad_loss && norm && grad_pred, "keypoints_loss_bwd: null pointer");
+  kp_loss_bwd_kernel<<<ceil_div((long)n_points * dim, kKpThreads), kKpThreads, 0, (cudaStream_t)stream>>>(
+      grad_loss, pred, gt, validity, norm, grad_pred, n_points, dim, kind, threshold, pow(threshold, 0.9));
+  LT_CHECK_LAUNCH("kp_loss_bwd_kernel");
+  return LT_OK;
+}
+
+// test hook: the kernels' term, derivative and summation order on the CPU (host pointers)
+extern "C" int lt_test_keypoints_loss_host(const float* pred, const float* gt, const float* validity, float* loss, double* norm,
+                                           const float* grad_loss, float* grad_pred, int kind, double threshold, int n_points,
+                                           int dim) {
+  const int rc = kp_check(pred, gt, validity, kind, n_points, dim);
+  if (rc != LT_OK) return rc;
+  LT_REQUIRE(loss && norm, "test_keypoints_loss_host: null pointer");
+  LT_REQUIRE(!grad_pred || grad_loss, "test_keypoints_loss_host: grad_pred needs grad_loss");
+  const double t09 = pow(threshold, 0.9);
+  double term[kKpThreads], sv[kKpThreads];
+  for (int tid = 0; tid < kKpThreads; ++tid) {
+    term[tid] = sv[tid] = 0.0;
+    for (int p = tid; p < n_points; p += kKpThreads) {
+      const double v = validity[p];
+      term[tid] += kp_term(pred + (long)p * dim, gt + (long)p * dim, v, dim, kind, threshold, t09);
+      sv[tid] += v;
+    }
+  }
+  for (int s = kKpThreads / 2; s > 0; s >>= 1) {
+    for (int tid = 0; tid < s; ++tid) {
+      term[tid] += term[tid + s];
+      sv[tid] += sv[tid + s];
+    }
+  }
+  *norm = kp_divisor(sv[0], dim, kind);
+  *loss = (float)(term[0] / *norm);
+  if (grad_pred) {
+    const double g = (double)*grad_loss / *norm;
+    for (long i = 0; i < (long)n_points * dim; ++i) {
+      const long p = i / dim;
+      grad_pred[i] = (float)kp_grad(pred + p * dim, gt + p * dim, validity[p], (int)(i - p * dim), dim, kind, threshold, t09, g);
+    }
+  }
+  return LT_OK;
+}

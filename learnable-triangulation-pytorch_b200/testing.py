@@ -229,3 +229,146 @@ def randomize_ransac_weights(model, seed=0, calib_size=64):
     """randomize_backbone_weights for a model whose heat maps are used raw (RANSACTriangulationNet): heat-map spread ~3."""
     randomize_backbone_weights(_BackboneHolder(model.backbone), seed=seed, calib_size=calib_size)
     return model.eval()
+
+
+# ---- restated training loop of the reference (train.py:185-263), for the TrainStep tests and tools/train_step_timing.py ----------
+
+CRITERIA = {"MSE": "mse", "MSESmooth": "mse_smooth", "MAE": "mae"}
+
+
+def reference_keypoints_loss(kind, pred, gt, validity, threshold=400):
+    """Restatement of the reference's keypoint criteria (mvn/models/loss.py:7-49), `kind` one of "mse", "mse_smooth", "mae", "l2":
+    the divisor read to the host with .item() and MSESmooth's boolean-mask replacement, as there.  Runs in the inputs' dtype
+    (float64 inputs give the float64 reference of the tests)."""
+    divisor = max(1, torch.sum(validity).item())
+    if kind == "l2":
+        return torch.sum(torch.sqrt(torch.sum((gt - pred) ** 2 * validity, dim=2))) / divisor
+    if kind == "mae":
+        terms = torch.abs(gt - pred) * validity
+    else:
+        terms = (gt - pred) ** 2 * validity
+        if kind == "mse_smooth":
+            over = terms > threshold
+            terms[over] = torch.pow(terms[over], 0.1) * (threshold ** 0.9)
+    return torch.sum(terms) / (pred.shape[-1] * divisor)
+
+
+def make_train_config(model_config, criterion="MAE", lr=1e-4, kind="human36m", **opt):
+    """A train.py config: `model_config` (make_config / make_alg_config) with a top-level `kind` and an `opt` section."""
+    cfg = AttrDict(model_config)
+    cfg.kind = kind
+    cfg.opt = AttrDict(dict(criterion=criterion, lr=lr, **opt))
+    return cfg
+
+
+def recipe_optimizer(model, config, **adam):
+    """train.py:428-439's Adam: per-module lrs for the volumetric model, the trainable parameters for the algebraic one."""
+    o = config.opt
+    if config.model.name == "vol":
+        groups = [{"params": model.backbone.parameters()},
+                  {"params": model.process_features.parameters(), "lr": getattr(o, "process_features_lr", o.lr)},
+                  {"params": model.volume_net.parameters(), "lr": getattr(o, "volume_net_lr", o.lr)}]
+        return torch.optim.Adam(groups, lr=o.lr, **adam)
+    return torch.optim.Adam([p for p in model.parameters() if p.requires_grad], lr=o.lr, **adam)
+
+
+def reference_train_step(model, optimizer, config, images_batch, keypoints_3d_gt, keypoints_3d_validity_gt, proj_matricies_batch,
+                         batch):
+    """One eager iteration of the reference's training loop body (train.py:185-263) restated: the model, the restated criterion,
+    lt_b200's native VolumetricCELoss, every .item() of the loop, the per-parameter .item() gradient norm of misc.calc_gradient_norm,
+    clip_grad_norm_ and the optimizer step.  base_point_l2 takes coco's hip midpoint from the ground truth.
+    -> (the model's outputs, metric_dict of Python floats)."""
+    from .loss import VolumetricCELoss
+    o = config.opt
+    outputs = model(images_batch, proj_matricies_batch, batch)
+    kp, gt = outputs[0], keypoints_3d_gt
+    J = kp.shape[1]
+    valid = (keypoints_3d_validity_gt > 0.0).type(torch.float32)
+    s = o.scale_keypoints_3d if hasattr(o, "scale_keypoints_3d") else 1.0
+    if images_batch.shape[1] == 1:
+        base_joint = {"human36m": 6, "coco": 11}[config.kind]
+        gt = gt.clone()
+        gt[:, torch.arange(J) != base_joint] -= gt[:, base_joint:base_joint + 1]
+        kp = kp.clone()
+        kp[:, torch.arange(J) != base_joint] -= kp[:, base_joint:base_joint + 1]
+    metrics = {}
+    threshold = o.mse_smooth_threshold if o.criterion == "MSESmooth" else 400
+    loss = reference_keypoints_loss(CRITERIA[o.criterion], kp * s, gt * s, valid, threshold)
+    total = 0.0 + loss
+    metrics[o.criterion] = loss.item()
+    if getattr(o, "use_volumetric_ce_loss", False):
+        ce = VolumetricCELoss(backend="native")(outputs[5], outputs[2], gt, valid)
+        metrics["volumetric_ce_loss"] = ce.item()
+        total = total + getattr(o, "volumetric_ce_loss_weight", 1.0) * ce
+    metrics["total_loss"] = total.item()
+    optimizer.zero_grad()
+    total.backward()
+    if hasattr(o, "grad_clip"):
+        torch.nn.utils.clip_grad_norm_(model.parameters(), o.grad_clip / o.lr)
+    norm2 = 0.0
+    for p in model.parameters():
+        if p.requires_grad:
+            norm2 += p.grad.data.norm(2).item() ** 2
+    metrics["grad_norm_times_lr"] = o.lr * norm2 ** 0.5
+    optimizer.step()
+    metrics["l2"] = reference_keypoints_loss("l2", kp * s, gt * s, valid).item()
+    if config.model.name == "vol":
+        base_pred = outputs[6]
+        per = []
+        for b in range(kp.shape[0]):
+            base_gt = (gt[b, 11, :3] + gt[b, 12, :3]) / 2 if config.model.kind == "coco" else gt[b, 6, :3]
+            per.append(torch.sqrt(torch.sum((base_pred[b] * s - base_gt * s) ** 2)).item())
+        metrics["base_point_l2"] = float(np.mean(per))
+    return outputs, metrics
+
+
+def prepare_batch(batch, images, device):
+    """images, keypoints_3d (B, J, 3), validity (B, J, 1), image-space projections as the reference's prepare_batch returns them
+    (datasets/utils.py:41-66) for a make_batch() dict."""
+    kp = torch.from_numpy(np.stack(batch["keypoints_3d"])).float()
+    return (images.to(device), kp[..., :3].to(device), kp[..., 3:].to(device),
+            torch.from_numpy(image_projections(batch)).to(device))
+
+
+def keypoint_case(name, dim=3, n=(3, 5), seed=0):
+    """(pred, gt, validity (B, J, 1)) float32 of one graded case of the keypoint criteria tests (KEYPOINT_CASES)."""
+    g = torch.Generator().manual_seed(seed)
+    B, J = n
+    gt = torch.randn(B, J, dim, generator=g) * 30
+    pred = gt + torch.randn(B, J, dim, generator=g) * 15
+    v = (torch.rand(B, J, 1, generator=g) > 0.3).float()
+    if name == "zero_validity":
+        v.zero_()
+    elif name == "fractional":
+        v = torch.rand(B, J, 1, generator=g)
+    elif name == "boundary":                    # (gt - pred)^2 v = 400 exactly, and just above it
+        v[0, 0], v[0, 1] = 1.0, 1.0
+        pred[0, 0, 0] = gt[0, 0, 0] - 20.0
+        pred[0, 1, 0] = gt[0, 1, 0] - 20.0009765625
+    elif name == "nan_invalid":
+        v[1, 2] = 0.0
+        pred[1, 2, 0] = float("nan")
+        v[0, 3] = 0.0
+        pred[0, 3, 1] = float("inf")
+    elif name == "nan_valid":
+        v[1, 1] = 1.0
+        pred[1, 1, 0] = float("nan")
+    elif name == "many":                        # more points than the CTA's threads
+        return keypoint_case("plain", dim, (20, 17), seed)
+    return pred, gt, v
+
+
+KEYPOINT_CASES = ("plain", "zero_validity", "fractional", "boundary", "nan_invalid", "nan_valid", "many")
+
+
+def reference_keypoints_loss64(kind, pred, gt, v, threshold=400.0):
+    """float64 loss, gradient wrt pred (grad_loss 1) and sum of |terms| of the restated reference."""
+    p = pred.double().requires_grad_(True)
+    loss = reference_keypoints_loss(kind, p, gt.double(), v.double(), threshold)
+    loss.backward()
+    with torch.no_grad():
+        r = gt.double() - pred.double()
+        terms = torch.abs(r) * v if kind == "mae" else r ** 2 * v.double()
+        if kind == "l2":
+            terms = torch.sqrt(terms.sum(-1))
+    return float(loss.detach()), p.grad, float(terms.abs().nansum())

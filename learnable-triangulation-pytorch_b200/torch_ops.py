@@ -117,3 +117,23 @@ def triangulate_batch_of_points(proj_matricies_batch, points_batch, confidences_
     _, _, vh = torch.linalg.svd(A.double(), full_matrices=False)
     X = vh[..., 3, :]
     return (X[..., :3] / X[..., 3:4]).to(points_batch.dtype)
+
+
+def keypoints_loss(pred, gt, validity, kind, threshold=400.0):
+    """The keypoint criteria of the reference (loss.py:7-49) with the divisor max(1, sum v) kept on the device: no host
+    synchronisation.  pred, gt (B, J, dim), validity (B, J, 1); `kind` is one of "mse", "mse_smooth", "mae", "l2".  MSESmooth's
+    replaced branch is a torch.where whose untaken pow sees 1, so its gradient is the reference's index_put gradient."""
+    r = gt - pred
+    divisor = torch.clamp(validity.sum(), min=1)
+    if kind == "l2":
+        return torch.sqrt((r ** 2 * validity).sum(dim=2)).sum() / divisor
+    if kind == "mae":
+        terms = torch.abs(r) * validity
+    else:
+        terms = r ** 2 * validity
+        if kind == "mse_smooth":
+            over = terms > threshold
+            terms = torch.where(over, torch.where(over, terms, torch.ones_like(terms)) ** 0.1 * threshold ** 0.9, terms)
+        elif kind != "mse":
+            raise ValueError("unknown keypoints loss kind {!r}".format(kind))
+    return terms.sum() / (pred.shape[-1] * divisor)

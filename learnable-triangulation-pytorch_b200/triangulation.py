@@ -104,7 +104,7 @@ def _check_train_graph(train_graph, backend):
 
 
 class _EngineOwner(nn.Module):
-    """Keeps the native engine's packed filters / CUDA graphs and the training graphs (train_graph.TrainGraphs) in step with the
+    """Keeps the native engine's packed filters / CUDA graphs and the training graphs (train_graph.TrainGraphs, TrainStep) in step with the
     module's tensors: `.to()/.cuda()/.float()` (`_apply`) and `load_state_dict` invalidate them explicitly (tensor versions alone
     miss `p.data` updates)."""
 
@@ -115,6 +115,8 @@ class _EngineOwner(nn.Module):
         graphs = self.__dict__.get("_train_graphs")
         if graphs is not None:
             graphs.invalidate()
+        for step in self.__dict__.get("_train_steps", ()):        # train_graph.TrainStep graphs of this model
+            step.invalidate()
 
     def _run_device(self, fn, inputs):
         """fn(*inputs): the device part of the forward, replayed from CUDA graphs with train_graph=True in a training forward."""
