@@ -281,6 +281,9 @@ typedef struct lt_conv_tc_launch_plan {
   int chunks;                /* K chunks of a tile: taps x Cin / 32 */
   int splits;                /* K split count, 1 = none */
   int grid;                  /* CTAs launched: min(m_tiles x n_tiles x splits, sm_count) */
+  int stages;                /* operand ring depth in shared memory */
+  int epi_buffers;           /* shared-memory epilogue tile buffers: 2 for at most 4 chunks, else 1; 0 for split launches and
+                                16-channel tiles, which keep no tile buffer */
 } lt_conv_tc_launch_plan;
 int lt_conv_tc_plan(const lt_conv_desc* desc, int sm_count, int splitk, lt_conv_tc_launch_plan* plan);
 int lt_conv_tc_pack_weights(const float* w_tap_ci_co, void* packed, int taps, int Cin, int Cout, void* stream);

@@ -39,7 +39,7 @@ class ConvDesc(ctypes.Structure):
 
 class ConvTcPlan(ctypes.Structure):
     """Mirror of `struct lt_conv_tc_launch_plan` (include/lt_b200.h)."""
-    _fields_ = [(n, c_int) for n in ("nt", "m_tiles", "n_tiles", "chunks", "splits", "grid")]
+    _fields_ = [(n, c_int) for n in ("nt", "m_tiles", "n_tiles", "chunks", "splits", "grid", "stages", "epi_buffers")]
 
 
 class ConvWgradPlan(ctypes.Structure):
@@ -332,7 +332,8 @@ def conv_nd(desc, inp, weight, scale, shift, residual, out, impl):
 
 
 def conv_tc_plan(desc, sm_count, splitk=1):
-    """Host-only work decomposition of an LT_CONV_TC launch (lt_conv_tc_plan): dict of nt, m_tiles, n_tiles, chunks, splits, grid."""
+    """Host-only work decomposition of an LT_CONV_TC launch (lt_conv_tc_plan): dict of nt, m_tiles, n_tiles, chunks, splits, grid,
+    stages, epi_buffers."""
     plan = ConvTcPlan()
     _check(lib().lt_conv_tc_plan(ctypes.byref(desc), sm_count, splitk, ctypes.byref(plan)), "lt_conv_tc_plan")
     return {name: getattr(plan, name) for name, _ in ConvTcPlan._fields_}

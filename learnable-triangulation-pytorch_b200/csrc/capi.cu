@@ -60,7 +60,7 @@ int conv_fold_fwd(const lt_conv_desc* d, const void* in, const void* weight, con
 
 }  // namespace lt
 
-extern "C" int lt_version(void) { return 203; }
+extern "C" int lt_version(void) { return 204; }
 
 extern "C" void lt_default_options(lt_options* o) {
   if (o) *o = lt::make_default_options();

@@ -16,7 +16,7 @@
 // Weights: [tap][Cin/32][CoutP rows][32 hi | 32 lo] fp16 (128-byte rows), so the K slices of both operands are descriptor offsets
 // (+0, +2 hi; +4, +6 lo, in 16-byte units).
 //
-// Warp roles (384 threads): warpgroup 0 = TMA producers (warp 0 fills the operand ring, warp 1 owns the epilogue buffer),
+// Warp roles (384 threads): warpgroup 0 = TMA producers (warp 0 fills the operand ring, warp 1 owns the epilogue buffers),
 // warpgroups 1 and 2 = MMA + epilogue for rows 0-63 and 64-127 of the M tile.  The operand ring is released per stage by one
 // arrival of each consumer warpgroup once its MMAs that read the stage have completed (wgmma.wait_group 1 keeps one chunk of MMAs
 // in flight behind the issue).
@@ -25,7 +25,8 @@
 // (the output may alias the residual): 32 dependent memory round trips per unit with the tensor cores idle.  So warp 1 TMA-loads
 // the unit's residual tile into a shared-memory buffer while the K loop runs, the consumers turn it into the output tile in place
 // with shared-memory accesses only, and warp 1 TMA-stores it while the next unit's K loop runs.  Warp 0 never waits on that
-// buffer.  16-channel tiles (half a 32-channel slab) keep the register store.
+// buffer.  Launches with short K loops (tc_layout) keep two such buffers and alternate between them, so the next unit's residual
+// load does not wait for this unit's epilogue and store.  16-channel tiles (half a 32-channel slab) keep the register store.
 //
 // Persistent grid: min(work units, SMs) CTAs stride over the work units (M tile x N tile x K split, N tile fastest).  Producer and
 // consumers keep one ring across unit boundaries, so the next unit's first boxes load while the consumers run the epilogue; on the
@@ -93,11 +94,11 @@ __global__ void __launch_bounds__(kTcThreads, 1) conv_tc_kernel(const __grid_con
   constexpr int kStage = kATileBytes + NT * 128;
   const int epi_bytes = tc_epi_bytes(NT, p.splits);
   const bool staged = epi_bytes > 0;
-  uint8_t* ebuf = smem + (size_t)p.stages * kStage;
-  uint64_t* full = reinterpret_cast<uint64_t*>(ebuf + epi_bytes);
+  uint8_t* ebuf = smem + (size_t)p.stages * kStage;   // p.epi_buffers tile buffers of epi_bytes
+  uint64_t* full = reinterpret_cast<uint64_t*>(ebuf + p.epi_buffers * epi_bytes);
   uint64_t* empty = full + p.stages;
-  uint64_t* efull = empty + p.stages;   // the epilogue buffer is free and holds the unit's residual
-  uint64_t* edone = efull + 1;          // both consumer warpgroups wrote the unit's output into it
+  uint64_t* efull = empty + p.stages;   // [b]: tile buffer b is free and holds its unit's residual
+  uint64_t* edone = efull + 2;          // [b]: both consumer warpgroups wrote their unit's output into tile buffer b
 
   const int wg = __shfl_sync(0xffffffffu, (int)(threadIdx.x >> 7), 0);
   const int lane = threadIdx.x & 31;
@@ -107,8 +108,7 @@ __global__ void __launch_bounds__(kTcThreads, 1) conv_tc_kernel(const __grid_con
 
   if (threadIdx.x == 0) {
     for (int s = 0; s < p.stages; ++s) { mbar_init(&full[s], 1); mbar_init(&empty[s], 2); }
-    mbar_init(efull, 1);
-    mbar_init(edone, 256);
+    for (int b = 0; b < 2; ++b) { mbar_init(&efull[b], 1); mbar_init(&edone[b], 256); }
     fence_barrier_init();
     prefetch_tmap(&tmA);
     prefetch_tmap(&tmB);
@@ -118,32 +118,53 @@ __global__ void __launch_bounds__(kTcThreads, 1) conv_tc_kernel(const __grid_con
   if (wg == 0) {
     regs_release_producer();
     if (staged && threadIdx.x == 32) {
-      // ================= epilogue buffer (warp 1, one lane): residual tile in, output tile out =================
-      // The residual load of unit u overlaps its K loop; its store overlaps the K loop of the next unit.
-      uint32_t eph = 0;
-      for (int u = blockIdx.x; u < units; u += gridDim.x) {
+      // ================= epilogue buffers (warp 1, one lane): residual tiles in, output tiles out =================
+      // The k-th unit of this CTA uses buffer k % epi_buffers.  With two buffers the next unit's residual load is issued as soon
+      // as the previous unit's store has read the other buffer, ahead of this unit's epilogue: it overlaps this unit's K loop,
+      // epilogue and store and the next unit's K loop, so the consumers find it there when they finish that K loop.  With one
+      // buffer it waits until this unit's store has read the buffer.  A unit's store overlaps the next unit's K loop either way.
+      const int nbuf = p.epi_buffers;
+      auto load_residual = [&](int u, int b) {
+        uint8_t* buf = ebuf + b * epi_bytes;
+        if (p.residual == LT_RES_NONE) {
+          mbar_arrive_local(&efull[b]);
+          return;
+        }
         const TcUnit w = tc_unit(p, u, m_tiles, nchunks_all);
         int ow0, oh0, od0, nb0;
         tc_tile_origin(p, w.m, ow0, oh0, od0, nb0);
-        bulk_wait_read0();                      // the previous unit's store has read the buffer
-        if (p.residual != LT_RES_NONE) {
-          mbar_expect_tx(efull, (uint32_t)epi_bytes);   // out-of-range positions and channels arrive as zeros
-          for (int sl = 0; sl < NT / 32; ++sl) {
-            int g, c;
-            epi_slab(p, w.n0 + 32 * sl, g, c);
-            tma_load_5d(ebuf + sl * kSlabBytes, &tmE.res[g], efull, c, ow0, oh0, od0, nb0);
-          }
-        } else {
-          mbar_arrive_local(efull);
+        mbar_expect_tx(&efull[b], (uint32_t)epi_bytes);   // out-of-range positions and channels arrive as zeros
+        for (int sl = 0; sl < NT / 32; ++sl) {
+          int g, c;
+          epi_slab(p, w.n0 + 32 * sl, g, c);
+          tma_load_5d(buf + sl * kSlabBytes, &tmE.res[g], &efull[b], c, ow0, oh0, od0, nb0);
         }
-        mbar_wait(edone, eph);
-        eph ^= 1u;
+      };
+      uint32_t eph = 0;   // bit b: phase of edone[b]
+      int b = 0;
+      if (blockIdx.x < units) load_residual(blockIdx.x, 0);
+      for (int u = blockIdx.x; u < units; u += gridDim.x) {
+        const int un = u + gridDim.x, bn = b ^ (nbuf - 1);
+        if (nbuf == 2 && un < units) {
+          bulk_wait_read0();                    // the previous unit's store has read buffer bn
+          load_residual(un, bn);
+        }
+        const TcUnit w = tc_unit(p, u, m_tiles, nchunks_all);
+        int ow0, oh0, od0, nb0;
+        tc_tile_origin(p, w.m, ow0, oh0, od0, nb0);
+        mbar_wait(&edone[b], (eph >> b) & 1u);
+        eph ^= 1u << b;
         for (int sl = 0; sl < NT / 32; ++sl) {  // clipped at the edges of the output grid and at FC
           int g, c;
           epi_slab(p, w.n0 + 32 * sl, g, c);
-          tma_store_5d(&tmE.out[g], ebuf + sl * kSlabBytes, c, ow0, oh0, od0, nb0);
+          tma_store_5d(&tmE.out[g], ebuf + b * epi_bytes + sl * kSlabBytes, c, ow0, oh0, od0, nb0);
         }
         bulk_commit();
+        if (nbuf == 1 && un < units) {
+          bulk_wait_read0();                    // this unit's store has read the buffer
+          load_residual(un, 0);
+        }
+        b = bn;
       }
       bulk_wait0();
     }
@@ -188,7 +209,9 @@ __global__ void __launch_bounds__(kTcThreads, 1) conv_tc_kernel(const __grid_con
   const int c2 = 2 * (lane & 3);
   const uint32_t ring0 = smem_u32(smem);
   int s = 0;
-  uint32_t ph = 0, eph = 0;
+  uint32_t ph = 0;
+  int eb = 0;          // tile buffer of this unit (staged epilogue)
+  uint32_t eph = 0;    // bit b: phase of efull[b]
   for (int u = blockIdx.x; u < units; u += gridDim.x) {
     const TcUnit w = tc_unit(p, u, m_tiles, nchunks_all);
     int prev = -1;
@@ -244,11 +267,11 @@ __global__ void __launch_bounds__(kTcThreads, 1) conv_tc_kernel(const __grid_con
       continue;
     }
     if constexpr (NT >= 32) {
-      // ---- staged: the residual comes from and the output goes to the epilogue buffer; warp 1 moves both with TMA ----
+      // ---- staged: the residual comes from and the output goes to tile buffer eb; warp 1 moves both with TMA ----
       // The arithmetic is conv_epilogue_row's.  A thread's residual and output elements share their addresses.
-      mbar_wait(efull, eph);
-      eph ^= 1u;
-      const uint32_t e0 = smem_u32(ebuf);
+      mbar_wait(&efull[eb], (eph >> eb) & 1u);
+      eph ^= 1u << eb;
+      const uint32_t e0 = smem_u32(ebuf + eb * epi_bytes);
       // Column group i + 1's scale and shift load while group i is processed: the compiler does not move loads across the
       // shared-memory accesses (volatile asm), so a load issued in its own iteration would wait a full L1 round trip.
       auto fc_ok = [&](int co) {
@@ -311,7 +334,8 @@ __global__ void __launch_bounds__(kTcThreads, 1) conv_tc_kernel(const __grid_con
         sh = sh_next;
       }
       fence_proxy_async();   // the generic-proxy writes become visible to the TMA store
-      mbar_arrive_local(edone);
+      mbar_arrive_local(&edone[eb]);
+      eb ^= p.epi_buffers - 1;
     } else {
       // ---- 16-channel tiles (half a slab): fused epilogue straight from the accumulator registers ----
       int ow0, oh0, od0, nb0;
@@ -556,8 +580,23 @@ static int make_epi_maps(const TcParams& p, TcEpiMaps* m) {
 }
 
 // one CTA per SM (the two consumer warpgroups hold up to 128 fp32 accumulators per thread): the shared memory beside the epilogue
-// buffer is pipeline depth (N tile 128: 5 stages beside the 64 KB buffer)
+// tile buffers is pipeline depth
 constexpr int kTcSmemBudget = 224 * 1024;
+
+// Shared-memory layout of one conv_tc launch (host only; launch_tc and lt_conv_tc_plan).  A second epilogue tile buffer lets the
+// next unit's residual tile load while this unit's output tile waits for its epilogue and store, but it takes ring stages: at N
+// tile 128 two 64 KB buffers leave 3 stages where one leaves 5.  Measured per layer class on an H100 80GB HBM3 (700 W), two
+// buffers win on the backbone's 1x1 expansions with 2 and 4 K chunks per unit (96^2 64 -> 256: 1.40 -> 1.04 ms, 48^2 128 -> 512:
+// 1.60 -> 1.39 ms per step) and lose from 8 chunks up, where the K loop needs the deeper ring (24^2 256 -> 1024, 8 chunks:
+// 4.18 -> 4.76 ms; 3x3 256 -> 256, 72 chunks: 4.49 -> 5.15 ms).  So staged launches of at most kTcShortK chunks per unit take
+// two buffers, longer ones one, and the ring gets the rest of the budget (N tile 128: 3 / 5 stages, 64: 6 / 8, 32: 8 / 8).
+constexpr int kTcShortK = 4;
+static void tc_layout(int nt, int splits, int chunks, int* stages, int* epi_buffers) {
+  const int epi_bytes = tc_epi_bytes(nt, splits);
+  *epi_buffers = epi_bytes == 0 ? 0 : (chunks <= kTcShortK ? 2 : 1);
+  const int s = (kTcSmemBudget - *epi_buffers * epi_bytes) / (kATileBytes + nt * 128);
+  *stages = s > 8 ? 8 : s;
+}
 
 static int launch_tc(const CUtensorMap& tmA, const CUtensorMap& tmB, TcParams& p, int n_tiles, cudaStream_t st, void* ws = nullptr,
                      size_t ws_bytes = 0) {
@@ -575,10 +614,8 @@ static int launch_tc(const CUtensorMap& tmA, const CUtensorMap& tmB, TcParams& p
   p.n_tiles = n_tiles;
   const int stage_bytes = kATileBytes + p.Nt * 128;
   const int epi_bytes = tc_epi_bytes(p.Nt, splits);
-  int stages = (kTcSmemBudget - epi_bytes) / stage_bytes;
-  if (stages > 8) stages = 8;
-  p.stages = stages;
-  const size_t smem = (size_t)stages * stage_bytes + epi_bytes + (2 * stages + 2) * 8 + 1024;
+  tc_layout(p.Nt, splits, p.KD * p.KH * p.KW * p.CB, &p.stages, &p.epi_buffers);
+  const size_t smem = (size_t)p.stages * stage_bytes + (size_t)p.epi_buffers * epi_bytes + (2 * p.stages + 4) * 8 + 1024;
   TcEpiMaps tmE{};
   int rc;
   if (epi_bytes) {
@@ -619,7 +656,7 @@ void fill_params(const lt_conv_desc* d, TcParams& p, int CB, int CoutP, int Nt, 
   p.osd = d->osd; p.osh = d->osh; p.osw = d->osw; p.ood = d->ood; p.ooh = d->ooh; p.oow = d->oow;
   p.relu = d->relu; p.residual = d->residual; p.out_format = d->out_format;
   p.scale = scale; p.shift = shift; p.res = residual; p.out = out;
-  p.splits = 1; p.ws = nullptr; p.ws_ld = 0; p.ws_gain = 1.0f; p.stages = 0; p.n_tiles = 1;
+  p.splits = 1; p.ws = nullptr; p.ws_ld = 0; p.ws_gain = 1.0f; p.stages = 0; p.n_tiles = 1; p.epi_buffers = 0;
   p.n_maps = out_groups(d);
   p.oc = p.n_maps > 1 ? d->Cout / p.n_maps : CoutP;
   p.gh = d->ogh > 1 ? d->ogh : 1; p.gw = d->ogw > 1 ? d->ogw : 1;
@@ -716,6 +753,7 @@ extern "C" int lt_conv_tc_plan(const lt_conv_desc* d, int sm_count, int splitk, 
   plan->chunks = d->KD * d->KH * d->KW * (d->Cin / 32);
   tc_plan(plan->m_tiles, plan->n_tiles, plan->nt, plan->chunks, 3, out_groups(d), d->workspace ? splitk : 0, d->workspace_bytes,
           sm_count, &plan->splits, &plan->grid);
+  tc_layout(plan->nt, plan->splits, plan->chunks, &plan->stages, &plan->epi_buffers);
   return LT_OK;
 }
 
@@ -757,7 +795,7 @@ extern "C" int lt_tc_gemm_selftest(const void* a, const void* b, float* d, int M
   p.relu = 0; p.residual = LT_RES_NONE; p.out_format = LT_FMT_F32;
   p.scale = ones; p.shift = zeros; p.res = nullptr; p.out = d;
   p.n_maps = 1; p.oc = N; p.gh = p.gw = 1;
-  p.splits = 1; p.ws = nullptr; p.ws_ld = 0; p.ws_gain = 1.0f; p.n_tiles = 1;
+  p.splits = 1; p.ws = nullptr; p.ws_ld = 0; p.ws_gain = 1.0f; p.n_tiles = 1; p.epi_buffers = 0;
   CUtensorMap tmA, tmB;
   {
     const uint64_t dims[5] = {(uint64_t)K, (uint64_t)M, 1, 1, 1};

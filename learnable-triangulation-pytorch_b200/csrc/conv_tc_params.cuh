@@ -29,6 +29,7 @@ struct TcParams {
   // grouped output (lt_conv_desc.ogd/ogh/ogw): output channel block g of `oc` channels goes to output map g (its own phase offset)
   int oc, n_maps;
   int gh, gw;    // output group grid (group g -> offset (g / (gh*gw), (g / gw) % gh, g % gw)); 1, 1 without groups
+  int epi_buffers;   // conv_tc_kernel's staged epilogue tile buffers: 2 (unit k uses buffer k & 1), 1, or 0 when not staged
 };
 
 // grouped output (lt_conv_desc.ogd/ogh/ogw): a k2 s2 transposed conv as ONE GEMM with N = 8 x Cout, group g = phase (a, b, c) of
