@@ -63,7 +63,8 @@ class UnprojectHeatmapsFn(torch.autograd.Function):
             grad_coord = grad_coord.reshape(coord_shape) if need_coord else None
         else:
             capi.unproject_aggregate_bwd(feats_cl, proj, coord, conf, g_cl, grad_feats, grad_conf, ctx.agg)
-        grad_heat = grad_feats.permute(0, 1, 4, 2, 3)                                       # (B, V, C, h, w) view
+        # grad_feats is the kernels' accumulation target even when the heat-maps need no gradient; it is returned only if they do
+        grad_heat = grad_feats.permute(0, 1, 4, 2, 3) if ctx.needs_input_grad[0] else None   # (B, V, C, h, w) view
         return grad_heat, grad_proj, grad_coord, (grad_conf.reshape(ctx.conf_shape) if need_conf else None), None
 
 
@@ -93,10 +94,11 @@ class IntegrateTensor3dFn(torch.autograd.Function):
         dev = probs.device
         g_kp = (grad_kp if grad_kp is not None else torch.zeros((B, J, 3), device=dev)).float().contiguous()
         g_vol = None if grad_vol is None else grad_vol.float().contiguous()
-        grad_logits = torch.empty_like(probs)
-        scratch = torch.empty(B * J, dtype=torch.float32, device=dev)
-        capi.softargmax3d_bwd(probs, coord, g_kp, g_vol, grad_logits, scratch, B, J, nvox, 1.0, ctx.softmax)
-        grad_coord = None
+        grad_logits = grad_coord = None
+        if ctx.needs_input_grad[0]:
+            grad_logits = torch.empty_like(probs)
+            scratch = torch.empty(B * J, dtype=torch.float32, device=dev)
+            capi.softargmax3d_bwd(probs, coord, g_kp, g_vol, grad_logits, scratch, B, J, nvox, 1.0, ctx.softmax)
         if ctx.needs_input_grad[1]:
             grad_coord = torch.empty((B, nvox, 3), dtype=torch.float32, device=dev)
             capi.softargmax3d_coord_bwd(probs.reshape(B, J, nvox), g_kp, grad_coord, B, J, nvox, ctx.softmax)

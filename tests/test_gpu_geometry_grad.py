@@ -114,8 +114,11 @@ def test_dlt_proj_bwd_device_matches_host_code():
     capi.triangulate_dlt_proj_bwd(*t, out, ws)
     torch.cuda.synchronize()
     assert guards_intact(buf) and bool(torch.isfinite(out).all())
-    # the same float64 solve; the device may contract operations differently, so a few ulps of the largest element
-    assert float((out.cpu().double() - torch.from_numpy(want).double()).abs().max()) <= 1e-5 * float(np.abs(want).max())
+    # the same float64 solve; the device may contract float64 operations differently: two float32 ulps of each element, or 1e-9 of
+    # the largest where an element is the difference of much larger terms (tests/test_gpu_geometry_grad_ref.py holds every element
+    # to the 50-digit reference)
+    got, want = out.cpu().double().numpy(), want.astype(np.float64)
+    assert (np.abs(got - want) <= 2 * 2.0 ** -23 * np.abs(want) + 1e-9 * np.abs(want).max()).all()
     out2 = torch.empty_like(out)
     capi.triangulate_dlt_proj_bwd(*t, out2, ws)
     assert torch.equal(out, out2)
