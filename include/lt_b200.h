@@ -186,6 +186,20 @@ int lt_unproject_aggregate_bwd_geom(const float* features, const float* proj, co
                                     const float* grad_out, float* grad_features, float* grad_conf, float* grad_proj, float* grad_coord,
                                     void* workspace, size_t workspace_bytes, int B, int V, int C, int h, int w, long nvox, int agg,
                                     void* stream);
+/* The fixed-order variant of lt_unproject_aggregate_bwd / lt_unproject_aggregate_bwd_geom (what training under
+ * torch.use_deterministic_algorithms runs): no float atomics.  Every element of grad_features is the sum of the same terms gs * w_k the
+ * atomic kernel adds, in one order fixed by the inputs (the four cells that have the pixel as a tap in a fixed order, each cell's
+ * voxels ascending); grad_conf sums fixed chunks of voxels in chunk order.  The result depends on no launch geometry, SM count or
+ * stream, and sample b's on no other sample.  grad_features / grad_conf are accumulated into (zero them first); grad_proj and
+ * grad_coord (either may be NULL, both NULL for no geometry gradient) are written, bit-identical to lt_unproject_aggregate_bwd_geom's.
+ * C % 4 == 0; with a geometry output C / 4 must be a power of two <= 32.  No host synchronisation.  workspace:
+ * lt_unproject_aggregate_bwd_det_workspace_bytes(B, V, C, h, w, nvox, agg, geom) bytes on the current device (geom: 1 if grad_proj or
+ * grad_coord will be given), about B V nvox (C + 16) * 4 bytes; 0 when the sizes are out of range or no device is present. */
+size_t lt_unproject_aggregate_bwd_det_workspace_bytes(int B, int V, int C, int h, int w, long nvox, int agg, int geom);
+int lt_unproject_aggregate_bwd_det(const float* features, const float* proj, const float* coord, const float* conf,
+                                   const float* grad_out, float* grad_features, float* grad_conf, float* grad_proj, float* grad_coord,
+                                   void* workspace, size_t workspace_bytes, int B, int V, int C, int h, int w, long nvox, int agg,
+                                   void* stream);
 
 /* ------------------------------------------------------------------------------------------
  * Volumetric soft-argmax.  Replaces op.integrate_tensor_3d_with_coordinates (op.py:84-96).
@@ -364,6 +378,12 @@ int lt_conv_fold_pack_weights(const float* w_tap_ci_co, void* packed, int K, int
 int lt_maxpool_fwd(const void* in, void* out, int format, int N, int ID, int IH, int IW, int C,
                    int kd, int kh, int kw, int sd, int sh, int sw, int pd, int ph, int pw,
                    int OD, int OH, int OW, void* stream);
+/* Backward of a float32 max pool with kernel == stride == k on all three axes and no padding (floor mode), as
+ * F.max_pool3d(x, k, k) computes it: grad_x[i] = 0 + grad_y[window] where x[i] is the window's arg-max by torch's rule (d, h, w
+ * scan order; greater or NaN replaces; the first element if none does), 0 elsewhere and in the dropped tail.  Written, not
+ * accumulated into.  x and grad_x share the element strides xs_* of (n, c, d, h, w); grad_y has gs_*.  No atomics. */
+int lt_maxpool3d_bwd(const float* x, const float* grad_y, float* grad_x, int N, int C, int D, int H, int W, long xs_n, long xs_c,
+                     long xs_d, long xs_h, long xs_w, long gs_n, long gs_c, long gs_d, long gs_h, long gs_w, int k, void* stream);
 
 /* ------------------------------------------------------------------------------------------
  * Algebraic-triangulation path and confidence heads (config #5; SURVEY 8f rows 2 and 4).
@@ -539,6 +559,11 @@ int lt_tc_gemm_selftest(const void* a_fp16, const void* b_fp16, float* d, int M,
 int lt_test_unproject_aggregate_bwd_host(const float* features, const float* proj, const float* coord, const float* conf,
                                          const float* grad_out, float* grad_features, float* grad_conf, int B, int V, int C, int h, int w,
                                          long nvox, int agg);
+int lt_test_unproject_aggregate_bwd_det_host(const float* features, const float* proj, const float* coord, const float* conf,
+                                             const float* grad_out, float* grad_features, float* grad_conf, float* grad_proj,
+                                             float* grad_coord, int B, int V, int C, int h, int w, long nvox, int agg);
+int lt_test_maxpool3d_bwd_host(const float* x, const float* grad_y, float* grad_x, int N, int C, int D, int H, int W, long xs_n,
+                               long xs_c, long xs_d, long xs_h, long xs_w, long gs_n, long gs_c, long gs_d, long gs_h, long gs_w, int k);
 int lt_test_softargmax3d_bwd_host(const float* probs, const float* coord, const float* grad_keypoints, const float* grad_volumes,
                                   float* grad_logits, int B, int J, long nvox, float multiplier, int softmax);
 int lt_test_triangulate_dlt_fwd_host(const float* proj, const float* keypoints_2d, const float* confidences, float* out, int B,

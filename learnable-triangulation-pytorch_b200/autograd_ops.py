@@ -13,6 +13,7 @@ matrices (unprojection, DLT) and coordinate volumes (unprojection, 3-D soft-argm
 requires no grad, so their training steps launch no geometry kernel.
 """
 import torch
+import torch.nn.functional as F
 
 from . import capi, engine
 from .engine import _round_up
@@ -52,7 +53,18 @@ class UnprojectHeatmapsFn(torch.autograd.Function):
         grad_conf = torch.zeros((B, V, C), dtype=torch.float32, device=feats_cl.device) if need_conf else None
         need_proj, need_coord = ctx.needs_input_grad[1], ctx.needs_input_grad[2]
         grad_proj = grad_coord = None
-        if need_proj or need_coord:
+        if torch.are_deterministic_algorithms_enabled():
+            # the fixed-order backward (no float atomics), whatever warn_only says: same terms, one summation order
+            dev = feats_cl.device
+            grad_proj = torch.empty((B, V, 12), dtype=torch.float32, device=dev) if need_proj else None
+            grad_coord = torch.empty((B, nvox, 3), dtype=torch.float32, device=dev) if need_coord else None
+            ws = torch.empty(capi.unproject_aggregate_bwd_det_workspace_bytes(B, V, C, h, w, nvox, ctx.agg, need_proj or need_coord),
+                             dtype=torch.uint8, device=dev)
+            capi.unproject_aggregate_bwd_det(feats_cl, proj, coord, conf, g_cl, grad_feats, grad_conf, grad_proj, grad_coord, ctx.agg, ws)
+            proj_shape, coord_shape = ctx.geom_shapes
+            grad_proj = grad_proj.reshape(proj_shape) if need_proj else None
+            grad_coord = grad_coord.reshape(coord_shape) if need_coord else None
+        elif need_proj or need_coord:
             dev = feats_cl.device
             grad_proj = torch.empty((B, V, 12), dtype=torch.float32, device=dev) if need_proj else None
             grad_coord = torch.empty((B, nvox, 3), dtype=torch.float32, device=dev) if need_coord else None
@@ -66,6 +78,26 @@ class UnprojectHeatmapsFn(torch.autograd.Function):
         # grad_feats is the kernels' accumulation target even when the heat-maps need no gradient; it is returned only if they do
         grad_heat = grad_feats.permute(0, 1, 4, 2, 3) if ctx.needs_input_grad[0] else None   # (B, V, C, h, w) view
         return grad_heat, grad_proj, grad_coord, (grad_conf.reshape(ctx.conf_shape) if need_conf else None), None
+
+
+class MaxPool3dFn(torch.autograd.Function):
+    """F.max_pool3d(x, k, k) with the native fixed-order backward (lt_maxpool3d_bwd): what V2V's pooling runs under
+    torch.use_deterministic_algorithms, where torch has no deterministic CUDA max_pool3d backward.  The forward is torch's."""
+
+    @staticmethod
+    def forward(ctx, x, k):
+        ctx.save_for_backward(x)
+        ctx.k = k
+        return F.max_pool3d(x, k, k)
+
+    @staticmethod
+    def backward(ctx, grad_y):
+        x, = ctx.saved_tensors
+        if x.dtype != torch.float32:
+            raise TypeError("the native max-pool backward takes float32 (got %s)" % x.dtype)
+        grad_x = torch.empty_like(x)
+        capi.maxpool3d_bwd(x, grad_y, grad_x, ctx.k)
+        return grad_x, None
 
 
 class IntegrateTensor3dFn(torch.autograd.Function):

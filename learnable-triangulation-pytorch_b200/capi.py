@@ -83,6 +83,11 @@ SIGNATURES = {
     "lt_unproject_aggregate_bwd_geom_workspace_bytes": (c_size_t, [c_int, c_int, c_long]),
     "lt_unproject_aggregate_bwd_geom": (c_int, [c_void_p] * 10 + [c_size_t] + [c_int] * 5 + [c_long, c_int, c_void_p]),
     "lt_softargmax3d_coord_bwd": (c_int, [c_void_p] * 3 + [c_int, c_int, c_long, c_int, c_void_p]),
+    "lt_unproject_aggregate_bwd_det_workspace_bytes": (c_size_t, [c_int] * 5 + [c_long, c_int, c_int]),
+    "lt_unproject_aggregate_bwd_det": (c_int, [c_void_p] * 10 + [c_size_t] + [c_int] * 5 + [c_long, c_int, c_void_p]),
+    "lt_test_unproject_aggregate_bwd_det_host": (c_int, [c_void_p] * 9 + [c_int] * 5 + [c_long, c_int]),
+    "lt_maxpool3d_bwd": (c_int, [c_void_p] * 3 + [c_int] * 5 + [c_long] * 10 + [c_int, c_void_p]),
+    "lt_test_maxpool3d_bwd_host": (c_int, [c_void_p] * 3 + [c_int] * 5 + [c_long] * 10 + [c_int]),
     "lt_test_unproject_aggregate_bwd_geom_host": (c_int, [c_void_p] * 9 + [c_int] * 5 + [c_long, c_int]),
     "lt_test_softargmax3d_coord_bwd_host": (c_int, [c_void_p] * 3 + [c_int, c_int, c_long]),
     "lt_test_unproject_aggregate_bwd_host": (c_int, [c_void_p] * 7 + [c_int] * 5 + [c_long, c_int]),
@@ -314,6 +319,34 @@ def unproject_aggregate_bwd_geom(features_cl, proj, coord, conf, grad_out_cl, gr
 
 def unproject_aggregate_bwd_geom_workspace_bytes(B, V, nvox):
     return lib().lt_unproject_aggregate_bwd_geom_workspace_bytes(B, V, nvox)
+
+
+def unproject_aggregate_bwd_det(features_cl, proj, coord, conf, grad_out_cl, grad_features_cl, grad_conf, grad_proj, grad_coord, agg,
+                                workspace):
+    """lt_unproject_aggregate_bwd_det, the fixed-order backward: arguments as unproject_aggregate_bwd_geom (grad_proj and grad_coord may
+    both be None); workspace: unproject_aggregate_bwd_det_workspace_bytes(...) bytes."""
+    B, V, h, w, C = features_cl.shape
+    nvox = coord.shape[1]
+    _check(lib().lt_unproject_aggregate_bwd_det(_ptr(features_cl), _ptr(proj), _ptr(coord), _ptr(conf), _ptr(grad_out_cl),
+                                                _ptr(grad_features_cl), _ptr(grad_conf), _ptr(grad_proj), _ptr(grad_coord), _ptr(workspace),
+                                                workspace.numel() * workspace.element_size(), B, V, C, h, w, nvox, agg, _stream()),
+           "lt_unproject_aggregate_bwd_det")
+
+
+def unproject_aggregate_bwd_det_workspace_bytes(B, V, C, h, w, nvox, agg, geom):
+    n = lib().lt_unproject_aggregate_bwd_det_workspace_bytes(B, V, C, h, w, nvox, agg, int(bool(geom)))
+    if n == 0:
+        raise RuntimeError("lt_unproject_aggregate_bwd_det_workspace_bytes: sizes out of range or no CUDA device")
+    return n
+
+
+def maxpool3d_bwd(x, grad_y, grad_x, k):
+    """lt_maxpool3d_bwd: grad_x (strides of x) written from float32 x and grad_y (N, C, D, H, W) tensors of any strides."""
+    N, C, D, H, W = x.shape
+    assert x.is_cuda and grad_y.is_cuda and grad_x.is_cuda and x.stride() == grad_x.stride()
+    assert x.dtype == grad_y.dtype == grad_x.dtype == torch.float32
+    _check(lib().lt_maxpool3d_bwd(x.data_ptr(), grad_y.data_ptr(), grad_x.data_ptr(), N, C, D, H, W, *x.stride(), *grad_y.stride(), int(k),
+                                  _stream()), "lt_maxpool3d_bwd")
 
 
 def softargmax3d_coord_bwd(probs, grad_keypoints, grad_coord, B, J, nvox, softmax):
@@ -583,6 +616,25 @@ def softargmax3d_bwd_host(probs, coord, grad_keypoints, grad_volumes, grad_logit
     _check(lib().lt_test_softargmax3d_bwd_host(_host_ptr(probs), _host_ptr(coord), _host_ptr(grad_keypoints), _host_ptr(grad_volumes),
                                                _host_ptr(grad_logits), B, J, nvox, float(multiplier), int(mode)),
            "lt_test_softargmax3d_bwd_host")
+
+
+def unproject_aggregate_bwd_det_host(features, proj, coord, conf, grad_out, grad_features, grad_conf, grad_proj, grad_coord, agg):
+    """lt_test_unproject_aggregate_bwd_det_host: the fixed-order backward's pass-1, gather and confidence items on CPU tensors (test hook,
+    no GPU needed).  Shapes as unproject_aggregate_bwd_det."""
+    B, V, h, w, C = features.shape
+    nvox = coord.shape[1]
+    _check(lib().lt_test_unproject_aggregate_bwd_det_host(_host_ptr(features), _host_ptr(proj), _host_ptr(coord), _host_ptr(conf),
+                                                          _host_ptr(grad_out), _host_ptr(grad_features), _host_ptr(grad_conf),
+                                                          _host_ptr(grad_proj), _host_ptr(grad_coord), B, V, C, h, w, nvox, agg),
+           "lt_test_unproject_aggregate_bwd_det_host")
+
+
+def maxpool3d_bwd_host(x, grad_y, grad_x, k):
+    """lt_test_maxpool3d_bwd_host: the max-pool backward's per-element code on CPU float32 tensors of any strides (grad_x: those of x)."""
+    N, C, D, H, W = x.shape
+    assert not x.is_cuda and x.stride() == grad_x.stride() and x.dtype == grad_y.dtype == grad_x.dtype == torch.float32
+    _check(lib().lt_test_maxpool3d_bwd_host(x.data_ptr(), grad_y.data_ptr(), grad_x.data_ptr(), N, C, D, H, W, *x.stride(), *grad_y.stride(),
+                                            int(k)), "lt_test_maxpool3d_bwd_host")
 
 
 def unproject_aggregate_bwd_geom_host(features, proj, coord, conf, grad_out, grad_features, grad_conf, grad_proj, grad_coord, agg):

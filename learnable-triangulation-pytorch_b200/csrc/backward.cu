@@ -18,9 +18,17 @@
 // the algebraic model (triangulation.py:131-200) trains through with the pixel grid (x, y, 0) as coordinates:
 //     mass:    d logit_i = mult * [p_i > 0] * (g_vol_i + (<g_kp, x_i> - <g_kp, kp>) / M)
 // The DLT backward of the algebraic model is in algebraic.cu (it shares the forward's eigen-solve).
+//
+// Fixed-order unprojection backward (lt_unproject_aggregate_bwd_det, selected by torch.use_deterministic_algorithms): no float
+// atomics.  Pass 1 runs the same per-item code but stores each (sample, view, voxel) sample gradient and the voxel's floor cell
+// instead of scattering; pass 2 sorts the voxels of every (sample, view) by cell, stably (voxel order within a cell); pass 3 gathers
+// per (pixel, channel quad) the terms gs * w_k of the four cells that have the pixel as a tap, in a fixed cell order and voxel order.
+// d conf sums fixed voxel chunks and merges them in chunk order.  Every sum depends only on the inputs of its own sample.
 #include "common.cuh"
+#include <cub/device/device_radix_sort.cuh>
 #include <math.h>
 #include <stdlib.h>
+#include <vector>
 
 // The per-item bodies are __host__ __device__: the kernels run them on the GPU, and lt_test_*_bwd_host (bottom of the file)
 // runs the SAME code on the CPU so that `-m "not gpu"` tests can check the gradient arithmetic against torch autograd
@@ -161,7 +169,34 @@ struct UnprojBwdParams {
   long nvox;
   float* geom_q;           // geometry variant: [B][V][nvox][3] q per (sample, view, voxel), written (the host hook accumulates
                            // (G_ix, G_iy) into its first two slots instead and forms q afterwards)
+  float* stage_gs;         // fixed-order pass 1: [B][V][nvox][C] sample gradient per (sample, view, voxel), written
+  unsigned* stage_key;     //   [B][V][nvox] sort key (b V + v) (cells + 1) + floor cell (det_cell), written
+  unsigned* stage_vox;     //   [B][V][nvox] the voxel index (the sort's values), written
 };
+
+// The (h + 1) x (w + 1) floor cells (xi, yi) of bwd_taps_impl whose taps can lie inside the map, xi, yi in [-1, size - 1], as
+// (yi + 1) (w + 1) + xi + 1, read off the first tap with a weight (such a tap is not clamped); (h + 1) (w + 1) when no tap has a
+// weight, i.e. the voxel adds nothing to this view.
+__host__ __device__ __forceinline__ unsigned det_cell(const BwdTaps& t, int h, int w) {
+#pragma unroll
+  for (int k = 0; k < 4; ++k)
+    if (t.w[k] != 0.0f) {
+      const int y = t.o[k] / w - (k >> 1), x = t.o[k] % w - (k & 1);
+      return (unsigned)((y + 1) * (w + 1) + x + 1);
+    }
+  return (unsigned)((h + 1) * (w + 1));
+}
+__host__ __device__ __forceinline__ long det_keys_per_view(int h, int w) { return (long)(h + 1) * (w + 1) + 1; }
+
+// pass 1 sink: what scatter4 would add for (b, v, vox, quad), stored; the voxel's first quad also stores its key and index
+__host__ __device__ __forceinline__ void det_stage(const UnprojBwdParams& p, int b, int v, long vox, int c0, const BwdTaps& t, float4 gs) {
+  const long row = ((long)b * p.V + v) * p.nvox + vox;
+  *reinterpret_cast<float4*>(p.stage_gs + row * p.C + c0) = gs;
+  if (c0 == 0) {
+    p.stage_key[row] = (unsigned)(((long)b * p.V + v) * det_keys_per_view(p.h, p.w) + det_cell(t, p.h, p.w));
+    p.stage_vox[row] = (unsigned)vox;
+  }
+}
 
 constexpr int kBwdSmemViews = 64;
 
@@ -192,7 +227,8 @@ __host__ __device__ __forceinline__ void geom_emit(const UnprojBwdParams& p, int
 // one (voxel, 4-channel quad) of sample b.  projs: the sample's first kBwdSmemViews projection matrices (shared memory on
 // the GPU) or null; gconf_acc: [V][C] accumulator of d conf (shared memory on the GPU, the output itself on the host) or null.
 // kGeom also hands every view's (G_ix, G_iy) to geom_emit, once per view on every path (the GPU lanes of a voxel meet there).
-template <bool kGeom>
+// kStage (the fixed-order path) stores every view's sample gradient with det_stage instead of scattering it.
+template <bool kGeom, bool kStage = false>
 __host__ __device__ __forceinline__ void unproject_bwd_item(const UnprojBwdParams& p, int b, long it, const float* projs, float* gconf_acc) {
   const int quads = p.C >> 2;
   const long map_elems = (long)p.h * p.w * p.C;
@@ -221,7 +257,8 @@ __host__ __device__ __forceinline__ void unproject_bwd_item(const UnprojBwdParam
           }
           gs = make_float4(g.x * cf.x, g.y * cf.y, g.z * cf.z, g.w * cf.w);
         }
-        scatter4(gb + v * map_elems, p.C, c0, t, gs);
+        if (kStage) det_stage(p, b, v, vox, c0, t, gs);
+        else scatter4(gb + v * map_elems, p.C, c0, t, gs);
         if (kGeom) geom_emit(p, b, v, vox, c0 >> 2, gt, geom_partial(fb + v * map_elems, p.C, c0, t, gt, gs));
       }
     } else if (p.agg == LT_AGG_MAX) {
@@ -240,8 +277,11 @@ __host__ __device__ __forceinline__ void unproject_bwd_item(const UnprojBwdParam
         if (kGeom) {
           GeomTaps gt;
           const BwdTaps t = bwd_taps_impl<true>(view_proj(v), X, Y, Z, p.h, p.w, &gt);
-          if (gs.x != 0.f || gs.y != 0.f || gs.z != 0.f || gs.w != 0.f) scatter4(gb + v * map_elems, p.C, c0, t, gs);
+          if (kStage) det_stage(p, b, v, vox, c0, t, gs);
+          else if (gs.x != 0.f || gs.y != 0.f || gs.z != 0.f || gs.w != 0.f) scatter4(gb + v * map_elems, p.C, c0, t, gs);
           geom_emit(p, b, v, vox, c0 >> 2, gt, geom_partial(fb + v * map_elems, p.C, c0, t, gt, gs));
+        } else if (kStage) {
+          det_stage(p, b, v, vox, c0, bwd_taps(view_proj(v), X, Y, Z, p.h, p.w), gs);
         } else if (gs.x != 0.f || gs.y != 0.f || gs.z != 0.f || gs.w != 0.f) {
           scatter4(gb + v * map_elems, p.C, c0, bwd_taps(view_proj(v), X, Y, Z, p.h, p.w), gs);
         }
@@ -268,7 +308,8 @@ __host__ __device__ __forceinline__ void unproject_bwd_item(const UnprojBwdParam
         const float4 s = sample4(fb + v * map_elems, p.C, c0, t);
         const float4 gs = make_float4(g.x * (expf(s.x - m.x) / den.x) * (1.0f + s.x - out.x), g.y * (expf(s.y - m.y) / den.y) * (1.0f + s.y - out.y),
                                       g.z * (expf(s.z - m.z) / den.z) * (1.0f + s.z - out.z), g.w * (expf(s.w - m.w) / den.w) * (1.0f + s.w - out.w));
-        scatter4(gb + v * map_elems, p.C, c0, t, gs);
+        if (kStage) det_stage(p, b, v, vox, c0, t, gs);
+        else scatter4(gb + v * map_elems, p.C, c0, t, gs);
         if (kGeom) geom_emit(p, b, v, vox, c0 >> 2, gt, geom_partial(fb + v * map_elems, p.C, c0, t, gt, gs));
       }
     }
@@ -386,6 +427,117 @@ __global__ void __launch_bounds__(256) unproject_geom_dx_kernel(const float* __r
   const long i = (long)blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= (long)B * nvox) return;
   geom_dx_item(proj, q, grad_coord, V, nvox, (int)(i / nvox), i % nvox);
+}
+
+// ---- fixed-order unprojection backward: passes 1 and 3 and the confidence gradient (see the top of the file) ----
+#ifdef __CUDA_ARCH__
+#define LT_ADD_PROD(acc, a, b) __fadd_rn((acc), __fmul_rn((a), (b)))    // the product rounded as the atomic kernel rounds it, then added
+#else
+#define LT_ADD_PROD(acc, a, b) ((acc) + (a) * (b))
+#endif
+
+__host__ __device__ __forceinline__ void add_prod4(float4& acc, float4 a, float b) {
+  acc.x = LT_ADD_PROD(acc.x, a.x, b); acc.y = LT_ADD_PROD(acc.y, a.y, b); acc.z = LT_ADD_PROD(acc.z, a.z, b); acc.w = LT_ADD_PROD(acc.w, a.w, b);
+}
+
+// d features of (b v, pixel pix, quad c0): the terms gs * w_k of the cells (y - 1, x - 1), (y - 1, x), (y, x - 1), (y, x) in that
+// order (the pixel is their tap k = 3, 2, 1, 0), each cell's voxels in ascending order (seg_begin / seg_end: the cell's range of
+// sorted_vox).  The taps are recomputed with bwd_taps, so w_k is the weight pass 1 and the atomic kernel use.
+__host__ __device__ __forceinline__ float4 det_gather_item(const UnprojBwdParams& p, const unsigned* __restrict__ seg_begin,
+                                                           const unsigned* __restrict__ seg_end, const unsigned* __restrict__ sorted_vox,
+                                                           int bv, int pix, int c0) {
+  const int b = bv / p.V, y = pix / p.w, x = pix % p.w;
+  const float* P = p.proj + (long)bv * 12;
+  const long kbase = (long)bv * det_keys_per_view(p.h, p.w);
+  float4 acc = make_float4(0.f, 0.f, 0.f, 0.f);
+  for (int k = 3; k >= 0; --k) {
+    const long key = kbase + (long)(y - (k >> 1) + 1) * (p.w + 1) + (x - (k & 1) + 1);
+    const unsigned e = LT_LD(seg_end + key);
+    for (unsigned i = LT_LD(seg_begin + key); i < e; ++i) {
+      const long vox = LT_LD(sorted_vox + i);
+      const float* cp = p.coord + ((long)b * p.nvox + vox) * 3;
+      const float wk = bwd_taps(P, LT_LD(cp), LT_LD(cp + 1), LT_LD(cp + 2), p.h, p.w).w[k];
+      if (wk != 0.0f) add_prod4(acc, LT_LD(reinterpret_cast<const float4*>(p.stage_gs + ((long)bv * p.nvox + vox) * p.C + c0)), wk);
+    }
+  }
+  return acc;
+}
+
+// d conf of (b v, quad c0) over one chunk of kDetConfChunk voxels: the terms g * s, voxels in order (the atomic kernel's terms)
+constexpr int kDetConfChunk = 256;
+__host__ __device__ __forceinline__ long det_conf_chunks(long nvox) { return (nvox + kDetConfChunk - 1) / kDetConfChunk; }
+
+__host__ __device__ __forceinline__ float4 det_conf_partial(const UnprojBwdParams& p, int bv, long chunk, int c0) {
+  const int b = bv / p.V;
+  const float* P = p.proj + (long)bv * 12;
+  const float* fmap = p.features + (long)bv * p.h * p.w * p.C;
+  const long v0 = chunk * kDetConfChunk, v1 = v0 + kDetConfChunk < p.nvox ? v0 + kDetConfChunk : p.nvox;
+  float4 acc = make_float4(0.f, 0.f, 0.f, 0.f);
+  for (long vox = v0; vox < v1; ++vox) {
+    const float* cp = p.coord + ((long)b * p.nvox + vox) * 3;
+    const float4 s = sample4(fmap, p.C, c0, bwd_taps(P, LT_LD(cp), LT_LD(cp + 1), LT_LD(cp + 2), p.h, p.w));
+    const float4 g = LT_LD(reinterpret_cast<const float4*>(p.grad_out + ((long)b * p.nvox + vox) * p.C + c0));
+    acc.x = LT_ADD_PROD(acc.x, g.x, s.x); acc.y = LT_ADD_PROD(acc.y, g.y, s.y);
+    acc.z = LT_ADD_PROD(acc.z, g.z, s.z); acc.w = LT_ADD_PROD(acc.w, g.w, s.w);
+  }
+  return acc;
+}
+
+// grad_conf[bv][c] += the chunk partials [bv][chunk][c] in chunk order
+__host__ __device__ __forceinline__ void det_conf_merge_item(const float* __restrict__ partial, float* __restrict__ grad_conf, int C, long chunks,
+                                                             long i) {
+  const long bv = i / C, c = i % C;
+  float s = 0.0f;
+  for (long k = 0; k < chunks; ++k) s += LT_LD(partial + (bv * chunks + k) * C + c);
+  grad_conf[i] += s;
+}
+
+template <bool kGeom>
+__global__ void __launch_bounds__(256) fo_unproj_bwd_stage_kernel(const UnprojBwdParams p) {
+  const long items = p.nvox * (p.C >> 2);
+  for (long it = (long)blockIdx.x * blockDim.x + threadIdx.x; it < items; it += (long)gridDim.x * blockDim.x)
+    unproject_bwd_item<kGeom, true>(p, blockIdx.y, it, nullptr, nullptr);
+}
+
+// each sorted key's segment [begin, end) of the sorted order; keys of no voxel keep the empty [0, 0)
+__global__ void __launch_bounds__(256) fo_unproj_bwd_bounds_kernel(const unsigned* __restrict__ keys, unsigned* __restrict__ seg_begin,
+                                                                    unsigned* __restrict__ seg_end, long n) {
+  const long i = (long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  const unsigned k = keys[i];
+  if (i == 0 || keys[i - 1] != k) seg_begin[k] = (unsigned)i;
+  if (i == n - 1 || keys[i + 1] != k) seg_end[k] = (unsigned)(i + 1);
+}
+
+// grid (pixel quads / 256, B V): grad_features, which the caller zero-fills, gets each total added once
+__global__ void __launch_bounds__(256) fo_unproj_bwd_gather_kernel(const UnprojBwdParams p, const unsigned* __restrict__ seg_begin,
+                                                                    const unsigned* __restrict__ seg_end, const unsigned* __restrict__ sorted_vox) {
+  const int quads = p.C >> 2, bv = blockIdx.y;
+  const long i = (long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= (long)p.h * p.w * quads) return;
+  const int pix = (int)(i / quads), c0 = (int)(i % quads) * 4;
+  const float4 a = det_gather_item(p, seg_begin, seg_end, sorted_vox, bv, pix, c0);
+  float4* dst = reinterpret_cast<float4*>(p.grad_features + ((long)bv * p.h * p.w + pix) * p.C + c0);
+  float4 d = *dst;
+  d.x += a.x; d.y += a.y; d.z += a.z; d.w += a.w;
+  *dst = d;
+}
+
+// grid (chunks x quads / 128, B V): partial[bv][chunk][C]
+__global__ void __launch_bounds__(128) fo_unproj_bwd_conf_partial_kernel(const UnprojBwdParams p, float* __restrict__ partial) {
+  const int quads = p.C >> 2, bv = blockIdx.y;
+  const long chunks = det_conf_chunks(p.nvox);
+  const long i = (long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= chunks * quads) return;
+  const long chunk = i / quads;
+  const int c0 = (int)(i % quads) * 4;
+  *reinterpret_cast<float4*>(partial + ((long)bv * chunks + chunk) * p.C + c0) = det_conf_partial(p, bv, chunk, c0);
+}
+
+__global__ void __launch_bounds__(128) fo_unproj_bwd_conf_merge_kernel(const float* __restrict__ partial, float* __restrict__ grad_conf, int C,
+                                                                        long chunks, long n) {
+  const long i = (long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i < n) det_conf_merge_item(partial, grad_conf, C, chunks, i);
 }
 
 // ---- soft-argmax backward, NCDHW: volumes / logits / grads are [B][J][nvox] ----
@@ -531,6 +683,23 @@ extern "C" size_t lt_unproject_aggregate_bwd_geom_workspace_bytes(int B, int V, 
   return geom_q_bytes(B, V, nvox) + (size_t)B * V * geom_chunks(nvox) * 12 * sizeof(double);
 }
 
+// dP (when grad_proj) and dX (when grad_coord) from the q of every (sample, view, voxel)
+static int geom_tail(const float* proj, const float* coord, const float* q, double* partial, float* grad_proj, float* grad_coord, int B, int V,
+                     long nvox, cudaStream_t st) {
+  if (grad_proj) {
+    const int chunks = geom_chunks(nvox);
+    unproject_geom_dp_partial_kernel<<<dim3((unsigned)chunks, (unsigned)(B * V)), kGeomThreads, 0, st>>>(coord, q, partial, V, nvox);
+    LT_CHECK_LAUNCH("unproject_geom_dp_partial_kernel");
+    unproject_geom_dp_merge_kernel<<<ceil_div((long)B * V * 12, 128), 128, 0, st>>>(partial, grad_proj, B * V, chunks);
+    LT_CHECK_LAUNCH("unproject_geom_dp_merge_kernel");
+  }
+  if (grad_coord) {
+    unproject_geom_dx_kernel<<<ceil_div((long)B * nvox, 256), 256, 0, st>>>(proj, q, grad_coord, B, V, nvox);
+    LT_CHECK_LAUNCH("unproject_geom_dx_kernel");
+  }
+  return LT_OK;
+}
+
 extern "C" int lt_unproject_aggregate_bwd_geom(const float* features, const float* proj, const float* coord, const float* conf,
                                                const float* grad_out, float* grad_features, float* grad_conf, float* grad_proj,
                                                float* grad_coord, void* workspace, size_t workspace_bytes, int B, int V, int C, int h,
@@ -556,16 +725,105 @@ extern "C" int lt_unproject_aggregate_bwd_geom(const float* features, const floa
   cudaStream_t st = (cudaStream_t)stream;
   unproject_bwd_geom_kernel<<<dim3((unsigned)blocks, (unsigned)B), 256, smem, st>>>(p);
   LT_CHECK_LAUNCH("unproject_bwd_geom_kernel");
-  if (grad_proj) {
-    const int chunks = geom_chunks(nvox);
-    unproject_geom_dp_partial_kernel<<<dim3((unsigned)chunks, (unsigned)(B * V)), kGeomThreads, 0, st>>>(coord, q, partial, V, nvox);
-    LT_CHECK_LAUNCH("unproject_geom_dp_partial_kernel");
-    unproject_geom_dp_merge_kernel<<<ceil_div((long)B * V * 12, 128), 128, 0, st>>>(partial, grad_proj, B * V, chunks);
-    LT_CHECK_LAUNCH("unproject_geom_dp_merge_kernel");
+  return geom_tail(proj, coord, q, partial, grad_proj, grad_coord, B, V, nvox, st);
+}
+
+// ---- fixed-order unprojection backward: workspace layout and launches ----
+struct DetLayout {
+  size_t gs, key0, key1, vox0, vox1, seg_begin, seg_end, conf, geom, sort, sort_bytes, total;
+  int key_bits;
+};
+
+static size_t det_align(size_t n) { return (n + 255) & ~(size_t)255; }
+
+// the sort's scratch is what cub::DeviceRadixSort asks for on the current device (0 with no device: the layout is then unusable)
+static DetLayout det_layout(int B, int V, int C, int h, int w, long nvox, bool want_conf, bool geom) {
+  DetLayout L{};
+  const long n = (long)B * V * nvox, nkeys = (long)B * V * det_keys_per_view(h, w);
+  size_t off = 0;
+  auto take = [&](size_t bytes) { const size_t o = off; off += det_align(bytes); return o; };
+  L.gs = take((size_t)n * C * sizeof(float));
+  L.key0 = take((size_t)n * 4); L.key1 = take((size_t)n * 4); L.vox0 = take((size_t)n * 4); L.vox1 = take((size_t)n * 4);
+  L.seg_begin = take((size_t)nkeys * 4); L.seg_end = take((size_t)nkeys * 4);
+  L.conf = take(want_conf ? (size_t)B * V * det_conf_chunks(nvox) * C * sizeof(float) : 0);
+  L.geom = take(geom ? lt_unproject_aggregate_bwd_geom_workspace_bytes(B, V, nvox) : 0);
+  L.key_bits = 1;
+  while (L.key_bits < 32 && (1L << L.key_bits) < nkeys) ++L.key_bits;
+  size_t sort_bytes = 0;
+  if (cub::DeviceRadixSort::SortPairs(nullptr, sort_bytes, (const unsigned*)nullptr, (unsigned*)nullptr, (const unsigned*)nullptr,
+                                      (unsigned*)nullptr, (int)n, 0, L.key_bits) != cudaSuccess) {
+    cudaGetLastError();
+    return DetLayout{};
   }
-  if (grad_coord) {
-    unproject_geom_dx_kernel<<<ceil_div((long)B * nvox, 256), 256, 0, st>>>(proj, q, grad_coord, B, V, nvox);
-    LT_CHECK_LAUNCH("unproject_geom_dx_kernel");
+  L.sort = take(sort_bytes);
+  L.sort_bytes = sort_bytes;
+  L.total = off;
+  return L;
+}
+
+static bool det_sizes_ok(int B, int V, int h, int w, long nvox) {
+  return B > 0 && V > 0 && h > 0 && w > 0 && nvox > 0 && (long)B * V <= 65535 && (long)B * V * nvox <= 0x7fffffffL &&
+         (long)B * V * det_keys_per_view(h, w) <= 0x7fffffffL;
+}
+
+extern "C" size_t lt_unproject_aggregate_bwd_det_workspace_bytes(int B, int V, int C, int h, int w, long nvox, int agg, int geom) {
+  if (!det_sizes_ok(B, V, h, w, nvox) || C <= 0) return 0;
+  return det_layout(B, V, C, h, w, nvox, agg == LT_AGG_CONF, geom != 0).total;
+}
+
+extern "C" int lt_unproject_aggregate_bwd_det(const float* features, const float* proj, const float* coord, const float* conf,
+                                              const float* grad_out, float* grad_features, float* grad_conf, float* grad_proj, float* grad_coord,
+                                              void* workspace, size_t workspace_bytes, int B, int V, int C, int h, int w, long nvox, int agg,
+                                              void* stream) {
+  LT_REQUIRE(features && proj && coord && grad_out && grad_features && workspace, "unproject_bwd_det: null pointer");
+  LT_REQUIRE(B > 0 && V > 0 && C > 0 && h > 0 && w > 0 && nvox > 0, "unproject_bwd_det: non-positive size");
+  LT_REQUIRE(det_sizes_ok(B, V, h, w, nvox), "unproject_bwd_det: too large (B V <= 65535, B V nvox and B V (h + 1) (w + 1) below 2^31)");
+  const bool geom = grad_proj != nullptr || grad_coord != nullptr;
+  LT_REQUIRE(C % 4 == 0 && (!geom || (C <= 128 && ((C / 4) & (C / 4 - 1)) == 0)),
+             "unproject_bwd_det: C %% 4 != 0, or with geometry outputs C / 4 not a power of two <= 32 (C=%d)", C);
+  LT_REQUIRE(agg >= LT_AGG_SUM && agg <= LT_AGG_CONF, "unproject_bwd_det: unknown aggregation %d", agg);
+  LT_REQUIRE(agg != LT_AGG_CONF || conf, "unproject_bwd_det: LT_AGG_CONF needs confidences");
+  const bool want_conf = grad_conf != nullptr && agg == LT_AGG_CONF;
+  const DetLayout L = det_layout(B, V, C, h, w, nvox, want_conf, geom);
+  LT_REQUIRE(L.total > 0 && workspace_bytes >= L.total, "unproject_bwd_det: workspace of %zu bytes, %zu needed", workspace_bytes, L.total);
+  char* ws = reinterpret_cast<char*>(workspace);
+  unsigned* key0 = reinterpret_cast<unsigned*>(ws + L.key0);
+  unsigned* key1 = reinterpret_cast<unsigned*>(ws + L.key1);
+  unsigned* vox0 = reinterpret_cast<unsigned*>(ws + L.vox0);
+  unsigned* vox1 = reinterpret_cast<unsigned*>(ws + L.vox1);
+  unsigned* seg_begin = reinterpret_cast<unsigned*>(ws + L.seg_begin);
+  unsigned* seg_end = reinterpret_cast<unsigned*>(ws + L.seg_end);
+  float* q = reinterpret_cast<float*>(ws + L.geom);
+  UnprojBwdParams p{features, proj, coord, conf, grad_out, grad_features, nullptr, B, V, C, h, w, agg, nvox, q,
+                    reinterpret_cast<float*>(ws + L.gs), key0, vox0};
+  cudaStream_t st = (cudaStream_t)stream;
+  const long n = (long)B * V * nvox, nkeys = (long)B * V * det_keys_per_view(h, w);
+  long blocks = (nvox * (C / 4) + 255) / 256;
+  const long cap = (long)sm_count() * 8;
+  if (blocks > cap) blocks = cap;
+  if (geom) fo_unproj_bwd_stage_kernel<true><<<dim3((unsigned)blocks, (unsigned)B), 256, 0, st>>>(p);
+  else fo_unproj_bwd_stage_kernel<false><<<dim3((unsigned)blocks, (unsigned)B), 256, 0, st>>>(p);
+  LT_CHECK_LAUNCH("fo_unproj_bwd_stage_kernel");
+  size_t sort_bytes = L.sort_bytes;
+  const cudaError_t se = cub::DeviceRadixSort::SortPairs(ws + L.sort, sort_bytes, key0, key1, vox0, vox1, (int)n, 0, L.key_bits, st);
+  LT_REQUIRE(se == cudaSuccess, "unproject_bwd_det: radix sort failed: %s", cudaGetErrorString(se));
+  LT_REQUIRE(cudaMemsetAsync(seg_begin, 0, (size_t)nkeys * 4, st) == cudaSuccess && cudaMemsetAsync(seg_end, 0, (size_t)nkeys * 4, st) == cudaSuccess,
+             "unproject_bwd_det: memset failed");
+  fo_unproj_bwd_bounds_kernel<<<ceil_div(n, 256), 256, 0, st>>>(key1, seg_begin, seg_end, n);
+  LT_CHECK_LAUNCH("fo_unproj_bwd_bounds_kernel");
+  fo_unproj_bwd_gather_kernel<<<dim3((unsigned)ceil_div((long)h * w * (C / 4), 256), (unsigned)(B * V)), 256, 0, st>>>(p, seg_begin, seg_end, vox1);
+  LT_CHECK_LAUNCH("fo_unproj_bwd_gather_kernel");
+  if (want_conf) {
+    float* partial = reinterpret_cast<float*>(ws + L.conf);
+    const long chunks = det_conf_chunks(nvox);
+    fo_unproj_bwd_conf_partial_kernel<<<dim3((unsigned)ceil_div(chunks * (C / 4), 128), (unsigned)(B * V)), 128, 0, st>>>(p, partial);
+    LT_CHECK_LAUNCH("fo_unproj_bwd_conf_partial_kernel");
+    fo_unproj_bwd_conf_merge_kernel<<<ceil_div((long)B * V * C, 128), 128, 0, st>>>(partial, grad_conf, C, chunks, (long)B * V * C);
+    LT_CHECK_LAUNCH("fo_unproj_bwd_conf_merge_kernel");
+  }
+  if (geom) {
+    double* partial = reinterpret_cast<double*>(reinterpret_cast<char*>(q) + geom_q_bytes(B, V, nvox));
+    return geom_tail(proj, coord, q, partial, grad_proj, grad_coord, B, V, nvox, st);
   }
   return LT_OK;
 }
@@ -617,6 +875,9 @@ extern "C" int lt_test_unproject_aggregate_bwd_host(const float* features, const
   return LT_OK;
 }
 
+static void geom_host_tail(const float* proj, const float* coord, float* q, float* grad_proj, float* grad_coord, int B, int V, int h, int w,
+                           long nvox);
+
 extern "C" int lt_test_unproject_aggregate_bwd_geom_host(const float* features, const float* proj, const float* coord, const float* conf,
                                                          const float* grad_out, float* grad_features, float* grad_conf, float* grad_proj,
                                                          float* grad_coord, int B, int V, int C, int h, int w, long nvox, int agg) {
@@ -630,6 +891,14 @@ extern "C" int lt_test_unproject_aggregate_bwd_geom_host(const float* features, 
   for (int b = 0; b < B; ++b)
     for (long it = 0; it < items; ++it)
       unproject_bwd_item<true>(p, b, it, nullptr, (grad_conf && agg == LT_AGG_CONF) ? grad_conf + (long)b * V * C : nullptr);
+  geom_host_tail(proj, coord, q, grad_proj, grad_coord, B, V, h, w, nvox);
+  free(q);
+  return LT_OK;
+}
+
+// (G_ix, G_iy) accumulated in q's first two slots -> q, then dP and dX, as the GPU's geometry passes form them
+static void geom_host_tail(const float* proj, const float* coord, float* q, float* grad_proj, float* grad_coord, int B, int V, int h, int w,
+                           long nvox) {
   for (int b = 0; b < B; ++b)       // (G_ix, G_iy) -> q, as the voxel's first lane forms it on the GPU
     for (int v = 0; v < V; ++v)
       for (long vox = 0; vox < nvox; ++vox) {
@@ -650,7 +919,51 @@ extern "C" int lt_test_unproject_aggregate_bwd_geom_host(const float* features, 
   }
   for (int b = 0; grad_coord && b < B; ++b)
     for (long vox = 0; vox < nvox; ++vox) geom_dx_item(proj, q, grad_coord, V, nvox, b, vox);
-  free(q);
+}
+
+// the fixed-order path on the CPU: pass 1 and the gather / confidence items of the GPU, with a host counting sort (stable: voxels in
+// order within a cell, the order cub's stable radix sort gives)
+extern "C" int lt_test_unproject_aggregate_bwd_det_host(const float* features, const float* proj, const float* coord, const float* conf,
+                                                        const float* grad_out, float* grad_features, float* grad_conf, float* grad_proj,
+                                                        float* grad_coord, int B, int V, int C, int h, int w, long nvox, int agg) {
+  LT_REQUIRE(features && proj && coord && grad_out && grad_features && C % 4 == 0 && det_sizes_ok(B, V, h, w, nvox),
+             "test_unproject_bwd_det_host: bad arguments");
+  LT_REQUIRE(agg >= LT_AGG_SUM && agg <= LT_AGG_CONF && (agg != LT_AGG_CONF || conf), "test_unproject_bwd_det_host: bad aggregation");
+  const bool geom = grad_proj != nullptr || grad_coord != nullptr;
+  const long n = (long)B * V * nvox, nkeys = (long)B * V * det_keys_per_view(h, w);
+  std::vector<float> gs((size_t)n * C + 4), q(geom ? (size_t)n * 3 : 0, 0.0f);
+  std::vector<unsigned> key(n), vox(n), sorted(n), seg_begin(nkeys, 0), seg_end(nkeys, 0);
+  UnprojBwdParams p{features, proj, coord, conf, grad_out, grad_features, nullptr, B, V, C, h, w, agg, nvox, geom ? q.data() : nullptr,
+                    gs.data(), key.data(), vox.data()};
+  const long items = nvox * (C / 4);
+  for (int b = 0; b < B; ++b)
+    for (long it = 0; it < items; ++it) {
+      if (geom) unproject_bwd_item<true, true>(p, b, it, nullptr, nullptr);
+      else unproject_bwd_item<false, true>(p, b, it, nullptr, nullptr);
+    }
+  for (long i = 0; i < n; ++i) ++seg_end[key[i]];
+  for (long k = 0, off = 0; k < nkeys; ++k) { seg_begin[k] = (unsigned)off; off += seg_end[k]; seg_end[k] = seg_begin[k]; }
+  for (long i = 0; i < n; ++i) sorted[seg_end[key[i]]++] = vox[i];
+  for (int bv = 0; bv < B * V; ++bv)
+    for (int pix = 0; pix < h * w; ++pix)
+      for (int c0 = 0; c0 < C; c0 += 4) {
+        const float4 a = det_gather_item(p, seg_begin.data(), seg_end.data(), sorted.data(), bv, pix, c0);
+        float* d = grad_features + ((long)bv * h * w + pix) * C + c0;
+        d[0] += a.x; d[1] += a.y; d[2] += a.z; d[3] += a.w;
+      }
+  if (grad_conf && agg == LT_AGG_CONF) {
+    const long chunks = det_conf_chunks(nvox);
+    std::vector<float> partial((size_t)B * V * chunks * C);
+    for (int bv = 0; bv < B * V; ++bv)
+      for (long ch = 0; ch < chunks; ++ch)
+        for (int c0 = 0; c0 < C; c0 += 4) {
+          const float4 a = det_conf_partial(p, bv, ch, c0);
+          float* d = partial.data() + ((long)bv * chunks + ch) * C + c0;
+          d[0] = a.x; d[1] = a.y; d[2] = a.z; d[3] = a.w;
+        }
+    for (long i = 0; i < (long)B * V * C; ++i) det_conf_merge_item(partial.data(), grad_conf, C, chunks, i);
+  }
+  if (geom) geom_host_tail(proj, coord, q.data(), grad_proj, grad_coord, B, V, h, w, nvox);
   return LT_OK;
 }
 

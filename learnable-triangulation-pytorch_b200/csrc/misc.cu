@@ -97,6 +97,55 @@ __global__ void __launch_bounds__(256) maxpool_kernel(const PoolParams p) {
 }
 
 
+// ---- max-pool backward, non-overlapping windows (kernel == stride, no padding), float32, any element strides ----------
+// The gather form of torch's max_pool3d backward: one thread per input element re-finds its window's arg-max with torch's rule
+// (scan d, h, w; a value is taken if greater than the running maximum or NaN, the window's first element if none is), and writes
+// 0 + grad_y there (torch adds into a zeroed gradient) and 0 elsewhere, including the tail floor mode drops.  No atomics.
+struct Pool3dBwdParams {
+  const float* x; const float* gy; float* gx;
+  int N, C, D, H, W, k;
+  long xs[5], gs[5];    // element strides (n, c, d, h, w) of x and grad_x, and of grad_y
+};
+
+__host__ __device__ __forceinline__ void pool3d_bwd_item(const Pool3dBwdParams& p, long i) {
+  int n, c, d, h, w;
+  long r = i;
+  if (p.xs[1] == 1 && p.C > 1) {   // channels-last: walk memory order, c fastest
+    c = (int)(r % p.C); r /= p.C; w = (int)(r % p.W); r /= p.W; h = (int)(r % p.H); r /= p.H; d = (int)(r % p.D); n = (int)(r / p.D);
+  } else {
+    w = (int)(r % p.W); r /= p.W; h = (int)(r % p.H); r /= p.H; d = (int)(r % p.D); r /= p.D; c = (int)(r % p.C); n = (int)(r / p.C);
+  }
+  const int k = p.k, od = d / k, oh = h / k, ow = w / k;
+  float out = 0.0f;
+  if (od < p.D / k && oh < p.H / k && ow < p.W / k) {
+    const float* xb = p.x + n * p.xs[0] + c * p.xs[1];
+    const int d0 = od * k, h0 = oh * k, w0 = ow * k;
+    float m = -INFINITY;
+    int best = 0;
+    for (int a = 0; a < k; ++a)
+      for (int b = 0; b < k; ++b)
+        for (int e = 0; e < k; ++e) {
+          const float v = xb[(d0 + a) * p.xs[2] + (h0 + b) * p.xs[3] + (w0 + e) * p.xs[4]];
+          if (v > m || v != v) { m = v; best = (a * k + b) * k + e; }
+        }
+    if (best == ((d - d0) * k + (h - h0)) * k + (w - w0))
+      out = 0.0f + p.gy[n * p.gs[0] + c * p.gs[1] + od * p.gs[2] + oh * p.gs[3] + ow * p.gs[4]];
+  }
+  p.gx[n * p.xs[0] + c * p.xs[1] + d * p.xs[2] + h * p.xs[3] + w * p.xs[4]] = out;
+}
+
+__global__ void __launch_bounds__(256) pool3d_bwd_kernel(const Pool3dBwdParams p, long total) {
+  for (long i = (long)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (long)gridDim.x * blockDim.x) pool3d_bwd_item(p, i);
+}
+
+static int pool3d_bwd_check(const float* x, const float* grad_y, float* grad_x, int N, int C, int D, int H, int W, int k) {
+  LT_REQUIRE(x && grad_y && grad_x, "maxpool3d_bwd: null pointer");
+  LT_REQUIRE(N > 0 && C > 0 && D > 0 && H > 0 && W > 0, "maxpool3d_bwd: non-positive size");
+  LT_REQUIRE(k >= 1 && k <= D && k <= H && k <= W, "maxpool3d_bwd: window %d must fit in the input (%d, %d, %d)", k, D, H, W);
+  return LT_OK;
+}
+
+
 // ---- batch image ingest ---------------------------------------------------------------------------
 // Host batches arrive as the dataset leaves them: [N][H][W][C] (HWC) uint8 / float32 / float64 (datasets/utils.py:24).
 // The reference transposes to CHW and casts on the CPU (image_batch_to_torch, img.py:96-99) after normalising per image
@@ -396,6 +445,27 @@ extern "C" int lt_maxpool_fwd(const void* in, void* out, int format, int N, int 
   PoolParams p{in, out, format, N, ID, IH, IW, C, kd, kh, kw, sd, sh, sw, pd, ph, pw, OD, OH, OW};
   maxpool_kernel<<<grid_for((long)N * OD * OH * OW * (C / 4)), 256, 0, (cudaStream_t)stream>>>(p);
   LT_CHECK_LAUNCH("maxpool_kernel");
+  return LT_OK;
+}
+
+extern "C" int lt_maxpool3d_bwd(const float* x, const float* grad_y, float* grad_x, int N, int C, int D, int H, int W, long xs_n, long xs_c,
+                                long xs_d, long xs_h, long xs_w, long gs_n, long gs_c, long gs_d, long gs_h, long gs_w, int k, void* stream) {
+  const int rc = pool3d_bwd_check(x, grad_y, grad_x, N, C, D, H, W, k);
+  if (rc != LT_OK) return rc;
+  const Pool3dBwdParams p{x, grad_y, grad_x, N, C, D, H, W, k, {xs_n, xs_c, xs_d, xs_h, xs_w}, {gs_n, gs_c, gs_d, gs_h, gs_w}};
+  const long total = (long)N * C * D * H * W;
+  pool3d_bwd_kernel<<<grid_for(total), 256, 0, (cudaStream_t)stream>>>(p, total);
+  LT_CHECK_LAUNCH("pool3d_bwd_kernel");
+  return LT_OK;
+}
+
+extern "C" int lt_test_maxpool3d_bwd_host(const float* x, const float* grad_y, float* grad_x, int N, int C, int D, int H, int W, long xs_n,
+                                          long xs_c, long xs_d, long xs_h, long xs_w, long gs_n, long gs_c, long gs_d, long gs_h, long gs_w, int k) {
+  const int rc = pool3d_bwd_check(x, grad_y, grad_x, N, C, D, H, W, k);
+  if (rc != LT_OK) return rc;
+  const Pool3dBwdParams p{x, grad_y, grad_x, N, C, D, H, W, k, {xs_n, xs_c, xs_d, xs_h, xs_w}, {gs_n, gs_c, gs_d, gs_h, gs_w}};
+  const long total = (long)N * C * D * H * W;
+  for (long i = 0; i < total; ++i) pool3d_bwd_item(p, i);
   return LT_OK;
 }
 

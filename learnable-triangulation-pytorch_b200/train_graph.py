@@ -143,11 +143,12 @@ class TrainGraphs:
 
 def _model_key(model, inputs):
     """What a graph of `model`'s step depends on besides the values it reads: input shapes / dtypes / devices, the parameters'
-    requires_grad mask, the data_ptr of every parameter and buffer, and the modules' training flags."""
+    requires_grad mask, the data_ptr of every parameter and buffer, the modules' training flags, and whether
+    torch.use_deterministic_algorithms is on (it selects the fixed-order backward kernels)."""
     params = list(model.parameters())
     return (tuple((tuple(t.shape), t.dtype, t.device) for t in inputs), tuple(p.requires_grad for p in params),
             tuple(p.data_ptr() for p in params), tuple(b.data_ptr() for b in model.buffers()),
-            tuple(m.training for m in model.modules()))
+            tuple(m.training for m in model.modules()), torch.are_deterministic_algorithms_enabled())
 
 
 def _capture_on_side_stream(cache, dev, state, warm_up, capture, what, reset=None):

@@ -9,9 +9,11 @@ Parameters live here; inference runs through the native planner in engine.py.
 The torch forward below is the autograd / CPU plumbing path (backend="torch").  Every forward takes the `conv` and `norm` hooks of
 layers.py: `conv` applies each Conv3d / ConvTranspose3d (v2v_backend="native": autograd_ops.v2v_conv), `norm` each BatchNorm3d
 together with the ReLU right after it and, in a Res3DBlock, the residual add (norm_backend="native": autograd_ops.batch_norm).
-None, the default, stands for the torch formulas in layers.py.  Pooling and the decoder's `upsample + skip` adds are always torch.
+None, the default, stands for the torch formulas in layers.py.  Pooling and the decoder's `upsample + skip` adds are always torch, but
+for the max-pool backward under torch.use_deterministic_algorithms (autograd_ops.MaxPool3dFn).
 A ReLU module right after a BatchNorm is applied by `norm`, not called as a module, so a forward hook registered on it does not fire.
 """
+import torch
 import torch.nn.functional as F
 from torch import nn
 
@@ -54,6 +56,9 @@ class Pool3DBlock(nn.Module):
         self.pool_size = pool_size
 
     def forward(self, x):
+        if torch.are_deterministic_algorithms_enabled() and x.is_cuda and torch.is_grad_enabled():
+            from .autograd_ops import MaxPool3dFn       # torch's CUDA max_pool3d backward is not deterministic
+            return MaxPool3dFn.apply(x, self.pool_size)
         return F.max_pool3d(x, self.pool_size, self.pool_size)
 
 
