@@ -17,13 +17,16 @@
 // which the warpgroup does not wait for (the slab is released after the next plane's first products are issued).  Work: the (n, h block, d) output planes in order, cut into one contiguous range per CTA (one
 // CTA per SM), so every SM computes the same number of planes to within one.  3^3 layers with W > 64 run on conv_tc_kernel.
 //
-// conv_fold_kernel (K = 7): tile 8 (w) x 16 (h) x 2 (d) whose 64-row m64 blocks are whole 8-wide W lines at 8 consecutive h of one
-// d plane; both consumer warpgroups on the same tile (two m64 blocks each).  An A stage holds ONE input halo box
-//   {64 channels, 8 + 6 (w), 16 + 6 (h), 2 (d)}   at input offset (-3, -3, kd - 3)
-// that serves every kw and kh of one kd.  TMA zero fill supplies the padding.  Each warp owns 16 rows of an m64 block, i.e. the W
-// lines 2 w' and 2 w' + 1 of the block (w' = warp in the warpgroup): the kw shift is a one-row offset, and along kh the fragments
-// of the second line are the first line of the next tap, so each kh step loads one new line per warp.  The filter streams through
-// its own ring, one slice per (kd, kw) = the 7 kh taps.  Products in (kd, kw, kh) order.
+// conv_fold_kernel (K = 7): tile 8 (w) x 16 (h) x BD = 64 / NC (d) outputs; consumer warpgroup g owns the 8-line h half g in all
+// BD output planes (m64 rows = whole 8-wide W lines at 8 consecutive h).  An A stage holds ONE input plane's halo box
+//   {64 channels, 8 + 6 (w), 16 + 6 (h), 1 (d)}
+// that serves every kw and kh of every output plane that reads it: the BD + 6 input planes of a tile are each loaded once.  TMA
+// zero fill supplies the padding.  Each warp owns 16 rows, i.e. the W lines 2 w' and 2 w' + 1 of its h half (w' = warp in the
+// warpgroup): the kw shift is a one-row offset, and along kh the fragments of the second line are the first line of the next tap,
+// so each kh step loads one new line per warp.  The output planes share these A fragments, so one m64 x 64 wgmma per K slice
+// computes all of them: N = the BD planes' NC columns, B = the taps kd = plane - b of one (kw, kh), one B stage per (plane, kw)
+// read as [kh][kd][NC] from the [kw][kd][kh] packing, zero-filled where kd falls outside the filter.  Every output still sees its
+// products in (kd, kw, kh) order.
 //
 // Weights: lt_conv_fold_pack_weights, rows of [32 hi | 32 lo] fp16, NC = round_up(Cout, 16) rows per tap: 3^3 as
 // [kd][kh][kw][NC] (a (kd, kh) slice is the 3 NC-row B operand of the kw-wide products), 7^3 as [kw][kd][kh][NC] (a (kd, kw) slice
@@ -403,22 +406,22 @@ static int conv_lines_run(const lt_conv_desc* d, const void* in, const void* wei
 template <int K, int NC>
 struct FoldCfg {
   static_assert(K == 7, "the 3^3 layers run on conv_lines_kernel");
-  static constexpr int BW = 8, BH = 16, BD = 2;
-  static constexpr int WBOX = BW + K - 1, HBOX = BH + K - 1, DBOX = BD;
-  static constexpr int A_BYTES = WBOX * HBOX * DBOX * 128;
-  static constexpr int ASTAGES = K;                    // A boxes per tile: one per kd
+  static constexpr int BW = 8, BH = 16;
+  static constexpr int BD = 64 / NC;                   // output planes per tile: N = BD NC = 64 per wgmma
+  static constexpr int WBOX = BW + K - 1, HBOX = BH + K - 1;
+  static constexpr int A_BYTES = WBOX * HBOX * 128;    // one input plane's halo box
+  static constexpr int A_STAGE = (A_BYTES + 1023) / 1024 * 1024;
   static constexpr int TAP = NC * 128;                 // one packed weight tap
-  static constexpr int B_SLICE = K * TAP;              // one (kd, kw) slice: the K kh taps
-  static constexpr int MB = 2;                         // m64 blocks per consumer warpgroup
+  static constexpr int B_KH = BD * TAP;                // one kh of a B stage: the taps of BD consecutive kd, the wide B operand
+  static constexpr int B_STAGE = K * B_KH;             // one (plane, kw) step: [kh][kd][NC]
   static constexpr int AVAIL = kFoldSmem - 1024 - 256;
   static constexpr int ARING = 2;
-  static constexpr int BRING_FIT = (AVAIL - ARING * A_BYTES) / B_SLICE;
-  static constexpr int BRING = BRING_FIT > 4 ? 4 : BRING_FIT;
-  static constexpr int A_OFF = BRING * B_SLICE;
-  static constexpr int BAR_OFF = A_OFF + ARING * A_BYTES;
+  static constexpr int BRING = (AVAIL - ARING * A_STAGE) / B_STAGE;
+  static constexpr int A_OFF = BRING * B_STAGE;
+  static constexpr int BAR_OFF = A_OFF + ARING * A_STAGE;
   static constexpr size_t SMEM = (size_t)BAR_OFF + 256 + 1024;
-  static_assert(BW * BH * BD == 256 && BH % 8 == 0, "two m64 blocks of whole 8-wide lines per warpgroup");
-  static_assert(A_BYTES % 1024 == 0 && B_SLICE % 1024 == 0, "boxes must start on 1024-byte swizzle atoms");
+  static_assert(BD * NC == 64 && BH == 16, "one 8-line h half of BD planes per consumer warpgroup, N <= 64 per wgmma");
+  static_assert(B_KH % 1024 == 0, "B operands must start on 1024-byte swizzle atoms");
   static_assert(BRING >= 2 && 2 * (ARING + BRING) * 8 <= 256 && SMEM <= (size_t)kFoldSmem, "shared memory");
 };
 
@@ -453,6 +456,39 @@ __device__ __forceinline__ void fold_tap(float (&d1)[NC / 2], float (&d2)[NC / 2
   wgmma_f16_rs<NC>(d2, a[1], bd + 6, 1u);
   wgmma_f16_rs<NC>(d2, a[2], bd, 1u);         // lo * hi
   wgmma_f16_rs<NC>(d2, a[3], bd + 2, 1u);
+}
+
+// The products of one input plane for every output block of the tile, kw by kw.  The blocks share their A fragments, so one
+// m64 x (BD NC) wgmma per K slice serves all of them: its B operand is the taps kd = pl - BD + 1 .. pl of one (kw, kh), adjacent
+// in the B stage (zero where kd is outside 0 .. K - 1, so a block only ever adds its own taps), and its accumulator columns are
+// the blocks' accumulators, stored in descending block order (slot BD - 1 - b) so that kd ascends with the column.  Each kh step
+// loads one new W line per warp.  The B stage of the previous (plane, kw) step is released once its MMAs have completed.
+template <int K, int NC>
+__device__ __forceinline__ void fold_plane(float (&d1)[FoldCfg<K, NC>::BD * NC / 2], float (&d2)[FoldCfg<K, NC>::BD * NC / 2],
+                                           uint32_t box, uint32_t row0, uint32_t mlane, uint32_t bsm0, uint64_t* bfull, uint64_t* bempty,
+                                           int& nbs, int& held, bool wg_lead) {
+  using C = FoldCfg<K, NC>;
+#pragma unroll 1
+  for (int kw = 0; kw < K; ++kw, ++nbs) {
+    const int sb = nbs % C::BRING;
+    mbar_wait(&bfull[sb], (uint32_t)(nbs / C::BRING) & 1u);
+    const uint32_t bstage = bsm0 + (uint32_t)(sb * C::B_STAGE);
+    uint32_t ln[K + 1][2][4];
+    fold_load_line(ln[0], box, row0 + kw, mlane);
+#pragma unroll
+    for (int kh = 0; kh < K; ++kh) {
+      fold_load_line(ln[kh + 1], box, row0 + kw + (uint32_t)((kh + 1) * C::WBOX), mlane);
+      wg_fence();
+      fold_tap<C::BD * NC>(d1, d2, ln[kh], ln[kh + 1], make_sw128_desc(bstage + (uint32_t)(kh * C::B_KH)), 1u);
+      wg_commit();
+      wg_wait<1>();
+      if (kh == 0 && held >= 0) {   // every MMA of the previous step has completed
+        if (wg_lead) mbar_arrive_local(&bempty[held % C::BRING]);
+        held = -1;
+      }
+    }
+    held = nbs;
+  }
 }
 
 template <int K, int NC>
@@ -490,19 +526,20 @@ __global__ void __launch_bounds__(kFoldThreads, 1) conv_fold_kernel(const __grid
       for (int t = blockIdx.x; t < ntiles; t += gridDim.x) {
         int ow0, oh0, od0, nb;
         fold_tile_origin(p, t, ow0, oh0, od0, nb);
-        for (int as = 0; as < C::ASTAGES; ++as) {
+        const int nvb = p.OD - od0 < C::BD ? p.OD - od0 : C::BD;
+        for (int pl = 0; pl < nvb + K - 1; ++pl) {
           mbar_wait(&aempty[sa], pa ^ 1u);
           if (elect_one()) {
             mbar_expect_tx(&afull[sa], (uint32_t)C::A_BYTES);
-            tma_load_5d(asm_ + (size_t)sa * C::A_BYTES, &tmA, &afull[sa], 0, ow0 - K / 2, oh0 - K / 2, od0 + as - K / 2, nb);
+            tma_load_5d(asm_ + (size_t)sa * C::A_STAGE, &tmA, &afull[sa], 0, ow0 - K / 2, oh0 - K / 2, od0 + pl - K / 2, nb);
           }
           __syncwarp();
           if (++sa == C::ARING) { sa = 0; pa ^= 1u; }
-          for (int kw = 0; kw < K; ++kw) {
+          for (int kw = 0; kw < K; ++kw) {   // taps kd = pl - BD + 1 .. pl of (kw, every kh); zero fill outside 0 .. K - 1
             mbar_wait(&bempty[sb], pb ^ 1u);
             if (elect_one()) {
-              mbar_expect_tx(&bfull[sb], (uint32_t)C::B_SLICE);
-              tma_load_3d(bsm + (size_t)sb * C::B_SLICE, &tmB, &bfull[sb], 0, 0, (kw * K + as) * K);
+              mbar_expect_tx(&bfull[sb], (uint32_t)C::B_STAGE);
+              tma_load_5d(bsm + (size_t)sb * C::B_STAGE, &tmB, &bfull[sb], 0, 0, pl - C::BD + 1, 0, kw);
             }
             __syncwarp();
             if (++sb == C::BRING) { sb = 0; pb ^= 1u; }
@@ -514,85 +551,54 @@ __global__ void __launch_bounds__(kFoldThreads, 1) conv_fold_kernel(const __grid
   }
 
   // ================= MMA + epilogue (warpgroups 1, 2) =================
+  // warpgroup g owns the 8-line h half g of the tile in all BD output planes (m64 block b = output plane od0 + b); each input
+  // plane's box and weight slices are shared by both warpgroups
   regs_claim_consumer();
   const int g = wg - 1, warp = (threadIdx.x >> 5) & 3;
-  float d1[C::MB][NC / 2], d2[C::MB][NC / 2];
-#pragma unroll
-  for (int b = 0; b < C::MB; ++b)
-#pragma unroll
-    for (int i = 0; i < NC / 2; ++i) { d1[b][i] = 0.f; d2[b][i] = 0.f; }
-  // m64 block b of this warpgroup: d plane dd and 8-line h block hb of the tile; this lane's box row for kw = kh = 0
-  int blk_dd[C::MB], blk_hb[C::MB];
-  uint32_t row0[C::MB];
-#pragma unroll
-  for (int b = 0; b < C::MB; ++b) {
-    const int blk = C::MB * g + b;
-    blk_dd[b] = blk / (C::BH / 8);
-    blk_hb[b] = blk % (C::BH / 8);
-    row0[b] = (uint32_t)((blk_dd[b] * C::HBOX + blk_hb[b] * 8 + 2 * warp) * C::WBOX + (lane & 7));
-  }
+  float d1[C::BD * NC / 2], d2[C::BD * NC / 2];   // output block b: the NC / 2 registers of slot BD - 1 - b
+  const uint32_t row0 = (uint32_t)((g * 8 + 2 * warp) * C::WBOX + (lane & 7));   // this lane's box row for kw = kh = 0
   const uint32_t mlane = (uint32_t)(lane >> 3);
   const int r_lo = warp * 16 + (lane >> 2);   // this thread's accumulator rows r_lo, r_lo + 8 of an m64 block
   const int c2 = 2 * (lane & 3);
   const uint32_t bsm0 = smem_u32(bsm), asm0 = smem_u32(asm_);
   const bool wg_lead = (threadIdx.x & 127) == 0;
-  int bprev = -1;
+  int na = 0, nbs = 0;   // input planes and B stages of this CTA so far (the producer's order)
+  int held = -1;         // the B stage of the previous (plane, kw) step until its MMAs have completed
   for (int kt = 0;; ++kt) {
     const int t = blockIdx.x + kt * gridDim.x;
     if (t >= ntiles) break;
+    int ow0, oh0, od0, nb;
+    fold_tile_origin(p, t, ow0, oh0, od0, nb);
+    const int nvb = p.OD - od0 < C::BD ? p.OD - od0 : C::BD;
+#pragma unroll
+    for (int i = 0; i < C::BD * NC / 2; ++i) { d1[i] = 0.f; d2[i] = 0.f; }   // the blocks of a tile start at different planes
 #pragma unroll 1
-    for (int as = 0; as < C::ASTAGES; ++as) {
-      const int na = kt * C::ASTAGES + as;
+    for (int pl = 0; pl < nvb + K - 1; ++pl, ++na) {
       const int sa = na % C::ARING;
       mbar_wait(&afull[sa], (uint32_t)(na / C::ARING) & 1u);
-      const uint32_t box = asm0 + (uint32_t)(sa * C::A_BYTES);
-#pragma unroll 1
-      for (int kw = 0; kw < K; ++kw) {
-        const int nbs = na * K + kw;
-        const int sb = nbs % C::BRING;
-        mbar_wait(&bfull[sb], (uint32_t)(nbs / C::BRING) & 1u);
-        const uint32_t bslice = bsm0 + (uint32_t)(sb * C::B_SLICE);
-        uint32_t ln[K + 1][C::MB][2][4];
-#pragma unroll
-        for (int b = 0; b < C::MB; ++b) fold_load_line(ln[0][b], box, row0[b] + kw, mlane);
-#pragma unroll
-        for (int kh = 0; kh < K; ++kh) {
-#pragma unroll
-          for (int b = 0; b < C::MB; ++b) fold_load_line(ln[kh + 1][b], box, row0[b] + kw + (uint32_t)((kh + 1) * C::WBOX), mlane);
-          wg_fence();
-          const uint64_t bd = make_sw128_desc(bslice + (uint32_t)(kh * C::TAP));
-          const uint32_t acc = (as == 0 && kw == 0 && kh == 0) ? 0u : 1u;
-#pragma unroll
-          for (int b = 0; b < C::MB; ++b) fold_tap<NC>(d1[b], d2[b], ln[kh][b], ln[kh + 1][b], bd, acc);
-          wg_commit();
-          wg_wait<1>();
-          if (kh == 0 && bprev >= 0) {   // every MMA of the previous weight slice has completed
-            if (wg_lead) mbar_arrive_local(&bempty[bprev]);
-            bprev = -1;
-          }
-        }
-        bprev = sb;
-      }
+      const uint32_t box = asm0 + (uint32_t)(sa * C::A_STAGE);
+      fold_plane<K, NC>(d1, d2, box, row0, mlane, bsm0, bfull, bempty, nbs, held, wg_lead);
       mbar_arrive_local(&aempty[sa]);   // this thread's ldmatrix reads of the box have completed
     }
     wg_wait<0>();
-    if (wg_lead) mbar_arrive_local(&bempty[bprev]);
-    bprev = -1;
-#pragma unroll
-    for (int b = 0; b < C::MB; ++b) { wg_fence_regs(d1[b]); wg_fence_regs(d2[b]); }
+    if (wg_lead) mbar_arrive_local(&bempty[held % C::BRING]);
+    held = -1;
+    wg_fence_regs(d1);
+    wg_fence_regs(d2);
 
     // ---- epilogue ----
-    int ow0, oh0, od0, nb;
-    fold_tile_origin(p, t, ow0, oh0, od0, nb);
 #pragma unroll
-    for (int b = 0; b < C::MB; ++b) {
+    for (int b = 0; b < C::BD; ++b) {
+      if (b >= nvb) continue;
 #pragma unroll
       for (int h = 0; h < 2; ++h) {
         const int r = r_lo + 8 * h;
-        const int ow = ow0 + (r & 7), oh = oh0 + blk_hb[b] * 8 + (r >> 3), od = od0 + blk_dd[b];
-        if (!(ow < p.OW && oh < p.OH && od < p.OD)) continue;
+        const int ow = ow0 + (r & 7), oh = oh0 + g * 8 + (r >> 3), od = od0 + b;
+        if (!(ow < p.OW && oh < p.OH)) continue;
         const long opix = (((long)nb * p.FD + od) * p.FH + oh) * p.FW + ow;
-        conv_epilogue_row<NC>(p, d1[b], d2[b], h, opix, 0, c2);
+        const int slot = (C::BD - 1 - b) * (NC / 2);
+        conv_epilogue_row<NC>(p, *reinterpret_cast<const float(*)[NC / 2]>(&d1[slot]), *reinterpret_cast<const float(*)[NC / 2]>(&d2[slot]),
+                              h, opix, 0, c2);
         if constexpr (NC == 16) {   // output channels 16..31: no weights
           const float z[8] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
           conv_epilogue_row<16>(p, z, z, h, opix, 16, c2);
@@ -613,12 +619,13 @@ static int conv_fold_run(const lt_conv_desc* d, const void* in, const void* weig
   p.tw = ceil_div(d->OW, p.bw); p.th = ceil_div(d->OH, p.bh); p.td = ceil_div(d->OD, p.bd); p.tn = d->N;
   p.stages = C::ARING;
   CUtensorMap tmA, tmB;
-  int rc = make_in_map(&tmA, d, C::WBOX, C::HBOX, C::DBOX, 1, in);
+  int rc = make_in_map(&tmA, d, C::WBOX, C::HBOX, 1, 1, in);
   if (rc) return rc;
-  const uint64_t dims[3] = {64, (uint64_t)NC, (uint64_t)K * K * K};
-  const uint64_t str[2] = {128, (uint64_t)NC * 128};
-  const uint32_t bx[3] = {64, (uint32_t)NC, (uint32_t)K};
-  rc = make_map(&tmB, weight, 3, dims, str, bx, nullptr, 1);
+  // packed [kw][kd][kh][NC] taps read as [kh][kd][NC] per kw: the BD kd of one kh are the N rows of one wide B operand
+  const uint64_t dims[5] = {64, (uint64_t)NC, (uint64_t)K, (uint64_t)K, (uint64_t)K};
+  const uint64_t str[4] = {128, (uint64_t)C::TAP * K, (uint64_t)C::TAP, (uint64_t)C::TAP * K * K};
+  const uint32_t bx[5] = {64, (uint32_t)NC, (uint32_t)C::BD, (uint32_t)K, 1};
+  rc = make_map(&tmB, weight, 5, dims, str, bx, nullptr, 1);
   if (rc) return rc;
   static DeviceOnce configured;
   if (configured.first()) {
