@@ -395,6 +395,25 @@ int lt_gap_mlp3_fwd(const void* in, int format, int N, int P, int C0, int H1, in
                     void* stream);
 /* conf[B][V][C] <- conf / sum_v conf + eps   (triangulation.py:173-174 with eps = 1e-5; :268-269 with eps = 0) */
 int lt_view_normalize_fwd(float* conf, int B, int V, int C, float eps, void* stream);
+/* Training tail of ConfidenceHead (head_backend="native"): x is the second head BatchNorm's output (N, C0, H, W), float32, element
+ * strides xs_* of (n, c, h, w) (NCHW and channels_last alike).  Per row n: 2x2 stride-2 max pool in floor mode (torch's rule: greater
+ * or NaN replaces), ReLU keeping NaN, mean over the P = (H/2)(W/2) pooled positions -> x0 (N, C0); Linear(C0,H1)+ReLU -> h1 (N, H1),
+ * Linear(H1,H2)+ReLU -> h2 (N, H2), Linear(H2,NO)+Sigmoid -> out (N, NO), the hidden ReLUs keeping NaN.  Fails for P = 0. */
+int lt_conf_head_tail_fwd(const float* x, int N, int C0, int H, int W, long xs_n, long xs_c, long xs_h, long xs_w, int H1, int H2, int NO,
+                          const float* w1, const float* b1, const float* w2, const float* b2, const float* w3, const float* b3, float* out,
+                          float* x0, float* h1, float* h2, void* stream);
+size_t lt_conf_head_tail_bwd_workspace_bytes(int N, int C0, int H1, int H2, int NO);
+/* Backward of lt_conf_head_tail_fwd from grad_y = dL/d(out) and the saved x, x0, h1, h2, out (= y): autograd's derivative of the torch
+ * formula (sigmoid backward g y (1 - y); ReLU masks !(h <= 0), so a NaN passes its gradient).  dW1..3, db1..3 (nn.Linear layouts)
+ * are sums over the N rows in order; grad_x (element strides gs_*) is written in one pass, dx0 / P at each window's arg-max when
+ * !(pooled <= 0), 0 elsewhere and in the tail floor mode drops.  No atomics; the caller passes the workspace. */
+int lt_conf_head_tail_bwd(const float* x, int N, int C0, int H, int W, long xs_n, long xs_c, long xs_h, long xs_w, long gs_n, long gs_c,
+                          long gs_h, long gs_w, int H1, int H2, int NO, const float* w1, const float* w2, const float* w3, const float* x0,
+                          const float* h1, const float* h2, const float* y, const float* grad_y, float* grad_x, float* dw1, float* db1,
+                          float* dw2, float* db2, float* dw3, float* db3, void* workspace, size_t workspace_bytes, void* stream);
+/* Backward of y_v = c_v / S + eps, S = sum_u c_u over the views: grad_conf[b][v][c] = g_v / S - (sum_u g_u c_u) / S^2, from the
+ * un-normalised conf [B][V][C]; float64 sums over the views in order. */
+int lt_view_normalize_bwd(const float* conf, const float* grad, float* grad_conf, int B, int V, int C, void* stream);
 /* confidence-weighted DLT (multiview.py:141-183): proj [B][V][3][4], keypoints_2d [B][V][J][2], confidences [B][V][J] or
  * NULL -> out [B][J][3]; float64 A^T A + Jacobi eigen-solve per (sample, joint). */
 int lt_triangulate_dlt_fwd(const float* proj, const float* keypoints_2d, const float* confidences, float* out, int B,
@@ -574,6 +593,12 @@ int lt_test_unproject_aggregate_bwd_geom_host(const float* features, const float
                                               const float* grad_out, float* grad_features, float* grad_conf, float* grad_proj,
                                               float* grad_coord, int B, int V, int C, int h, int w, long nvox, int agg);
 int lt_test_softargmax3d_coord_bwd_host(const float* probs, const float* grad_keypoints, float* grad_coord, int B, int J, long nvox);
+/* lt_conf_head_tail_fwd (+ lt_conf_head_tail_bwd when grad_y is not NULL) on host pointers, with the kernels' per-item code. */
+int lt_test_conf_head_tail_host(const float* x, int N, int C0, int H, int W, long xs_n, long xs_c, long xs_h, long xs_w, long gs_n,
+                                long gs_c, long gs_h, long gs_w, int H1, int H2, int NO, const float* w1, const float* b1, const float* w2,
+                                const float* b2, const float* w3, const float* b3, float* out, float* x0, float* h1, float* h2,
+                                const float* grad_y, float* grad_x, float* dw1, float* db1, float* dw2, float* db2, float* dw3, float* db3);
+int lt_test_view_normalize_bwd_host(const float* conf, const float* grad, float* grad_conf, int B, int V, int C);
 int lt_test_triangulate_dlt_proj_bwd_host(const float* proj, const float* keypoints_2d, const float* confidences, const float* grad_out,
                                           float* grad_proj, int B, int V, int J);
 /* lt_volumetric_ce_fwd (+ lt_volumetric_ce_bwd when grad_probs is not NULL, grad_loss then a HOST pointer) on host pointers, with

@@ -820,3 +820,80 @@ def batch_norm(module, x, relu=False, residual=None):
         module.num_batches_tracked.add_(1)
     return BatchNormActFn.apply(x, module.weight, module.bias, residual, module.running_mean, module.running_var, module.eps,
                                 module.momentum, module.training, relu)
+
+
+# ---- The confidence heads' tail for training (head_backend="native"): csrc/algebraic.cu's lt_conf_head_tail_fwd / _bwd and
+# lt_view_normalize_fwd / _bwd.  No cuBLAS: the head's Linear layers and their gradients are fixed-order kernels of the project.
+
+class ConfHeadTailFn(torch.autograd.Function):
+    """MaxPool2d(2) -> ReLU -> mean over the pooled positions -> Linear + ReLU -> Linear + ReLU -> Linear + Sigmoid of a (N, C0, H, W)
+    float32 map of any element strides (NCHW or channels_last, read in place): lt_conf_head_tail_fwd, which keeps the mean x0 and the
+    hidden activations h1, h2 for lt_conf_head_tail_bwd.  Gradients reach the map and the six Linear parameters."""
+
+    @staticmethod
+    def forward(ctx, x, w1, b1, w2, b2, w3, b3):
+        N, dev = x.shape[0], x.device
+        lins = tuple((w.detach().float().contiguous(), b.detach().float().contiguous()) for w, b in ((w1, b1), (w2, b2), (w3, b3)))
+        out, x0, h1, h2 = (torch.empty((N, k), dtype=torch.float32, device=dev)
+                           for k in (lins[2][0].shape[0], x.shape[1], lins[0][0].shape[0], lins[1][0].shape[0]))
+        capi.conf_head_tail(x.detach(), *lins, out, x0, h1, h2)
+        ctx.save_for_backward(x, lins[0][0], lins[1][0], lins[2][0], x0, h1, h2, out)
+        return out
+
+    @staticmethod
+    def backward(ctx, grad_out):
+        x, w1, w2, w3, x0, h1, h2, y = ctx.saved_tensors
+        N, C0 = x0.shape
+        dev = x.device
+        grad_x = torch.empty_like(x)
+        grads = tuple(torch.empty(shape, dtype=torch.float32, device=dev)
+                      for shape in (w1.shape, w1.shape[:1], w2.shape, w2.shape[:1], w3.shape, w3.shape[:1]))
+        ws = torch.empty(capi.conf_head_tail_bwd_workspace_bytes(N, C0, w1.shape[0], w2.shape[0], w3.shape[0]), dtype=torch.uint8,
+                         device=dev)
+        capi.conf_head_tail_bwd(x.detach(), w1, w2, w3, x0, h1, h2, y, grad_out.float().contiguous(), grad_x, grads, ws)
+        return (grad_x,) + grads
+
+
+def conf_head_tail(head, x):
+    """The `tail` hook of pose_resnet.ConfidenceHead: its second max pool, ReLU, global mean and `head` MLP applied to the second
+    BatchNorm's output x through ConfHeadTailFn.  ValueError for a map the kernels do not take; RuntimeError for CPU tensors."""
+    lin = [m for m in head.head if isinstance(m, torch.nn.Linear)]
+    if x.dim() != 4 or x.shape[1] != lin[0].in_features:
+        raise ValueError("native confidence head: expected a (N, %d, H, W) map, got %s" % (lin[0].in_features, tuple(x.shape)))
+    if x.shape[2] < 2 or x.shape[3] < 2:
+        raise ValueError("native confidence head: a %dx%d map is too small for the 2x2 max pool" % tuple(x.shape[2:]))
+    if x.dtype != torch.float32:
+        raise TypeError("native confidence head: float32 maps only (got %s)" % x.dtype)
+    if not x.is_cuda:
+        raise RuntimeError("lt_b200 native confidence head needs CUDA tensors (got %s)" % x.device)
+    return ConfHeadTailFn.apply(x, lin[0].weight, lin[0].bias, lin[1].weight, lin[1].bias, lin[2].weight, lin[2].bias)
+
+
+class ViewNormalizeFn(torch.autograd.Function):
+    """conf / conf.sum(dim=1, keepdim=True) + eps for (B, V, C) float32 confidences: lt_view_normalize_fwd on a copy (the backward
+    reads the un-normalised values), lt_view_normalize_bwd."""
+
+    @staticmethod
+    def forward(ctx, conf, eps):
+        c = conf.detach().float().contiguous()
+        out = c.clone()
+        B, V, C = c.shape
+        capi.view_normalize(out, B, V, C, eps)
+        ctx.save_for_backward(c)
+        return out
+
+    @staticmethod
+    def backward(ctx, grad_out):
+        c, = ctx.saved_tensors
+        grad = torch.empty_like(c)
+        capi.view_normalize_bwd(c, grad_out.float().contiguous(), grad)
+        return grad, None
+
+
+def view_normalize(conf, eps):
+    """(B, V, C) confidences normalised over the views (dim 1), plus eps, on the native kernels."""
+    if conf.dim() != 3:
+        raise ValueError("view_normalize: expected (B, V, C) confidences, got %s" % (tuple(conf.shape),))
+    if not conf.is_cuda:
+        raise RuntimeError("lt_b200 native view normalisation needs CUDA tensors (got %s)" % conf.device)
+    return ViewNormalizeFn.apply(conf, eps)

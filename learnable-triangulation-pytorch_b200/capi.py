@@ -117,6 +117,12 @@ SIGNATURES = {
     "lt_maxpool_fwd": (c_int, [c_void_p, c_void_p] + [c_int] * 18 + [c_void_p]),
     "lt_gap_mlp3_fwd": (c_int, [c_void_p] + [c_int] * 7 + [c_void_p] * 7 + [c_void_p]),
     "lt_view_normalize_fwd": (c_int, [c_void_p, c_int, c_int, c_int, c_float, c_void_p]),
+    "lt_conf_head_tail_fwd": (c_int, [c_void_p] + [c_int] * 4 + [c_long] * 4 + [c_int] * 3 + [c_void_p] * 10 + [c_void_p]),
+    "lt_conf_head_tail_bwd_workspace_bytes": (c_size_t, [c_int] * 5),
+    "lt_conf_head_tail_bwd": (c_int, [c_void_p] + [c_int] * 4 + [c_long] * 8 + [c_int] * 3 + [c_void_p] * 16 + [c_size_t, c_void_p]),
+    "lt_test_conf_head_tail_host": (c_int, [c_void_p] + [c_int] * 4 + [c_long] * 8 + [c_int] * 3 + [c_void_p] * 18),
+    "lt_view_normalize_bwd": (c_int, [c_void_p] * 3 + [c_int] * 3 + [c_void_p]),
+    "lt_test_view_normalize_bwd_host": (c_int, [c_void_p] * 3 + [c_int] * 3),
     "lt_triangulate_dlt_fwd": (c_int, [c_void_p] * 4 + [c_int] * 3 + [c_void_p]),
     "lt_triangulate_dlt_bwd": (c_int, [c_void_p] * 6 + [c_int] * 3 + [c_void_p]),
     "lt_test_triangulate_dlt_fwd_host": (c_int, [c_void_p] * 4 + [c_int] * 3),
@@ -440,6 +446,42 @@ def view_normalize(conf, B, V, C, eps):
     _check(lib().lt_view_normalize_fwd(_ptr(conf), B, V, C, float(eps), _stream()), "lt_view_normalize_fwd")
 
 
+def _map_dims(x):
+    """(N, C, H, W) and element strides of a float32 map of any strides (lt_conf_head_tail_*)."""
+    assert x.dim() == 4 and x.dtype == torch.float32, "the confidence-head tail takes a float32 (N, C, H, W) map"
+    return tuple(x.shape), tuple(x.stride())
+
+
+def conf_head_tail(x, lin1, lin2, lin3, out, x0, h1, h2):
+    """lt_conf_head_tail_fwd: x (N, C0, H, W) float32 CUDA of any element strides, lin* = (weight, bias) of the three nn.Linear layers
+    -> out (N, NO), x0 (N, C0), h1 (N, H1), h2 (N, H2) written."""
+    (N, C0, H, W), xs = _map_dims(x)
+    assert x.is_cuda
+    _check(lib().lt_conf_head_tail_fwd(x.data_ptr(), N, C0, H, W, *xs, lin1[0].shape[0], lin2[0].shape[0], lin3[0].shape[0],
+                                       _ptr(lin1[0]), _ptr(lin1[1]), _ptr(lin2[0]), _ptr(lin2[1]), _ptr(lin3[0]), _ptr(lin3[1]), _ptr(out),
+                                       _ptr(x0), _ptr(h1), _ptr(h2), _stream()), "lt_conf_head_tail_fwd")
+
+
+def conf_head_tail_bwd_workspace_bytes(N, C0, H1, H2, NO):
+    return lib().lt_conf_head_tail_bwd_workspace_bytes(N, C0, H1, H2, NO)
+
+
+def conf_head_tail_bwd(x, w1, w2, w3, x0, h1, h2, y, grad_y, grad_x, grads, workspace):
+    """lt_conf_head_tail_bwd: grad_x (any element strides, the shape of x) and grads = (dW1, db1, dW2, db2, dW3, db3) written."""
+    (N, C0, H, W), xs = _map_dims(x)
+    assert x.is_cuda and tuple(grad_x.shape) == (N, C0, H, W)
+    _check(lib().lt_conf_head_tail_bwd(x.data_ptr(), N, C0, H, W, *xs, *grad_x.stride(), w1.shape[0], w2.shape[0], w3.shape[0], _ptr(w1),
+                                       _ptr(w2), _ptr(w3), _ptr(x0), _ptr(h1), _ptr(h2), _ptr(y), _ptr(grad_y), grad_x.data_ptr(),
+                                       *[_ptr(t) for t in grads], _ptr(workspace), workspace.numel() * workspace.element_size(), _stream()),
+           "lt_conf_head_tail_bwd")
+
+
+def view_normalize_bwd(conf, grad, grad_conf):
+    """lt_view_normalize_bwd: conf, grad, grad_conf (B, V, C) float32 contiguous."""
+    B, V, C = conf.shape
+    _check(lib().lt_view_normalize_bwd(_ptr(conf), _ptr(grad), _ptr(grad_conf), B, V, C, _stream()), "lt_view_normalize_bwd")
+
+
 def triangulate_dlt(proj, kp2d, conf, out):
     B, V, J = kp2d.shape[:3]
     _check(lib().lt_triangulate_dlt_fwd(_ptr(proj), _ptr(kp2d), _ptr(conf), _ptr(out), B, V, J, _stream()), "lt_triangulate_dlt_fwd")
@@ -722,3 +764,29 @@ def cl_to_cf(inp, out, N, P, Cs, C):
 
 def tc_gemm_selftest(a_fp16, b_fp16, d, M, N, K, variant=0):
     _check(lib().lt_tc_gemm_selftest(_ptr(a_fp16), _ptr(b_fp16), _ptr(d), M, N, K, variant, _stream()), "lt_tc_gemm_selftest")
+
+
+def conf_head_tail_host(x, lin1, lin2, lin3, grad_y=None):
+    """lt_test_conf_head_tail_host: the confidence-head tail kernels' per-item code on CPU float32 tensors (test hook, no GPU needed).
+    x (N, C0, H, W) of any element strides.  -> (out, x0, h1, h2), and with grad_y (N, NO) also (grad_x with the strides of
+    torch.empty_like(x), (dW1, db1, dW2, db2, dW3, db3))."""
+    (N, C0, H, W), xs = _map_dims(x)
+    assert not x.is_cuda
+    H1, H2, NO = lin1[0].shape[0], lin2[0].shape[0], lin3[0].shape[0]
+    out, x0, h1, h2 = (torch.empty(N, k) for k in (NO, C0, H1, H2))
+    gx = torch.empty_like(x) if grad_y is not None else None
+    grads = tuple(torch.empty(t.shape) for lin in (lin1, lin2, lin3) for t in lin) if grad_y is not None else (None,) * 6
+    _check(lib().lt_test_conf_head_tail_host(x.data_ptr(), N, C0, H, W, *xs, *(gx.stride() if gx is not None else (0,) * 4), H1, H2, NO,
+                                             *[_host_ptr(t) for lin in (lin1, lin2, lin3) for t in lin], _host_ptr(out), _host_ptr(x0),
+                                             _host_ptr(h1), _host_ptr(h2), _host_ptr(grad_y), None if gx is None else gx.data_ptr(),
+                                             *[_host_ptr(t) for t in grads]), "lt_test_conf_head_tail_host")
+    return (out, x0, h1, h2) if grad_y is None else (out, x0, h1, h2, gx, grads)
+
+
+def view_normalize_bwd_host(conf, grad):
+    """lt_test_view_normalize_bwd_host: the view-normalisation backward's per-item code on CPU (B, V, C) float32 tensors."""
+    B, V, C = conf.shape
+    out = torch.empty_like(conf)
+    _check(lib().lt_test_view_normalize_bwd_host(_host_ptr(conf), _host_ptr(grad), _host_ptr(out), B, V, C),
+           "lt_test_view_normalize_bwd_host")
+    return out

@@ -1,6 +1,8 @@
 // Small kernels of the algebraic-triangulation path and the confidence heads (SURVEY section 8f rows 2 and 4):
 //   - global-average-pool + 3-layer MLP + sigmoid tail of GlobalAveragePoolingHead (pose_resnet.py:163-174)
-//   - normalisation of per-view confidences (triangulation.py:173-174, :268-269)
+//   - the same tail for training (head_backend="native"): the second 2x2 max pool, ReLU, mean and MLP forward, saving what the
+//     backward reads, and its backward (weight, bias and input-map gradients), every sum in a fixed order without atomics
+//   - normalisation of per-view confidences (triangulation.py:173-174, :268-269) and its backward
 //   - confidence-weighted DLT triangulation (multiview.py:141-183) and its backward, one thread per (sample, joint); the
 //     projection-matrix gradient as per-(sample, joint) partials summed over the joints in a fixed order
 #include "common.cuh"
@@ -10,8 +12,40 @@
 
 namespace lt {
 
-// One CTA per image: mean over P positions of C0 channels, then Linear(C0,H1)+ReLU, Linear(H1,H2)+ReLU,
-// Linear(H2,NO)+Sigmoid.  Weights are row-major [out][in] float32 (nn.Linear layout).  Dynamic smem: C0+H1+H2 floats.
+// ---- the confidence heads' MLP tail: Linear(C0,H1)+ReLU, Linear(H1,H2)+ReLU, Linear(H2,NO)+Sigmoid on one row --------------------
+// Weights are row-major [out][in] float32 (nn.Linear layout).  Every output is b[o] followed by one fmaf per input in input order, so
+// the inference tail (gap_mlp3_kernel), the training tail (conf_head_fwd_kernel) and the host test hook compute the same floats.
+__host__ __device__ __forceinline__ float linear_item(const float* __restrict__ w, const float* __restrict__ b, const float* x, int in,
+                                                      int o) {
+  float acc = b[o];
+  for (int i = 0; i < in; ++i) acc = fmaf(w[(long)o * in + i], x[i], acc);
+  return acc;
+}
+
+__host__ __device__ __forceinline__ float sigmoid_f(float v) { return 1.0f / (1.0f + expf(-v)); }
+// dL/dv of y = sigmoid(v) from y and g = dL/dy, as autograd's sigmoid backward: g y (1 - y)
+__host__ __device__ __forceinline__ float sigmoid_bwd(float g, float y) { return g * y * (1.0f - y); }
+
+// The ReLU of the hidden layers.  kTorchRelu: torch's rule (a NaN stays NaN), which training follows so that its forward and the
+// backward's masks are autograd's; otherwise fmaxf, which maps NaN to 0, as the inference tail always has.
+template <bool kTorchRelu>
+__host__ __device__ __forceinline__ float hidden_relu(float v) { return kTorchRelu ? (v <= 0.0f ? 0.0f : v) : fmaxf(v, 0.0f); }
+
+// The three layers of row x0 (C0 floats) by the CTA: x1 (H1) and x2 (H2) are the post-ReLU activations, in shared memory, complete on
+// return; out (NO) is the sigmoid.  x0 must be complete (after a barrier) on entry.
+template <bool kTorchRelu>
+__device__ __forceinline__ void mlp3_row(const float* x0, float* x1, float* x2, int C0, int H1, int H2, int NO,
+                                         const float* __restrict__ w1, const float* __restrict__ b1, const float* __restrict__ w2,
+                                         const float* __restrict__ b2, const float* __restrict__ w3, const float* __restrict__ b3,
+                                         float* __restrict__ out) {
+  for (int o = threadIdx.x; o < H1; o += blockDim.x) x1[o] = hidden_relu<kTorchRelu>(linear_item(w1, b1, x0, C0, o));
+  __syncthreads();
+  for (int o = threadIdx.x; o < H2; o += blockDim.x) x2[o] = hidden_relu<kTorchRelu>(linear_item(w2, b2, x1, H1, o));
+  __syncthreads();
+  for (int o = threadIdx.x; o < NO; o += blockDim.x) out[o] = sigmoid_f(linear_item(w3, b3, x2, H2, o));
+}
+
+// One CTA per image: mean over P positions of C0 channels, then the MLP tail (mlp3_row).  Dynamic smem: C0+H1+H2 floats.
 __global__ void __launch_bounds__(256) gap_mlp3_kernel(const void* __restrict__ in, int format, int P, int C0, int H1, int H2, int NO,
                                                        const float* __restrict__ w1, const float* __restrict__ b1,
                                                        const float* __restrict__ w2, const float* __restrict__ b2,
@@ -35,23 +69,166 @@ __global__ void __launch_bounds__(256) gap_mlp3_kernel(const void* __restrict__ 
     x0[c] = acc / (float)P;
   }
   __syncthreads();
-  for (int o = threadIdx.x; o < H1; o += blockDim.x) {
-    float acc = b1[o];
-    for (int i = 0; i < C0; ++i) acc = fmaf(w1[(long)o * C0 + i], x0[i], acc);
-    x1[o] = fmaxf(acc, 0.0f);
+  mlp3_row<false>(x0, x1, x2, C0, H1, H2, NO, w1, b1, w2, b2, w3, b3, out + (long)n * NO);
+}
+
+// ---- training tail of ConfidenceHead (pose_resnet.py): from the second BatchNorm's output x (N, C0, H, W), float32, any element
+// strides, through MaxPool2d(2) -> ReLU -> mean over the P = (H/2)(W/2) pooled positions -> the MLP tail, and its backward.
+//   forward  conf_head_fwd_kernel, one CTA per row: x0 = mean(relu(pool(x))) with torch's pooling rule (pool_max of misc.cu: a value
+//            replaces the running maximum if greater or NaN; floor mode) and a NaN-keeping ReLU, then mlp3_row<true>.  x0, h1, h2
+//            are saved for the backward.
+//   backward conf_head_bwd_rows_kernel, one CTA per row: d3 = g y (1 - y), d2 = [!(h2 <= 0)] W3^T d3, d1 = [!(h1 <= 0)] W2^T d2,
+//            dx0 = W1^T d1 (torch's threshold_backward masks: a NaN activation passes its gradient), into the workspace;
+//            conf_head_wgrad_kernel, one thread per weight or bias: the sum over the rows n = 0..N-1 in order;
+//            conf_head_dx_kernel, one thread per element of x: dx0 / P at its window's arg-max when !(pooled <= 0), 0 elsewhere
+//            (including the last row / column floor mode drops).  No atomics: every sum has one fixed order.
+struct HeadMap {
+  const float* x; int N, C, H, W; long xs[4];   // element strides (n, c, h, w)
+};
+
+// the window of pooled position (ph, pw) of row n, channel c: its maximum under torch's rule and the index (2 a + b) of the element
+// holding it (the first one; 0 if no element is taken)
+__host__ __device__ __forceinline__ float head_window_max(const HeadMap& m, int n, int c, int ph, int pw, int* arg) {
+  const float* xb = m.x + n * m.xs[0] + c * m.xs[1] + (2 * ph) * m.xs[2] + (2 * pw) * m.xs[3];
+  float mx = -INFINITY;
+  int best = 0;
+  for (int a = 0; a < 2; ++a)
+    for (int b = 0; b < 2; ++b) {
+      const float v = xb[a * m.xs[2] + b * m.xs[3]];
+      if (v > mx || v != v) { mx = v; best = 2 * a + b; }
+    }
+  *arg = best;
+  return mx;
+}
+
+// x0[n][c]: the pooled, rectified values summed in row-major pooled order, over P
+__host__ __device__ __forceinline__ float head_gap_item(const HeadMap& m, int n, int c) {
+  const int OH = m.H / 2, OW = m.W / 2;
+  float acc = 0.0f;
+  for (int ph = 0; ph < OH; ++ph)
+    for (int pw = 0; pw < OW; ++pw) {
+      int arg;
+      const float v = head_window_max(m, n, c, ph, pw, &arg);
+      acc += v <= 0.0f ? 0.0f : v;
+    }
+  return acc / (float)(OH * OW);
+}
+
+// sum_o w[o][i] d[o] over the `out` rows of an [out][in] weight, o in order
+__host__ __device__ __forceinline__ float linear_bwd_item(const float* __restrict__ w, const float* d, int out, int in, int i) {
+  float acc = 0.0f;
+  for (int o = 0; o < out; ++o) acc = fmaf(w[(long)o * in + i], d[o], acc);
+  return acc;
+}
+
+// Workspace of the backward: per row d3 (NO), d2 (H2), d1 (H1) and dx0 (C0), float32
+__host__ __device__ __forceinline__ long head_ws_row(int C0, int H1, int H2, int NO) { return (long)NO + H2 + H1 + C0; }
+
+// one weight or bias gradient: element e of the flattened [dW1 | db1 | dW2 | db2 | dW3 | db3], summed over the rows in order
+__host__ __device__ __forceinline__ void head_wgrad_item(const float* __restrict__ ws, const float* __restrict__ x0,
+                                                         const float* __restrict__ h1, const float* __restrict__ h2, int N, int C0, int H1,
+                                                         int H2, int NO, long e, float* __restrict__ dw1, float* __restrict__ db1,
+                                                         float* __restrict__ dw2, float* __restrict__ db2, float* __restrict__ dw3,
+                                                         float* __restrict__ db3) {
+  const long row = head_ws_row(C0, H1, H2, NO);
+  // the gradient's array, the layer's deltas (offset in a workspace row), its input activations (nullptr for a bias) and their width
+  float* dst;
+  const float* act = nullptr;
+  long doff;
+  int in = 1;
+  if (e < (long)H1 * C0) { dst = dw1; act = x0; in = C0; doff = (long)NO + H2; }
+  else if ((e -= (long)H1 * C0) < H1) { dst = db1; doff = (long)NO + H2; }
+  else if ((e -= H1) < (long)H2 * H1) { dst = dw2; act = h1; in = H1; doff = NO; }
+  else if ((e -= (long)H2 * H1) < H2) { dst = db2; doff = NO; }
+  else if ((e -= H2) < (long)NO * H2) { dst = dw3; act = h2; in = H2; doff = 0; }
+  else { e -= (long)NO * H2; dst = db3; doff = 0; }
+  const long o = act ? e / in : e, i = act ? e % in : 0;
+  float acc = 0.0f;
+  for (int n = 0; n < N; ++n) {
+    const float d = ws[n * row + doff + o];
+    acc = act ? fmaf(d, act[(long)n * in + i], acc) : acc + d;
   }
-  __syncthreads();
-  for (int o = threadIdx.x; o < H2; o += blockDim.x) {
-    float acc = b2[o];
-    for (int i = 0; i < H1; ++i) acc = fmaf(w2[(long)o * H1 + i], x1[i], acc);
-    x2[o] = fmaxf(acc, 0.0f);
+  dst[e] = acc;
+}
+
+// grad_x at element i of the map, walked in the memory order of grad_x (channels fastest when its channel stride is 1)
+__host__ __device__ __forceinline__ void head_dx_item(const HeadMap& m, const long gs[4], const float* __restrict__ ws, int C0, int H1,
+                                                      int H2, int NO, float* __restrict__ gx, long i) {
+  int n, c, h, w;
+  long r = i;
+  if (gs[1] == 1 && m.C > 1) {
+    c = (int)(r % m.C); r /= m.C; w = (int)(r % m.W); r /= m.W; h = (int)(r % m.H); n = (int)(r / m.H);
+  } else {
+    w = (int)(r % m.W); r /= m.W; h = (int)(r % m.H); r /= m.H; c = (int)(r % m.C); n = (int)(r / m.C);
   }
+  const int OH = m.H / 2, OW = m.W / 2, ph = h / 2, pw = w / 2;
+  float out = 0.0f;
+  if (ph < OH && pw < OW) {
+    int arg;
+    const float mx = head_window_max(m, n, c, ph, pw, &arg);
+    if (arg == 2 * (h - 2 * ph) + (w - 2 * pw) && !(mx <= 0.0f))
+      out = ws[n * head_ws_row(C0, H1, H2, NO) + (long)NO + H2 + H1 + c] / (float)(OH * OW);
+  }
+  gx[n * gs[0] + c * gs[1] + h * gs[2] + w * gs[3]] = out;
+}
+
+__global__ void __launch_bounds__(256) conf_head_fwd_kernel(const HeadMap m, int H1, int H2, int NO, const float* __restrict__ w1,
+                                                            const float* __restrict__ b1, const float* __restrict__ w2,
+                                                            const float* __restrict__ b2, const float* __restrict__ w3,
+                                                            const float* __restrict__ b3, float* __restrict__ out,
+                                                            float* __restrict__ x0_out, float* __restrict__ h1_out,
+                                                            float* __restrict__ h2_out) {
+  extern __shared__ float sm[];
+  const int C0 = m.C, n = blockIdx.x;
+  float* x0 = sm;
+  float* x1 = x0 + C0;
+  float* x2 = x1 + H1;
+  for (int c = threadIdx.x; c < C0; c += blockDim.x) x0_out[(long)n * C0 + c] = x0[c] = head_gap_item(m, n, c);
   __syncthreads();
+  mlp3_row<true>(x0, x1, x2, C0, H1, H2, NO, w1, b1, w2, b2, w3, b3, out + (long)n * NO);
+  for (int o = threadIdx.x; o < H1; o += blockDim.x) h1_out[(long)n * H1 + o] = x1[o];
+  for (int o = threadIdx.x; o < H2; o += blockDim.x) h2_out[(long)n * H2 + o] = x2[o];
+}
+
+// Dynamic smem: NO + H2 + H1 floats (the row's deltas, also written to its workspace row)
+__global__ void __launch_bounds__(256) conf_head_bwd_rows_kernel(int C0, int H1, int H2, int NO, const float* __restrict__ w1,
+                                                                 const float* __restrict__ w2, const float* __restrict__ w3,
+                                                                 const float* __restrict__ h1, const float* __restrict__ h2,
+                                                                 const float* __restrict__ y, const float* __restrict__ g,
+                                                                 float* __restrict__ ws) {
+  extern __shared__ float sm[];
+  float* d3 = sm;
+  float* d2 = d3 + NO;
+  float* d1 = d2 + H2;
+  const int n = blockIdx.x;
+  float* wrow = ws + n * head_ws_row(C0, H1, H2, NO);
   for (int o = threadIdx.x; o < NO; o += blockDim.x) {
-    float acc = b3[o];
-    for (int i = 0; i < H2; ++i) acc = fmaf(w3[(long)o * H2 + i], x2[i], acc);
-    out[(long)n * NO + o] = 1.0f / (1.0f + expf(-acc));
+    wrow[o] = d3[o] = sigmoid_bwd(g[(long)n * NO + o], y[(long)n * NO + o]);
   }
+  __syncthreads();
+  for (int i = threadIdx.x; i < H2; i += blockDim.x)
+    wrow[NO + i] = d2[i] = !(h2[(long)n * H2 + i] <= 0.0f) ? linear_bwd_item(w3, d3, NO, H2, i) : 0.0f;
+  __syncthreads();
+  for (int i = threadIdx.x; i < H1; i += blockDim.x)
+    wrow[NO + H2 + i] = d1[i] = !(h1[(long)n * H1 + i] <= 0.0f) ? linear_bwd_item(w2, d2, H2, H1, i) : 0.0f;
+  __syncthreads();
+  for (int i = threadIdx.x; i < C0; i += blockDim.x) wrow[NO + H2 + H1 + i] = linear_bwd_item(w1, d1, H1, C0, i);
+}
+
+__global__ void __launch_bounds__(256) conf_head_wgrad_kernel(const float* __restrict__ ws, const float* __restrict__ x0,
+                                                              const float* __restrict__ h1, const float* __restrict__ h2, int N, int C0,
+                                                              int H1, int H2, int NO, long total, float* __restrict__ dw1,
+                                                              float* __restrict__ db1, float* __restrict__ dw2, float* __restrict__ db2,
+                                                              float* __restrict__ dw3, float* __restrict__ db3) {
+  for (long e = (long)blockIdx.x * blockDim.x + threadIdx.x; e < total; e += (long)gridDim.x * blockDim.x)
+    head_wgrad_item(ws, x0, h1, h2, N, C0, H1, H2, NO, e, dw1, db1, dw2, db2, dw3, db3);
+}
+
+__global__ void __launch_bounds__(256) conf_head_dx_kernel(const HeadMap m, const long4 gs4, const float* __restrict__ ws, int H1, int H2,
+                                                           int NO, float* __restrict__ gx, long total) {
+  const long gs[4] = {gs4.x, gs4.y, gs4.z, gs4.w};
+  for (long i = (long)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (long)gridDim.x * blockDim.x)
+    head_dx_item(m, gs, ws, m.C, H1, H2, NO, gx, i);
 }
 
 // conf[B][V][C] /= sum over views; += eps
@@ -62,6 +239,29 @@ __global__ void view_normalize_kernel(float* __restrict__ conf, int B, int V, in
   float s = 0.0f;
   for (int v = 0; v < V; ++v) s += conf[((long)b * V + v) * C + c];
   for (int v = 0; v < V; ++v) conf[((long)b * V + v) * C + c] = conf[((long)b * V + v) * C + c] / s + eps;
+}
+
+// Backward of y_v = c_v / S + eps, S = sum_u c_u, for one (b, c): dc_v = g_v / S - (sum_u g_u c_u) / S^2, the sums over the views in
+// order, in float64, rounded once.
+__host__ __device__ __forceinline__ void view_normalize_bwd_item(const float* __restrict__ conf, const float* __restrict__ grad,
+                                                                 float* __restrict__ grad_conf, int V, int C, int b, int c) {
+  double s = 0.0, t = 0.0;
+  for (int v = 0; v < V; ++v) {
+    const long k = ((long)b * V + v) * C + c;
+    s += (double)conf[k];
+    t += (double)grad[k] * (double)conf[k];
+  }
+  for (int v = 0; v < V; ++v) {
+    const long k = ((long)b * V + v) * C + c;
+    grad_conf[k] = (float)((double)grad[k] / s - t / (s * s));
+  }
+}
+
+__global__ void view_normalize_bwd_kernel(const float* __restrict__ conf, const float* __restrict__ grad, float* __restrict__ grad_conf,
+                                          int B, int V, int C) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= B * C) return;
+  view_normalize_bwd_item(conf, grad, grad_conf, V, C, i / C, i % C);
 }
 
 // Weighted DLT (Hartley & Zisserman 12.2): rows c*(x*P[2] - P[0]), c*(y*P[2] - P[1]); the solution is the right singular
@@ -310,6 +510,63 @@ extern "C" int lt_view_normalize_fwd(float* conf, int B, int V, int C, float eps
   return LT_OK;
 }
 
+static int conf_head_check(const float* x, int N, int C0, int H, int W, int H1, int H2, int NO) {
+  LT_REQUIRE(x, "conf_head_tail: null input map");
+  LT_REQUIRE(N > 0 && C0 > 0 && H > 0 && W > 0 && H1 > 0 && H2 > 0 && NO > 0, "conf_head_tail: non-positive size");
+  LT_REQUIRE(H >= 2 && W >= 2, "conf_head_tail: a %dx%d map is too small for the 2x2 max pool", H, W);
+  LT_REQUIRE((size_t)(C0 + H1 + H2) * sizeof(float) <= 48 * 1024, "conf_head_tail: layer widths too large");
+  return LT_OK;
+}
+
+extern "C" int lt_conf_head_tail_fwd(const float* x, int N, int C0, int H, int W, long xs_n, long xs_c, long xs_h, long xs_w, int H1,
+                                     int H2, int NO, const float* w1, const float* b1, const float* w2, const float* b2, const float* w3,
+                                     const float* b3, float* out, float* x0, float* h1, float* h2, void* stream) {
+  const int rc = conf_head_check(x, N, C0, H, W, H1, H2, NO);
+  if (rc != LT_OK) return rc;
+  LT_REQUIRE(w1 && b1 && w2 && b2 && w3 && b3 && out && x0 && h1 && h2, "conf_head_tail_fwd: null pointer");
+  const HeadMap m{x, N, C0, H, W, {xs_n, xs_c, xs_h, xs_w}};
+  conf_head_fwd_kernel<<<N, 256, (size_t)(C0 + H1 + H2) * sizeof(float), (cudaStream_t)stream>>>(m, H1, H2, NO, w1, b1, w2, b2, w3, b3,
+                                                                                                 out, x0, h1, h2);
+  LT_CHECK_LAUNCH("conf_head_fwd_kernel");
+  return LT_OK;
+}
+
+extern "C" size_t lt_conf_head_tail_bwd_workspace_bytes(int N, int C0, int H1, int H2, int NO) {
+  return (N > 0 && C0 > 0 && H1 > 0 && H2 > 0 && NO > 0) ? (size_t)N * head_ws_row(C0, H1, H2, NO) * sizeof(float) : 0;
+}
+
+extern "C" int lt_conf_head_tail_bwd(const float* x, int N, int C0, int H, int W, long xs_n, long xs_c, long xs_h, long xs_w, long gs_n,
+                                     long gs_c, long gs_h, long gs_w, int H1, int H2, int NO, const float* w1, const float* w2,
+                                     const float* w3, const float* x0, const float* h1, const float* h2, const float* y,
+                                     const float* grad_y, float* grad_x, float* dw1, float* db1, float* dw2, float* db2, float* dw3,
+                                     float* db3, void* workspace, size_t workspace_bytes, void* stream) {
+  const int rc = conf_head_check(x, N, C0, H, W, H1, H2, NO);
+  if (rc != LT_OK) return rc;
+  LT_REQUIRE(w1 && w2 && w3 && x0 && h1 && h2 && y && grad_y && grad_x && dw1 && db1 && dw2 && db2 && dw3 && db3 && workspace,
+             "conf_head_tail_bwd: null pointer");
+  const size_t need = lt_conf_head_tail_bwd_workspace_bytes(N, C0, H1, H2, NO);
+  LT_REQUIRE(workspace_bytes >= need, "conf_head_tail_bwd: workspace of %zu bytes, %zu needed", workspace_bytes, need);
+  cudaStream_t st = (cudaStream_t)stream;
+  float* ws = static_cast<float*>(workspace);
+  conf_head_bwd_rows_kernel<<<N, 256, (size_t)(NO + H2 + H1) * sizeof(float), st>>>(C0, H1, H2, NO, w1, w2, w3, h1, h2, y, grad_y, ws);
+  LT_CHECK_LAUNCH("conf_head_bwd_rows_kernel");
+  const long nw = (long)H1 * C0 + H1 + (long)H2 * H1 + H2 + (long)NO * H2 + NO;
+  conf_head_wgrad_kernel<<<ceil_div(nw, 256), 256, 0, st>>>(ws, x0, h1, h2, N, C0, H1, H2, NO, nw, dw1, db1, dw2, db2, dw3, db3);
+  LT_CHECK_LAUNCH("conf_head_wgrad_kernel");
+  const HeadMap m{x, N, C0, H, W, {xs_n, xs_c, xs_h, xs_w}};
+  const long total = (long)N * C0 * H * W;
+  conf_head_dx_kernel<<<ceil_div(total, 256), 256, 0, st>>>(m, make_long4(gs_n, gs_c, gs_h, gs_w), ws, H1, H2, NO, grad_x, total);
+  LT_CHECK_LAUNCH("conf_head_dx_kernel");
+  return LT_OK;
+}
+
+extern "C" int lt_view_normalize_bwd(const float* conf, const float* grad, float* grad_conf, int B, int V, int C, void* stream) {
+  LT_REQUIRE(conf && grad && grad_conf && B > 0 && V > 0 && C > 0, "view_normalize_bwd: bad arguments");
+  view_normalize_bwd_kernel<<<ceil_div((long)B * C, 128), 128, 0, (cudaStream_t)stream>>>(conf, grad, grad_conf, B, V, C);
+  LT_CHECK_LAUNCH("view_normalize_bwd_kernel");
+  return LT_OK;
+}
+
 extern "C" int lt_triangulate_dlt_fwd(const float* proj, const float* keypoints_2d, const float* confidences, float* out, int B,
                                       int V, int J, void* stream) {
   LT_REQUIRE(proj && keypoints_2d && out && B > 0 && V > 0 && J > 0, "triangulate_dlt: bad arguments");
@@ -361,6 +618,54 @@ extern "C" int lt_test_triangulate_dlt_bwd_host(const float* proj, const float* 
              "test_triangulate_dlt_bwd_host: bad arguments");
   for (int b = 0; b < B; ++b)
     for (int j = 0; j < J; ++j) dlt_bwd_item(proj, keypoints_2d, confidences, grad_out, grad_keypoints_2d, grad_confidences, b, j, V, J);
+  return LT_OK;
+}
+
+// The forward kernel's and (grad_y not null) the backward kernels' per-item code on host pointers, row by row as the CTAs run it.
+extern "C" int lt_test_conf_head_tail_host(const float* x, int N, int C0, int H, int W, long xs_n, long xs_c, long xs_h, long xs_w,
+                                           long gs_n, long gs_c, long gs_h, long gs_w, int H1, int H2, int NO, const float* w1,
+                                           const float* b1, const float* w2, const float* b2, const float* w3, const float* b3, float* out,
+                                           float* x0, float* h1, float* h2, const float* grad_y, float* grad_x, float* dw1, float* db1,
+                                           float* dw2, float* db2, float* dw3, float* db3) {
+  const int rc = conf_head_check(x, N, C0, H, W, H1, H2, NO);
+  if (rc != LT_OK) return rc;
+  LT_REQUIRE(w1 && b1 && w2 && b2 && w3 && b3 && out && x0 && h1 && h2, "test_conf_head_tail_host: null pointer");
+  LT_REQUIRE(!grad_y || (grad_x && dw1 && db1 && dw2 && db2 && dw3 && db3), "test_conf_head_tail_host: null gradient pointer");
+  const HeadMap m{x, N, C0, H, W, {xs_n, xs_c, xs_h, xs_w}};
+  for (int n = 0; n < N; ++n) {
+    float* r0 = x0 + (long)n * C0;
+    float* r1 = h1 + (long)n * H1;
+    float* r2 = h2 + (long)n * H2;
+    for (int c = 0; c < C0; ++c) r0[c] = head_gap_item(m, n, c);
+    for (int o = 0; o < H1; ++o) r1[o] = hidden_relu<true>(linear_item(w1, b1, r0, C0, o));
+    for (int o = 0; o < H2; ++o) r2[o] = hidden_relu<true>(linear_item(w2, b2, r1, H1, o));
+    for (int o = 0; o < NO; ++o) out[(long)n * NO + o] = sigmoid_f(linear_item(w3, b3, r2, H2, o));
+  }
+  if (!grad_y) return LT_OK;
+  const long row = head_ws_row(C0, H1, H2, NO);
+  float* ws = static_cast<float*>(malloc((size_t)N * row * sizeof(float)));
+  LT_REQUIRE(ws, "test_conf_head_tail_host: out of memory");
+  for (int n = 0; n < N; ++n) {
+    float* d3 = ws + n * row;
+    float* d2 = d3 + NO;
+    float* d1 = d2 + H2;
+    for (int o = 0; o < NO; ++o) d3[o] = sigmoid_bwd(grad_y[(long)n * NO + o], out[(long)n * NO + o]);
+    for (int i = 0; i < H2; ++i) d2[i] = !(h2[(long)n * H2 + i] <= 0.0f) ? linear_bwd_item(w3, d3, NO, H2, i) : 0.0f;
+    for (int i = 0; i < H1; ++i) d1[i] = !(h1[(long)n * H1 + i] <= 0.0f) ? linear_bwd_item(w2, d2, H2, H1, i) : 0.0f;
+    for (int i = 0; i < C0; ++i) d1[H1 + i] = linear_bwd_item(w1, d1, H1, C0, i);
+  }
+  const long nw = (long)H1 * C0 + H1 + (long)H2 * H1 + H2 + (long)NO * H2 + NO;
+  for (long e = 0; e < nw; ++e) head_wgrad_item(ws, x0, h1, h2, N, C0, H1, H2, NO, e, dw1, db1, dw2, db2, dw3, db3);
+  const long gs[4] = {gs_n, gs_c, gs_h, gs_w};
+  for (long i = 0; i < (long)N * C0 * H * W; ++i) head_dx_item(m, gs, ws, C0, H1, H2, NO, grad_x, i);
+  free(ws);
+  return LT_OK;
+}
+
+extern "C" int lt_test_view_normalize_bwd_host(const float* conf, const float* grad, float* grad_conf, int B, int V, int C) {
+  LT_REQUIRE(conf && grad && grad_conf && B > 0 && V > 0 && C > 0, "test_view_normalize_bwd_host: bad arguments");
+  for (int b = 0; b < B; ++b)
+    for (int c = 0; c < C; ++c) view_normalize_bwd_item(conf, grad, grad_conf, V, C, b, c);
   return LT_OK;
 }
 

@@ -15,8 +15,10 @@ layers.py: `conv` applies each Conv2d / ConvTranspose2d (backbone_backend=
 "native": autograd_ops.backbone_conv), `norm` each BatchNorm2d together with
 the ReLU right after it and, at the end of a residual unit, the shortcut add
 (norm_backend="native": autograd_ops.batch_norm).  None, the default, stands
-for the torch formulas in layers.py.  Max-pool and the heads' Linear layers
-are always torch modules.  A ReLU module right after a BatchNorm is applied by
+for the torch formulas in layers.py.  The trunk's max-pool and the heads'
+first max-pool are always torch modules; the heads' second max-pool, ReLU,
+mean and Linear layers are torch modules unless a `tail` hook replaces them
+(head_backend="native": autograd_ops.conf_head_tail).  A ReLU module right after a BatchNorm is applied by
 `norm`, not called as a module, so a forward hook registered on it does not
 fire.
 """
@@ -103,9 +105,13 @@ class ConfidenceHead(nn.Module):
             nn.Linear(256, n_classes), nn.Sigmoid(),
         )
 
-    def forward(self, x, conv=None, norm=None):
-        x = run(self.features, x, conv, norm)
-        return self.head(x.flatten(2).mean(dim=-1))
+    def forward(self, x, conv=None, norm=None, tail=None):
+        """`tail`, a function (head, x) -> confidences, replaces everything after the second BatchNorm (its max pool and ReLU, the
+        global mean and `head`); None runs the torch modules (head_backend="native": autograd_ops.conf_head_tail)."""
+        if tail is None:
+            x = run(self.features, x, conv, norm)
+            return self.head(x.flatten(2).mean(dim=-1))
+        return tail(self, run(self.features[:6], x, conv, norm))
 
 
 class PoseResNet(nn.Module):
@@ -154,12 +160,12 @@ class PoseResNet(nn.Module):
                 x = unit(x, conv, norm)
         return x
 
-    def forward(self, x, conv=None, norm=None):
-        """-> (heatmaps, features, alg_confidences, vol_confidences), reference :293-318."""
+    def forward(self, x, conv=None, norm=None, tail=None):
+        """-> (heatmaps, features, alg_confidences, vol_confidences), reference :293-318.  `tail` goes to the confidence heads."""
         conv, norm = defaults(conv, norm)
         x = self.trunk(x, conv, norm)
-        alg = self.alg_confidences(x, conv, norm) if hasattr(self, "alg_confidences") else None
-        vol = self.vol_confidences(x, conv, norm) if hasattr(self, "vol_confidences") else None
+        alg = self.alg_confidences(x, conv, norm, tail) if hasattr(self, "alg_confidences") else None
+        vol = self.vol_confidences(x, conv, norm, tail) if hasattr(self, "vol_confidences") else None
         features = run(self.deconv_layers, x, conv, norm)
         return conv(self.final_layer, features), features, alg, vol
 

@@ -58,7 +58,7 @@ def _place_cuboids(base, sides):
 _NO_V2V = object()      # the v2v_backend of a model without a V2V net (None stays an unknown v2v_backend)
 
 
-def _check_backends(backend, conv_mode, backbone_backend, norm_backend, v2v_backend=_NO_V2V):
+def _check_backends(backend, conv_mode, backbone_backend, norm_backend, v2v_backend=_NO_V2V, head_backend="torch"):
     """ValueError unless the training switches are known values in a supported combination.
 
     v2v_backend="native" / backbone_backend="native": every Conv3d / ConvTranspose3d of volume_net / every Conv2d / ConvTranspose2d
@@ -66,7 +66,10 @@ def _check_backends(backend, conv_mode, backbone_backend, norm_backend, v2v_back
     tensor-core kernels.  Both need backend="hybrid" and conv_mode="tc".
     norm_backend="native": every BatchNorm2d / BatchNorm3d of the backbone, its confidence heads and the V2V net, fused with the ReLU
     after it and the residual add of a residual unit, trains on the native kernels.  The kernels read the channels-last maps the
-    native convolutions produce, so it needs backend="hybrid" and every conv switch of the model "native"."""
+    native convolutions produce, so it needs backend="hybrid" and every conv switch of the model "native".
+    head_backend="native": the confidence heads' tail (second max pool, ReLU, global mean, the three Linear layers and the sigmoid) and
+    the normalisation of the confidences over the views train on the native kernels, forward and backward, without cuBLAS.  It needs
+    backend="hybrid" and composes with every other switch; a model without confidence heads runs unchanged."""
     convs = [("backbone_backend", backbone_backend)] + ([] if v2v_backend is _NO_V2V else [("v2v_backend", v2v_backend)])
     for name, value in reversed(convs):     # the V2V switch first
         if value not in ("torch", "native"):
@@ -78,6 +81,10 @@ def _check_backends(backend, conv_mode, backbone_backend, norm_backend, v2v_back
     if norm_backend == "native" and (backend != "hybrid" or any(value != "native" for _, value in convs)):
         raise ValueError("norm_backend='native' needs backend='hybrid' and %s (got backend=%r, %s)"
                          % (" and ".join("%s='native'" % name for name, _ in convs), backend, ", ".join("%s=%r" % c for c in convs)))
+    if head_backend not in ("torch", "native"):
+        raise ValueError("unknown head_backend {!r}".format(head_backend))
+    if head_backend == "native" and backend != "hybrid":
+        raise ValueError("head_backend='native' needs backend='hybrid' (got %r)" % (backend,))
 
 
 def _hooks(backbone_backend, norm_backend, v2v_backend="torch"):
@@ -86,6 +93,11 @@ def _hooks(backbone_backend, norm_backend, v2v_backend="torch"):
     return (autograd_ops.backbone_conv if backbone_backend == "native" else layers.torch_conv,
             autograd_ops.v2v_conv if v2v_backend == "native" else layers.torch_conv,
             autograd_ops.batch_norm if norm_backend == "native" else layers.torch_norm)
+
+
+def _head_tail(head_backend):
+    """The confidence heads' `tail` hook of a checked head_backend: None (the torch modules) or autograd_ops.conf_head_tail."""
+    return autograd_ops.conf_head_tail if head_backend == "native" else None
 
 
 def _upload(device, *arrays, dtype=torch.float32):
@@ -137,7 +149,7 @@ class _EngineOwner(nn.Module):
 
 class VolumetricTriangulationNet(_EngineOwner):
     def __init__(self, config, device="cuda:0", backend=None, conv_mode=None, use_cuda_graph=True, v2v_backend="torch",
-                 backbone_backend="torch", norm_backend="torch", train_graph=False):
+                 backbone_backend="torch", norm_backend="torch", train_graph=False, head_backend="torch"):
         super().__init__()
         m = config.model
         self.num_joints = m.backbone.num_joints
@@ -166,9 +178,10 @@ class VolumetricTriangulationNet(_EngineOwner):
 
         self.backend = backend or os.environ.get("LT_B200_BACKEND", "native")
         self.conv_mode = conv_mode or os.environ.get("LT_B200_CONV", "tc")
-        _check_backends(self.backend, self.conv_mode, backbone_backend, norm_backend, v2v_backend)
+        _check_backends(self.backend, self.conv_mode, backbone_backend, norm_backend, v2v_backend, head_backend)
         _check_train_graph(train_graph, self.backend)
         self.v2v_backend = v2v_backend
+        self.head_backend = head_backend
         self.backbone_backend = backbone_backend
         self.norm_backend = norm_backend
         self.use_cuda_graph = use_cuda_graph
@@ -259,7 +272,7 @@ class VolumetricTriangulationNet(_EngineOwner):
         B, V = images.shape[:2]
         flat = images.reshape(-1, *images.shape[2:])
         conv, v2v_conv, norm = _hooks(self.backbone_backend, self.norm_backend, self.v2v_backend)
-        heatmaps, features, _, vol_conf = self.backbone(flat, conv, norm)
+        heatmaps, features, _, vol_conf = self.backbone(flat, conv, norm, _head_tail(self.head_backend))
         hm_shape = (backbone_map_size(images.shape[3]), backbone_map_size(images.shape[4]))
         if tuple(heatmaps.shape[2:]) != hm_shape:
             raise RuntimeError("heat-map size %s differs from the size %s used for the projection matrices"
@@ -267,7 +280,10 @@ class VolumetricTriangulationNet(_EngineOwner):
         if vol_conf is not None:
             vol_conf = vol_conf.view(B, V, *vol_conf.shape[1:])
             if self.volume_aggregation_method == "conf_norm":
-                vol_conf = vol_conf / vol_conf.sum(dim=1, keepdim=True)
+                if self.head_backend == "native":
+                    vol_conf = autograd_ops.view_normalize(vol_conf, 0.0)
+                else:
+                    vol_conf = vol_conf / vol_conf.sum(dim=1, keepdim=True)
         n = self.volume_size
         idx = torch.arange(n, device=dev, dtype=torch.float)
         grid = torch.stack(torch.meshgrid(idx, idx, idx, indexing="ij"), dim=-1)              # (n, n, n, 3)
@@ -293,7 +309,7 @@ class AlgebraicTriangulationNet(_EngineOwner):
     with their backward kernels (trains, any mode)."""
 
     def __init__(self, config, device="cuda:0", backend=None, conv_mode=None, backbone_backend="torch", norm_backend="torch",
-                 train_graph=False):
+                 train_graph=False, head_backend="torch"):
         super().__init__()
         self.use_confidences = config.model.use_confidences
         config.model.backbone.alg_confidences = False
@@ -305,8 +321,9 @@ class AlgebraicTriangulationNet(_EngineOwner):
         self.heatmap_multiplier = config.model.heatmap_multiplier
         self.backend = backend or os.environ.get("LT_B200_BACKEND", "native")
         self.conv_mode = conv_mode or os.environ.get("LT_B200_CONV", "tc")
-        _check_backends(self.backend, self.conv_mode, backbone_backend, norm_backend)
+        _check_backends(self.backend, self.conv_mode, backbone_backend, norm_backend, head_backend=head_backend)
         _check_train_graph(train_graph, self.backend)
+        self.head_backend = head_backend
         self.backbone_backend = backbone_backend
         self.norm_backend = norm_backend
         self.clone_outputs = True
@@ -341,14 +358,17 @@ class AlgebraicTriangulationNet(_EngineOwner):
         ops_backend = "hybrid" if self.backend == "hybrid" else "torch"
         B, V = images.shape[:2]
         conv, _, norm = _hooks(self.backbone_backend, self.norm_backend)
-        heatmaps, _, alg_conf, _ = self.backbone(images.reshape(-1, *images.shape[2:]), conv, norm)
+        heatmaps, _, alg_conf, _ = self.backbone(images.reshape(-1, *images.shape[2:]), conv, norm, _head_tail(self.head_backend))
         if not self.use_confidences:
             alg_conf = torch.ones(B * V, heatmaps.shape[1], dtype=torch.float, device=images.device)
         kp2d, heatmaps = op.integrate_tensor_2d(heatmaps * self.heatmap_multiplier, self.heatmap_softmax, backend=ops_backend)
         heatmaps = heatmaps.view(B, V, *heatmaps.shape[1:])
         kp2d = kp2d.view(B, V, *kp2d.shape[1:])
         alg_conf = alg_conf.view(B, V, -1)
-        alg_conf = alg_conf / alg_conf.sum(dim=1, keepdim=True) + 1e-5
+        if self.use_confidences and self.head_backend == "native":
+            alg_conf = autograd_ops.view_normalize(alg_conf, 1e-5)
+        else:
+            alg_conf = alg_conf / alg_conf.sum(dim=1, keepdim=True) + 1e-5
         h, w = heatmaps.shape[3:]
         H, W = images.shape[3:]
         # the (W / w, H / h) scale is filled on the device: a host-to-device copy would synchronise and cannot be captured
