@@ -300,6 +300,32 @@ typedef struct lt_conv_tc_launch_plan {
                                 16-channel tiles, which keep no tile buffer */
 } lt_conv_tc_launch_plan;
 int lt_conv_tc_plan(const lt_conv_desc* desc, int sm_count, int splitk, lt_conv_tc_launch_plan* plan);
+
+/* Chain mode of the LT_CONV_TC / TC1 kernel: `blocks` identical bottleneck blocks in ONE persistent launch.  descs[0..2] are the
+ * lt_conv_nd_fwd descriptors of a block's 1x1 reduce, its 3x3 and its 1x1 expansion (residual BEFORE or AFTER ReLU): stride 1, split-
+ * fp16 in and out, one output grid for all three, every Cout a multiple of 128 (N tile 128, never split along K).  The chain runs in
+ * place on x (the first block's input, the last block's output); bufs = {Y1 even, Y1 odd, Y2 even, Y2 odd} hold the reduce and 3x3
+ * outputs of even / odd blocks.  weights / scales / shifts: 3 x blocks entries, layer 3 k + c.  Every unit (layer, M tile, N tile)
+ * computes the bits its own lt_conv_nd_fwd launch would.  counters: lt_conv_tc_chain_plan.counters unsigned ints of device scratch,
+ * zeroed in the stream by the call.  At most 36 blocks per call. */
+typedef struct lt_conv_tc_chain_launch_plan {
+  int m_tiles;               /* output tiles of 128 positions, shared by every layer */
+  int n_tiles[3];            /* N tiles of 128 channels of the reduce, the 3x3 and the expansion */
+  int units;                 /* work units of the launch, numbered layer-major, then M tile, then N tile */
+  int grid;                  /* CTAs launched: min(units, sm_count) */
+  int counters;              /* unsigned ints of the counter scratch: the unit dispenser + one per (layer, M tile) */
+} lt_conv_tc_chain_launch_plan;
+int lt_conv_tc_chain_plan(const lt_conv_desc* descs, int blocks, int sm_count, lt_conv_tc_chain_launch_plan* plan);
+/* What unit `unit` of that chain waits for before it loads: all of tiles[0..n_deps) of layer src_layer (-1: nothing, the first
+ * layer) must have `need` N tiles stored.  At most `cap` tiles are written. */
+typedef struct lt_conv_tc_chain_unit {
+  int layer, m_tile, n_tile;
+  int src_layer, need, n_deps;
+} lt_conv_tc_chain_unit;
+int lt_conv_tc_chain_deps(const lt_conv_desc* descs, int blocks, int unit, lt_conv_tc_chain_unit* info, int* tiles, int cap);
+int lt_conv_tc_chain_fwd(const lt_conv_desc* descs, int blocks, void* x, void* const* bufs, const void* const* weights,
+                         const float* const* scales, const float* const* shifts, void* counters, size_t counters_bytes, int impl,
+                         void* stream);
 int lt_conv_tc_pack_weights(const float* w_tap_ci_co, void* packed, int taps, int Cin, int Cout, void* stream);
 
 /* Weight preparation (once per parameter version, engine.prepare()).

@@ -42,6 +42,16 @@ class ConvTcPlan(ctypes.Structure):
     _fields_ = [(n, c_int) for n in ("nt", "m_tiles", "n_tiles", "chunks", "splits", "grid", "stages", "epi_buffers")]
 
 
+class ConvTcChainPlan(ctypes.Structure):
+    """Mirror of `struct lt_conv_tc_chain_launch_plan` (include/lt_b200.h)."""
+    _fields_ = [("m_tiles", c_int), ("n_tiles", c_int * 3), ("units", c_int), ("grid", c_int), ("counters", c_int)]
+
+
+class ConvTcChainUnit(ctypes.Structure):
+    """Mirror of `struct lt_conv_tc_chain_unit` (include/lt_b200.h)."""
+    _fields_ = [(n, c_int) for n in ("layer", "m_tile", "n_tile", "src_layer", "need", "n_deps")]
+
+
 class ConvWgradPlan(ctypes.Structure):
     """Mirror of `struct lt_conv_wgrad_launch_plan` (include/lt_b200.h)."""
     _fields_ = [(n, c_int) for n in ("nwg", "ngroups", "m_tiles", "splits", "stages")]
@@ -99,6 +109,10 @@ SIGNATURES = {
     "lt_conv_tc_weight_bytes": (c_size_t, [c_int, c_int, c_int]),
     "lt_conv_tc_plan": (c_int, [ctypes.POINTER(ConvDesc), c_int, c_int, ctypes.POINTER(ConvTcPlan)]),
     "lt_conv_tc_pack_weights": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_void_p]),
+    "lt_conv_tc_chain_plan": (c_int, [ctypes.POINTER(ConvDesc), c_int, c_int, ctypes.POINTER(ConvTcChainPlan)]),
+    "lt_conv_tc_chain_deps": (c_int, [ctypes.POINTER(ConvDesc), c_int, c_int, ctypes.POINTER(ConvTcChainUnit), ctypes.POINTER(c_int), c_int]),
+    "lt_conv_tc_chain_fwd": (c_int, [ctypes.POINTER(ConvDesc), c_int, c_void_p] + [ctypes.POINTER(c_void_p)] * 4 + [c_void_p, c_size_t, c_int,
+                                                                                                              c_void_p]),
     "lt_absmax_fwd": (c_int, [c_void_p, c_long, c_void_p, c_void_p]),
     "lt_conv_gather_weights_fwd": (c_int, [c_void_p] + [c_long] * 6 + [c_int] * 7 + [c_void_p, c_void_p, c_int, c_int, c_void_p]),
     "lt_fold_bn_fwd": (c_int, [c_void_p] * 5 + [c_float, c_int, c_int, c_void_p, c_int, c_void_p, c_void_p, c_void_p]),
@@ -376,6 +390,37 @@ def conv_tc_plan(desc, sm_count, splitk=1):
     plan = ConvTcPlan()
     _check(lib().lt_conv_tc_plan(ctypes.byref(desc), sm_count, splitk, ctypes.byref(plan)), "lt_conv_tc_plan")
     return {name: getattr(plan, name) for name, _ in ConvTcPlan._fields_}
+
+
+def _chain_descs(descs):
+    assert len(descs) == 3
+    return (ConvDesc * 3)(*descs)
+
+
+def conv_tc_chain_plan(descs, blocks, sm_count):
+    """Host-only work decomposition of a chain launch (lt_conv_tc_chain_plan) of `blocks` blocks whose three layers the ConvDescs
+    `descs` describe: dict of m_tiles, n_tiles (3), units, grid, counters."""
+    plan = ConvTcChainPlan()
+    _check(lib().lt_conv_tc_chain_plan(_chain_descs(descs), blocks, sm_count, ctypes.byref(plan)), "lt_conv_tc_chain_plan")
+    return {"m_tiles": plan.m_tiles, "n_tiles": list(plan.n_tiles), "units": plan.units, "grid": plan.grid, "counters": plan.counters}
+
+
+def conv_tc_chain_deps(descs, blocks, unit, cap=64):
+    """lt_conv_tc_chain_deps: (layer, m_tile, n_tile, src_layer, need, [tiles of src_layer unit `unit` waits for])."""
+    info = ConvTcChainUnit()
+    tiles = (c_int * cap)()
+    _check(lib().lt_conv_tc_chain_deps(_chain_descs(descs), blocks, unit, ctypes.byref(info), tiles, cap), "lt_conv_tc_chain_deps")
+    return info.layer, info.m_tile, info.n_tile, info.src_layer, info.need, list(tiles[:info.n_deps])
+
+
+def conv_tc_chain(descs, blocks, x, bufs, weights, scales, shifts, counters, impl):
+    """lt_conv_tc_chain_fwd: `blocks` bottleneck blocks in one launch, in place on tensor x; bufs: the 4 intermediate tensors (Y1 even,
+    Y1 odd, Y2 even, Y2 odd); weights / scales / shifts: 3 x blocks tensors; counters: device scratch of plan["counters"] int32."""
+    n = 3 * blocks
+    assert len(bufs) == 4 and len(weights) == len(scales) == len(shifts) == n
+    arr = lambda ts: (c_void_p * len(ts))(*[t.data_ptr() for t in ts])
+    _check(lib().lt_conv_tc_chain_fwd(_chain_descs(descs), blocks, _ptr(x), arr(bufs), arr(weights), arr(scales), arr(shifts), _ptr(counters),
+                                      counters.numel() * counters.element_size(), impl, _stream()), "lt_conv_tc_chain_fwd")
 
 
 def conv_tc_weight_bytes(taps, cin, cout):

@@ -49,6 +49,7 @@ constexpr int kTcThreads = 384;
 // in time and the A boxes are L2 hits for all but the first; then M tile; the K split z outermost.
 struct TcUnit {
   int m, n0, z, q_begin, nchunks;
+  int k, c;   // chain mode: block and layer class (0 otherwise)
 };
 __device__ __forceinline__ TcUnit tc_unit(const TcParams& p, int u, int m_tiles, int nchunks_all) {
   TcUnit w;
@@ -59,6 +60,7 @@ __device__ __forceinline__ TcUnit tc_unit(const TcParams& p, int u, int m_tiles,
   w.n0 = n * p.Nt;
   w.q_begin = (int)(((long)w.z * nchunks_all) / p.splits);
   w.nchunks = (int)(((long)(w.z + 1) * nchunks_all) / p.splits) - w.q_begin;
+  w.k = w.c = 0;
   return w;
 }
 __device__ __forceinline__ void tc_tile_origin(const TcParams& p, int t, int& ow0, int& oh0, int& od0, int& nb0) {
@@ -85,10 +87,82 @@ __device__ __forceinline__ uint32_t sw128(int row, int b) {
   return (uint32_t)(row * 128 + ((((b >> 4) ^ row) & 7) << 4) + (b & 15));
 }
 
-template <int NT>
-__global__ void __launch_bounds__(kTcThreads, 1) conv_tc_kernel(const __grid_constant__ CUtensorMap tmA,
-                                                                const __grid_constant__ CUtensorMap tmB,
-                                                                const __grid_constant__ TcEpiMaps tmE, const TcParams p) {
+// ---- chain mode (lt_conv_tc_chain_fwd): one persistent launch over a run of identical bottleneck blocks ----
+// Layer c of block k (c = 0: 1x1 reduce, 1: the 3x3, 2: 1x1 expansion + residual) is layer 3k + c of the chain.  All layers share
+// the output grid and the M-tile box of the launch's TcParams; what differs per layer class is below, per block the filter and the
+// folded scale / shift.  Units are numbered layer-major, then M tile, then N tile, so every unit's inputs come from units with
+// smaller numbers: CTAs take units in that order from one global counter and start each once the tiles it reads are stored.
+constexpr int kChainMaxBlocks = 36;
+constexpr int kChainRing = 4;   // unit ids in flight between a CTA's dispatching warp and its other roles
+struct TcChainGeom {
+  int blocks, m_tiles, units_per_block;
+  int tw, th, td, tn, bw, bh, bd, bn, OW, OH, OD;
+  int n_tiles[3], chunks[3], CB[3], KW[3], KH[3], KD[3], pw[3], ph[3], pd[3], CoutP[3], FC[3], residual[3], relu[3];
+};
+struct TcChain {
+  CUtensorMap a[3][2];     // [class][block parity]: the A operand (block input X, Y1, Y2)
+  CUtensorMap out[3][2];   // [class][block parity]: the output (Y1, Y2, X); the expansion writes its residual X in place
+  CUtensorMap res;         // the expansion's residual: X
+  CUtensorMap b[kChainMaxBlocks][3];
+  const float* scale[kChainMaxBlocks][3];
+  const float* shift[kChainMaxBlocks][3];
+  unsigned* counters;      // [0]: next unit to take; [1 + layer * m_tiles + m]: N tiles of (layer, M tile m) stored
+  TcChainGeom g;
+};
+
+__host__ __device__ inline void chain_unit(const TcChainGeom& g, int u, int& k, int& c, int& m, int& n) {
+  k = u / g.units_per_block;
+  int r = u - k * g.units_per_block;
+  c = 0;
+  while (c < 2 && r >= g.m_tiles * g.n_tiles[c]) { r -= g.m_tiles * g.n_tiles[c]; ++c; }
+  m = r / g.n_tiles[c];
+  n = r - m * g.n_tiles[c];
+}
+
+// The tiles unit (block k, class c, M tile m) reads: tiles lo..hi per axis (w, h, d, batch) of layer `src` = 3k + c - 1, the one
+// that writes its input, each complete once `need` (that layer's N tiles) units have stored it.  The receptive field of the tile
+// is clipped to the grid: what lies outside is padding, which TMA zero-fills.  false: the chain's first layer reads the input X.
+__host__ __device__ inline bool chain_deps(const TcChainGeom& g, int k, int c, int m, int& src, int& need, int lo[4], int hi[4]) {
+  if (k == 0 && c == 0) return false;
+  src = 3 * k + c - 1;
+  need = g.n_tiles[(c + 2) % 3];
+  const int tile[3] = {m % g.tw, (m / g.tw) % g.th, (m / (g.tw * g.th)) % g.td};
+  const int box[3] = {g.bw, g.bh, g.bd}, ext[3] = {g.OW, g.OH, g.OD};
+  const int kk[3] = {g.KW[c], g.KH[c], g.KD[c]}, pad[3] = {g.pw[c], g.ph[c], g.pd[c]};
+  for (int a = 0; a < 3; ++a) {
+    int p0 = tile[a] * box[a] - pad[a], p1 = tile[a] * box[a] + box[a] - 1 - pad[a] + kk[a] - 1;
+    p0 = p0 < 0 ? 0 : p0;
+    p1 = p1 > ext[a] - 1 ? ext[a] - 1 : p1;
+    lo[a] = p0 / box[a];
+    hi[a] = p1 / box[a];
+  }
+  lo[3] = hi[3] = m / (g.tw * g.th * g.td);
+  return true;
+}
+
+__device__ __forceinline__ unsigned ld_acquire_gpu(const unsigned* a) {
+  unsigned v;
+  asm volatile("ld.acquire.gpu.global.u32 %0, [%1];" : "=r"(v) : "l"(a) : "memory");
+  return v;
+}
+__device__ __forceinline__ void red_release_gpu_add(unsigned* a, unsigned v) {
+  asm volatile("red.release.gpu.global.add.u32 [%0], %1;" ::"l"(a), "r"(v) : "memory");
+}
+// orders generic-proxy accesses to global memory against the async proxy (TMA) of this thread
+__device__ __forceinline__ void fence_proxy_async_global() { asm volatile("fence.proxy.async.global;" ::: "memory"); }
+// Bounded like mbar_wait: a protocol bug traps instead of hanging the GPU.
+__device__ __forceinline__ void wait_count(const unsigned* a, unsigned need) {
+  if (ld_acquire_gpu(a) >= need) return;
+  const long long t0 = clock64();
+  while (ld_acquire_gpu(a) < need) {
+    __nanosleep(100);
+    if (clock64() - t0 > 4000000000LL) __trap();
+  }
+}
+
+template <int NT, bool CHAIN>
+__device__ __forceinline__ void conv_tc_body(const CUtensorMap* tmA, const CUtensorMap* tmB, const TcEpiMaps* tmE, const TcParams& p,
+                                             const TcChain* cp) {
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
   constexpr int kStage = kATileBytes + NT * 128;
@@ -99,19 +173,47 @@ __global__ void __launch_bounds__(kTcThreads, 1) conv_tc_kernel(const __grid_con
   uint64_t* empty = full + p.stages;
   uint64_t* efull = empty + p.stages;   // [b]: tile buffer b is free and holds its unit's residual
   uint64_t* edone = efull + 2;          // [b]: both consumer warpgroups wrote their unit's output into tile buffer b
+  // chain: ring slot i holds the id of a unit taken by warp 0 (ufull) until warp 1's lane and the 8 consumer warps read it (uempty)
+  uint64_t* ufull = edone + 2;
+  uint64_t* uempty = ufull + kChainRing;
+  volatile int* uid = reinterpret_cast<volatile int*>(uempty + kChainRing);
 
   const int wg = __shfl_sync(0xffffffffu, (int)(threadIdx.x >> 7), 0);
   const int lane = threadIdx.x & 31;
   const int m_tiles = p.tw * p.th * p.td * p.tn;
-  const int units = m_tiles * p.n_tiles * p.splits;
+  int units = m_tiles * p.n_tiles * p.splits;
+  if constexpr (CHAIN) units = cp->g.blocks * cp->g.units_per_block;
   const int nchunks_all = p.KD * p.KH * p.KW * p.CB;
+  auto unit_of = [&](int u) {
+    if constexpr (CHAIN) {
+      TcUnit w;
+      int n;
+      chain_unit(cp->g, u, w.k, w.c, w.m, n);
+      w.n0 = n * NT;
+      w.z = 0;
+      w.q_begin = 0;
+      w.nchunks = cp->g.chunks[w.c];
+      return w;
+    } else {
+      return tc_unit(p, u, m_tiles, nchunks_all);
+    }
+  };
 
   if (threadIdx.x == 0) {
     for (int s = 0; s < p.stages; ++s) { mbar_init(&full[s], 1); mbar_init(&empty[s], 2); }
     for (int b = 0; b < 2; ++b) { mbar_init(&efull[b], 1); mbar_init(&edone[b], 256); }
+    if constexpr (CHAIN) {
+      for (int i = 0; i < kChainRing; ++i) { mbar_init(&ufull[i], 1); mbar_init(&uempty[i], 9); }
+    }
     fence_barrier_init();
-    prefetch_tmap(&tmA);
-    prefetch_tmap(&tmB);
+    if constexpr (CHAIN) {
+      for (int c = 0; c < 3; ++c)
+        for (int q = 0; q < 2; ++q) { prefetch_tmap(&cp->a[c][q]); prefetch_tmap(&cp->out[c][q]); }
+      prefetch_tmap(&cp->res);
+    } else {
+      prefetch_tmap(tmA);
+      prefetch_tmap(tmB);
+    }
   }
   __syncthreads();
 
@@ -126,73 +228,154 @@ __global__ void __launch_bounds__(kTcThreads, 1) conv_tc_kernel(const __grid_con
       const int nbuf = p.epi_buffers;
       auto load_residual = [&](int u, int b) {
         uint8_t* buf = ebuf + b * epi_bytes;
-        if (p.residual == LT_RES_NONE) {
+        const TcUnit w = unit_of(u);
+        int res_mode = p.residual;
+        if constexpr (CHAIN) res_mode = cp->g.residual[w.c];
+        if (res_mode == LT_RES_NONE) {
           mbar_arrive_local(&efull[b]);
           return;
         }
-        const TcUnit w = tc_unit(p, u, m_tiles, nchunks_all);
         int ow0, oh0, od0, nb0;
         tc_tile_origin(p, w.m, ow0, oh0, od0, nb0);
+        if constexpr (CHAIN) fence_proxy_async_global();   // the tiles were stored by other CTAs (warp 0 acquired them)
         mbar_expect_tx(&efull[b], (uint32_t)epi_bytes);   // out-of-range positions and channels arrive as zeros
         for (int sl = 0; sl < NT / 32; ++sl) {
           int g, c;
           epi_slab(p, w.n0 + 32 * sl, g, c);
-          tma_load_5d(buf + sl * kSlabBytes, &tmE.res[g], &efull[b], c, ow0, oh0, od0, nb0);
+          tma_load_5d(buf + sl * kSlabBytes, CHAIN ? &cp->res : &tmE->res[g], &efull[b], c, ow0, oh0, od0, nb0);
         }
       };
       uint32_t eph = 0;   // bit b: phase of edone[b]
-      int b = 0;
-      if (blockIdx.x < units) load_residual(blockIdx.x, 0);
-      for (int u = blockIdx.x; u < units; u += gridDim.x) {
-        const int un = u + gridDim.x, bn = b ^ (nbuf - 1);
-        if (nbuf == 2 && un < units) {
-          bulk_wait_read0();                    // the previous unit's store has read buffer bn
-          load_residual(un, bn);
+      if constexpr (CHAIN) {
+        // One buffer.  A unit counts as stored once its TMA store has completed (not only read shared memory); its (layer, M tile)
+        // counter is raised before this lane waits for the next unit id, which may be a unit that depends on this one.
+        int rs = 0;
+        uint32_t rph = 0;
+        auto take = [&]() {
+          mbar_wait(&ufull[rs], rph);
+          const int v = uid[rs];
+          mbar_arrive_local(&uempty[rs]);
+          if (++rs == kChainRing) { rs = 0; rph ^= 1u; }
+          return v;
+        };
+        int u = take();
+        if (u < units) load_residual(u, 0);
+        while (u < units) {
+          const TcUnit w = unit_of(u);
+          int ow0, oh0, od0, nb0;
+          tc_tile_origin(p, w.m, ow0, oh0, od0, nb0);
+          mbar_wait(&edone[0], eph & 1u);
+          eph ^= 1u;
+          for (int sl = 0; sl < NT / 32; ++sl) {
+            int g, c;
+            epi_slab(p, w.n0 + 32 * sl, g, c);
+            tma_store_5d(&cp->out[w.c][w.k & 1], ebuf + sl * kSlabBytes, c, ow0, oh0, od0, nb0);
+          }
+          bulk_commit();
+          bulk_wait0();
+          fence_proxy_async_global();
+          red_release_gpu_add(cp->counters + 1 + (size_t)(3 * w.k + w.c) * m_tiles + w.m, 1u);
+          u = take();
+          if (u < units) load_residual(u, 0);
         }
-        const TcUnit w = tc_unit(p, u, m_tiles, nchunks_all);
-        int ow0, oh0, od0, nb0;
-        tc_tile_origin(p, w.m, ow0, oh0, od0, nb0);
-        mbar_wait(&edone[b], (eph >> b) & 1u);
-        eph ^= 1u << b;
-        for (int sl = 0; sl < NT / 32; ++sl) {  // clipped at the edges of the output grid and at FC
-          int g, c;
-          epi_slab(p, w.n0 + 32 * sl, g, c);
-          tma_store_5d(&tmE.out[g], ebuf + b * epi_bytes + sl * kSlabBytes, c, ow0, oh0, od0, nb0);
+      } else {
+        int b = 0;
+        if (blockIdx.x < units) load_residual(blockIdx.x, 0);
+        for (int u = blockIdx.x; u < units; u += gridDim.x) {
+          const int un = u + gridDim.x, bn = b ^ (nbuf - 1);
+          if (nbuf == 2 && un < units) {
+            bulk_wait_read0();                    // the previous unit's store has read buffer bn
+            load_residual(un, bn);
+          }
+          const TcUnit w = tc_unit(p, u, m_tiles, nchunks_all);
+          int ow0, oh0, od0, nb0;
+          tc_tile_origin(p, w.m, ow0, oh0, od0, nb0);
+          mbar_wait(&edone[b], (eph >> b) & 1u);
+          eph ^= 1u << b;
+          for (int sl = 0; sl < NT / 32; ++sl) {  // clipped at the edges of the output grid and at FC
+            int g, c;
+            epi_slab(p, w.n0 + 32 * sl, g, c);
+            tma_store_5d(&tmE->out[g], ebuf + b * epi_bytes + sl * kSlabBytes, c, ow0, oh0, od0, nb0);
+          }
+          bulk_commit();
+          if (nbuf == 1 && un < units) {
+            bulk_wait_read0();                    // this unit's store has read the buffer
+            load_residual(un, 0);
+          }
+          b = bn;
         }
-        bulk_commit();
-        if (nbuf == 1 && un < units) {
-          bulk_wait_read0();                    // this unit's store has read the buffer
-          load_residual(un, 0);
-        }
-        b = bn;
+        bulk_wait0();
       }
-      bulk_wait0();
     }
     // ================= TMA producer (warp 0 runs the loop; one elected lane issues) =================
     // The ring slot / phase run on across units: the next unit's boxes load while the consumers run the previous epilogue.
     if (threadIdx.x < 32) {
       int s = 0;
       uint32_t ph = 0;
-      for (int u = blockIdx.x; u < units; u += gridDim.x) {
-        const TcUnit w = tc_unit(p, u, m_tiles, nchunks_all);
+      int rs = 0;
+      uint32_t rph = 0;
+      // chain: take the next unit, wait until the tiles it reads are stored, then hand its id to the other roles
+      auto take = [&]() {
+        mbar_wait(&uempty[rs], rph ^ 1u);
+        int u = 0;
+        if (lane == 0) u = (int)atomicAdd(cp->counters, 1u);
+        u = __shfl_sync(0xffffffffu, u, 0);
+        u = u < units ? u : units;
+        if (u < units) {
+          int k, c, m, n, src, need, lo[4], hi[4];
+          chain_unit(cp->g, u, k, c, m, n);
+          if (chain_deps(cp->g, k, c, m, src, need, lo, hi)) {
+            const int nw = hi[0] - lo[0] + 1, nh = hi[1] - lo[1] + 1, nd = hi[2] - lo[2] + 1;
+            for (int i = lane; i < nw * nh * nd; i += 32) {
+              const int t = ((hi[3] * cp->g.td + lo[2] + i / (nw * nh)) * cp->g.th + lo[1] + (i / nw) % nh) * cp->g.tw + lo[0] + i % nw;
+              wait_count(cp->counters + 1 + (size_t)src * m_tiles + t, (unsigned)need);
+            }
+            __syncwarp();
+            fence_proxy_async_global();   // the TMA loads below read what the acquired stores wrote
+          }
+        }
+        if (lane == 0) {
+          uid[rs] = u;
+          mbar_arrive_local(&ufull[rs]);
+        }
+        __syncwarp();
+        if (++rs == kChainRing) { rs = 0; rph ^= 1u; }
+        return u;
+      };
+      int u;
+      if constexpr (CHAIN) u = take();
+      else u = blockIdx.x;
+      while (u < units) {
+        const TcUnit w = unit_of(u);
         int ow0, oh0, od0, nb0;
         tc_tile_origin(p, w.m, ow0, oh0, od0, nb0);
+        int CB = p.CB, KW = p.KW, KH = p.KH, pw = p.pw, ph_ = p.ph, pd = p.pd, b_step1 = p.b_step1;
+        const CUtensorMap* mA = tmA;
+        const CUtensorMap* mB = tmB;
+        if constexpr (CHAIN) {
+          const TcChainGeom& g = cp->g;
+          CB = g.CB[w.c]; KW = g.KW[w.c]; KH = g.KH[w.c]; pw = g.pw[w.c]; ph_ = g.ph[w.c]; pd = g.pd[w.c]; b_step1 = g.CoutP[w.c];
+          mA = &cp->a[w.c][w.k & 1];
+          mB = &cp->b[w.k][w.c];
+        }
         // chunk -> (tap, channel block) advanced incrementally: no integer division in the loop
-        int tap = w.q_begin / p.CB, cb = w.q_begin - tap * p.CB;
-        int kw = tap % p.KW, kh = (tap / p.KW) % p.KH, kd = tap / (p.KW * p.KH);
-        const int ax = ow0 * p.sw - p.pw, ay = oh0 * p.sh - p.ph, az = od0 * p.sd - p.pd, bn0 = w.n0 * p.b_nmul;
+        int tap = w.q_begin / CB, cb = w.q_begin - tap * CB;
+        int kw = tap % KW, kh = (tap / KW) % KH, kd = tap / (KW * KH);
+        const int ax = ow0 * p.sw - pw, ay = oh0 * p.sh - ph_, az = od0 * p.sd - pd, bn0 = w.n0 * p.b_nmul;
         for (int q = 0, qa = w.q_begin; q < w.nchunks; ++q, ++qa) {
           mbar_wait(&empty[s], ph ^ 1u);
           uint8_t* a_dst = smem + (size_t)s * kStage;
           if (elect_one()) {
             mbar_expect_tx(&full[s], (uint32_t)kStage);
-            tma_load_5d(a_dst, &tmA, &full[s], cb * 64, ax + kw, ay + kh, az + kd, nb0);
-            tma_load_2d(a_dst + kATileBytes, &tmB, &full[s], qa * p.b_step0, qa * p.b_step1 + bn0);
+            tma_load_5d(a_dst, mA, &full[s], cb * 64, ax + kw, ay + kh, az + kd, nb0);
+            tma_load_2d(a_dst + kATileBytes, mB, &full[s], qa * p.b_step0, qa * b_step1 + bn0);
           }
           __syncwarp();
-          if (++cb == p.CB) { cb = 0; if (++kw == p.KW) { kw = 0; if (++kh == p.KH) { kh = 0; ++kd; } } }
+          if (++cb == CB) { cb = 0; if (++kw == KW) { kw = 0; if (++kh == KH) { kh = 0; ++kd; } } }
           if (++s == p.stages) { s = 0; ph ^= 1u; }
         }
+        if constexpr (CHAIN) u = take();
+        else u += gridDim.x;
       }
     }
     return;
@@ -212,8 +395,21 @@ __global__ void __launch_bounds__(kTcThreads, 1) conv_tc_kernel(const __grid_con
   uint32_t ph = 0;
   int eb = 0;          // tile buffer of this unit (staged epilogue)
   uint32_t eph = 0;    // bit b: phase of efull[b]
-  for (int u = blockIdx.x; u < units; u += gridDim.x) {
-    const TcUnit w = tc_unit(p, u, m_tiles, nchunks_all);
+  int rs = 0;
+  uint32_t rph = 0;
+  auto take = [&]() {  // chain: every thread reads the id, one arrival per warp
+    mbar_wait(&ufull[rs], rph);
+    const int v = uid[rs];
+    __syncwarp();
+    if (lane == 0) mbar_arrive_local(&uempty[rs]);
+    if (++rs == kChainRing) { rs = 0; rph ^= 1u; }
+    return v;
+  };
+  int u;
+  if constexpr (CHAIN) u = take();
+  else u = blockIdx.x;
+  for (; u < units; u = CHAIN ? take() : u + (int)gridDim.x) {
+    const TcUnit w = unit_of(u);
     int prev = -1;
     for (int q = 0; q < w.nchunks; ++q) {
       mbar_wait(&full[s], ph);
@@ -269,6 +465,14 @@ __global__ void __launch_bounds__(kTcThreads, 1) conv_tc_kernel(const __grid_con
     if constexpr (NT >= 32) {
       // ---- staged: the residual comes from and the output goes to tile buffer eb; warp 1 moves both with TMA ----
       // The arithmetic is conv_epilogue_row's.  A thread's residual and output elements share their addresses.
+      int FC = p.FC, res_mode = p.residual, relu = p.relu;
+      const float* scale = p.scale;
+      const float* shift = p.shift;
+      if constexpr (CHAIN) {
+        FC = cp->g.FC[w.c]; res_mode = cp->g.residual[w.c]; relu = cp->g.relu[w.c];
+        scale = cp->scale[w.k][w.c];
+        shift = cp->shift[w.k][w.c];
+      }
       mbar_wait(&efull[eb], (eph >> eb) & 1u);
       eph ^= 1u << eb;
       const uint32_t e0 = smem_u32(ebuf + eb * epi_bytes);
@@ -278,12 +482,12 @@ __global__ void __launch_bounds__(kTcThreads, 1) conv_tc_kernel(const __grid_con
         int ch;
         long pix;
         epilogue_target(p, co, 0, ch, pix);
-        return ch < p.FC;
+        return ch < FC;
       };
       float2 sc = make_float2(0.f, 0.f), sh = sc;
       if (fc_ok(w.n0 + c2)) {
-        sc = __ldg(reinterpret_cast<const float2*>(p.scale + w.n0 + c2));
-        sh = __ldg(reinterpret_cast<const float2*>(p.shift + w.n0 + c2));
+        sc = __ldg(reinterpret_cast<const float2*>(scale + w.n0 + c2));
+        sh = __ldg(reinterpret_cast<const float2*>(shift + w.n0 + c2));
       }
 #pragma unroll
       for (int i = 0; i < NT / 8; ++i) {
@@ -291,8 +495,8 @@ __global__ void __launch_bounds__(kTcThreads, 1) conv_tc_kernel(const __grid_con
         const bool ok = fc_ok(co);
         float2 sc_next = sc, sh_next = sh;
         if (i + 1 < NT / 8 && fc_ok(co + 8)) {
-          sc_next = __ldg(reinterpret_cast<const float2*>(p.scale + co + 8));
-          sh_next = __ldg(reinterpret_cast<const float2*>(p.shift + co + 8));
+          sc_next = __ldg(reinterpret_cast<const float2*>(scale + co + 8));
+          sh_next = __ldg(reinterpret_cast<const float2*>(shift + co + 8));
         }
         const uint32_t slab = e0 + (uint32_t)((i >> 2) * kSlabBytes);
         const int cc = 8 * (i & 3) + c2;   // column in the slab
@@ -307,23 +511,23 @@ __global__ void __launch_bounds__(kTcThreads, 1) conv_tc_kernel(const __grid_con
           if (p.out_format == LT_FMT_F32) {
             const uint32_t a = slab + sw128(row, 4 * cc);
             float2 r = make_float2(0.f, 0.f);
-            if (p.residual != LT_RES_NONE) r = lds_f2(a);
-            if (p.residual == LT_RES_BEFORE_RELU) { v0 += r.x; v1 += r.y; }
-            if (p.relu) { v0 = fmaxf(v0, 0.f); v1 = fmaxf(v1, 0.f); }
-            if (p.residual == LT_RES_AFTER_RELU) { v0 += r.x; v1 += r.y; }
+            if (res_mode != LT_RES_NONE) r = lds_f2(a);
+            if (res_mode == LT_RES_BEFORE_RELU) { v0 += r.x; v1 += r.y; }
+            if (relu) { v0 = fmaxf(v0, 0.f); v1 = fmaxf(v1, 0.f); }
+            if (res_mode == LT_RES_AFTER_RELU) { v0 += r.x; v1 += r.y; }
             sts_f2(a, make_float2(v0, v1));
           } else {
             const uint32_t ahi = slab + sw128(row, 2 * cc), alo = slab + sw128(row, 64 + 2 * cc);
             float2 r = make_float2(0.f, 0.f);
-            if (p.residual != LT_RES_NONE) {
+            if (res_mode != LT_RES_NONE) {
               const uint32_t rh = lds32(ahi), rl = lds32(alo);
               const float2 a = __half22float2(*reinterpret_cast<const __half2*>(&rh));
               const float2 b = __half22float2(*reinterpret_cast<const __half2*>(&rl));
               r = make_float2(fmaf(b.x, kLoInv, a.x), fmaf(b.y, kLoInv, a.y));
             }
-            if (p.residual == LT_RES_BEFORE_RELU) { v0 += r.x; v1 += r.y; }
-            if (p.relu) { v0 = fmaxf(v0, 0.f); v1 = fmaxf(v1, 0.f); }
-            if (p.residual == LT_RES_AFTER_RELU) { v0 += r.x; v1 += r.y; }
+            if (res_mode == LT_RES_BEFORE_RELU) { v0 += r.x; v1 += r.y; }
+            if (relu) { v0 = fmaxf(v0, 0.f); v1 = fmaxf(v1, 0.f); }
+            if (res_mode == LT_RES_AFTER_RELU) { v0 += r.x; v1 += r.y; }
             uint32_t hi2, lo2;
             split_s32x2(v0, v1, hi2, lo2);
             sts32(ahi, hi2);
@@ -353,6 +557,19 @@ __global__ void __launch_bounds__(kTcThreads, 1) conv_tc_kernel(const __grid_con
       }
     }
   }
+}
+
+template <int NT>
+__global__ void __launch_bounds__(kTcThreads, 1) conv_tc_kernel(const __grid_constant__ CUtensorMap tmA,
+                                                                const __grid_constant__ CUtensorMap tmB,
+                                                                const __grid_constant__ TcEpiMaps tmE, const TcParams p) {
+  conv_tc_body<NT, false>(&tmA, &tmB, &tmE, p, nullptr);
+}
+
+// Chain mode of conv_tc_kernel<128>: the K loop, products, epilogue and tile box are the per-layer kernel's, so every unit computes
+// the bits its per-layer launch computes.  `p` holds what the chain's layers share (box, grid, format, terms, ring depth).
+__global__ void __launch_bounds__(kTcThreads, 1) conv_tc_chain_kernel(const __grid_constant__ TcChain chain, const TcParams p) {
+  conv_tc_body<128, true>(nullptr, nullptr, nullptr, p, &chain);
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -712,6 +929,117 @@ int conv_tc_fwd_terms(const lt_conv_desc* d, const void* in, const void* weight,
   return launch_tc(tmA, tmB, p, CoutP / Nt, (cudaStream_t)stream, d->workspace, d->workspace_bytes);
 }
 
+// ---- chain mode (lt_conv_tc_chain_fwd) ----
+// Geometry of a chain of `blocks` bottleneck blocks whose three launches `d` describes (host only): what the kernel and the
+// planner need to number the units and find their dependencies.
+static int chain_geom(const lt_conv_desc* d, int blocks, TcChainGeom* g) {
+  LT_REQUIRE(d && g, "conv_tc_chain: null pointer");
+  LT_REQUIRE(blocks >= 1 && blocks <= kChainMaxBlocks, "conv_tc_chain: %d blocks, 1 to %d per launch", blocks, kChainMaxBlocks);
+  for (int c = 0; c < 3; ++c) {
+    const lt_conv_desc& e = d[c];
+    LT_REQUIRE(e.in_format == LT_FMT_S32 && e.out_format == LT_FMT_S32, "conv_tc_chain: layer %d must be split-fp16 in and out", c);
+    LT_REQUIRE(e.N == d[0].N && e.OD == d[0].OD && e.OH == d[0].OH && e.OW == d[0].OW && e.ID == e.OD && e.IH == e.OH && e.IW == e.OW &&
+                   e.FD == e.OD && e.FH == e.OH && e.FW == e.OW && e.N > 0 && e.OD > 0 && e.OH > 0 && e.OW > 0,
+               "conv_tc_chain: layer %d must map the chain's output grid onto itself", c);
+    LT_REQUIRE(e.sd == 1 && e.sh == 1 && e.sw == 1 && e.osd == 1 && e.osh == 1 && e.osw == 1 && e.ood == 0 && e.ooh == 0 && e.oow == 0 &&
+                   out_groups(&e) == 1,
+               "conv_tc_chain: layer %d must be a stride-1 conv with a plain output", c);
+    LT_REQUIRE(e.KD > 0 && e.KH > 0 && e.KW > 0 && 2 * e.pd == e.KD - 1 && 2 * e.ph == e.KH - 1 && 2 * e.pw == e.KW - 1,
+               "conv_tc_chain: layer %d must pad to its own output size", c);
+    LT_REQUIRE(e.Cin % 32 == 0 && e.Cout % 128 == 0 && e.FC == e.Cout && e.Cin == d[(c + 2) % 3].Cout,
+               "conv_tc_chain: layer %d channels %d -> %d (FC %d) do not chain at N tile 128", c, e.Cin, e.Cout, e.FC);
+    LT_REQUIRE(c == 2 ? (e.residual == LT_RES_BEFORE_RELU || e.residual == LT_RES_AFTER_RELU) : e.residual == LT_RES_NONE,
+               "conv_tc_chain: only the expansion (layer 2) adds the residual");
+  }
+  int box[4];
+  pick_box(d[0].OW, d[0].OH, d[0].OD, d[0].N, box);
+  g->blocks = blocks;
+  g->bw = box[0]; g->bh = box[1]; g->bd = box[2]; g->bn = box[3];
+  g->OW = d[0].OW; g->OH = d[0].OH; g->OD = d[0].OD;
+  g->tw = ceil_div(g->OW, g->bw); g->th = ceil_div(g->OH, g->bh); g->td = ceil_div(g->OD, g->bd); g->tn = ceil_div(d[0].N, g->bn);
+  g->m_tiles = g->tw * g->th * g->td * g->tn;
+  g->units_per_block = 0;
+  for (int c = 0; c < 3; ++c) {
+    const lt_conv_desc& e = d[c];
+    g->n_tiles[c] = e.Cout / 128;
+    g->CB[c] = e.Cin / 32;
+    g->KW[c] = e.KW; g->KH[c] = e.KH; g->KD[c] = e.KD;
+    g->pw[c] = e.pw; g->ph[c] = e.ph; g->pd[c] = e.pd;
+    g->chunks[c] = e.KD * e.KH * e.KW * g->CB[c];
+    g->CoutP[c] = e.Cout;
+    g->FC[c] = e.FC;
+    g->residual[c] = e.residual;
+    g->relu[c] = e.relu;
+    g->units_per_block += g->m_tiles * g->n_tiles[c];
+  }
+  LT_REQUIRE((long)g->units_per_block * blocks < (1L << 30), "conv_tc_chain: too many work units");
+  return LT_OK;
+}
+
+// one launch's parameters: the chain's kernel parameter block, beside TcParams, must stay within the 32764 bytes a launch takes
+static_assert(sizeof(TcChain) + sizeof(TcParams) + 64 <= 32764, "conv_tc_chain_kernel parameters exceed the launch limit");
+
+static int launch_chain(const lt_conv_desc* d, int blocks, void* x, void* const* bufs, const void* const* weights,
+                        const float* const* scales, const float* const* shifts, void* counters, size_t counters_bytes, int terms,
+                        cudaStream_t st) {
+  static thread_local TcChain ch;   // ~17 KB: kept off the stack
+  memset(&ch, 0, sizeof(ch));
+  int rc = chain_geom(d, blocks, &ch.g);
+  if (rc) return rc;
+  const TcChainGeom& g = ch.g;
+  LT_REQUIRE(x && bufs && weights && scales && shifts && counters, "conv_tc_chain: null pointer");
+  const size_t ncount = 1 + (size_t)3 * blocks * g.m_tiles;
+  LT_REQUIRE(counters_bytes >= ncount * sizeof(unsigned), "conv_tc_chain: counters need %zu bytes", ncount * sizeof(unsigned));
+  void* in_of[3][2] = {{x, x}, {bufs[0], bufs[1]}, {bufs[2], bufs[3]}};
+  void* out_of[3][2] = {{bufs[0], bufs[1]}, {bufs[2], bufs[3]}, {x, x}};
+  for (int i = 0; i < 4; ++i) LT_REQUIRE(bufs[i] && reinterpret_cast<uintptr_t>(bufs[i]) % 16 == 0, "conv_tc_chain: buffer %d", i);
+  LT_REQUIRE(reinterpret_cast<uintptr_t>(x) % 16 == 0, "conv_tc_chain: x must be 16-byte aligned (TMA global addresses)");
+  TcParams p;
+  fill_params(&d[0], p, g.CB[0], g.CoutP[0], 128, terms, nullptr, nullptr, nullptr, x);
+  tc_layout(128, 1, kTcShortK + 1, &p.stages, &p.epi_buffers);   // one tile buffer, the deep ring: every chained layer has > 4 chunks
+  for (int c = 0; c < 3; ++c) {
+    for (int q = 0; q < 2; ++q) {
+      rc = make_in_map(&ch.a[c][q], &d[c], p.bw, p.bh, p.bd, p.bn, in_of[c][q]);
+      if (rc) return rc;
+      TcParams lp;
+      fill_params(&d[c], lp, g.CB[c], g.CoutP[c], 128, terms, nullptr, nullptr, c == 2 ? x : nullptr, out_of[c][q]);
+      TcEpiMaps em;
+      rc = make_epi_maps(lp, &em);
+      if (rc) return rc;
+      ch.out[c][q] = em.out[0];
+      if (c == 2) ch.res = em.res[0];
+    }
+  }
+  for (int k = 0; k < blocks; ++k)
+    for (int c = 0; c < 3; ++c) {
+      const int l = 3 * k + c;
+      LT_REQUIRE(weights[l] && scales[l] && shifts[l], "conv_tc_chain: null filter, scale or shift of layer %d", l);
+      const uint64_t dims[2] = {64, (uint64_t)g.chunks[c] * g.CoutP[c]};
+      const uint64_t str[1] = {128};
+      const uint32_t bx[2] = {64, 128};
+      rc = make_map(&ch.b[k][c], weights[l], 2, dims, str, bx, nullptr, 1);
+      if (rc) return rc;
+      ch.scale[k][c] = scales[l];
+      ch.shift[k][c] = shifts[l];
+    }
+  ch.counters = static_cast<unsigned*>(counters);
+  cudaError_t e = cudaMemsetAsync(counters, 0, ncount * sizeof(unsigned), st);
+  if (e != cudaSuccess) return fail(LT_ERR_CUDA, "conv_tc_chain: cudaMemsetAsync: %s", cudaGetErrorString(e));
+  const long units = (long)g.units_per_block * blocks;
+  const int grid = (int)(units < sm_count() ? units : sm_count());
+  const size_t smem = (size_t)p.stages * (kATileBytes + 128 * 128) + (size_t)p.epi_buffers * tc_epi_bytes(128, 1) + (2 * p.stages + 4) * 8 +
+                      kChainRing * (2 * 8 + 4) + 1024;
+  static DeviceOnce configured;
+  if (configured.first()) {
+    e = cudaFuncSetAttribute(conv_tc_chain_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(227 * 1024));
+    if (e != cudaSuccess) return fail(LT_ERR_CUDA, "conv_tc_chain: cudaFuncSetAttribute: %s", cudaGetErrorString(e));
+  }
+  conv_tc_chain_kernel<<<grid, kTcThreads, smem, st>>>(ch, p);
+  e = cudaGetLastError();
+  if (e != cudaSuccess) return fail(LT_ERR_CUDA, "conv_tc_chain_kernel: %s", cudaGetErrorString(e));
+  return LT_OK;
+}
+
 // ---- weight packing: fp32 [taps][Cin][Cout] -> fp16 [taps][Cin/32][CoutP][32 hi | 32 lo] (128-byte rows) ----------
 __global__ void __launch_bounds__(256) pack_weights_kernel(const float* __restrict__ w, sh_t* __restrict__ out,
                                                            int taps, int Cin, int Cout, int CoutP) {
@@ -755,6 +1083,54 @@ extern "C" int lt_conv_tc_plan(const lt_conv_desc* d, int sm_count, int splitk, 
           sm_count, &plan->splits, &plan->grid);
   tc_layout(plan->nt, plan->splits, plan->chunks, &plan->stages, &plan->epi_buffers);
   return LT_OK;
+}
+
+extern "C" int lt_conv_tc_chain_plan(const lt_conv_desc* descs, int blocks, int sm_count, lt_conv_tc_chain_launch_plan* plan) {
+  LT_REQUIRE(plan && sm_count > 0, "conv_tc_chain_plan: bad arguments");
+  TcChainGeom g;
+  const int rc = chain_geom(descs, blocks, &g);
+  if (rc) return rc;
+  plan->m_tiles = g.m_tiles;
+  for (int c = 0; c < 3; ++c) plan->n_tiles[c] = g.n_tiles[c];
+  plan->units = g.units_per_block * blocks;
+  plan->grid = plan->units < sm_count ? plan->units : sm_count;
+  plan->counters = 1 + 3 * blocks * g.m_tiles;
+  return LT_OK;
+}
+
+extern "C" int lt_conv_tc_chain_deps(const lt_conv_desc* descs, int blocks, int unit, lt_conv_tc_chain_unit* info, int* tiles, int cap) {
+  LT_REQUIRE(info && (tiles || cap == 0), "conv_tc_chain_deps: bad arguments");
+  TcChainGeom g;
+  const int rc = chain_geom(descs, blocks, &g);
+  if (rc) return rc;
+  LT_REQUIRE(unit >= 0 && unit < g.units_per_block * blocks, "conv_tc_chain_deps: unit %d out of range", unit);
+  int k, c, m, n, src, need, lo[4], hi[4];
+  chain_unit(g, unit, k, c, m, n);
+  info->layer = 3 * k + c;
+  info->m_tile = m;
+  info->n_tile = n;
+  info->src_layer = -1;
+  info->need = 0;
+  info->n_deps = 0;
+  if (!chain_deps(g, k, c, m, src, need, lo, hi)) return LT_OK;
+  info->src_layer = src;
+  info->need = need;
+  for (int tn = lo[3]; tn <= hi[3]; ++tn)
+    for (int td = lo[2]; td <= hi[2]; ++td)
+      for (int th = lo[1]; th <= hi[1]; ++th)
+        for (int tw = lo[0]; tw <= hi[0]; ++tw) {
+          LT_REQUIRE(info->n_deps < cap, "conv_tc_chain_deps: more than %d tiles", cap);
+          tiles[info->n_deps++] = ((tn * g.td + td) * g.th + th) * g.tw + tw;
+        }
+  return LT_OK;
+}
+
+extern "C" int lt_conv_tc_chain_fwd(const lt_conv_desc* descs, int blocks, void* x, void* const* bufs, const void* const* weights,
+                                    const float* const* scales, const float* const* shifts, void* counters, size_t counters_bytes, int impl,
+                                    void* stream) {
+  LT_REQUIRE(impl == LT_CONV_TC || impl == LT_CONV_TC1, "conv_tc_chain: impl %d is not a tensor-core conv", impl);
+  return launch_chain(descs, blocks, x, bufs, weights, scales, shifts, counters, counters_bytes, impl == LT_CONV_TC ? 3 : 1,
+                      (cudaStream_t)stream);
 }
 
 extern "C" size_t lt_conv_tc_weight_bytes(int taps, int Cin, int Cout) {

@@ -276,6 +276,7 @@ def conv_desc(N, in_dims, cin, cout, k, stride, pad, out_dims, out_full, out_c, 
 
 
 SPLITK_WS_BYTES = 32 << 20
+CHAIN_MAX_BLOCKS = 36     # bottleneck blocks per lt_conv_tc_chain_fwd launch (its kernel parameter block holds 3 filter maps per block)
 _SPLITK_WS = {}
 
 
@@ -359,6 +360,7 @@ class NativeEngine:
         self._grids2d = {}         # (h, w, B*V, device) -> pixel_grid of the algebraic forward's 2-D soft-argmax
         self.launches = 0          # kernels launched by the last eager forward (our own kernels only)
         self.timeline = None       # set to [] to record (label, flops, bytes, start_evt, end_evt) per launch
+        self._chain_runs = {}      # (layer, block, input shape) -> _chain_run's answer for the current packs
         capi.lib()                 # fail loudly if the extension is missing
 
     # ------------------------------------------------------------------ weight packing
@@ -423,6 +425,7 @@ class NativeEngine:
                                              for i in (0, 2, 4)]
             if not hasattr(m, "volume_net"):
                 self._packs, self._packs_version = P, ver
+                self._chain_runs = {}
                 self._graphs = {}
                 return
             P["process_features"] = self._pack_conv(m.process_features[0], None, out_fmt=FMT_F32)
@@ -452,6 +455,7 @@ class NativeEngine:
             P["back2"] = self._pack_conv(v.back_layers[2].block[0], v.back_layers[2].block[1])
             P["output"] = self._pack_conv(v.output_layer, None, out_fmt=FMT_F32)
         self._packs, self._packs_version = P, ver
+        self._chain_runs = {}
         self._graphs = {}
 
     # ------------------------------------------------------------------ op helpers
@@ -568,7 +572,15 @@ class NativeEngine:
         x = self._maxpool(x, (1, 3, 3), (1, 2, 2), (0, 1, 1))
         bb = self.model.backbone
         for li in range(1, 5):
-            for ui, unit in enumerate(getattr(bb, "layer%d" % li)):
+            units = getattr(bb, "layer%d" % li)
+            ui = 0
+            while ui < len(units):
+                run = self._chain_run(x, li, ui, units)
+                if run:
+                    x = self._chain(x, ["layer%d.%d" % (li, ui + i) for i in range(run[0])], run[1])
+                    ui += run[0]
+                    continue
+                unit = units[ui]
                 key = "layer%d.%d" % (li, ui)
                 n_st = len(unit.stages())
                 identity = self._conv(x, P[key + ".ds"], relu=False) if unit.downsample is not None else x
@@ -576,6 +588,74 @@ class NativeEngine:
                 for si in range(n_st - 1):
                     y = self._conv(y, P["%s.c%d" % (key, si)], relu=True)
                 x = self._conv(y, P["%s.c%d" % (key, n_st - 1)], relu=True, residual=identity, res_mode=RES_BEFORE_RELU)
+                ui += 1
+        return x
+
+    def _chain_descs(self, x, pks):
+        """The lt_conv_nd_fwd descriptors of one bottleneck block (1x1 reduce, 3x3, 1x1 expansion + residual) over Act x."""
+        dims = (x.D, x.H, x.W)
+        return [conv_desc(x.N, dims, pk.cin, pk.cout_p, pk.k, pk.stride, pk.pad, dims, dims, pk.cout_p, FMT_S32, FMT_S32, relu=True,
+                          res_mode=RES_BEFORE_RELU if i == 2 else RES_NONE) for i, pk in enumerate(pks)]
+
+    def _chain_run(self, x, li, ui, units):
+        """(blocks, descs) of the chain launch (lt_conv_tc_chain_fwd) that runs blocks ui.. of backbone layer li, or None: the
+        per-layer launches run them.  A run is the longest stretch of bottleneck blocks without downsample whose three layers map the
+        grid of x onto itself at N tile 128 (stride 1, Cout a multiple of 128) and whose per-layer launches would not split K: the
+        chain runs exactly their products and epilogues, so its outputs are bit-identical to theirs."""
+        if not x.data.is_cuda or x.fmt != FMT_S32 or self.tc_impl == CONV_SIMT:
+            return None
+        P = self._packs
+        key = (li, ui, x.N, x.D, x.H, x.W, x.C)
+        cache = self._chain_runs
+        if key in cache:
+            return cache[key]
+
+        def block(i):
+            u = units[i]
+            if u.downsample is not None or len(u.stages()) != 3:
+                return None
+            pks = [P["layer%d.%d.c%d" % (li, i, si)] for si in range(3)]
+            if any(pk.impl != self.tc_impl or pk.w_fold is not None or pk.cout_p % 128 or tuple(pk.stride) != (1, 1, 1) for pk in pks):
+                return None
+            return pks
+
+        run, descs = 0, None
+        first = block(ui)
+        if first is not None and x.C == first[2].cout_p == first[0].cin:
+            descs = self._chain_descs(x, first)
+            ws = splitk_workspace(x.data.device) if self._splitk_ws is None else self._splitk_ws
+            sms = torch.cuda.get_device_properties(x.data.device).multi_processor_count
+            plans = []
+            for d in descs:
+                d.workspace, d.workspace_bytes = ws.data_ptr(), ws.numel()
+                plans.append(capi.conv_tc_plan(d, sms, capi.get_options()["tc_splitk"]))
+                d.workspace, d.workspace_bytes = None, 0
+            if all(p["splits"] == 1 and p["nt"] == 128 for p in plans):
+                shape = [(pk.k, pk.pad, pk.cin, pk.cout_p) for pk in first]
+                run = 1
+                while ui + run < len(units) and run < CHAIN_MAX_BLOCKS:
+                    nxt = block(ui + run)
+                    if nxt is None or [(pk.k, pk.pad, pk.cin, pk.cout_p) for pk in nxt] != shape:
+                        break
+                    run += 1
+                capi.conv_tc_chain_plan(descs, run, sms)   # the C side's own checks
+        cache[key] = (run, descs) if run else None
+        return cache[key]
+
+    def _chain(self, x, keys, descs):
+        """Blocks `keys` of the backbone as one chain launch, in place on x (lt_conv_tc_chain_fwd)."""
+        P = self._packs
+        pks = [P["%s.c%d" % (k, si)] for k in keys for si in range(3)]
+        dev = x.data.device
+        mid = pks[0].cout_p
+        bufs = [Act(x.N, x.D, x.H, x.W, mid, FMT_S32, dev).data for _ in range(4)]
+        plan = capi.conv_tc_chain_plan(descs, len(keys), 1)
+        counters = torch.empty(plan["counters"], dtype=torch.int32, device=dev)
+        flops = sum(2.0 * x.N * x.D * x.H * x.W * pk.kmacs for pk in pks)
+        with self._timed("conv_tc", flops=flops, desc="chain %s..%s N%d %dx%d Cin%d" % (keys[0], keys[-1], x.N, x.H, x.W, x.C)):
+            capi.conv_tc_chain(descs, len(keys), x.data, bufs, [pk.w for pk in pks], [pk.scale for pk in pks], [pk.shift for pk in pks],
+                               counters, self.tc_impl)
+        self.launches += 1
         return x
 
     def unproject(self, feats, B, V, proj, coord, agg, conf=None):
