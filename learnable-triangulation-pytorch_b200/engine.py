@@ -357,6 +357,7 @@ class NativeEngine:
         self._packs_version = None
         self._epoch = 0
         self._graphs = {}
+        self.captures = 0          # CUDA graphs captured by replay()
         self._grids2d = {}         # (h, w, B*V, device) -> pixel_grid of the algebraic forward's 2-D soft-argmax
         self.launches = 0          # kernels launched by the last eager forward (our own kernels only)
         self.timeline = None       # set to [] to record (label, flops, bytes, start_evt, end_evt) per launch
@@ -1009,25 +1010,39 @@ class NativeEngine:
     def forward(self, images, proj, position, center, step, rot):
         """All inputs are CUDA float32 tensors. Returns (keypoints, features, volumes, coord_volumes)."""
         self.prepare()
+        inputs = (images, proj, position, center, step, rot)
         if not self.use_graph:
-            return self._device_forward(images, proj, position, center, step, rot)
-        key = (tuple(images.shape), images.device.index)
+            return self._device_forward(*inputs)
+        return self.replay((tuple(images.shape), images.device.index), self._device_forward, inputs)
+
+    def algebraic_forward_graphed(self, images, proj, heatmap_multiplier, use_confidences, heatmap_softmax=True):
+        """algebraic_forward replayed from one CUDA graph per (images shape, device): -> the graph's static outputs."""
+        self.prepare()
+        fn = lambda im, pr: self.algebraic_forward(im, pr, heatmap_multiplier, use_confidences, heatmap_softmax)
+        return self.replay(("algebraic", tuple(images.shape), images.device.index), fn, (images, proj))
+
+    def replay(self, key, fn, inputs):
+        """fn(*inputs), a device forward of the prepared packs, replayed from the CUDA graph cached under `key` -> its static
+        outputs, overwritten by the next replay.  A miss runs fn eagerly on a side stream first (module loads, function attributes,
+        the split-K scratch, the soft-argmax grids), then captures it there, reading static copies of the inputs; `captures` counts
+        them.  The capture is thread_local: a DataLoader's pin-memory thread may make CUDA calls meanwhile (a validation pass captures
+        at its first batch, when that thread is prefetching).  prepare() and invalidate() drop the graphs with the packs they read."""
         g = self._graphs.get(key)
         if g is None:
-            static_in = [t.clone() for t in (images, proj, position, center, step, rot)]
-            s = torch.cuda.Stream(device=images.device)
+            static_in = [t.clone() for t in inputs]
+            s = torch.cuda.Stream(device=inputs[0].device)
             s.wait_stream(torch.cuda.current_stream())
             with torch.cuda.stream(s):
-                self._device_forward(*static_in)      # warm-up (module load, func attributes)
+                fn(*static_in)
             torch.cuda.current_stream().wait_stream(s)
             torch.cuda.synchronize()
             graph = torch.cuda.CUDAGraph()
-            with torch.cuda.graph(graph):
-                static_out = self._device_forward(*static_in)
-            g = (graph, static_in, static_out, self.launches)
-            self._graphs[key] = g
+            with torch.cuda.graph(graph, stream=s, capture_error_mode="thread_local"):
+                static_out = fn(*static_in)
+            g = self._graphs[key] = (graph, static_in, static_out, self.launches)
+            self.captures += 1
         graph, static_in, static_out, launches = g
-        for dst, src in zip(static_in, (images, proj, position, center, step, rot)):
+        for dst, src in zip(static_in, inputs):
             dst.copy_(src, non_blocking=True)
         graph.replay()
         self.launches = launches

@@ -224,7 +224,8 @@ class TrainStep:
     opt.load_state_dict and model.to()); a capture replaces the graphs of the same input shapes.  A capture first runs the whole
     step eagerly on a side stream and then restores the parameters, the optimizer state (a state that was empty goes back to zeros
     and step 0) and every BatchNorm buffer, so the first replay is the first update.  `captures` counts captures.  clone_outputs
-    False returns the graph's own output and metric buffers, valid until the next call.
+    False returns the graph's own output and metric buffers, valid until the next call.  Every call invalidates the model's native
+    engine, so an eval_backend="native" forward after it re-packs the updated weights.
 
     DistributedDataParallel is not supported (the gradient all-reduce would have to run inside the graph)."""
 
@@ -300,6 +301,7 @@ class TrainStep:
             self._entries[self._key(inputs)] = entry        # the capture created an empty optimizer state
         for dst, src in zip(entry.static_in, inputs):
             dst.copy_(src)
+        m._invalidate_native_eval()             # the replayed Adam and BatchNorm updates bump no tensor version
         entry.graph.replay()
         for p, g in entry.grads:
             p.grad = g

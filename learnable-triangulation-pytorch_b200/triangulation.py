@@ -58,8 +58,12 @@ def _place_cuboids(base, sides):
 _NO_V2V = object()      # the v2v_backend of a model without a V2V net (None stays an unknown v2v_backend)
 
 
-def _check_backends(backend, conv_mode, backbone_backend, norm_backend, v2v_backend=_NO_V2V, head_backend="torch"):
+def _check_backends(backend, conv_mode, backbone_backend, norm_backend, v2v_backend=_NO_V2V, head_backend="torch", eval_backend=None):
     """ValueError unless the training switches are known values in a supported combination.
+
+    eval_backend="native": an eval-mode forward without gradients of a backend="torch" / "hybrid" model runs the native engine, as
+    a backend="native" model with the same weights does (packed filters, folded BatchNorm, CUDA graphs).  Every other forward is
+    unchanged; with backend="native" it changes nothing.  None (the default) never uses the engine.
 
     v2v_backend="native" / backbone_backend="native": every Conv3d / ConvTranspose3d of volume_net / every Conv2d / ConvTranspose2d
     of the backbone, its confidence heads and `process_features` runs forward, data gradient and weight gradient on the native
@@ -85,6 +89,8 @@ def _check_backends(backend, conv_mode, backbone_backend, norm_backend, v2v_back
         raise ValueError("unknown head_backend {!r}".format(head_backend))
     if head_backend == "native" and backend != "hybrid":
         raise ValueError("head_backend='native' needs backend='hybrid' (got %r)" % (backend,))
+    if eval_backend not in (None, "native"):
+        raise ValueError("unknown eval_backend {!r} (None or 'native')".format(eval_backend))
 
 
 def _hooks(backbone_backend, norm_backend, v2v_backend="torch"):
@@ -131,10 +137,26 @@ class _EngineOwner(nn.Module):
             step.invalidate()
 
     def _run_device(self, fn, inputs):
-        """fn(*inputs): the device part of the forward, replayed from CUDA graphs with train_graph=True in a training forward."""
+        """fn(*inputs): the device part of a torch / hybrid forward, replayed from CUDA graphs with train_graph=True in a training
+        forward.  A train-mode forward invalidates the native engine (_invalidate_native_eval)."""
+        if self.training:
+            self._invalidate_native_eval()
         if self._train_graphs is not None and self.training and torch.is_grad_enabled():
             return self._train_graphs.run(self, fn, inputs, self.clone_outputs)
         return fn(*inputs)
+
+    def _invalidate_native_eval(self):
+        """Drop the native engine's packed filters and graphs, keeping the training graphs: training changes weights and BatchNorm
+        statistics where NativeEngine._param_version cannot see it (TrainStep's captured Adam, replayed BatchNorm updates, the native
+        BatchNorm's pointer writes).  Called by every train-mode forward and every TrainStep call, so the next eval_backend="native"
+        forward re-packs and re-captures, and the eval graphs and packs are not held during training."""
+        eng = self.__dict__.get("_engine")
+        if eng is not None:
+            eng.invalidate()
+
+    def _native_eval(self):
+        """Whether this forward of a torch / hybrid model runs on the native engine: eval_backend="native", eval mode, no grad."""
+        return self.eval_backend == "native" and not self.training and not torch.is_grad_enabled()
 
     def _apply(self, fn, *args, **kwargs):
         out = super()._apply(fn, *args, **kwargs)
@@ -149,7 +171,7 @@ class _EngineOwner(nn.Module):
 
 class VolumetricTriangulationNet(_EngineOwner):
     def __init__(self, config, device="cuda:0", backend=None, conv_mode=None, use_cuda_graph=True, v2v_backend="torch",
-                 backbone_backend="torch", norm_backend="torch", train_graph=False, head_backend="torch"):
+                 backbone_backend="torch", norm_backend="torch", train_graph=False, head_backend="torch", eval_backend=None):
         super().__init__()
         m = config.model
         self.num_joints = m.backbone.num_joints
@@ -178,10 +200,11 @@ class VolumetricTriangulationNet(_EngineOwner):
 
         self.backend = backend or os.environ.get("LT_B200_BACKEND", "native")
         self.conv_mode = conv_mode or os.environ.get("LT_B200_CONV", "tc")
-        _check_backends(self.backend, self.conv_mode, backbone_backend, norm_backend, v2v_backend, head_backend)
+        _check_backends(self.backend, self.conv_mode, backbone_backend, norm_backend, v2v_backend, head_backend, eval_backend)
         _check_train_graph(train_graph, self.backend)
         self.v2v_backend = v2v_backend
         self.head_backend = head_backend
+        self.eval_backend = eval_backend
         self.backbone_backend = backbone_backend
         self.norm_backend = norm_backend
         self.use_cuda_graph = use_cuda_graph
@@ -217,11 +240,15 @@ class VolumetricTriangulationNet(_EngineOwner):
 
     # ---------------------------------------------------------------- forward
     def forward(self, images, proj_matricies, batch):
-        if self.backend in ("torch", "hybrid"):
+        if self.backend in ("torch", "hybrid") and not self._native_eval():
             # "hybrid": torch/cuDNN convolutions with the native custom ops (forward + backward kernels) in the autograd graph
             return self._forward_torch(images, batch)
-        if self.backend != "native":
+        if self.backend not in ("native", "torch", "hybrid"):
             raise ValueError("unknown backend {!r}".format(self.backend))
+        return self._forward_native(images, batch)
+
+    def _forward_native(self, images, batch):
+        """The native engine's forward: backend="native", and the eval forwards of eval_backend="native"."""
         if not images.is_cuda:
             raise RuntimeError("lt_b200 native backend needs CUDA tensors (got %s); construct the model with "
                                "backend='torch' for the CPU/autograd path" % images.device)
@@ -235,14 +262,11 @@ class VolumetricTriangulationNet(_EngineOwner):
         hm_shape = (backbone_map_size(H), backbone_map_size(W))   # == H // 4 only when H is a multiple of 32
         proj, base, position, step, rots, cuboids = self._host_geometry(batch, B, (H, W), hm_shape)
         dev = images.device
-
-        def up(a):
-            return torch.from_numpy(np.ascontiguousarray(a, dtype=np.float32)).to(dev, non_blocking=True)
-
         with torch.cuda.device(dev):      # launches go to the model's device, whatever the caller's current device is
-            outs = self.engine().forward(
-                images.float().contiguous(), up(proj), up(position), up(base), up(step), up(rots.reshape(B, 9)))
-            base_points = up(base)
+            # one page-locked upload: a pageable copy would wait for the host, and a replayed forward synchronises nowhere
+            geometry = _upload(dev, proj, position, base, step, rots.reshape(B, 9))
+            outs = self.engine().forward(images.float().contiguous(), *geometry)
+            base_points = geometry[2]
         if self.clone_outputs and self.use_cuda_graph:
             outs = tuple(o.clone() for o in outs)
         kp, features, volumes, coord = outs[:4]
@@ -309,7 +333,7 @@ class AlgebraicTriangulationNet(_EngineOwner):
     with their backward kernels (trains, any mode)."""
 
     def __init__(self, config, device="cuda:0", backend=None, conv_mode=None, backbone_backend="torch", norm_backend="torch",
-                 train_graph=False, head_backend="torch"):
+                 train_graph=False, head_backend="torch", eval_backend=None):
         super().__init__()
         self.use_confidences = config.model.use_confidences
         config.model.backbone.alg_confidences = False
@@ -321,9 +345,10 @@ class AlgebraicTriangulationNet(_EngineOwner):
         self.heatmap_multiplier = config.model.heatmap_multiplier
         self.backend = backend or os.environ.get("LT_B200_BACKEND", "native")
         self.conv_mode = conv_mode or os.environ.get("LT_B200_CONV", "tc")
-        _check_backends(self.backend, self.conv_mode, backbone_backend, norm_backend, head_backend=head_backend)
+        _check_backends(self.backend, self.conv_mode, backbone_backend, norm_backend, head_backend=head_backend, eval_backend=eval_backend)
         _check_train_graph(train_graph, self.backend)
         self.head_backend = head_backend
+        self.eval_backend = eval_backend
         self.backbone_backend = backbone_backend
         self.norm_backend = norm_backend
         self.clone_outputs = True
@@ -337,20 +362,30 @@ class AlgebraicTriangulationNet(_EngineOwner):
         return self._engine
 
     def forward(self, images, proj_matricies, batch):
-        if self.backend == "torch":
-            return self._forward_torch(images, proj_matricies)
-        if self.backend == "hybrid":
-            # torch/cuDNN backbone with the native 2-D soft-argmax and DLT (forward + backward kernels) in the autograd graph
-            if not images.is_cuda:
+        if self.backend in ("torch", "hybrid") and not self._native_eval():
+            # "hybrid": torch/cuDNN backbone with the native 2-D soft-argmax and DLT (forward + backward kernels) in the autograd graph
+            if self.backend == "hybrid" and not images.is_cuda:
                 raise RuntimeError("lt_b200 hybrid backend needs CUDA tensors (native custom ops); use backend='torch' on CPU")
             return self._run_device(self._forward_torch, (images, proj_matricies))
+        return self._forward_native(images, proj_matricies)
+
+    def _forward_native(self, images, proj_matricies):
+        """The native engine's forward: backend="native" eagerly; the eval forwards of eval_backend="native" from one CUDA graph per
+        input shape, with the volumetric model's clone_outputs semantics."""
         if not images.is_cuda:
             raise RuntimeError("lt_b200 native backend needs CUDA tensors; construct the model with backend='torch' for CPU/autograd")
         if self.training or torch.is_grad_enabled():
             raise RuntimeError("lt_b200 native backend is inference-only: use model.eval() under torch.no_grad(), or backend='torch'")
+        H, W = images.shape[3:]
+        if self.conv_mode != "simt" and (H % 2 or W % 2):      # the exact-fp32 mode's stem is an ordinary conv and takes odd sides
+            raise ValueError("lt_b200 native backend needs even image sides (space-to-depth stem), got %dx%d" % (H, W))
+        args = (images.float().contiguous(), proj_matricies.float().contiguous(), self.heatmap_multiplier, self.use_confidences,
+                self.heatmap_softmax)
         with torch.cuda.device(images.device):
-            return self.engine().algebraic_forward(images.float().contiguous(), proj_matricies.float().contiguous(),
-                                                   self.heatmap_multiplier, self.use_confidences, self.heatmap_softmax)
+            if self.backend == "native":
+                return self.engine().algebraic_forward(*args)
+            outs = self.engine().algebraic_forward_graphed(*args)
+        return tuple(o.clone() for o in outs) if self.clone_outputs else outs
 
     def _forward_torch(self, images, proj_matricies):
         """The reference forward on torch autograd, (images, proj_matricies) -> (kp3d, kp2d, heatmaps, alg_conf): everything runs on
